@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — learner gradient-steps/sec (BASELINE.json metric) on N B200s.
+"""bench.py — learner gradient-steps/sec (BASELINE.json metric) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
 
 One "step" = one `learn()` call of the hot path (`ReplayBuffer.sample ->
 PolicyLearner.learn()`) with `training_rounds = --rounds` gradient steps at
@@ -9,7 +9,7 @@ batch 256 on a 1e6-transition replay buffer (BASELINE cfg2: obs=128, A=16,
 hidden [64,64]); value = K * rounds * n_gpus / max-over-ranks device time.
 Timing: CUDA events on the launch stream around the K timed calls, barrier +
 synchronize on both sides, W >= 3 warm-up calls; the 1.04 GB buffer is larger
-than the 126 MB L2, so sampled rows come from HBM.
+than the 50 MB L2, so sampled rows come from HBM.
 
   value : buffer already resident in HBM, private device RNG stream
   e2e   : through the plugin API with HOST data — every step pushes `rounds`
@@ -21,6 +21,10 @@ than the 126 MB L2, so sampled rows come from HBM.
   cpu_baseline  : the oracle port (oracle/pearl_oracle.py — eager PyTorch on the
                   host cores, the reference's own algorithm) on a bounded sample
 `--impl reference` times that CPU port alone (rank 0), same metric/config.
+`--dump-outputs DIR` writes what the last timed learn() returned and left behind (per-round loss
+reports and the flat parameter vectors of the first 32 learners) as DIR/<name>.npy; buffers, initial
+parameters and index streams are seeded and do not depend on how many learners fit in memory, so
+two builds can be compared output for output.
 N > 1: one process per GPU, each with its own buffer shard (see DESIGN.md §multi-GPU).
 """
 from __future__ import annotations
@@ -38,9 +42,7 @@ sys.path.insert(0, ROOT)
 
 OBS, N_ACT, HIDDEN, BATCH = 128, 16, (64, 64), 256
 METRIC = "learner gradient-steps/sec (batch=256, 1e6 replay)"
-
-
-TC_DRAM_BYTES_PER_STEP = 1.165e6   # measured under ncu (4.042 GB read + 1.327 GB written over 144 learners x 32 rounds), profiles/r2b_k_dqn_tc_final_ncu_raw.csv
+DUMP_LEARNERS = 32   # --dump-outputs: learners written, independent of how many the GPU holds
 
 
 def flops_per_step(obs=OBS, A=N_ACT, H1=HIDDEN[0], H2=HIDDEN[1], B=BATCH, double=False):
@@ -97,7 +99,7 @@ def peaks() -> dict:
         d = json.load(open(p))
         return {"bf16_tflops": d["bf16_tflops"], "bf16_tflops_sustained": d.get("bf16_tflops_sustained"),
                 "hbm_gbs": d["hbm_gbs"], "source": "measured"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "source": "fallback"}
+    return {"bf16_tflops": 989.0, "bf16_tflops_sustained": None, "hbm_gbs": 3350.0, "source": "NVIDIA H100 SXM data sheet (700 W)"}
 
 
 # ----------------------------------------------------------------------------- CPU reference arm
@@ -212,7 +214,7 @@ def run_reference(args) -> None:
                    "training_rounds_per_step": args.ref_rounds, "hidden": list(HIDDEN), "cpu_buffer": args.ref_capacity,
                    "same_config": False,
                    "differences": "the CPU learners sample from deques of 20k transitions (not 1e6) and run 40 rounds per learn() "
-                                  "(the B200 arm: 512); neither changes the cost of a gradient step"},
+                                  "(the GPU arm: 512); neither changes the cost of a gradient step"},
         "cpu_baseline": r,
         "e2e": {"value": r["value"], "unit": "gradient-steps/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
         "gpu_launches": 0,
@@ -220,7 +222,7 @@ def run_reference(args) -> None:
     print(json.dumps(line), flush=True)
 
 
-# ----------------------------------------------------------------------------- B200 arm
+# ----------------------------------------------------------------------------- GPU arm
 class Space:
     def __init__(self, n):
         import torch
@@ -293,11 +295,19 @@ def run_b200(args) -> None:
     kernel_ms = []
     e0.record()
     for _ in range(args.steps):
-        group.learn()
+        reports = group.learn()
         kernel_ms.append(group.last_kernel_ms())
     e1.record()
     barrier()
     clk = clocks.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        # the first DUMP_LEARNERS learners: learner i's buffer, parameters and index stream do not depend on how many fit
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        n_dump = min(R, DUMP_LEARNERS)
+        np.save(os.path.join(args.dump_outputs, "loss.npy"), np.asarray([r["loss"] for r in reports[:n_dump]], dtype=np.float32))
+        np.save(os.path.join(args.dump_outputs, "parameters.npy"),
+                torch.stack([l.flat_parameters for l in learners[:n_dump]]).float().cpu().numpy())
     t = torch.tensor([e0.elapsed_time(e1)], device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -416,12 +426,8 @@ def run_b200(args) -> None:
             "gpu_launches": args.steps * launches_group,
             "clocks": clk,
             "roofline": {"bound": "tensor", "kernel": "k_dqn_tc", "achieved": achieved, "peak": peak, "unit": "TFLOP/s",
-                         "frac": achieved / peak, "traffic": TC_DRAM_BYTES_PER_STEP * rounds * R,
-                         "traffic_source": "dram__bytes_read.sum + dram__bytes_write.sum of the `ncu --set full` capture of k_dqn_tc in "
-                                           "profiles/r2b_k_dqn_tc_final_ncu_raw.csv (1.17 MB per gradient step with 144 learners' parameters, AdamW state and operand "
-                                           "tiles competing for L2; algorithmic gather 266 KB), "
-                                           "scaled to the gradient steps of one bench launch",
-                         "peak_source": f"{pk['source']} bf16 dense (sustained: kernel timed inside a long step)",
+                         "frac": achieved / peak,
+                         "peak_source": f"{pk['source']} bf16 dense",
                          "flops_per_gradient_step_factored": fact, "flops_per_gradient_step_as_written": as_written,
                          "kernel_ms_per_launch": k_ms, "gradient_steps_per_launch": rounds * R,
                          "note": "3xTF32: every algorithmic FLOP is issued 3x on the TF32 pipe (half the bf16 rate), so the "
@@ -645,9 +651,8 @@ def other_paths(dev, args) -> dict:
                       "kernels_per_step": kps,
                       "engine": "automatic contraction engine: at batch 512 every product runs on the fp32 SIMT tiles with the contraction "
                                 "axis sliced over 4 warp groups (k_gemm<32,32,2,4>); CUDA-graph replay",
-                      "with_tcgen05_contractions_forced": {"value": R / sec2, "us_per_step": sec2 / R * 1e6,
-                                                           "note": "engine 2: every product on k_gemm_tc (3xTF32 tcgen05, 128 x 64 tiles); slower at this "
-                                                                   "batch size, see profiles/r2_gemm_tc.md"}}
+                      "with_tensor_core_contractions_forced": {"value": R / sec2, "us_per_step": sec2 / R * 1e6,
+                                                           "note": "engine 2: every product on k_gemm_tc (3xTF32 wgmma, 128 x 64 tiles)"}}
         del buf
         if not args.no_cpu:
             from oracle.sac_oracle import OracleSAC
@@ -682,7 +687,7 @@ def other_paths(dev, args) -> dict:
                       "preprocess_ms": pre_sec * 1e3, "preprocess_transitions_per_s": n / pre_sec,
                       "value": R / (sec - pre_sec), "unit": "gradient-steps/s (actor + critic steps, preprocessing excluded)",
                       "learn_ms": sec * 1e3, "training_rounds": R,
-                      "engine": "rollout passes (8192 rows each): 3xTF32 tcgen05 contractions (k_gemm_tc); training rounds at batch 256: fp32 SIMT "
+                      "engine": "rollout passes (8192 rows each): 3xTF32 wgmma contractions (k_gemm_tc); training rounds at batch 256: fp32 SIMT "
                                 "tiles (k_gemm<32,32,2,*>), CUDA-graph replay",
                       "with_simt_contractions_only": {"value": R / (sec0 - pre0), "preprocess_ms": pre0 * 1e3}}
         del buf
@@ -809,6 +814,8 @@ def main() -> None:
     ap.add_argument("--no-dp", action="store_true", help="N > 1: skip the sharded-replay single-learner record")
     ap.add_argument("--dp-rounds", type=int, default=256)
     ap.add_argument("--no-extras", action="store_true", help="skip the SAC / PPO / prioritized-replay side measurements")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's loss reports and parameters of the first 32 learners to DIR/<name>.npy")
     ap.add_argument("--extras-only", action="store_true", help="developer: run only the side measurements on cuda:0")
     args = ap.parse_args()
     # stdout carries the ONE JSON line and nothing else: libraries that print there (NCCL's version banner, torch warnings

@@ -1,4 +1,4 @@
-/* pearl_b200.h — C ABI of libpearlb200.so: the B200-native learner hot path of
+/* pearl_b200.h — C ABI of libpearlb200.so: the H100-native learner hot path of
  * facebookresearch/Pearl (`ReplayBuffer.sample -> PolicyLearner.learn()`).
  *
  * Conventions
@@ -38,8 +38,8 @@ extern "C" {
 
 /* ---- library ----------------------------------------------------------- */
 int prl_abi_version(void);
-/* Select `device` for the calling thread and check it is sm_100 (B200).
- * There is no CPU fallback: without a B200 this returns PRL_EUNSUPPORTED. */
+/* Select `device` for the calling thread and check it is sm_90 (H100).
+ * There is no CPU fallback: without an H100 this returns PRL_EUNSUPPORTED. */
 int prl_init(int device);
 const char *prl_last_error(void);
 /* multiprocessor count of the current device (grid sizing, reported by bench) */
@@ -274,8 +274,8 @@ int prl_dqn_set_comm(prl_dqn *dqn, prl_comm *comm);
 /* ---- tensor-core learner, one SM per learner (aggregate mode) -----------------------------
  * PolicyLearner.learn() for `count` INDEPENDENT learners (seeds / agents; the reference runs those
  * as separate OS processes, utils/scripts/benchmark.py:80-116) in one launch: CTA i trains learner
- * dqns[i] on buffer bufs[i] for `rounds` gradient steps with every dense contraction on tcgen05
- * (3xTF32, fp32 accumulation in TMEM).  Same arithmetic contract and outputs as prl_dqn_learn, per
+ * dqns[i] on buffer bufs[i] for `rounds` gradient steps with every dense contraction on wgmma
+ * (3xTF32, fp32 accumulation in registers).  Same arithmetic contract and outputs as prl_dqn_learn, per
  * learner; out_mae (required) / out_q / out_y / out_logical are arrays of `count` device pointers
  * (the optional arrays and their entries may be NULL).  Shape class: hidden [64,64], obs % 8 == 0
  * and <= 128, n_actions in {1,2,4,8,16}, DeepQLearning (not DoubleDQN), batch 128 or 256, all
@@ -456,25 +456,25 @@ int prl_dqn_set_timing(prl_dqn *dqn, int enable);
 int prl_dqn_set_profile(prl_dqn *dqn, long long *stamps_dev);
 int prl_dqn_last_kernel_ms(prl_dqn *dqn, float *ms);
 
-/* Self-test of the tcgen05 / TMEM building block used by the learner kernels: one CTA computes
+/* Self-test of the wgmma building block used by the learner kernels: one CTA computes
  * D[128][n] = A[128][k] * B[n][k]^T (device fp32 row-major arrays) with plain TF32 (passes = 1) or
  * the 3xTF32 split the learner uses for fp32 parity (passes = 3).  Test infrastructure hook. */
 int prl_test_umma_gemm(const float *a_dev, const float *b_dev, float *d_dev, int n, int k, int passes,
                        void *stream);
-/* Same product with the A operand in tensor memory (written by tcgen05.st), B in shared memory;
- * k <= 64; reps > 1 prints a throughput probe. */
+/* Same product with the A operand in registers (RS form), B in shared memory;
+ * k <= 64, n = 32 or a multiple of 64; `reps` is ignored. */
 int prl_test_umma_gemm_ts(const float *a_dev, const float *b_dev, float *d_dev, int n, int k, int reps, void *stream);
 /* General self-test: D[m][n] = A[m][k] * B[n][k]^T with m in {64,128} and a free operand chunk pitch
- * `lbo` (128 dense / 144 transposed-write friendly, see csrc/umma.cuh).  draw_dev receives the raw
- * accumulator: 128 TMEM lanes x n columns (for m = 64, row i is lane 32*(i/16) + i%16). */
+ * `lbo` (128 dense / 144 transposed-write friendly, see csrc/umma.cuh).  draw_dev receives the
+ * product, row-major [m x n]. */
 int prl_test_umma_gemm2(const float *a_dev, const float *b_dev, float *draw_dev, int m, int n, int k, int lbo,
                         void *stream);
 
 /* ---- contraction engine of the actor-critic learners (SAC, PPO, TD3 / DDPG) --------------------------------
  * The dense layers of those learners (the torch matmuls of pearl/neural_networks/common/utils.py:mlp_block as used by
- * actor_networks.py / value_networks.py, forward and autograd backward) run as 3xTF32 tcgen05 tiles or as fp32 SIMT tiles:
- * engine 1 (default) picks per product whichever is faster on a B200 (profiles/r2_gemm_tc.md), 0 = SIMT only,
- * 2 = tcgen05 always.  Process-wide; read when a learner's round is launched or captured into its CUDA graph, so set it
+ * actor_networks.py / value_networks.py, forward and autograd backward) run as 3xTF32 wgmma tiles or as fp32 SIMT tiles:
+ * engine 1 (default) uses the tensor-core tiles for products with at least 4096 output rows (a threshold not measured on H100), 0 = SIMT only,
+ * 2 = tensor cores always.  Process-wide; read when a learner's round is launched or captured into its CUDA graph, so set it
  * before the first learn() of a learner. */
 int prl_set_contraction_engine(int engine);
 int prl_get_contraction_engine(void);
@@ -482,15 +482,11 @@ int prl_get_contraction_engine(void);
  *   op 0  c[M x N]   = act(x W^T + bias)      a = x [M x K] (or [M x split] and a2 = [M x (K - split)]), b = W [N x K]
  *   op 1  c[M x K] (+)= dy W, masked          a = dy [M x N], b = W [N x K], mask [M x K] (keep where mask > 0)
  *   op 2  c[N x K]   = dy^T x, c_tail = dy^T 1  a = dy [M x N], b = x [M x K] (or split with a2)
- * engine: -1 library default, 0 SIMT, 1 automatic, 2 tcgen05 always; 64 / 32: the shared-memory-operand form with that tile
- * width, 164 / 132: the tensor-memory-operand form with tile width 64 / 32. */
+ * engine: -1 library default, 0 SIMT, 1 automatic, 2 tensor cores always; 64 / 32: the shared-memory-operand form with that tile
+ * width, 164 / 132: the register-operand form with tile width 64 / 32. */
 int prl_test_contraction(int op, int engine, int M, int N, int K, const float *a, const float *b, const float *a2, int split,
                          const float *bias, const float *mask, int relu, int accumulate, float *c, float *c_tail, int nets,
                          void *stream);
-/* Developer profiling of the tcgen05 contraction: device int64[33][8] receiving SM-clock stamps of CTA 0 (per 32-deep
- * chunk: loader warp 0 at iteration start / loads issued / stage free / tile stored, issuer at operands ready / MMAs
- * issued) for the following prl_test_contraction calls; NULL = off. */
-int prl_test_contraction_stamps(long long *stamps_dev);
 
 #ifdef __cplusplus
 }

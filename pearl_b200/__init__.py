@@ -1,4 +1,4 @@
-"""pearl_b200 — B200-native (sm_100a) learner hot path of facebookresearch/Pearl:
+"""pearl_b200 — H100-native (sm_90a) learner hot path of facebookresearch/Pearl:
 `ReplayBuffer.sample -> PolicyLearner.learn()` behind Pearl's own plugin API.
 
     from pearl_b200 import B200ReplayBuffer, B200DeepQLearning, B200DoubleDQN

@@ -1,7 +1,7 @@
 """ctypes binding of libpearlb200.so (include/pearl_b200.h).
 
 The product path has NO CPU fallback: if the shared library is missing or the
-process has no B200, `load()` / `init()` raise.
+process has no H100, `load()` / `init()` raise.
 """
 from __future__ import annotations
 
@@ -155,7 +155,6 @@ _SIGNATURES = {
     "prl_set_contraction_engine": (C.c_int, [C.c_int]),
     "prl_get_contraction_engine": (C.c_int, []),
     "prl_test_contraction": (C.c_int, [C.c_int] * 5 + [_P, _P, _P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P, C.c_int, _P]),
-    "prl_test_contraction_stamps": (C.c_int, [_P]),
     "prl_dqn_last_launch_info": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                            C.POINTER(C.c_int32)]),
 }

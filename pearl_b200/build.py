@@ -1,5 +1,5 @@
-"""Build pearl_b200/libpearlb200.so in-tree with nvcc for sm_100a (no JIT cache:
-the built .so travels to the GPU box with the repo snapshot)."""
+"""Build pearl_b200/libpearlb200.so in-tree with nvcc for sm_90a (no JIT cache: the library
+is built once, next to the package that loads it)."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ HDR = [os.path.join(HERE, "csrc", "common.cuh"), os.path.join(HERE, "csrc", "sam
 OUT = os.path.join(HERE, "libpearlb200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
     "-Xptxas", "-v",

@@ -1,37 +1,35 @@
 // dqn_tc.cu — tensor-core DQN learner: ONE SM (one CTA) runs one complete learner, every dense
-// contraction of the step on tcgen05 (3xTF32 UMMA, fp32 accumulators in TMEM), so that a launch
-// with L CTAs trains L independent learners (seeds / agents) concurrently — the aggregate mode that
-// fills a B200 — and a single learner needs one SM instead of 65.
+// contraction of the step on Hopper's warpgroup tensor-core instruction (wgmma, 3xTF32, fp32 accumulators in
+// registers), so that a launch with L CTAs trains L independent learners (seeds / agents) concurrently — the
+// aggregate mode that fills the chip — and a single learner needs one SM instead of a cooperative grid.
 //
 // Same semantics as the cooperative SIMT kernel in dqn.cu (DeepQLearning.learn: sample -> Q(s,a) ->
 // max_a' Q_target(s',a') -> MSE -> backward -> AdamW(amsgrad) -> scheduled soft target update; reference
 // call sites in include/pearl_b200.h).  Supported shape class: two hidden layers of 64, obs % 8 == 0,
 // obs <= 128, n_actions in {1,2,4,8,16}, batch in {128, 256}; everything else stays on the SIMT kernel.
 //
-// Per gradient step (256 threads, thread (m = tid % 128, h = tid / 128) owns batch row m of the
-// current 128-row tile = TMEM lane m, and column half h):
-//   phase T  target net: T1 = S' W1s^T per row tile (K chunks of 64 staged through smem); then one
-//            128 x 64 x 64 product per (row tile, action slot): A tile row m = relu(T1[m] + W1a[:,a] + b1)
-//            built from registers, two thread groups ping-pong (own A buffer + own accumulator) so the
-//            tensor pipe always has the other group's tile; running max over action slots in registers.
-//   phase O  online net forward (same tiles), loss gradient, dZ2, dH1 = dZ2 W2 (B operand = W2^T tile),
-//            and the weight gradients as tensor-core products over the batch dimension:
+// Per gradient step (256 threads = two warpgroups; warpgroup h owns the 64 batch rows 128 i + 64 h .. of row tile i,
+// a thread the elements of those rows that the wgmma accumulator layout gives it, umma.cuh):
+//   layer 1  T1 = X W1s^T: the rows are gathered into shared memory by cp.async (K chunks of 64) and read back
+//            as register A fragments (RS form); B = the W1 tile.
+//   phase T  target net: per action slot one 64 x 64 x 64 product whose A operand relu(T1 + W1a[:,a] + b1) is
+//            built in registers from the layer-1 accumulator and never leaves them; running max over the slots.
+//   phase O  online net forward the same way, loss gradient, dZ2, dH1 = dZ2 W2 (B operand = W2^T tile), all on
+//            register operands; then the weight gradients as products over the batch dimension:
 //            dW2 = dZ2^T H1, dW1s = dZ1^T S, and [db | dW1a] = dZ^T E with E = [1 | onehot(action)];
 //            their operands are explicitly transposed tiles written with a 144-byte chunk pitch
-//            (bank-conflict-free column scatter).  Accumulators for all of these live in TMEM.
-//   AdamW    gradients TMEM -> shared staging (M = 64 lane map), then one coalesced 16-byte sweep over the flat parameter
+//            (bank-conflict-free column scatter), 64 batch rows per pass, the two warpgroups taking
+//            different output columns.  Their accumulators stay in registers for the whole step.
+//   AdamW    gradients registers -> shared staging, then one coalesced 16-byte sweep over the flat parameter
 //            vector (parameters / moments in L2) that also writes the operand-layout weight tiles.
 //
-// Round 2: the weights are kept in global memory a second time IN THE UMMA OPERAND LAYOUT (hi tile = the fp32 values —
-// the tensor core truncates them to TF32 — and lo tile = x - trunc_tf32(x)), written by AdamW / the soft target update
-// next to the flat torch-order vectors, so staging a network's B operands is three TMA bulk copies
-// (cp.async.bulk + mbarrier complete_tx) issued by one thread instead of a SIMT split-and-scatter pass of all 256
-// threads (18.5 k of 172 k clk per round in round 1); the online W1 tiles travel while the all-actions products run.
-// A warp-specialised rewrite of this kernel (row groups + issuer / loader / tile-builder warps) was built and measured
-// in round 2 as well — bit-correct but slower; see profiles/r2_k_dqn_tc_summary.md.  What a source-level stall profile of
-// THIS kernel found instead (profiles/r2b_k_dqn_tc_stalls.md): the MMA issue code must sit under elect.sync
-// (umma::elect_one), the target network's small vectors are cached in shared memory between soft updates, AdamW walks one
-// flat list with two groups of loads in flight, the soft target update is applied to the tiles in tile order.
+// The weights are kept in global memory a second time IN THE OPERAND LAYOUT (hi tile = the fp32 values — the tensor
+// core truncates them to TF32 — and lo tile = x - trunc_tf32(x)), written by AdamW / the soft target update next to the
+// flat torch-order vectors, so staging a network's B operands is three TMA bulk copies (cp.async.bulk + mbarrier
+// complete_tx) issued by one thread.  The W2 tiles store their K axis in the order umma::kperm, which is the order in
+// which an accumulator's columns feed the next product's register A operand.  The target network's small vectors are
+// cached in shared memory between soft updates, AdamW walks one flat list with two groups of loads in flight, the soft
+// target update is applied to the tiles in tile order.
 #include <math.h>
 #include <stdarg.h>
 #include <stdlib.h>
@@ -51,17 +49,14 @@ namespace {
 constexpr int NTH = 256;
 constexpr int HID = 64;
 constexpr int MAX_B = 256;
-// shared memory regions (bytes)
+// shared memory regions (bytes): 1 = W1 hi | lo tiles, 2 = row staging of layer 1 / gradient staging of AdamW,
+// 3 = W2 hi | lo | W2^T hi | lo tiles
 constexpr int REG1 = 0, REG2 = 65536, REG3 = 131072, MISC_OFF = 196608;
 constexpr int HALF = 32768;          // hi tile at region base, lo tile at base + HALF
+constexpr int SBUF = 16384;          // layer-1 row staging of one warpgroup: [64 rows][64 floats]
 // transposed-tile arena (regions 1+2) for the weight-gradient products, 64 batch rows per pass
 constexpr int TL = 144;              // chunk pitch of transposed tiles
 constexpr int AR_A_HI = 0, AR_A_LO = 18432, AR_B_HI = 36864, AR_B_LO = 73728, AR_E = 110592;
-// TMEM columns
-constexpr int TM_T1 = 0, TM_ACC0 = 128, TM_ACC1 = 192, TM_DW2 = 256, TM_DW1 = 320, TM_DE2 = 448, TM_DE1 = 480;
-// A operands held in tensor memory (TS products) while the weight-gradient accumulators are not live:
-// group g: hi at TM_A + 128 g, lo 64 columns further
-constexpr int TM_A = 256;
 
 struct TcLearner {            // one per CTA, in global memory
     const uint32_t *records;
@@ -96,14 +91,11 @@ struct Misc {
     // a scheduled soft update, so they are loaded then and in the prologue, not every round)
     struct Smalls { float watb[16][HID]; float b2[HID], w3[HID]; float b3, pad0[3]; } sm[2];
     float y[MAX_B];
-    float vpart[128][2];
-    float vmax2[2][128];
     int act[MAX_B], cnt[MAX_B], slot[MAX_B];
     float rew[MAX_B], term[MAX_B];
-    float redw[8][32];
+    float redw[8][HID];
     float redmae[8], reddb3[8];
-    unsigned long long bar[10];   // 1,2: per-group MMA; 3,4,5: phase-O products; 6: target tiles; 7: online W1 tiles; 8: online W2 tiles
-    uint32_t tmem_base;
+    unsigned long long bar[3];   // 0: target tiles; 1: online W1 tiles; 2: online W2 tiles
 };
 
 __device__ __forceinline__ void cp_async16_zfill_tc(void *smem_dst, const void *gmem_src, int src_bytes) {
@@ -112,14 +104,6 @@ __device__ __forceinline__ void cp_async16_zfill_tc(void *smem_dst, const void *
 }
 
 __device__ __forceinline__ void group_sync(int g) { asm volatile("bar.sync %0, %1;" ::"r"(1 + g), "r"(128) : "memory"); }
-
-__device__ __forceinline__ void st_split4(float *hi_base, float *lo_base, int idx, float4 v) {
-    float4 h, l;
-    umma::split_tf32(v.x, h.x, l.x); umma::split_tf32(v.y, h.y, l.y);
-    umma::split_tf32(v.z, h.z, l.z); umma::split_tf32(v.w, h.w, l.w);
-    *reinterpret_cast<float4 *>(hi_base + idx) = h;
-    *reinterpret_cast<float4 *>(lo_base + idx) = l;
-}
 
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(umma::smem_u32(bar)), "r"(bytes) : "memory");
@@ -131,12 +115,11 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gmem_src, u
                  : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ float tf32_lo(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
+using umma::tf32_lo;
 
 // Operand-layout copies of one network's matrices in global memory (floats):
-//   [W1 hi: 64 x obs][W1 lo][W2 hi: 64 x 64][W2 lo]      (the shared-memory images, tile by tile; the W2^T tiles of the
-//   online network are transposed out of the W2 tiles in shared memory: keeping them in global memory too cost AdamW eight
-//   scattered 4-byte stores per 16-byte group, more than the transposition)
+//   [W1 hi: 64 x obs][W1 lo][W2 hi: 64 x 64][W2 lo]      (the shared-memory images, tile by tile; the W2 tiles with their
+//   K axis in umma::kperm order; the W2^T tiles of the online network are transposed out of the W2 tiles in shared memory)
 struct NetTiles { float *w1hi, *w1lo, *w2; };   // w2: the 2 x 4096-float block W2 hi | W2 lo
 __host__ __device__ inline int net_tile_floats(int obs) { return 128 * obs + 2 * HID * HID; }
 __device__ __forceinline__ NetTiles net_tiles(float *base, int obs) { return NetTiles{base, base + 64 * obs, base + 128 * obs}; }
@@ -151,7 +134,7 @@ __device__ void rebuild_tiles(const float *__restrict__ net, const Dims &d, cons
     for (int e = tid; e < HID * HID; e += NTH) {
         const int j = e >> 6, k = e & 63;
         const float x = __ldcg(net + d.oW2 + e);
-        const int i1 = umma::tile_index(j, k, HID);
+        const int i1 = umma::tile_index(j, umma::kperm(k), HID);
         t.w2[i1] = x; t.w2[4096 + i1] = tf32_lo(x);
     }
 }
@@ -184,9 +167,6 @@ __device__ __forceinline__ float fast_sqrt(float x) {
 }
 struct AdamScalarsTc : AdamScalars { float inv_bc2_sqrt; };
 
-// AdamW on parameters [i0, i0 + valid) with gradients g[OFF .. OFF + COUNT): COUNT is a compile-time
-// multiple of 16 so that g stays in registers; `valid` <= COUNT masks the tail.  Per 16-parameter batch:
-// all loads first (one L2 round trip), then arithmetic, then stores.
 __device__ __forceinline__ float adam_math(float w, float &m, float &v, float &x, float g, const AdamScalarsTc &hs) {
     float p = __fmul_rn(w, hs.decay);
     m = fmaf(hs.omb1, g - m, m);
@@ -197,86 +177,53 @@ __device__ __forceinline__ float adam_math(float w, float &m, float &v, float &x
     const float denom = __fadd_rn(__fmul_rn(fast_sqrt(x), hs.inv_bc2_sqrt), hs.eps);
     return __fadd_rn(p, __fdividef(__fmul_rn(-hs.step_size, m), denom));
 }
-// T1[tile] = X[tile rows] W1s^T, X = state (online) or next_state (target).  The two 128-thread groups
-// take alternate row tiles; each thread streams its own row from global memory, splits it and writes it
-// straight into tensor memory (TS product: no shared-memory staging of A), 64 columns of K per pass.
-__device__ void layer1_all_tiles(const TcArgs &a, const TcLearner &L, Misc &mi, char *smem, int field_off, uint32_t tm,
-                                 uint32_t tlane, uint32_t &parg, int round = 0, bool stamp = false) {
-    const int m = threadIdx.x & 127, g = threadIdx.x >> 7;
-    const int ntiles = a.B >> 7;
+
+// t1[64 x 64] = X[rows row0 .. row0 + 64) W1s^T for this warpgroup, X = state (online) or next_state (target).  The rows
+// arrive by coalesced 16-byte cp.async (16 lanes per row) in a staging buffer [64 rows][64 floats] whose 16-byte chunk c
+// of row r sits at chunk position c ^ (r & 7), which makes the fragment reads below (8 rows x 4 consecutive k per warp
+// and load) conflict free; 64 columns of K per pass.
+__device__ __forceinline__ void layer1_block(const TcArgs &a, const TcLearner &L, const Misc &mi, char *smem, int field_off, int row0,
+                                             float (&t1)[32]) {
+    const int m = threadIdx.x & 127, g = threadIdx.x >> 7, t = threadIdx.x & 3;
     const umma::Tile B_hi = umma::make_tile(smem + REG1, a.d.obs, 128), B_lo = umma::make_tile(smem + REG1 + HALF, a.d.obs, 128);
-    const uint32_t a_hi = TM_A + 128 * g, a_lo = a_hi + 64;
-    uint64_t *bar = reinterpret_cast<uint64_t *>(mi.bar);
-    // staging buffer of this group in region 2: [128 rows][64 floats], 16-byte chunk c of row r stored at
-    // chunk position c ^ (r & 7): rows arrive by coalesced 16-byte cp.async (16 lanes per row), and the
-    // row-owning thread reads its row back with conflict-free 128-bit loads.
-    float *sbuf = reinterpret_cast<float *>(smem + REG2 + g * 32768);
-    for (int t = g; t < ntiles; t += 2) {
-        for (int kc = 0; kc * 64 < a.d.obs; kc++) {
-            if (stamp && kc == 1) TC_STAMP(10);
+    float *sbuf = reinterpret_cast<float *>(smem + REG2 + g * SBUF);
+    for (int kc = 0; kc * 64 < a.d.obs; kc++) {
 #pragma unroll 4
-            for (int i = 0; i < 16; i++) {
-                const int item = i * 128 + m, rr = item >> 4, c = item & 15, k = kc * 64 + c * 4;
-                const float *src = reinterpret_cast<const float *>(L.records + (size_t)mi.slot[t * 128 + rr] * a.lay.record_words) +
-                                   field_off + k;
-                const int nb = k < a.d.obs ? 16 : 0;
-                cp_async16_zfill_tc(sbuf + rr * 64 + ((c ^ (rr & 7)) << 2), nb ? src : reinterpret_cast<const float *>(L.records), nb);
-            }
-            cp_async_commit();
-            cp_async_wait<0>();
-            group_sync(g);
-#pragma unroll
-            for (int half = 0; half < 2; half++) {
-                float hi[32], lo[32];
-#pragma unroll
-                for (int i = 0; i < 8; i++) {
-                    const int c = half * 8 + i;
-                    const float4 v = *reinterpret_cast<const float4 *>(sbuf + m * 64 + ((c ^ (m & 7)) << 2));
-                    umma::split_tf32(v.x, hi[4 * i + 0], lo[4 * i + 0]); umma::split_tf32(v.y, hi[4 * i + 1], lo[4 * i + 1]);
-                    umma::split_tf32(v.z, hi[4 * i + 2], lo[4 * i + 2]); umma::split_tf32(v.w, hi[4 * i + 3], lo[4 * i + 3]);
-                }
-                umma::tmem_st32(tlane + a_hi + half * 32, hi);
-                umma::tmem_st32(tlane + a_lo + half * 32, lo);
-            }
-            umma::tmem_st_wait();
-            if (stamp && kc == 1) TC_STAMP(11);
-            umma::fence_before_thread_sync();
-            group_sync(g);
-            if (stamp && kc == 1) TC_STAMP(12);
-            if (m < 32 && umma::elect_one()) {
-                umma::fence_after_thread_sync();
-                const int keff = min(64, a.d.obs - kc * 64);
-                umma::gemm3_ts(tm + TM_T1 + t * 64, tm + a_hi, tm + a_lo, B_hi.shifted(kc * 2048), B_lo.shifted(kc * 2048), 128, HID,
-                               keff, kc > 0);
-                umma::mma_commit(&bar[1 + g]);
-            }
-            if (stamp && kc == 1) TC_STAMP(13);
-            umma::mbar_wait(&bar[1 + g], parg);
-            parg ^= 1;
-            umma::fence_after_thread_sync();
-            if (stamp && kc == 1) TC_STAMP(14);
+        for (int i = 0; i < 8; i++) {
+            const int item = i * 128 + m, rr = item >> 4, c = item & 15, k = kc * 64 + c * 4;
+            const float *src = reinterpret_cast<const float *>(L.records + (size_t)mi.slot[row0 + rr] * a.lay.record_words) + field_off + k;
+            const int nb = k < a.d.obs ? 16 : 0;
+            cp_async16_zfill_tc(sbuf + rr * 64 + ((c ^ (rr & 7)) << 2), nb ? src : reinterpret_cast<const float *>(L.records), nb);
         }
+        cp_async_commit();
+        cp_async_wait<0>();
+        group_sync(g);
+        float hi[32], lo[32];
+#pragma unroll
+        for (int ks = 0; ks < 8; ks++)
+#pragma unroll
+            for (int q = 0; q < 2; q++)
+#pragma unroll
+                for (int p = 0; p < 2; p++) {
+                    const int r = umma::acc_row(p), k = 8 * ks + t + 4 * q;
+                    umma::split_tf32(sbuf[r * 64 + (((k >> 2) ^ (r & 7)) << 2) + (k & 3)], hi[4 * ks + 2 * q + p], lo[4 * ks + 2 * q + p]);
+                }
+        const int keff = min(64, a.d.obs - kc * 64);
+        umma::gemm3_rs<HID, 8>(t1, hi, lo, B_hi.shifted(kc * 2048), B_lo.shifted(kc * 2048), kc > 0, keff >> 3);
+        umma::wg_commit();
+        umma::wg_wait<0>();
+        group_sync(g);   // the staging buffer is free for the next pass
     }
-    if (stamp) TC_STAMP(15);
-    umma::fence_before_thread_sync();
-    __syncthreads();
-    umma::fence_after_thread_sync();
 }
 
-// v[c] = this lane's (row's) value of column c; returns, in lane c, the sum of column c over the warp's
-// 32 rows: reduce-scatter butterfly, 31 shuffles instead of 32 x 5.
-__device__ __forceinline__ float warp_colsum32(float *v, int lane) {
+// register A fragments (hi / lo) of the next product from values in accumulator order: v[4 j + 2 p + e] -> a[4 j + 2 e + p]
+__device__ __forceinline__ void acc_to_frag(const float (&v)[32], float (&hi)[32], float (&lo)[32]) {
 #pragma unroll
-    for (int n = 16; n >= 1; n >>= 1) {
-        const bool up = (lane & n) != 0;
+    for (int j = 0; j < 8; j++)
 #pragma unroll
-        for (int i = 0; i < n; i++) {
-            const float send = up ? v[i] : v[i + n];
-            const float keep = up ? v[i + n] : v[i];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, n);
-        }
-    }
-    return v[0];
+        for (int p = 0; p < 2; p++)
+#pragma unroll
+            for (int e = 0; e < 2; e++) umma::split_tf32(v[4 * j + 2 * p + e], hi[4 * j + 2 * e + p], lo[4 * j + 2 * e + p]);
 }
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -284,6 +231,19 @@ __device__ __forceinline__ float warp_sum(float v) {
     for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
 }
+__device__ __forceinline__ float quad_sum(float v) {
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// d[64 x n] (+)= A B^T over 64 batch rows, n in {8, 16, 32, 64}
+__device__ __forceinline__ void gemm3_n(int n, float *d, umma::Tile ah, umma::Tile al, umma::Tile bh, umma::Tile bl, bool accumulate) {
+    if (n == 64) umma::gemm3<64>(d, ah, al, bh, bl, 64, accumulate);
+    else if (n == 32) umma::gemm3<32>(d, ah, al, bh, bl, 64, accumulate);
+    else if (n == 16) umma::gemm3<16>(d, ah, al, bh, bl, 64, accumulate);
+    else umma::gemm3<8>(d, ah, al, bh, bl, 64, accumulate);
+}
+__host__ __device__ inline int pow2_cols(int n) { return n > 32 ? 64 : n > 16 ? 32 : n > 8 ? 16 : 8; }
 
 __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     extern __shared__ __align__(1024) char smem[];
@@ -299,9 +259,10 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     }
     const Dims &d = a.d;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int m = tid & 127, h = tid >> 7;
+    const int h = tid >> 7, t4 = tid & 3;
     const int ntiles = a.B >> 7;
     const int W = a.lay.record_words;
+    const int rA = umma::acc_row(0), rB = umma::acc_row(1);   // this thread's two rows of its warpgroup's 64-row block
 
     // De-phase the learners: identical CTAs started together run in lock-step and hit L2 / HBM with their AdamW sweeps
     // (432 KB each) and row gathers all at once; a start offset of up to ~50 us spreads those bursts over the round.
@@ -309,17 +270,15 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
         const long long t0 = clock64(), wait = (long long)(blockIdx.x % 48) * 2000;
         while (clock64() - t0 < wait) __nanosleep(100);
     }
-    if (warp == 0) umma::tmem_alloc(&mi.tmem_base, 512);
+    uint64_t *bar = reinterpret_cast<uint64_t *>(mi.bar);
     if (tid == 0)
-        for (int i = 0; i < 10; i++) umma::mbar_init(reinterpret_cast<uint64_t *>(&mi.bar[i]), 1);
+        for (int i = 0; i < 3; i++) umma::mbar_init(bar + i, 1);
     // the operand-layout tiles follow the flat parameters (which the host may have changed between calls)
     const NetTiles To = net_tiles(L.tiles, d.obs), Tt = net_tiles(L.tiles + net_tile_floats(d.obs), d.obs);
     rebuild_tiles(L.w, d, To, tid);
     rebuild_tiles(L.wt, d, Tt, tid);
     fence_proxy_async_all();
-    umma::fence_before_thread_sync();
     __syncthreads();
-    umma::fence_after_thread_sync();
     const uint32_t w1_bytes = 64u * d.obs * 4, w2_bytes = 2u * HID * HID * 4;
     // B-operand tiles of one network by TMA: W1 hi / lo into region 1, the W2 block into region 3
     auto tma_w1 = [&](const NetTiles &t, uint64_t *b) {
@@ -331,10 +290,12 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
         mbar_expect_tx(b, w2_bytes);
         bulk_g2s(smem + REG3, t.w2, w2_bytes, b);
     };
-    const uint32_t tm = mi.tmem_base;
-    const uint32_t tlane = tm + ((uint32_t)((warp & 3) * 32) << 16);   // this warp's 32 TMEM lanes
-    uint32_t parg = 0, par3 = 0, par4 = 0, par5 = 0;                  // mbarrier phase parities
-    uint64_t *bar = reinterpret_cast<uint64_t *>(mi.bar);
+    uint32_t par_w1 = 0;   // phase parity of bar[1] (one completion per row tile)
+    const umma::Tile W2_hi = umma::make_tile(smem + REG3, 64, 128), W2_lo = umma::make_tile(smem + REG3 + 16384, 64, 128);
+    const umma::Tile W2T_hi = umma::make_tile(smem + REG3 + 32768, 64, 128), W2T_lo = umma::make_tile(smem + REG3 + 49152, 64, 128);
+    // weight-gradient products: warpgroup 0 accumulates dW2 (g1) and columns [0, 64) of dW1s (g2), warpgroup 1
+    // [db2 | .] (g1[0..16)), [db1 | dW1a] (g1[16..32)) and columns [64, obs) of dW1s (g2)
+    const int n_dw1 = h == 0 ? pow2_cols(min(d.obs, 64)) : (d.obs > 64 ? pow2_cols(d.obs - 64) : 0);
 
     for (int round = 0; round < a.rounds; round++) {
         TC_STAMP(0);
@@ -379,226 +340,192 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
         // ================= phase T: y = max_a' Q_target(s', a') * gamma * (1 - term) + r =================
         TC_STAMP(1);
         if (tid == 0) {   // target tiles: three TMA bulk copies (regions 1 and 3 are free: every product of the last round was waited for)
-            mbar_expect_tx(bar + 6, 2 * w1_bytes + w2_bytes);
-            bulk_g2s(smem + REG1, Tt.w1hi, w1_bytes, bar + 6);
-            bulk_g2s(smem + REG1 + HALF, Tt.w1lo, w1_bytes, bar + 6);
-            bulk_g2s(smem + REG3, Tt.w2, w2_bytes, bar + 6);
+            mbar_expect_tx(bar + 0, 2 * w1_bytes + w2_bytes);
+            bulk_g2s(smem + REG1, Tt.w1hi, w1_bytes, bar + 0);
+            bulk_g2s(smem + REG1 + HALF, Tt.w1lo, w1_bytes, bar + 0);
+            bulk_g2s(smem + REG3, Tt.w2, w2_bytes, bar + 0);
         }
         if (soft_upd || round == 0) load_smalls(L.wt, d, mi.sm[1]);   // the target's small vectors only change at a soft update
-        umma::mbar_wait(bar + 6, round & 1);
+        umma::mbar_wait(bar + 0, round & 1);
         __syncthreads();
         TC_STAMP(2);
-        layer1_all_tiles(a, L, mi, smem, a.lay.off_next_state, tm, tlane, parg);
-        if (tid == 0) tma_w1(To, bar + 7);      // region 1 is free again: the online W1 tiles travel while the all-actions products run
-        TC_STAMP(3);
-        {
-            // group g = h: own A operand in tensor memory and own accumulator; the two groups ping-pong
-            const umma::Tile B_hi = umma::make_tile(smem + REG3, 64, 128), B_lo = umma::make_tile(smem + REG3 + 16384, 64, 128);
-            const uint32_t acc_col = h ? TM_ACC1 : TM_ACC0;
-            const uint32_t a_hi = TM_A + 128 * h, a_lo = a_hi + 64;
-            for (int t = 0; t < ntiles; t++) {
-                const int row = t * 128 + m;
-                float t1[64];
-                umma::tmem_ld32(tlane + TM_T1 + t * 64, t1);
-                umma::tmem_ld32(tlane + TM_T1 + t * 64 + 32, t1 + 32);
-                const int cnt = mi.cnt[row];
-                const uint8_t *ids = reinterpret_cast<const uint8_t *>(L.records + (size_t)mi.slot[row] * W + a.lay.off_avail);
-                float best = -INFINITY;
-                for (int act = h; act < d.A; act += 2) {
-                    int id = act;
-                    if ((L.buf_flags & PRL_BUF_DYNAMIC_ACTIONS) && act < cnt) id = ids[act];
+        for (int i = 0; i < ntiles; i++) {
+            const int row0 = i * 128 + h * 64;
+            float t1[32];
+            layer1_block(a, L, mi, smem, a.lay.off_next_state, row0, t1);
+            const int rows[2] = {row0 + rA, row0 + rB};
+            int cnt[2];
+            const uint8_t *ids[2];
+            float best[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-                    for (int half = 0; half < 2; half++) {
-                        float hi[32], lo[32];
-#pragma unroll
-                        for (int c4 = 0; c4 < 8; c4++) {
-                            const float4 wv = *reinterpret_cast<const float4 *>(&mi.sm[1].watb[id][half * 32 + 4 * c4]);
-                            const int c = half * 32 + 4 * c4;
-                            umma::split_tf32(fmaxf(t1[c + 0] + wv.x, 0.f), hi[4 * c4 + 0], lo[4 * c4 + 0]);
-                            umma::split_tf32(fmaxf(t1[c + 1] + wv.y, 0.f), hi[4 * c4 + 1], lo[4 * c4 + 1]);
-                            umma::split_tf32(fmaxf(t1[c + 2] + wv.z, 0.f), hi[4 * c4 + 2], lo[4 * c4 + 2]);
-                            umma::split_tf32(fmaxf(t1[c + 3] + wv.w, 0.f), hi[4 * c4 + 3], lo[4 * c4 + 3]);
-                        }
-                        umma::tmem_st32(tlane + a_hi + half * 32, hi);
-                        umma::tmem_st32(tlane + a_lo + half * 32, lo);
-                    }
-                    umma::tmem_st_wait();
-                    
-                    umma::fence_before_thread_sync();
-                    group_sync(h);
-                    
-                    if (m < 32 && umma::elect_one()) {
-                        umma::fence_after_thread_sync();
-                        umma::gemm3_ts(tm + acc_col, tm + a_hi, tm + a_lo, B_hi, B_lo, 128, HID, HID, false);
-                        umma::mma_commit(&bar[1 + h]);
-                    }
-                    
-                    umma::mbar_wait(&bar[1 + h], parg);
-                    parg ^= 1;
-                    umma::fence_after_thread_sync();
-                    
-                    float acc[64];
-                    umma::tmem_ld32(tlane + acc_col, acc);
-                    umma::tmem_ld32(tlane + acc_col + 32, acc + 32);
-                    float q = 0.f;
-#pragma unroll
-                    for (int c4 = 0; c4 < 16; c4++) {
-                        const float4 w3v = *reinterpret_cast<const float4 *>(&mi.sm[1].w3[4 * c4]);
-                        const float4 b2v = *reinterpret_cast<const float4 *>(&mi.sm[1].b2[4 * c4]);
-                        q = fmaf(w3v.x, fmaxf(acc[4 * c4 + 0] + b2v.x, 0.f), q);
-                        q = fmaf(w3v.y, fmaxf(acc[4 * c4 + 1] + b2v.y, 0.f), q);
-                        q = fmaf(w3v.z, fmaxf(acc[4 * c4 + 2] + b2v.z, 0.f), q);
-                        q = fmaf(w3v.w, fmaxf(acc[4 * c4 + 3] + b2v.w, 0.f), q);
-                    }
-                    q += mi.sm[1].b3;
-                    if (act >= cnt) q = -INFINITY;   // next_state_action_values[mask] = -inf
-                    best = fmaxf(best, q);
-                    
-                    
-                }
-                mi.vmax2[h][m] = best;
-                umma::fence_before_thread_sync();
-                __syncthreads();
-                if (h == 0) {
-                    const float v = fmaxf(mi.vmax2[0][m], mi.vmax2[1][m]);
-                    mi.y[row] = __fadd_rn(__fmul_rn(__fmul_rn(v, a.gamma), 1.f - mi.term[row]), mi.rew[row]);
-                }
-                __syncthreads();
+            for (int p = 0; p < 2; p++) {
+                cnt[p] = mi.cnt[rows[p]];
+                ids[p] = reinterpret_cast<const uint8_t *>(L.records + (size_t)mi.slot[rows[p]] * W + a.lay.off_avail);
             }
+            for (int act = 0; act < d.A; act++) {
+                float hi[32], lo[32], acc[32];
+#pragma unroll
+                for (int p = 0; p < 2; p++) {
+                    int id = act;
+                    if ((L.buf_flags & PRL_BUF_DYNAMIC_ACTIONS) && act < cnt[p]) id = ids[p][act];
+#pragma unroll
+                    for (int j = 0; j < 8; j++) {
+                        const float2 wv = *reinterpret_cast<const float2 *>(&mi.sm[1].watb[id][8 * j + 2 * t4]);
+                        umma::split_tf32(fmaxf(t1[4 * j + 2 * p] + wv.x, 0.f), hi[4 * j + p], lo[4 * j + p]);
+                        umma::split_tf32(fmaxf(t1[4 * j + 2 * p + 1] + wv.y, 0.f), hi[4 * j + 2 + p], lo[4 * j + 2 + p]);
+                    }
+                }
+                umma::gemm3_rs<HID, 8>(acc, hi, lo, W2_hi, W2_lo, false);
+                umma::wg_commit();
+                umma::wg_wait<0>();
+                float q[2] = {0.f, 0.f};
+#pragma unroll
+                for (int j = 0; j < 8; j++) {
+                    const float2 w3v = *reinterpret_cast<const float2 *>(&mi.sm[1].w3[8 * j + 2 * t4]);
+                    const float2 b2v = *reinterpret_cast<const float2 *>(&mi.sm[1].b2[8 * j + 2 * t4]);
+#pragma unroll
+                    for (int p = 0; p < 2; p++) {
+                        q[p] = fmaf(w3v.x, fmaxf(acc[4 * j + 2 * p] + b2v.x, 0.f), q[p]);
+                        q[p] = fmaf(w3v.y, fmaxf(acc[4 * j + 2 * p + 1] + b2v.y, 0.f), q[p]);
+                    }
+                }
+#pragma unroll
+                for (int p = 0; p < 2; p++) {
+                    float v = quad_sum(q[p]) + mi.sm[1].b3;
+                    if (act >= cnt[p]) v = -INFINITY;   // next_state_action_values[mask] = -inf
+                    best[p] = fmaxf(best[p], v);
+                }
+            }
+            if (t4 == 0)
+#pragma unroll
+                for (int p = 0; p < 2; p++)
+                    mi.y[rows[p]] = __fadd_rn(__fmul_rn(__fmul_rn(best[p], a.gamma), 1.f - mi.term[rows[p]]), mi.rew[rows[p]]);
         }
+        __syncthreads();   // both warpgroups are done with the target tiles
 
         // ================= phase O: online forward, loss, backward =================
-        TC_STAMP(4);
-        if (tid == 0) tma_w2(To, bar + 8);         // region 3 held the target W2 until the last all-actions product
+        TC_STAMP(3);
+        if (tid == 0) { tma_w1(To, bar + 1); tma_w2(To, bar + 2); }
         load_smalls(L.w, d, mi.sm[0]);
-        umma::mbar_wait(bar + 8, round & 1);
-        {   // W2^T tiles (B operand of dH1 = dZ2 W2) out of the W2 tiles: element (k, j) <- (j, k)
+        umma::mbar_wait(bar + 2, round & 1);
+        {   // W2^T tiles (B operand of dH1 = dZ2 W2, contraction over W2's rows) out of the W2 tiles
             const float *w2 = reinterpret_cast<const float *>(smem + REG3);
             float *w2t = reinterpret_cast<float *>(smem + REG3 + 32768);
             for (int e = tid; e < HID * HID; e += NTH) {
-                const int j = e >> 6, k = e & 63, i1 = umma::tile_index(j, k, HID), i2 = umma::tile_index(k, j, HID);
+                const int j = e >> 6, k = e & 63, i1 = umma::tile_index(j, umma::kperm(k), HID), i2 = umma::tile_index(k, umma::kperm(j), HID);
                 w2t[i2] = w2[i1]; w2t[4096 + i2] = w2[4096 + i1];
             }
             umma::fence_async_smem();
         }
-        umma::mbar_wait(bar + 7, round & 1);
-        __syncthreads();
-        TC_STAMP(5);
-        layer1_all_tiles(a, L, mi, smem, a.lay.off_state, tm, tlane, parg, round, true);
-        TC_STAMP(6);
-        float dw3_acc = 0.f, mae_acc = 0.f, db3_acc = 0.f;
-        const umma::Tile W2_hi = umma::make_tile(smem + REG3, 64, 128), W2_lo = umma::make_tile(smem + REG3 + 16384, 64, 128);
-        const umma::Tile W2T_hi = umma::make_tile(smem + REG3 + 32768, 64, 128), W2T_lo = umma::make_tile(smem + REG3 + 49152, 64, 128);
-        float *r2hi = reinterpret_cast<float *>(smem + REG2), *r2lo = r2hi + HALF / 4;
-        const umma::Tile R2_hi = umma::make_tile(r2hi, 64, 128), R2_lo = umma::make_tile(r2lo, 64, 128);
-        for (int t = 0; t < ntiles; t++) {
-            const int row = t * 128 + m, c0 = h * 32;
-            float h1[32];
-            umma::tmem_ld32(tlane + TM_T1 + t * 64 + c0, h1);
-            {
-                const int ai = mi.act[row];
+        TC_STAMP(4);
+        float dw3[16], g1[32], g2[32];
+        float mae_acc = 0.f, db3_acc = 0.f;
 #pragma unroll
-                for (int c = 0; c < 32; c++) h1[c] = fmaxf(h1[c] + mi.sm[0].watb[ai][c0 + c], 0.f);
+        for (int c = 0; c < 16; c++) dw3[c] = 0.f;
+        float *arena = reinterpret_cast<float *>(smem);
+        const umma::Tile TA_hi = umma::make_tile(smem + AR_A_HI, 64, TL), TA_lo = umma::make_tile(smem + AR_A_LO, 64, TL);
+        const umma::Tile TB_hi = umma::make_tile(smem + AR_B_HI, 64, TL), TB_lo = umma::make_tile(smem + AR_B_LO, 64, TL);
+        const umma::Tile TE = umma::make_tile(smem + AR_E, 64, TL);
+        for (int i = 0; i < ntiles; i++) {
+            if (i > 0 && tid == 0) tma_w1(To, bar + 1);   // the arena of the last tile overwrote region 1
+            umma::mbar_wait(bar + 1, par_w1);
+            par_w1 ^= 1;
+            __syncthreads();   // also: the W2^T tiles are complete
+            const int row0 = i * 128 + h * 64;
+            const int rows[2] = {row0 + rA, row0 + rB};
+            float h1[32], z[32], hi[32], lo[32];
+            layer1_block(a, L, mi, smem, a.lay.off_state, row0, h1);
+            if (i == 0) TC_STAMP(5);
+            int ai[2];
 #pragma unroll
-                for (int c4 = 0; c4 < 8; c4++)
-                    st_split4(r2hi, r2lo, umma::tile_index(m, c0 + 4 * c4, 64),
-                              make_float4(h1[4 * c4], h1[4 * c4 + 1], h1[4 * c4 + 2], h1[4 * c4 + 3]));
+            for (int p = 0; p < 2; p++) {
+                ai[p] = mi.act[rows[p]];
+#pragma unroll
+                for (int j = 0; j < 8; j++) {
+                    const float2 wv = *reinterpret_cast<const float2 *>(&mi.sm[0].watb[ai[p]][8 * j + 2 * t4]);
+                    h1[4 * j + 2 * p] = fmaxf(h1[4 * j + 2 * p] + wv.x, 0.f);
+                    h1[4 * j + 2 * p + 1] = fmaxf(h1[4 * j + 2 * p + 1] + wv.y, 0.f);
+                }
             }
-            umma::fence_async_smem();
-            umma::fence_before_thread_sync();
-            __syncthreads();
-            if (warp == 0 && umma::elect_one()) {
-                umma::fence_after_thread_sync();
-                umma::gemm3(tm + TM_ACC0, R2_hi, R2_lo, W2_hi, W2_lo, 128, HID, HID, false);
-                umma::mma_commit(&bar[4]);
-            }
-            umma::mbar_wait(&bar[4], par4);
-            par4 ^= 1;
-            umma::fence_after_thread_sync();
-            float z[32];   // h2, then dz2
-            umma::tmem_ld32(tlane + TM_ACC0 + c0, z);
-            float part = 0.f;
+            acc_to_frag(h1, hi, lo);
+            umma::gemm3_rs<HID, 8>(z, hi, lo, W2_hi, W2_lo, false);
+            umma::wg_commit();
+            umma::wg_wait<0>();
+            float part[2] = {0.f, 0.f}, dq[2];
 #pragma unroll
-            for (int c = 0; c < 32; c++) { z[c] = fmaxf(z[c] + mi.sm[0].b2[c0 + c], 0.f); part = fmaf(mi.sm[0].w3[c0 + c], z[c], part); }
-            mi.vpart[m][h] = part;
-            umma::fence_before_thread_sync();
-            __syncthreads();
-            const float q = mi.vpart[m][0] + mi.vpart[m][1] + mi.sm[0].b3;
-            const float y = mi.y[row];
-            const float dq = (q - y) * a.inv_b2;
-            if (h == 0) {
-                if (L.out_q) L.out_q[(size_t)round * a.B + row] = q;
-                if (L.out_y) L.out_y[(size_t)round * a.B + row] = y;
-                mae_acc += fabsf(q - y);
-                db3_acc += dq;
-            }
-            // dW3[c0 + c] += sum_rows dq * h2 : reduce over this warp's 32 rows, lane c keeps column c
-            {
-                float cs[32];
+            for (int j = 0; j < 8; j++) {
+                const float2 w3v = *reinterpret_cast<const float2 *>(&mi.sm[0].w3[8 * j + 2 * t4]);
+                const float2 b2v = *reinterpret_cast<const float2 *>(&mi.sm[0].b2[8 * j + 2 * t4]);
 #pragma unroll
-                for (int c = 0; c < 32; c++) cs[c] = dq * z[c];
-                dw3_acc += warp_colsum32(cs, lane);   // lane c receives the sum of column c over the 32 rows
+                for (int p = 0; p < 2; p++) {
+                    z[4 * j + 2 * p] = fmaxf(z[4 * j + 2 * p] + b2v.x, 0.f);
+                    z[4 * j + 2 * p + 1] = fmaxf(z[4 * j + 2 * p + 1] + b2v.y, 0.f);
+                    part[p] = fmaf(w3v.x, z[4 * j + 2 * p], part[p]);
+                    part[p] = fmaf(w3v.y, z[4 * j + 2 * p + 1], part[p]);
+                }
             }
 #pragma unroll
-            for (int c = 0; c < 32; c++) z[c] = (z[c] > 0.f) ? dq * mi.sm[0].w3[c0 + c] : 0.f;   // dZ2
-#pragma unroll
-            for (int c4 = 0; c4 < 8; c4++)
-                st_split4(r2hi, r2lo, umma::tile_index(m, c0 + 4 * c4, 64),
-                          make_float4(z[4 * c4], z[4 * c4 + 1], z[4 * c4 + 2], z[4 * c4 + 3]));
-            umma::fence_async_smem();
-            umma::fence_before_thread_sync();
-            __syncthreads();
-            if (warp == 0 && umma::elect_one()) {
-                umma::fence_after_thread_sync();
-                umma::gemm3(tm + TM_ACC1, R2_hi, R2_lo, W2T_hi, W2T_lo, 128, HID, HID, false);   // dH1 = dZ2 W2
-                umma::mma_commit(&bar[5]);
+            for (int p = 0; p < 2; p++) {
+                const float q = quad_sum(part[p]) + mi.sm[0].b3;
+                const float y = mi.y[rows[p]];
+                dq[p] = (q - y) * a.inv_b2;
+                if (t4 == 0) {
+                    if (L.out_q) L.out_q[(size_t)round * a.B + rows[p]] = q;
+                    if (L.out_y) L.out_y[(size_t)round * a.B + rows[p]] = y;
+                    mae_acc += fabsf(q - y);
+                    db3_acc += dq[p];
+                }
             }
-            umma::mbar_wait(&bar[5], par5);
-            par5 ^= 1;
-            umma::fence_after_thread_sync();
+            // dW3 partial sums over this thread's two rows, then dZ2 in place of h2
+#pragma unroll
+            for (int j = 0; j < 8; j++) {
+                const float2 w3v = *reinterpret_cast<const float2 *>(&mi.sm[0].w3[8 * j + 2 * t4]);
+                dw3[2 * j] += dq[0] * z[4 * j] + dq[1] * z[4 * j + 2];
+                dw3[2 * j + 1] += dq[0] * z[4 * j + 1] + dq[1] * z[4 * j + 3];
+#pragma unroll
+                for (int p = 0; p < 2; p++) {
+                    z[4 * j + 2 * p] = z[4 * j + 2 * p] > 0.f ? dq[p] * w3v.x : 0.f;
+                    z[4 * j + 2 * p + 1] = z[4 * j + 2 * p + 1] > 0.f ? dq[p] * w3v.y : 0.f;
+                }
+            }
             float dz1[32];
-            umma::tmem_ld32(tlane + TM_ACC1 + c0, dz1);
-            if (t == 0) TC_STAMP(7);
+            acc_to_frag(z, hi, lo);
+            umma::gemm3_rs<HID, 8>(dz1, hi, lo, W2T_hi, W2T_lo, false);   // dH1 = dZ2 W2
+            umma::wg_commit();
+            umma::wg_wait<0>();
 #pragma unroll
             for (int c = 0; c < 32; c++) dz1[c] = (h1[c] > 0.f) ? dz1[c] : 0.f;
+            if (i == 0) TC_STAMP(6);
 
-            // ---- weight gradients: contractions over the batch rows, 64 rows per pass
-            float *arena = reinterpret_cast<float *>(smem);
-            const umma::Tile TA_hi = umma::make_tile(smem + AR_A_HI, 64, TL), TA_lo = umma::make_tile(smem + AR_A_LO, 64, TL);
-            const umma::Tile TB_hi = umma::make_tile(smem + AR_B_HI, 64, TL), TB_lo = umma::make_tile(smem + AR_B_LO, 64, TL);
-            const umma::Tile TE = umma::make_tile(smem + AR_E, 64, TL);
+            // ---- weight gradients: contractions over the batch rows, 64 rows (one warpgroup's block) per pass
             for (int hf = 0; hf < 2; hf++) {
-                const bool mine = (m >> 6) == hf;
-                const int rr = m & 63;
-                const bool first = (t == 0 && hf == 0);
-                umma::fence_before_thread_sync();
+                const bool mine = h == hf;
+                const bool first = (i == 0 && hf == 0);
                 __syncthreads();   // previous products have been waited for: the arena is free
                 if (mine) {
 #pragma unroll
-                    for (int c = 0; c < 32; c++) {
-                        const int idx = umma::tile_index2(c0 + c, rr, 64, TL);
-                        float hi, lo;
-                        umma::split_tf32(z[c], hi, lo);            // dZ2^T
-                        arena[AR_A_HI / 4 + idx] = hi; arena[AR_A_LO / 4 + idx] = lo;
-                        umma::split_tf32(h1[c], hi, lo);           // H1^T
-                        arena[AR_B_HI / 4 + idx] = hi; arena[AR_B_LO / 4 + idx] = lo;
-                    }
-                    const int ai = mi.act[row];
+                    for (int j = 0; j < 8; j++)
 #pragma unroll
-                    for (int e = 0; e < 16; e++) {                 // E^T: [1 | onehot(action)]
-                        const int er = h * 16 + e;
-                        arena[AR_E / 4 + umma::tile_index2(er, rr, 64, TL)] = (er == 0 || er == ai + 1) ? 1.f : 0.f;
-                    }
+                        for (int p = 0; p < 2; p++)
+#pragma unroll
+                            for (int e = 0; e < 2; e++) {
+                                const int idx = umma::tile_index2(8 * j + 2 * t4 + e, p ? rB : rA, 64, TL), c = 4 * j + 2 * p + e;
+                                arena[AR_A_HI / 4 + idx] = z[c]; arena[AR_A_LO / 4 + idx] = tf32_lo(z[c]);       // dZ2^T
+                                arena[AR_B_HI / 4 + idx] = h1[c]; arena[AR_B_LO / 4 + idx] = tf32_lo(h1[c]);     // H1^T
+                            }
+#pragma unroll
+                    for (int p = 0; p < 2; p++)
+#pragma unroll
+                        for (int x = 0; x < 8; x++) {                 // E^T: [1 | onehot(action)]
+                            const int er = t4 * 8 + x;
+                            arena[AR_E / 4 + umma::tile_index2(er, p ? rB : rA, 64, TL)] = (er == 0 || er == ai[p] + 1) ? 1.f : 0.f;
+                        }
                 }
                 umma::fence_async_smem();
-                umma::fence_before_thread_sync();
                 __syncthreads();
-                if (warp == 0 && umma::elect_one()) {
-                    umma::fence_after_thread_sync();
-                    umma::gemm3(tm + TM_DW2, TA_hi, TA_lo, TB_hi, TB_lo, 64, HID, 64, !first);
-                    umma::gemm3(tm + TM_DE2, TA_hi, TA_lo, TE, TE, 64, 32, 64, !first, false, true);
-                    umma::mma_commit(&bar[3]);
-                }
+                if (h == 0) umma::gemm3<64>(g1, TA_hi, TA_lo, TB_hi, TB_lo, 64, !first);
+                else umma::gemm3<32>(g1, TA_hi, TA_lo, TE, TE, 64, !first, false, true);
+                umma::wg_commit();
                 // S^T: every warp reads whole state rows of this half coalesced (lane = k) and scatters them into column rq of
                 // the transposed tile; the first four rows are requested BEFORE waiting for the dW2 product
                 float sv[4][4];
@@ -606,7 +533,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
 #pragma unroll
                     for (int ri = 0; ri < 4; ri++) {
                         const int rq = warp + 8 * (r0 + ri);
-                        const float *src = reinterpret_cast<const float *>(L.records + (size_t)mi.slot[t * 128 + hf * 64 + rq] * W) + a.lay.off_state;
+                        const float *src = reinterpret_cast<const float *>(L.records + (size_t)mi.slot[i * 128 + hf * 64 + rq] * W) + a.lay.off_state;
 #pragma unroll
                         for (int jj = 0; jj < 4; jj++) sv[ri][jj] = (lane + 32 * jj < d.obs) ? __ldg(src + lane + 32 * jj) : 0.f;
                     }
@@ -618,92 +545,76 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
 #pragma unroll
                         for (int jj = 0; jj < 4; jj++)
                             if (lane + 32 * jj < d.obs) {
-                                float hi, lo;
-                                umma::split_tf32(sv[ri][jj], hi, lo);
                                 const int idx = umma::tile_index2(lane + 32 * jj, rq, 64, TL);
-                                arena[AR_B_HI / 4 + idx] = hi; arena[AR_B_LO / 4 + idx] = lo;
+                                arena[AR_B_HI / 4 + idx] = sv[ri][jj]; arena[AR_B_LO / 4 + idx] = tf32_lo(sv[ri][jj]);
                             }
                     }
                 };
                 st_rows_load(0);
-                umma::mbar_wait(&bar[3], par3);
-                par3 ^= 1;
-                umma::fence_after_thread_sync();
-                umma::fence_before_thread_sync();
+                umma::wg_wait<0>();
                 __syncthreads();
                 if (mine) {
 #pragma unroll
-                    for (int c = 0; c < 32; c++) {
-                        const int idx = umma::tile_index2(c0 + c, rr, 64, TL);
-                        float hi, lo;
-                        umma::split_tf32(dz1[c], hi, lo);          // dZ1^T
-                        arena[AR_A_HI / 4 + idx] = hi; arena[AR_A_LO / 4 + idx] = lo;
-                    }
+                    for (int j = 0; j < 8; j++)
+#pragma unroll
+                        for (int p = 0; p < 2; p++)
+#pragma unroll
+                            for (int e = 0; e < 2; e++) {
+                                const int idx = umma::tile_index2(8 * j + 2 * t4 + e, p ? rB : rA, 64, TL), c = 4 * j + 2 * p + e;
+                                arena[AR_A_HI / 4 + idx] = dz1[c]; arena[AR_A_LO / 4 + idx] = tf32_lo(dz1[c]);   // dZ1^T
+                            }
                 }
                 st_rows_scatter(0);
                 st_rows_load(4);
                 st_rows_scatter(4);
                 umma::fence_async_smem();
-                umma::fence_before_thread_sync();
                 __syncthreads();
-                if (warp == 0 && umma::elect_one()) {
-                    umma::fence_after_thread_sync();
-                    umma::gemm3(tm + TM_DW1, TA_hi, TA_lo, TB_hi, TB_lo, 64, d.obs, 64, !first);
-                    umma::gemm3(tm + TM_DE1, TA_hi, TA_lo, TE, TE, 64, 32, 64, !first, false, true);
-                    umma::mma_commit(&bar[3]);
-                }
-                umma::mbar_wait(&bar[3], par3);
-                par3 ^= 1;
-                umma::fence_after_thread_sync();
+                if (n_dw1) gemm3_n(n_dw1, g2, TA_hi, TA_lo, TB_hi.rows_from(64 * h), TB_lo.rows_from(64 * h), !first);
+                if (h == 1) umma::gemm3<32>(g1 + 16, TA_hi, TA_lo, TE, TE, 64, !first, false, true);
+                umma::wg_commit();
+                umma::wg_wait<0>();
             }
+            umma::fence_async_smem();   // the arena was written through the generic proxy, the next W1 copy is a TMA write
+            __syncthreads();            // the arena is free: the next tile's W1 copy / the gradient staging may overwrite it
         }
 
         TC_STAMP(8);
-        // ================= AdamW (gradients straight from TMEM; M = 64 rows live in lanes 32q + (0..15)) ==========
-        mi.redw[warp][lane] = dw3_acc;
-        if (lane == 0) { mi.redmae[warp] = 0.f; mi.reddb3[warp] = 0.f; }
+        // ================= AdamW ==========
+        // column sums of dW3 over the warp's rows: lanes with equal lane % 4 hold the same columns
+#pragma unroll
+        for (int c = 0; c < 16; c++) {
+            float v = dw3[c];
+            v += __shfl_xor_sync(0xffffffffu, v, 4);
+            v += __shfl_xor_sync(0xffffffffu, v, 8);
+            v += __shfl_xor_sync(0xffffffffu, v, 16);
+            if (lane < 4) mi.redw[warp][8 * (c >> 1) + 2 * lane + (c & 1)] = v;
+        }
         {
             const float ms = warp_sum(mae_acc), ds = warp_sum(db3_acc);
             if (lane == 0) { mi.redmae[warp] = ms; mi.reddb3[warp] = ds; }
         }
-        umma::fence_before_thread_sync();
-        __syncthreads();
-        umma::fence_after_thread_sync();
         {
-            // 1) gradients TMEM -> shared staging in region 2 (the arena is free).  Row
-            //    pitches are odd, so the 16 live lanes of a warp (rows 16q .. 16q+15) hit distinct banks.
+            // 1) gradients registers -> shared staging in region 2 (the arena is free)
             float *gs_w2 = reinterpret_cast<float *>(smem + REG2);     // [64][65]
             const int pitch1 = d.D | 1;
             float *gs_w1 = gs_w2 + 64 * 65;                            // [64][pitch1]   (state cols, then action cols)
             float *gs_b1 = gs_w1 + 64 * pitch1, *gs_b2 = gs_b1 + 64;
-            const int j = (warp & 3) * 16 + (lane & 15);               // M = 64 lane map: lanes >= 16 hold nothing
-            const bool live = lane < 16;
-            float g[32];
-            umma::tmem_ld32(tlane + TM_DW2 + h * 32, g);
-            if (live)
 #pragma unroll
-                for (int c = 0; c < 32; c++) gs_w2[j * 65 + h * 32 + c] = g[c];
-            for (int cc = 0; cc < 2; cc++) {
-                const int kbase = h * 64 + cc * 32;
-                if (kbase < d.obs) {   // warp-uniform
-                    umma::tmem_ld32(tlane + TM_DW1 + kbase, g);
-                    if (live)
+            for (int p = 0; p < 2; p++) {
+                const int j = p ? rB : rA;                             // the gradient's row = hidden unit
 #pragma unroll
-                        for (int c = 0; c < 32; c++)
-                            if (kbase + c < d.obs) gs_w1[j * pitch1 + kbase + c] = g[c];
-                }
+                for (int jb = 0; jb < 8; jb++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const int c = 8 * jb + 2 * t4 + e, k = 64 * h + c;
+                        if (h == 0) gs_w2[j * 65 + c] = g1[4 * jb + 2 * p + e];
+                        if (c < n_dw1 && k < d.obs) gs_w1[j * pitch1 + k] = g2[4 * jb + 2 * p + e];
+                        if (h == 1 && jb < 4) {                        // [db | dW1a] columns: 0 = bias, 1 + k = action k
+                            if (c == 0) { gs_b2[j] = g1[4 * jb + 2 * p + e]; gs_b1[j] = g1[16 + 4 * jb + 2 * p + e]; }
+                            else if (c - 1 < d.A) gs_w1[j * pitch1 + d.obs + c - 1] = g1[16 + 4 * jb + 2 * p + e];
+                        }
+                    }
             }
-            umma::tmem_ld32(tlane + (h ? TM_DE1 : TM_DE2), g);
-            if (live) {
-                if (h == 0) gs_b2[j] = g[0];
-                else {
-                    gs_b1[j] = g[0];
-#pragma unroll
-                    for (int k = 0; k < 16; k++)
-                        if (k < d.A) gs_w1[j * pitch1 + d.obs + k] = g[1 + k];
-                }
-            }
-            umma::fence_before_thread_sync();
             __syncthreads();
             // 2) AdamW over the flat parameter vector, all 256 threads, fully coalesced 16-byte accesses.  The sweep is bound by
             //    L2 round trips, not bytes: W1 | W2 are walked as ONE flat list of 16-byte groups (no 4-lane tail passes per W1
@@ -717,14 +628,17 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             float sg = 0.f, sw = 0.f, sm = 0.f, sv2 = 0.f, sx = 0.f;
             if (tid < 64) { si = d.ob1 + tid; sg = gs_b1[tid]; }
             else if (tid < 128) { si = d.ob2 + tid - 64; sg = gs_b2[tid - 64]; }
-            else if (tid < 192) {       // W3: sum the four row-quarter partials of this column in fixed order
-                const int col = tid - 128, hh = col >> 5, c = col & 31;
-                sg = ((mi.redw[hh * 4 + 0][c] + mi.redw[hh * 4 + 1][c]) + mi.redw[hh * 4 + 2][c]) + mi.redw[hh * 4 + 3][c];
+            else if (tid < 192) {       // W3: sum the eight warps' partials of this column in fixed order
+                const int col = tid - 128;
+                sg = 0.f;
+#pragma unroll
+                for (int w8 = 0; w8 < 8; w8++) sg += mi.redw[w8][col];
                 si = d.oW3 + col;
             } else if (tid == 192) {
-                sg = ((mi.reddb3[0] + mi.reddb3[1]) + mi.reddb3[2]) + mi.reddb3[3];
+                float e = 0.f;
+#pragma unroll
+                for (int w8 = 0; w8 < 8; w8++) { sg += mi.reddb3[w8]; e += mi.redmae[w8]; }
                 si = d.ob3;
-                const float e = ((mi.redmae[0] + mi.redmae[1]) + mi.redmae[2]) + mi.redmae[3];
                 L.out_mae[round] = e / (float)a.B;   // reported "loss": mean |q - y|
             }
             if (si >= 0) { sw = __ldcg(L.w + si); sm = __ldcg(L.m + si); sv2 = __ldcg(L.v + si); sx = __ldcg(L.vmax + si); }
@@ -747,30 +661,37 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                     for (int u = 0; u < U; u++) {
                         const int q = q0 + u * NTH;
                         if (q < ntot) {
-                            int i;
+                            const bool is_w1 = q < n1;
+                            int i, row, c;
                             const float *gp;
-                            float *thi, *tlo;             // the same 16-byte chunk of the operand-layout tiles (hi = the value, lo = residual)
-                            if (q < n1) {
-                                const int row = q / D4, c = (q - row * D4) * 4;
+                            if (is_w1) {
+                                row = q / D4; c = (q - row * D4) * 4;
                                 i = d.oW1 + q * 4;
                                 gp = gs_w1 + row * pitch1 + c;
-                                const int ti = umma::tile_index(row, c, d.obs);
-                                thi = c < d.obs ? To.w1hi + ti : nullptr; tlo = To.w1lo + ti;
                             } else {
-                                const int q4 = q - n1, row = q4 >> 4, c = (q4 & 15) * 4;
+                                const int q4 = q - n1;
+                                row = q4 >> 4; c = (q4 & 15) * 4;
                                 i = d.oW2 + q4 * 4;
                                 gp = gs_w2 + row * 65 + c;
-                                const int ti = umma::tile_index(row, c, HID);
-                                thi = To.w2 + ti; tlo = To.w2 + 4096 + ti;
                             }
                             float4 w = w4[u], mm = m4[u], vv = v4[u], xx = x4[u];
                             w.x = adam_math(w.x, mm.x, vv.x, xx.x, gp[0], hs); w.y = adam_math(w.y, mm.y, vv.y, xx.y, gp[1], hs);
                             w.z = adam_math(w.z, mm.z, vv.z, xx.z, gp[2], hs); w.w = adam_math(w.w, mm.w, vv.w, xx.w, gp[3], hs);
                             *reinterpret_cast<float4 *>(L.w + i) = w; *reinterpret_cast<float4 *>(L.m + i) = mm;
                             *reinterpret_cast<float4 *>(L.v + i) = vv; *reinterpret_cast<float4 *>(L.vmax + i) = xx;
-                            if (thi) {
-                                *reinterpret_cast<float4 *>(thi) = w;
-                                *reinterpret_cast<float4 *>(tlo) = make_float4(tf32_lo(w.x), tf32_lo(w.y), tf32_lo(w.z), tf32_lo(w.w));
+                            // the same values in the operand-layout tiles (hi = the value, lo = residual)
+                            if (is_w1) {
+                                if (c < d.obs) {
+                                    const int ti = umma::tile_index(row, c, d.obs);
+                                    *reinterpret_cast<float4 *>(To.w1hi + ti) = w;
+                                    *reinterpret_cast<float4 *>(To.w1lo + ti) = make_float4(tf32_lo(w.x), tf32_lo(w.y), tf32_lo(w.z), tf32_lo(w.w));
+                                }
+                            } else {   // kperm order: columns c, c + 2 and c + 1, c + 3 are neighbours
+                                const int te = umma::tile_index(row, umma::kperm(c), HID), to = umma::tile_index(row, umma::kperm(c + 1), HID);
+                                *reinterpret_cast<float2 *>(To.w2 + te) = make_float2(w.x, w.z);
+                                *reinterpret_cast<float2 *>(To.w2 + to) = make_float2(w.y, w.w);
+                                *reinterpret_cast<float2 *>(To.w2 + 4096 + te) = make_float2(tf32_lo(w.x), tf32_lo(w.z));
+                                *reinterpret_cast<float2 *>(To.w2 + 4096 + to) = make_float2(tf32_lo(w.y), tf32_lo(w.w));
                             }
                         }
                     }
@@ -798,12 +719,9 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 L.m[si] = sm; L.v[si] = sv2; L.vmax[si] = sx;
             }
         }
-        umma::fence_before_thread_sync();
         __syncthreads();
-        umma::fence_after_thread_sync();
         TC_STAMP(9);
     }
-    if (warp == 0) umma::tmem_dealloc(tm, 512);
 }
 
 // a few microseconds of nothing: lets the learner CTAs of the main stream take their SMs before the next chunk's

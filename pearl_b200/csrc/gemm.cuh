@@ -45,7 +45,6 @@ struct GemmArgs {
     int relu;                                                   // max(., 0)
     const float *mask; int ldm; long long mask_net_stride;     // keep only where mask[i][j] > 0
     int accumulate;                                             // C += (before relu / mask)
-    long long *stamps;                                          // developer profiling of k_gemm_tc (CTA 0): [chunk][8] SM clocks
 };
 
 constexpr int GK = 32;   // contraction chunk
@@ -182,9 +181,9 @@ __global__ void __launch_bounds__((TM / MR) * (TN / 4) * KS) k_gemm(const GemmAr
     }
 }
 
-// gemm_tc.cu: the same contraction on tcgen05 (3xTF32).  Returns false when the engine is off / the shape is not covered.
+// gemm_tc.cu: the same contraction on wgmma (3xTF32).  Returns false when the engine is off / the shape is not covered.
 bool gemm_tc_launch(const GemmArgs &g, int nets, bool ao, bool bo, cudaStream_t st, int engine);
-// the TS form (the 128-row operand in tensor memory); gs in the kernel's own orientation, see gemm_tc.cu
+// the RS form (the 128-row operand in registers); gs in the kernel's own orientation, see gemm_tc.cu
 bool gemm_ts_launch(const GemmArgs &gs, int nets, bool bo, bool swap, cudaStream_t st, int engine);
 void transpose_weights(int rows, int cols, int nets, const float *src, float *dst, cudaStream_t st);
 cudaError_t gemm_tc_prepare();
@@ -192,12 +191,10 @@ cudaError_t gemm_tc_prepare();
 struct GemmLauncher {
     cudaStream_t st;
     int count = 0;
-    long long *stamps = nullptr;
     bool fixed_order = false;   // SIMT tiles: never slice the contraction axis (a row's sum must not depend on the launch's shape)
-    int engine = -1;   // -1: library default (prl_set_contraction_engine); 0: SIMT tiles; 1 / 64 / 32: tcgen05 tiles
+    int engine = -1;   // -1: library default (prl_set_contraction_engine); 0: SIMT tiles; 1 / 64 / 32: tensor-core tiles
     template <bool AO, bool BO>
     void run(const GemmArgs &g, int nets) {
-        if (stamps) { GemmArgs gs = g; gs.stamps = stamps; if (gemm_tc_launch(gs, nets, AO, BO, st, engine)) { count++; return; } }
         if (gemm_tc_launch(g, nets, AO, BO, st, engine)) { count++; return; }
         const long long big = (long long)((g.Mo + 63) / 64) * ((g.No + 63) / 64) * nets;
         if (big >= 96) {       // enough 64x64 tiles to occupy the chip
@@ -216,14 +213,14 @@ struct GemmLauncher {
         g.tail_col = -1;
         return g;
     }
-    // y[M x N] = act(x W^T + b).  Wt (optional): W transposed, [K x N] with row pitch ldwt — offered to the TS-form kernel
+    // y[M x N] = act(x W^T + b).  Wt (optional): W transposed, [K x N] with row pitch ldwt — offered to the RS-form kernel
     void fwd(Mat X, int M, const float *W, int ldw, long long w_ns, const float *b, long long b_ns, int N, int K, bool relu, float *Y,
              int ldy, long long y_ns, int nets = 1, const float *Wt = nullptr, int ldwt = 0, long long wt_ns = 0) {
         GemmArgs g = base();
         g.Mo = M; g.No = N; g.Kc = K; g.C = Y; g.ldc = ldy; g.c_net_stride = y_ns; g.bias = b; g.bias_net_stride = b_ns; g.relu = relu;
         if (Wt) {                                        // D[n][m] = sum_k Wt[k][n] x[m][k]
             GemmArgs t = g;
-            t.A = mat(Wt, ldwt, wt_ns); t.B = X; t.Mo = N; t.No = M; t.stamps = stamps;
+            t.A = mat(Wt, ldwt, wt_ns); t.B = X; t.Mo = N; t.No = M;
             if (gemm_ts_launch(t, nets, true, true, st, engine)) { count++; return; }
         }
         g.A = X; g.B = mat(W, ldw, w_ns);
@@ -239,7 +236,7 @@ struct GemmLauncher {
         g.mask = mask; g.ldm = ldm; g.mask_net_stride = m_ns; g.accumulate = accumulate;
         {                                                // D[k][m] = sum_n W[n][col0 + k] dy[m][n]
             GemmArgs t = g;
-            t.A = g.B; t.B = g.A; t.Mo = Kx; t.No = M; t.stamps = stamps;
+            t.A = g.B; t.B = g.A; t.Mo = Kx; t.No = M;
             if (gemm_ts_launch(t, nets, true, true, st, engine)) { count++; return; }
         }
         run<true, false>(g, nets);
@@ -255,7 +252,6 @@ struct GemmLauncher {
         g.C_tail = db; g.tail_col = K; g.tail_net_stride = db_ns;
         {
             GemmArgs t = g;
-            t.stamps = stamps;
             if (gemm_ts_launch(t, nets, false, false, st, engine)) { count++; return; }
         }
         run<false, false>(g, nets);

@@ -1,37 +1,29 @@
-// gemm_tc.cu — the actor-critic learners' contraction (gemm.cuh: C[i][j] = sum_c A(i, c) * B(j, c)) on the 5th-generation
-// tensor cores: tcgen05.mma kind::tf32 with the 3xTF32 operand split of umma.cuh (hi*hi + hi*lo + lo*hi accumulated in
-// fp32 in tensor memory), so the products keep fp32 parity with the reference's torch matmuls (1e-4 gate, ~1e-6 measured).
+// gemm_tc.cu — the actor-critic learners' contraction (gemm.cuh: C[i][j] = sum_c A(i, c) * B(j, c)) on Hopper's tensor
+// cores: wgmma.mma_async of kind tf32 with the 3xTF32 operand split of umma.cuh (hi*hi + hi*lo + lo*hi accumulated in
+// fp32 registers), so the products keep fp32 parity with the reference's torch matmuls (1e-4 gate).
 //
-// One CTA computes a 128 x TN tile of C (TN = 64 or 32).  The contraction axis is walked in chunks of 32:
-//   * all 8 warps are loaders: they read the chunk's A (128 x 32) and B (TN x 32) elements from global memory exactly as
-//     gemm.cuh's `Mat` describes them (two concatenated sources, a ones column, stacked networks; either the row or the
-//     feature axis of the Mat is the contraction axis), TWO chunks ahead of the one being multiplied (three register
-//     sets), split them into hi / lo and store them as 16-byte chunks into K-major no-swizzle UMMA tiles with a 144-byte
-//     chunk pitch — with that pitch both global layouts give conflict-free STS.128 and fully coalesced global loads;
-//   * three shared-memory stages; one thread issues the 12 MMAs of a chunk (4 K-steps x 3 split terms) and commits them
-//     to the stage's mbarrier, which is what the loaders wait on before they overwrite the stage three chunks later;
-//   * epilogue: tcgen05.ld of the accumulator (warp w: lanes 32(w%4).., columns 32(w/4)..), a per-warp transpose through
-//     shared memory so that bias / mask / accumulate reads and the C stores are coalesced along j.
-// What bounds it (profiles/r2_gemm_tc.md): not the tensor pipe (12 % active) and not shared memory (the TS form below, which
-// keeps the 128-row operand out of shared memory altogether, runs at the same speed) but the operand loads: a CTA moves
-// 24 KB from L2 per 32-deep chunk of its 128 x 64 tile, ~1500 clk per chunk alone and ~2800 clk with every SM busy, i.e.
-// 21 FLOP per byte at the ~2.5 TB/s the chip delivers to this access pattern = the measured 52 TFLOP/s on 65536 x 256 x
-// 256.  That is 2.1x the SIMT tiles on large products and a tie (or a loss) on the learners' own batch-256 / 512 products,
-// which is how gemm_tc_launch chooses.
+// One CTA (two warpgroups) computes a 128 x TN tile of C (TN = 64 or 32), each warpgroup 64 rows of it.  The contraction
+// axis is walked in chunks of 32:
+//   * all 8 warps read the chunk's A (128 x 32) and B (TN x 32) elements from global memory exactly as gemm.cuh's `Mat`
+//     describes them (two concatenated sources, a ones column, stacked networks; either the row or the feature axis of
+//     the Mat is the contraction axis), TWO chunks ahead of the one being multiplied (three register sets), split them
+//     into hi / lo and store them as 16-byte chunks into K-major no-swizzle tiles with a 144-byte chunk pitch — with that
+//     pitch both global layouts give conflict-free STS.128 and fully coalesced global loads;
+//   * three shared-memory stages, the products of one chunk stay in flight while the next chunk is stored;
+//   * epilogue: the register accumulators are staged through shared memory so that bias / mask / accumulate reads and
+//     the C stores are coalesced along j.
+// gemm_tc_launch sends products with fewer than 4096 output rows to the SIMT tiles.  That threshold was chosen for the
+// tcgen05 kernel this one replaces and has not been measured again on H100 (tools/gemm_bench.py times both engines).
 #include "gemm.cuh"
 #include "umma.cuh"
 
 namespace prl {
 
-int g_contraction_engine = 1;   // 1: tcgen05 tiles, 0: SIMT tiles (prl_set_contraction_engine)
+int g_contraction_engine = 1;   // 1: tensor-core tiles, 0: SIMT tiles (prl_set_contraction_engine)
 
 namespace {
 
-constexpr int TM = 128, GKT = 32, LBO = 144, SBO = 8 * LBO, NSTAGE = 3, NSET = 3, NLOAD = 256, NTHR = NLOAD + 32;
-
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(umma::smem_u32(bar)) : "memory");
-}
+constexpr int TM = 128, GKT = 32, LBO = 144, SBO = 8 * LBO, NSTAGE = 3, NSET = 3, NLOAD = 256;
 
 // which (row of the tile, 16-byte K chunk) a thread's slot u covers.  XO: the Mat's rows are the tile's rows (features are
 // contracted, contiguous along k): 8 lanes read one row's 128 contiguous bytes.  !XO: the Mat's rows are contracted
@@ -62,7 +54,7 @@ struct Operand {
     const float *zb1, *zb2;     // part bases with the network offset applied (zb2 also with -split)
     int off1[S], off2[S];       // XO: float offset of the slot's row in part 1 / part 2
     int kcu[S];                 // !XO: first contraction index of slot u inside a chunk
-    int soff[S];                // byte offset of the slot's 16-byte chunk inside the UMMA tile
+    int soff[S];                // byte offset of the slot's 16-byte chunk inside the operand tile
     const float *fbase;         // !XO: this thread's feature column
     int fld;                    // !XO: its row pitch
     bool isone, vec1, vec2;
@@ -151,7 +143,7 @@ struct Operand {
         if (con >= Kc) v = 0.f;
         return v;
     }
-    // split into hi (the value itself: the tensor core truncates) / lo and store as 16-byte chunks of the UMMA tiles
+    // split into hi (the value itself: the tensor core truncates) / lo and store as 16-byte chunks of the operand tiles
     __device__ __forceinline__ void store(int c, const float (&reg)[S][4], unsigned char *hi, unsigned char *lo) const {
         if (edge(c)) {                               // uniform branch, taken for at most two chunks of a product
 #pragma unroll
@@ -176,290 +168,173 @@ struct Operand {
             *reinterpret_cast<float4 *>(lo + soff[u]) = make_float4(l[0], l[1], l[2], l[3]);
         }
     }
-    // ROWS = 128, !XO only: this thread's 16 values of chunk c (tile row = 32 (w % 4) + lane, k = 16 (w / 4) .. + 16) go to
-    // tensor memory as the A operand of the TS-form MMA: hi at column a_col + 16 (w / 4), lo 32 columns further
-    __device__ __forceinline__ void store_tmem(int c, const float (&reg)[S][4], uint32_t taddr_hi) const {
-        static_assert(!XO || ROWS != 128, "TMEM operands are loaded with the lanes along the tile rows");
-        const bool is_edge = edge(c);
-        float v[16], l[16];
-#pragma unroll
-        for (int u = 0; u < 4; u++)
-#pragma unroll
-            for (int e = 0; e < 4; e++) v[u * 4 + e] = reg[u][e];
-        if (is_edge) {
-#pragma unroll
-            for (int u = 0; u < 4; u++)
-#pragma unroll
-                for (int e = 0; e < 4; e++) v[u * 4 + e] = edge_elem(c, u, e, v[u * 4 + e]);
-        }
-#pragma unroll
-        for (int i = 0; i < 16; i++) l[i] = v[i] - __uint_as_float(__float_as_uint(v[i]) & 0xffffe000u);
-        umma::tmem_st16(taddr_hi, v);
-        umma::tmem_st16(taddr_hi + 32, l);
-    }
 };
 
-// warps 0-7: loaders + epilogue; warp 8: TMEM owner, one lane issues the MMAs.  288 threads put three warps on one
-// sub-partition, which caps the kernel at 168 registers per thread.
-template <int TN, bool AO, bool BO>
-__global__ void __maxnreg__(168) k_gemm_tc(const GemmArgs g) {
-    extern __shared__ __align__(128) unsigned char dsm[];
-    __shared__ __align__(8) uint64_t full[NSTAGE], empty[NSTAGE], done;
-    __shared__ uint32_t tmem_slot;
-    constexpr int A_B = (TM / 8) * SBO, B_B = (TN / 8) * SBO, STAGE_B = 2 * A_B + 2 * B_B;
-    const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31, z = blockIdx.z;
-    const int i0 = blockIdx.x * TM, j0 = blockIdx.y * TN;
-    const int nch = (g.Kc + GKT - 1) / GKT;
-    const bool prof = g.stamps != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && z == 0 && lane == 0 && (w == 0 || w == 8);
-
-    if (w == 8) {
-        umma::tmem_alloc(&tmem_slot, TN);
-        if (lane == 0) {
-            for (int b = 0; b < NSTAGE; b++) { umma::mbar_init(&full[b], NLOAD / 32); umma::mbar_init(&empty[b], 1); }
-            umma::mbar_init(&done, 1);
-        }
-        umma::fence_before_thread_sync();
-        __syncthreads();
-        umma::fence_after_thread_sync();
-        if (umma::elect_one()) {   // one lane of the converged issuer warp: back-to-back UTCHMMA, descriptor math on the uniform datapath
-            const uint32_t tmem = tmem_slot, idesc = umma::make_idesc_tf32(TM, TN);
-            const uint64_t dproto = umma::make_desc2(0, LBO, SBO);
-            const uint32_t base = umma::smem_u32(dsm);
-            for (int c = 0; c < nch; c++) {
-                const int s = c % NSTAGE;
-                umma::mbar_wait(&full[s], (c / NSTAGE) & 1);
-                if (prof && c < 32) g.stamps[c * 8 + 5] = clock64();
-                umma::fence_after_thread_sync();
-                const uint32_t a = (base + s * STAGE_B) >> 4;
-                const uint64_t ah = dproto + a, al = ah + (A_B >> 4), bh = al + (A_B >> 4), bl = bh + (B_B >> 4);
-#pragma unroll
-                for (int ks = 0; ks < GKT / 8; ks++) {
-                    const uint64_t o = (uint64_t)(ks * ((2 * LBO) >> 4));
-                    umma::mma_tf32(tmem, al + o, bh + o, idesc, c > 0 || ks > 0);   // small terms first
-                    umma::mma_tf32(tmem, ah + o, bl + o, idesc, true);
-                    umma::mma_tf32(tmem, ah + o, bh + o, idesc, true);
-                }
-                umma::mma_commit(&empty[s]);      // arrives when the MMAs that read stage s have completed
-                if (prof && c < 32) g.stamps[c * 8 + 6] = clock64();
-            }
-            umma::mma_commit(&done);
-        }
-        __syncwarp();
-    } else {
-        const Operand<TM, AO> opA(g.A, z, i0, g.Mo, g.Kc, w, lane);
-        const Operand<TN, BO> opB(g.B, z, j0, g.No, g.Kc, w, lane);
-        float ra[NSET][TM / 32][4], rb[NSET][TN / 32][4];
-#pragma unroll
-        for (int p = 0; p < NSET - 1; p++)
-            if (p < nch) { opA.fetch(p, ra[p]); opB.fetch(p, rb[p]); }
-        if (prof) g.stamps[32 * 8 + 2] = clock64();
-        __syncthreads();   // barriers initialised, TMEM allocated
-        if (prof) g.stamps[32 * 8 + 3] = clock64();
-        static_assert(NSET == NSTAGE, "stage index == register set index");
-        for (int c0 = 0; c0 < nch; c0 += NSET) {
-#pragma unroll
-            for (int u = 0; u < NSET; u++) {
-                const int c = c0 + u;
-                if (c < nch) {
-                    if (prof && c < 32) g.stamps[c * 8 + 0] = clock64();
-                    if (c + NSET - 1 < nch) {       // two chunks ahead of the one being stored
-                        opA.fetch(c + NSET - 1, ra[(u + NSET - 1) % NSET]);
-                        opB.fetch(c + NSET - 1, rb[(u + NSET - 1) % NSET]);
-                    }
-                    if (prof && c < 32) g.stamps[c * 8 + 1] = clock64();
-                    if (c >= NSTAGE) umma::mbar_wait(&empty[u], ((c / NSTAGE) - 1) & 1);
-                    if (prof && c < 32) g.stamps[c * 8 + 2] = clock64();
-                    unsigned char *st = dsm + u * STAGE_B;
-                    opA.store(c, ra[u], st, st + A_B);
-                    opB.store(c, rb[u], st + 2 * A_B, st + 2 * A_B + B_B);
-                    if (prof && c < 32) g.stamps[c * 8 + 4] = clock64();
-                    umma::fence_async_smem();       // generic-proxy writes -> visible to the tensor core's async proxy
-                    __syncwarp();
-                    if (prof && c < 32) g.stamps[c * 8 + 3] = clock64();
-                    if (lane == 0) mbar_arrive(&full[u]);
-                }
-            }
-        }
-        umma::mbar_wait(&done, 0);
-        if (prof) g.stamps[32 * 8 + 0] = clock64();
-        umma::fence_after_thread_sync();
-
-        const uint32_t tmem = tmem_slot;
-        const int q = w & 3, h = w >> 2;
-        if (h * 32 < TN) {
-            float v[32];
-            umma::tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(h * 32), v);
-            float *tb = reinterpret_cast<float *>(dsm) + w * (32 * 33);   // the stages are free: every MMA has completed
-#pragma unroll
-            for (int t = 0; t < 32; t++) tb[lane * 33 + t] = v[t];
-            __syncwarp();
-            const int j = j0 + h * 32 + lane;
-            if (j < g.No) {
-                const float bj = g.bias ? __ldg(g.bias + z * g.bias_net_stride + j) : 0.f;
-                const bool tail = g.C_tail && j == g.tail_col;
-#pragma unroll 4
-                for (int rr = 0; rr < 32; rr++) {
-                    const int i = i0 + q * 32 + rr;
-                    if (i >= g.Mo) break;
-                    float x = tb[rr * 33 + lane];
-                    if (tail) { g.C_tail[z * g.tail_net_stride + i] = x; continue; }
-                    float *dst = g.C + z * g.c_net_stride + (size_t)i * g.ldc + j;
-                    if (g.bias) x += bj;
-                    if (g.accumulate) x += *dst;
-                    if (g.relu) x = fmaxf(x, 0.f);
-                    if (g.mask && !(__ldg(g.mask + z * g.mask_net_stride + (size_t)i * g.ldm + j) > 0.f)) x = 0.f;
-                    *dst = x;
-                }
-            }
-        }
-        umma::fence_before_thread_sync();
-        if (prof) g.stamps[32 * 8 + 1] = clock64();
-    }
+// Both warpgroups' accumulators (rows 64 wg .. of the tile) -> C, staged through shared memory (the operand stages are
+// free: every product has completed) so that the bias / mask / accumulate reads and the C stores are coalesced along C's
+// contiguous axis.  SWAP: the accumulator is C transposed (tile rows = C's column index).
+template <int TN, bool SWAP>
+__device__ __forceinline__ void epilogue(const GemmArgs &g, int z, const float *d, float *tb, int a0, int b0) {
+    const int tid = threadIdx.x, wg = tid >> 7;
     __syncthreads();
-    if (w == 8) {
-        umma::fence_after_thread_sync();
-        umma::tmem_dealloc(tmem_slot, TN);
+#pragma unroll
+    for (int j = 0; j < TN / 8; j++)
+#pragma unroll
+        for (int p = 0; p < 2; p++)
+#pragma unroll
+            for (int e = 0; e < 2; e++) tb[(wg * 64 + umma::acc_row(p)) * (TN + 1) + umma::acc_col(j, e)] = d[4 * j + 2 * p + e];
+    __syncthreads();
+    for (int o = tid; o < TM * TN; o += NLOAD) {
+        const int r = SWAP ? o % TM : o / TN, c = SWAP ? o / TM : o % TN;
+        const int i = SWAP ? b0 + c : a0 + r, j = SWAP ? a0 + r : b0 + c;
+        if (i < (SWAP ? g.No : g.Mo) && j < (SWAP ? g.Mo : g.No)) gemm_emit(g, z, i, j, tb[r * (TN + 1) + c]);
     }
 }
 
-// ---- TS form: the A operand lives in tensor memory -----------------------------------------------------------------
+// SS form: 8 warps = two warpgroups; every thread is loader and consumer.  Per chunk: store the chunk's tiles into stage
+// c % 3, make them visible to the tensor core, one block barrier, then each warpgroup issues the 12 wgmma of its 64 rows
+// (4 K-steps x 3 split terms) and leaves them in flight: the wait before the NEXT barrier only asks for the chunk before
+// to have completed, which is what frees the stage written after that barrier.
+template <int TN, bool AO, bool BO>
+__global__ void __launch_bounds__(NLOAD, 1) k_gemm_tc(const GemmArgs g) {
+    extern __shared__ __align__(128) unsigned char dsm[];
+    constexpr int A_B = (TM / 8) * SBO, B_B = (TN / 8) * SBO, STAGE_B = 2 * A_B + 2 * B_B;
+    const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31, wg = tid >> 7, z = blockIdx.z;
+    const int i0 = blockIdx.x * TM, j0 = blockIdx.y * TN;
+    const int nch = (g.Kc + GKT - 1) / GKT;
+    const uint32_t base = umma::smem_u32(dsm);
+
+    const Operand<TM, AO> opA(g.A, z, i0, g.Mo, g.Kc, w, lane);
+    const Operand<TN, BO> opB(g.B, z, j0, g.No, g.Kc, w, lane);
+    float ra[NSET][TM / 32][4], rb[NSET][TN / 32][4];
+    float d[TN / 2];
+#pragma unroll
+    for (int p = 0; p < NSET - 1; p++)
+        if (p < nch) { opA.fetch(p, ra[p]); opB.fetch(p, rb[p]); }
+    static_assert(NSET == NSTAGE, "stage index == register set index");
+    for (int c0 = 0; c0 < nch; c0 += NSET) {
+#pragma unroll
+        for (int u = 0; u < NSET; u++) {
+            const int c = c0 + u;
+            if (c < nch) {
+                if (c + NSET - 1 < nch) {       // two chunks ahead of the one being stored
+                    opA.fetch(c + NSET - 1, ra[(u + NSET - 1) % NSET]);
+                    opB.fetch(c + NSET - 1, rb[(u + NSET - 1) % NSET]);
+                }
+                unsigned char *st = dsm + u * STAGE_B;
+                opA.store(c, ra[u], st, st + A_B);
+                opB.store(c, rb[u], st + 2 * A_B, st + 2 * A_B + B_B);
+                umma::fence_async_smem();       // generic-proxy writes -> visible to the tensor core's async proxy
+                umma::wg_wait<1>();             // chunk c - 2 has completed: after the barrier its stage may be overwritten
+                __syncthreads();
+                const umma::Tile ah{base + u * STAGE_B + wg * (64 / 8) * SBO, LBO, SBO}, al = ah.shifted(A_B);
+                const umma::Tile bh{base + u * STAGE_B + 2 * A_B, LBO, SBO}, bl = bh.shifted(B_B);
+                umma::gemm3<TN>(d, ah, al, bh, bl, GKT, c > 0);
+                umma::wg_commit();
+            }
+        }
+    }
+    umma::wg_wait<0>();
+    epilogue<TN, false>(g, z, d, reinterpret_cast<float *>(dsm), i0, j0);
+}
+
+// ---- RS form: the A operand lives in registers ---------------------------------------------------------------------
 // The SS kernel above moves 120 KB through shared memory per 32-deep chunk of a 128 x 64 tile (48 KB of hi / lo stores and
-// 72 KB of operand reads by the 12 MMAs).  This form was written to test whether that is what bounds it — it is not: the two
-// run within 10 % of each other.  Here the 128-row operand never touches shared memory: it must be the operand whose Mat
-// has the tile rows along the contiguous axis ("rows contracted"), so that lane l of warp w loads row 32 (w % 4) + l for
-// 16 consecutive contraction indices with coalesced loads and writes hi / lo straight into its own TMEM lane
-// (tcgen05.st).  Shared memory only carries the TN-row operand: 16 KB of stores + 24 KB of MMA reads per chunk.
+// 72 KB of operand reads by the 12 MMAs).  Here the 128-row operand never touches shared memory: it must be the operand
+// whose Mat has the tile rows along the contiguous axis ("rows contracted"); every thread loads exactly the elements of
+// its own wgmma A fragments (8 consecutive tile rows x 4 contraction indices per warp and load: whole 32-byte sectors).
+// Shared memory only carries the TN-row operand: 16 KB of stores + 24 KB of MMA reads per chunk.  The fragments of a chunk
+// are the operands of products in flight, so a chunk's products are waited for before the next chunk's split.
 //   nn.Linear forward     D[n][m] = sum_k Wt[k][n] x[m][k]     A = a transposed copy of W kept by the learner, SWAP
 //   backward-data         D[k][m] = sum_n W[n][k] dy[m][n]      A = W as stored, SWAP
 //   backward-weight       D[n][k] = sum_m dy[m][n] x[m][k]      A = dy as stored
-// SWAP: the accumulator is C transposed (lanes = C's column index): the epilogue stores straight from registers, coalesced.
-constexpr int TS_ACC_COLS = 64, TS_STAGE_COLS = 64, TS_TMEM_COLS = 256;
+// SWAP: the accumulator is C transposed (tile rows = C's column index).
+struct FragA {
+    const float *base[2];   // this thread's two tile rows (Mat features) at contraction index 0
+    int fld[2];
+    bool one[2];
+    int Kc, t;
+    __device__ __forceinline__ FragA(const Mat &m, int z, int out0, int out_lim, int Kc_) : Kc(Kc_), t(threadIdx.x & 3) {
+        const float *zb1 = m.p1 + z * m.net_stride1, *zb2 = m.p2 + z * m.net_stride2 - m.split;
+#pragma unroll
+        for (int p = 0; p < 2; p++) {
+            const int out = out0 + (threadIdx.x >> 7) * 64 + umma::acc_row(p);
+            one[p] = out == m.ones_at && out < out_lim;
+            int f = min(out, out_lim - 1);
+            if (f == m.ones_at) f = 0;                      // any valid address: the value is replaced by 1.0 / never used
+            base[p] = f < m.split ? zb1 + f : zb2 + f;
+            fld[p] = f < m.split ? m.ld1 : m.ld2;
+        }
+    }
+    // reg[4 ks + 2 q + p] = A[row p][32 c + 8 ks + t + 4 q]; indices past the contraction axis repeat the last one
+    __device__ __forceinline__ void fetch(int c, float (&reg)[16]) const {
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+            const int k = c * GKT + 8 * (i >> 2) + t + 4 * ((i >> 1) & 1);
+            reg[i] = __ldg(base[i & 1] + (size_t)min(k, Kc - 1) * fld[i & 1]);
+        }
+    }
+    __device__ __forceinline__ void split(int c, const float (&reg)[16], float (&hi)[16], float (&lo)[16]) const {
+#pragma unroll
+        for (int i = 0; i < 16; i++) {
+            const int k = c * GKT + 8 * (i >> 2) + t + 4 * ((i >> 1) & 1);
+            float v = one[i & 1] ? 1.f : reg[i];
+            if (k >= Kc) v = 0.f;
+            umma::split_tf32(v, hi[i], lo[i]);
+        }
+    }
+};
 
 template <int TN, bool BO, bool SWAP>
-__global__ void __maxnreg__(168) k_gemm_ts(const GemmArgs g) {
+__global__ void __launch_bounds__(NLOAD, 1) k_gemm_ts(const GemmArgs g) {
     extern __shared__ __align__(128) unsigned char dsm[];
-    __shared__ __align__(8) uint64_t full[NSTAGE], empty[NSTAGE], done;
-    __shared__ uint32_t tmem_slot;
     constexpr int B_B = (TN / 8) * SBO, STAGE_B = 2 * B_B;
-    static_assert(TN <= TS_ACC_COLS && TS_ACC_COLS + NSTAGE * TS_STAGE_COLS <= TS_TMEM_COLS, "TMEM column budget");
     const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31, z = blockIdx.z;
     const int a0 = blockIdx.x * TM, b0 = blockIdx.y * TN;
     const int nch = (g.Kc + GKT - 1) / GKT;
+    const uint32_t base = umma::smem_u32(dsm);
 
-    if (w == 8) {
-        umma::tmem_alloc(&tmem_slot, TS_TMEM_COLS);
-        if (lane == 0) {
-            for (int b = 0; b < NSTAGE; b++) { umma::mbar_init(&full[b], NLOAD / 32); umma::mbar_init(&empty[b], 1); }
-            umma::mbar_init(&done, 1);
-        }
-        umma::fence_before_thread_sync();
-        __syncthreads();
-        umma::fence_after_thread_sync();
-        if (umma::elect_one()) {   // one lane of the converged issuer warp: back-to-back UTCHMMA, descriptor math on the uniform datapath
-            const uint32_t tmem = tmem_slot, idesc = umma::make_idesc_tf32(TM, TN);
-            const uint64_t dproto = umma::make_desc2(0, LBO, SBO);
-            const uint32_t base = umma::smem_u32(dsm);
-            for (int c = 0; c < nch; c++) {
-                const int s = c % NSTAGE;
-                umma::mbar_wait(&full[s], (c / NSTAGE) & 1);
-                umma::fence_after_thread_sync();
-                const uint64_t bh = dproto + ((base + s * STAGE_B) >> 4), bl = bh + (B_B >> 4);
-                const uint32_t ah = tmem + TS_ACC_COLS + s * TS_STAGE_COLS, al = ah + 32;
+    const FragA opA(g.A, z, a0, g.Mo, g.Kc);
+    const Operand<TN, BO> opB(g.B, z, b0, g.No, g.Kc, w, lane);
+    float ra[NSET][16], rb[NSET][TN / 32][4];
+    float hi[16], lo[16], d[TN / 2];
 #pragma unroll
-                for (int ks = 0; ks < GKT / 8; ks++) {
-                    const uint64_t o = (uint64_t)(ks * ((2 * LBO) >> 4));
-                    umma::mma_tf32_ts(tmem, al + ks * 8, bh + o, idesc, c > 0 || ks > 0);   // small terms first
-                    umma::mma_tf32_ts(tmem, ah + ks * 8, bl + o, idesc, true);
-                    umma::mma_tf32_ts(tmem, ah + ks * 8, bh + o, idesc, true);
+    for (int p = 0; p < NSET - 1; p++)
+        if (p < nch) { opA.fetch(p, ra[p]); opB.fetch(p, rb[p]); }
+    for (int c0 = 0; c0 < nch; c0 += NSET) {
+#pragma unroll
+        for (int u = 0; u < NSET; u++) {
+            const int c = c0 + u;
+            if (c < nch) {
+                if (c + NSET - 1 < nch) {
+                    opA.fetch(c + NSET - 1, ra[(u + NSET - 1) % NSET]);
+                    opB.fetch(c + NSET - 1, rb[(u + NSET - 1) % NSET]);
                 }
-                umma::mma_commit(&empty[s]);
-            }
-            umma::mma_commit(&done);
-        }
-        __syncwarp();
-    } else {
-        const Operand<TM, false> opA(g.A, z, a0, g.Mo, g.Kc, w, lane);
-        const Operand<TN, BO> opB(g.B, z, b0, g.No, g.Kc, w, lane);
-        float ra[NSET][TM / 32][4], rb[NSET][TN / 32][4];
-#pragma unroll
-        for (int p = 0; p < NSET - 1; p++)
-            if (p < nch) { opA.fetch(p, ra[p]); opB.fetch(p, rb[p]); }
-        __syncthreads();   // barriers initialised, TMEM allocated
-        const uint32_t tmem = tmem_slot;
-        const uint32_t my_a = tmem + ((uint32_t)((w & 3) * 32) << 16) + TS_ACC_COLS + (w >> 2) * 16;   // this warp's lanes, its half of the chunk
-        for (int c0 = 0; c0 < nch; c0 += NSET) {
-#pragma unroll
-            for (int u = 0; u < NSET; u++) {
-                const int c = c0 + u;
-                if (c < nch) {
-                    if (c + NSET - 1 < nch) {
-                        opA.fetch(c + NSET - 1, ra[(u + NSET - 1) % NSET]);
-                        opB.fetch(c + NSET - 1, rb[(u + NSET - 1) % NSET]);
-                    }
-                    if (c >= NSTAGE) {
-                        umma::mbar_wait(&empty[u], ((c / NSTAGE) - 1) & 1);
-                        umma::fence_after_thread_sync();
-                    }
-                    unsigned char *st = dsm + u * STAGE_B;
-                    opA.store_tmem(c, ra[u], my_a + u * TS_STAGE_COLS);
-                    opB.store(c, rb[u], st, st + B_B);
-                    umma::tmem_st_wait();
-                    umma::fence_async_smem();
-                    umma::fence_before_thread_sync();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&full[u]);
-                }
+                umma::wg_wait<0>();             // hi / lo are the operands of the previous chunk's products
+                opA.split(c, ra[u], hi, lo);
+                unsigned char *st = dsm + u * STAGE_B;
+                opB.store(c, rb[u], st, st + B_B);
+                umma::fence_async_smem();
+                __syncthreads();
+                const umma::Tile bh{base + u * STAGE_B, LBO, SBO}, bl = bh.shifted(B_B);
+                umma::gemm3_rs<TN, GKT / 8>(d, hi, lo, bh, bl, c > 0);
+                umma::wg_commit();
             }
         }
-        umma::mbar_wait(&done, 0);
-        umma::fence_after_thread_sync();
-
-        const int q = w & 3, h = w >> 2;
-        if (h * 32 < TN) {
-            float v[32];
-            umma::tmem_ld32(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(h * 32), v);
-            if (SWAP) {      // lane = C's column j, accumulator column = C's row i: every store instruction covers 32 consecutive j
-                const int j = a0 + q * 32 + lane;
-                if (j < g.Mo) {
-#pragma unroll
-                    for (int t = 0; t < 32; t++) {
-                        const int i = b0 + h * 32 + t;
-                        if (i < g.No) gemm_emit(g, z, i, j, v[t]);
-                    }
-                }
-            } else {         // lane = C's row: transpose through shared memory (the stages are free) for coalesced stores
-                float *tb = reinterpret_cast<float *>(dsm) + w * (32 * 33);
-#pragma unroll
-                for (int t = 0; t < 32; t++) tb[lane * 33 + t] = v[t];
-                __syncwarp();
-                const int j = b0 + h * 32 + lane;
-                if (j < g.No) {
-#pragma unroll 4
-                    for (int rr = 0; rr < 32; rr++) {
-                        const int i = a0 + q * 32 + rr;
-                        if (i < g.Mo) gemm_emit(g, z, i, j, tb[rr * 33 + lane]);
-                    }
-                }
-            }
-        }
-        umma::fence_before_thread_sync();
     }
-    __syncthreads();
-    if (w == 8) {
-        umma::fence_after_thread_sync();
-        umma::tmem_dealloc(tmem_slot, TS_TMEM_COLS);
-    }
+    umma::wg_wait<0>();
+    epilogue<TN, SWAP>(g, z, d, reinterpret_cast<float *>(dsm), a0, b0);
 }
 
 template <int TN>
 constexpr int ts_smem_bytes() {
-    constexpr int stages = NSTAGE * 2 * (TN / 8) * SBO, transpose = 8 * 32 * 33 * 4;
+    constexpr int stages = NSTAGE * 2 * (TN / 8) * SBO, transpose = TM * (TN + 1) * 4;
     return stages > transpose ? stages : transpose;
 }
 template <int TN, bool BO, bool SWAP>
 void launch_ts(const GemmArgs &g, int nets, cudaStream_t st) {
     dim3 grid((g.Mo + TM - 1) / TM, (g.No + TN - 1) / TN, nets);
-    k_gemm_ts<TN, BO, SWAP><<<grid, NTHR, ts_smem_bytes<TN>(), st>>>(g);
+    k_gemm_ts<TN, BO, SWAP><<<grid, NLOAD, ts_smem_bytes<TN>(), st>>>(g);
 }
 
 template <int TN>
@@ -473,7 +348,7 @@ cudaError_t prepare_one() {
 template <int TN, bool AO, bool BO>
 void launch_one(const GemmArgs &g, int nets, cudaStream_t st) {
     dim3 grid((g.Mo + TM - 1) / TM, (g.No + TN - 1) / TN, nets);
-    k_gemm_tc<TN, AO, BO><<<grid, NTHR, smem_bytes<TN>(), st>>>(g);
+    k_gemm_tc<TN, AO, BO><<<grid, NLOAD, smem_bytes<TN>(), st>>>(g);
 }
 
 template <bool AO, bool BO>
@@ -500,15 +375,15 @@ cudaError_t gemm_tc_prepare() {
     return cudaSuccess;
 }
 
-// engine: -1 = the library default (g_contraction_engine); 0 = SIMT tiles; 1 = automatic: tcgen05 tiles from 4096 output
-// rows on, where they are the faster of the two (see the header of this file), SIMT tiles below; 2 = tcgen05 always (callers
-// whose results must not depend on how many rows a launch sees: PPO's rollout passes); 64 / 32 = tcgen05 with that tile width.
+// engine: -1 = the library default (g_contraction_engine); 0 = SIMT tiles; 1 = automatic: tensor-core tiles from 4096 output
+// rows on (see the header of this file), SIMT tiles below; 2 = tensor cores always (callers whose results must not depend
+// on how many rows a launch sees: PPO's rollout passes); 64 / 32 = tensor cores with that tile width.
 bool gemm_tc_launch(const GemmArgs &g, int nets, bool ao, bool bo, cudaStream_t st, int engine) {
     if (engine < 0) engine = g_contraction_engine;
     if (engine == 0 || g.Mo <= 0 || g.No <= 0 || g.Kc <= 0) return false;
     if (!ao && bo) return false;   // not a shape the learners use
     if (engine == 1 && g.Mo < 4096) return false;
-    if (engine == 164 || engine == 132) engine = 2;    // the TS form declined the shape
+    if (engine == 164 || engine == 132) engine = 2;    // the RS form declined the shape
     const int tn = engine == 64 || engine == 32 ? engine : (g.No > 32 ? 64 : 32);
     if (ao && bo) launch_tn<true, true>(g, nets, st, tn);
     else if (ao) launch_tn<true, false>(g, nets, st, tn);
@@ -516,11 +391,9 @@ bool gemm_tc_launch(const GemmArgs &g, int nets, bool ao, bool bo, cudaStream_t 
     return true;
 }
 
-// TS form.  gs is already in the kernel's orientation: gs.A = the 128-row operand (its Mat rows are contracted), gs.Mo its
+// RS form.  gs is already in the kernel's orientation: gs.A = the 128-row operand (its Mat rows are contracted), gs.Mo its
 // extent, gs.B / gs.No the other operand; swap = the accumulator is C transposed.  Only on request (engine 164 / 132 = this
-// form with tile width 64 / 32): measured on a B200 it is within +-10 % of the SS form on every shape of the learners
-// (profiles/r2_gemm_tc.md) — neither form is bound by shared-memory bandwidth or by the tensor pipe, both wait for the
-// global loads of their operands — so the automatic choice never needs it and no learner has to keep transposed weights.
+// form with tile width 64 / 32): the automatic choice uses the SS form, for which no learner has to keep transposed weights.
 bool gemm_ts_launch(const GemmArgs &gs, int nets, bool bo, bool swap, cudaStream_t st, int engine) {
     if (engine < 0) engine = g_contraction_engine;
     if ((engine != 164 && engine != 132) || gs.Mo <= 0 || gs.No <= 0 || gs.Kc <= 0) return false;
@@ -531,7 +404,7 @@ bool gemm_ts_launch(const GemmArgs &gs, int nets, bool bo, bool swap, cudaStream
     return true;
 }
 
-// dst[z][c][r] = src[z][r][c]  (the transposed weight copies the TS-form forward reads)
+// dst[z][c][r] = src[z][r][c]  (the transposed weight copies the RS-form forward reads)
 __global__ void k_transpose(int rows, int cols, const float *__restrict__ src, float *__restrict__ dst) {
     __shared__ float t[32][33];
     const size_t zo = (size_t)blockIdx.z * rows * cols;
@@ -550,15 +423,12 @@ void transpose_weights(int rows, int cols, int nets, const float *src, float *ds
 }  // namespace prl
 
 extern "C" int prl_set_contraction_engine(int engine) {
-    PRL_REQUIRE(engine >= 0 && engine <= 2, "engine must be 0 (SIMT tiles), 1 (automatic) or 2 (tcgen05 tiles always)");
+    PRL_REQUIRE(engine >= 0 && engine <= 2, "engine must be 0 (SIMT tiles), 1 (automatic) or 2 (tensor-core tiles always)");
     prl::g_contraction_engine = engine;
     return PRL_OK;
 }
 extern "C" int prl_get_contraction_engine(void) { return prl::g_contraction_engine; }
 
-static long long *g_test_stamps = nullptr;
-/* developer profiling: device int64[33][8] receiving SM-clock stamps of CTA 0 of the next prl_test_contraction calls */
-extern "C" int prl_test_contraction_stamps(long long *stamps_dev) { g_test_stamps = stamps_dev; return PRL_OK; }
 
 // Test hook: one contraction of the learners' three kinds through GemmLauncher.
 //   op 0  y[M x N]  = act(x W^T + b)          a = x [M x K] (or [M x split] with a2 = [M x (K - split)]), b = W [N x K]
@@ -573,7 +443,6 @@ extern "C" int prl_test_contraction(int op, int engine, int M, int N, int K, con
     GemmLauncher L;   // prl_init has prepared the kernels
     L.st = (cudaStream_t)stream;
     L.engine = engine;
-    L.stamps = g_test_stamps;
     const long long MK = (long long)M * K, MN = (long long)M * N, NK = (long long)N * K;
     if (op == 0) {
         Mat X = a2 ? mat2(a, split, split, a2, K - split, (long long)M * split, (long long)M * (K - split)) : mat(a, K, MK);

@@ -35,8 +35,8 @@ extern "C" int prl_init(int device) {
     PRL_CUDA(cudaSetDevice(device));
     cudaDeviceProp p;
     PRL_CUDA(cudaGetDeviceProperties(&p, device));
-    if (p.major != 10)
-        return fail(PRL_EUNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_100a only",
+    if (p.major != 9)
+        return fail(PRL_EUNSUPPORTED, "device %d is sm_%d%d; this library is built for sm_90a only",
                     device, p.major, p.minor);
     PRL_CUDA(prl::gemm_tc_prepare());
     return PRL_OK;

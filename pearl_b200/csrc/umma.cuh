@@ -1,18 +1,25 @@
-// umma.cuh — thin inline-PTX layer over Blackwell's 5th-generation tensor cores
-// (tcgen05.mma with TMEM accumulators) for the dense contractions of the learner.
+// umma.cuh — thin inline-PTX layer over Hopper's warpgroup tensor-core instruction
+// (wgmma.mma_async, sm_90a) for the dense contractions of the learners.
 //
 // fp32 parity needs more than one TF32 pass: every fp32 operand x is split
 //   x = hi + lo,  hi = trunc_tf32(x) (done by the hardware),  lo = x - hi
-// and a product is accumulated as hi*hi + hi*lo + lo*hi in the fp32 TMEM
+// and a product is accumulated as hi*hi + hi*lo + lo*hi in the fp32 register
 // accumulator ("3xTF32"): relative error ~2^-21 per product instead of 2^-11.
 //
-// Operand tiles live in shared memory in the canonical K-major NO-SWIZZLE
-// ("interleaved") UMMA layout, written directly by SIMT code:
+// A product is issued by one whole warpgroup (128 threads, 4 consecutive warps):
+// D[64 x N] (+)= A[64 x 8] * B[N x 8]^T, the accumulator spread over the warpgroup's registers:
+//   thread (warp w of the warpgroup, g = lane / 4, t = lane % 4), register d[4 j + 2 p + e]
+//   holds D[16 w + g + 8 p][8 j + 2 t + e]                                   (acc_row / acc_col below)
+// B always comes from shared memory, A from shared memory (SS form) or from registers (RS form):
+//   a[2 q + p] = A[16 w + g + 8 p][t + 4 q].
+//
+// Shared-memory operand tiles are in the canonical K-major NO-SWIZZLE ("interleaved") layout,
+// written directly by SIMT code:
 //   16-byte chunk c = k/4 of row r sits at  (r/8)*SBO + c*LBO + (r%8)*16
 //   (8 rows x 16 B = one 128-byte core matrix; LBO = 128 B so the core matrices
 //    of one 8-row group are contiguous along K; SBO = (K/4)*128 B)
-// One tcgen05.mma.kind::tf32 consumes K = 8 (two chunks); the next K step
-// advances the descriptor start address by 2*LBO.
+// One wgmma of kind tf32 consumes K = 8 (two chunks); the next K step advances the
+// descriptor start address by 2*LBO.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -31,63 +38,23 @@ __device__ __forceinline__ int tile_index(int r, int k, int K) {
     return (r >> 3) * (tile_sbo(K) >> 2) + (k >> 2) * 32 + (r & 7) * 4 + (k & 3);
 }
 
-__device__ __forceinline__ float tf32_rna(float x) {
-    uint32_t u;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(u) : "f"(x));
-    return __uint_as_float(u);
-}
-// The tensor core TRUNCATES fp32 operands to TF32 (measured, tests/test_gpu_umma.py), so the "hi" operand
+// The tensor core TRUNCATES fp32 operands to TF32 (the 3xTF32 cases of tests/test_gpu_umma.py only reach 4e-6 if it
+// does: with rounding, hi + lo would not add up to x), so the "hi" operand
 // can be x itself and lo = x - trunc_tf32(x) (exact in fp32; its own truncation costs 2^-21 relative).
+__device__ __forceinline__ float tf32_lo(float x) { return x - __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 __device__ __forceinline__ void split_tf32(float x, float &hi, float &lo) {
     hi = x;
-    lo = x - __uint_as_float(__float_as_uint(x) & 0xffffe000u);
+    lo = tf32_lo(x);
 }
 
 // ---- descriptors ------------------------------------------------------------
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout): start address>>4 [0,14),
-// LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48), layout type [61,64) = 0 (no swizzle)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, int sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
-    d |= (uint64_t)((LBO >> 4) & 0x3fff) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
-}
-// instruction descriptor for kind::tf32, fp32 accumulate, both operands K-major
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, M x N x 8
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n"
-        ::"r"(tmem_d), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-
-// same with the A operand in tensor memory (lanes = rows, one 32-bit column per K element): no shared
-// memory traffic for A, which at N = 64 is what bounds the SS form (6 KB of operands per MMA at 128 B/clk)
-__device__ __forceinline__ void mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t b_desc, uint32_t idesc,
-                                            bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}\n"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate)
-        : "memory");
-}
-
-// generic descriptor: explicit LBO / SBO (bytes)
+// shared-memory matrix descriptor: start address>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46),
+// layout type [62,64) = 0 (no swizzle)
 __device__ __forceinline__ uint64_t make_desc2(uint32_t smem_addr, int lbo_bytes, int sbo_bytes) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3fff);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3fff) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3fff) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
 
@@ -97,8 +64,7 @@ __device__ __forceinline__ uint64_t make_desc2(uint32_t smem_addr, int lbo_bytes
 // lbo = 144: "transposed-write friendly": when 32 lanes write the SAME row r and consecutive k
 //            (a thread that owns batch row k scatters its values into column k of the tile), the
 //            addresses (k/4)*144 + (k%4)*4 hit 32 distinct banks.
-// MN-major tf32 operands are NOT usable with the no-swizzle layout (measured: garbage), so the backward
-// pass builds explicitly transposed tiles instead.
+// wgmma has no MN-major form for tf32 operands, so the backward pass builds explicitly transposed tiles.
 struct Tile {
     uint32_t addr;  // shared-memory byte address
     int lbo, sbo;   // bytes
@@ -112,93 +78,117 @@ __device__ __forceinline__ int tile_index2(int r, int k, int K, int lbo) {
 }
 __device__ __forceinline__ Tile make_tile(const void *p, int K, int lbo) { return Tile{smem_u32(p), lbo, (K >> 2) * lbo}; }
 
-// One lane of a CONVERGED warp (call it under a warp-uniform condition, all 32 lanes executing).  MMA issue code must sit
-// under `if (elect_one())`, not under `if (lane == 0)`: tcgen05.mma is a uniform-datapath instruction (UTCHMMA, operands in
-// uniform registers).  Behind a thread-index predicate nvcc wraps EVERY mma in a serialisation loop over the active lanes
-// (ELECT + 4 R2UR.BROADCAST + PLOP3 + BRA.U.ANY: ~13 dependent instructions, 53 clk per 128 x 64 x 8 product against a
-// tensor-pipe floor of 32); behind elect.sync it knows exactly one lane runs and emits back-to-back UTCHMMA with the
-// descriptor arithmetic on the uniform datapath (ncu source view: profiles/r2_k_dqn_tc_stalls.md).
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}\n" : "=r"(pred));
-    return pred != 0;
-}
+// ---- accumulator / register-operand coordinates of this thread -----------------
+__device__ __forceinline__ int acc_row(int p) { return ((threadIdx.x >> 5) & 3) * 16 + ((threadIdx.x & 31) >> 2) + 8 * p; }  // p = 0, 1
+__device__ __forceinline__ int acc_col(int j, int e) { return 8 * j + 2 * (threadIdx.x & 3) + e; }                            // e = 0, 1
+// A product whose A operand is a previous accumulator (RS form) contracts over the accumulator's columns: K slot t of
+// step j is fed from column 8 j + 2 t and slot t + 4 from column 8 j + 2 t + 1.  The B tile of such a product stores
+// column k of its matrix at the K position kperm(k), which makes the pairing right without moving a register.
+__host__ __device__ constexpr int kperm(int k) { return (k & ~7) | ((k & 1) << 2) | ((k & 7) >> 1); }
 
-// 3xTF32: D[M x N] (+)= A[M x K] * B[N x K]^T; issued by ONE thread.  *_exact: the operand is exactly
-// representable in TF32 (0/1 indicators), its lo tile is not needed.  Descriptors are built once; a K
-// step of 8 only adds (2*lbo)>>4 to the 14-bit start-address field.
-__device__ __forceinline__ void gemm3(uint32_t tmem_d, Tile a_hi, Tile a_lo, Tile b_hi, Tile b_lo, int M, int N, int K,
-                                      bool accumulate_first, bool a_exact = false, bool b_exact = false) {
-    const uint32_t idesc = make_idesc_tf32(M, N);
+// ---- synchronisation of the asynchronous tensor-core proxy -------------------------
+// registers written by ordinary instructions (accumulators, RS operands) -> visible to the next wgmma
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+// make generic-proxy shared-memory writes visible to the tensor core (async proxy)
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ---- one wgmma: D[64 x N] (+)= A[64 x 8] B[N x 8]^T, N in {8, 16, 32, 64}; d: N / 2 registers -----------
+template <int N> struct Mma;
+
+#define UMMA_D4(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3])
+#define UMMA_D8(o) UMMA_D4(o), UMMA_D4(o + 4)
+#define UMMA_D16(o) UMMA_D8(o), UMMA_D8(o + 8)
+#define UMMA_D32(o) UMMA_D16(o), UMMA_D16(o + 16)
+#define UMMA_DEFINE(N, DREGS, DOPS, A0, B0, P0)                                                                         \
+    template <> struct Mma<N> {                                                                                         \
+        static __device__ __forceinline__ void ss(float *d, uint64_t a_desc, uint64_t b_desc, bool accumulate) {        \
+            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #P0 ", 0;\n\t"                                        \
+                         "wgmma.mma_async.sync.aligned.m64n" #N "k8.f32.tf32.tf32 " DREGS ", %" #A0 ", %" #B0 ", p, 1, 1;\n\t}\n" \
+                         : DOPS                                                                                         \
+                         : "l"(a_desc), "l"(b_desc), "r"((uint32_t)accumulate));                                        \
+        }                                                                                                               \
+    };
+UMMA_DEFINE(8, "{%0, %1, %2, %3}", UMMA_D4(0), 4, 5, 6)
+UMMA_DEFINE(16, "{%0, %1, %2, %3, %4, %5, %6, %7}", UMMA_D8(0), 8, 9, 10)
+UMMA_DEFINE(32, "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}", UMMA_D16(0), 16, 17, 18)
+UMMA_DEFINE(64,
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+            "%24, %25, %26, %27, %28, %29, %30, %31}",
+            UMMA_D32(0), 32, 33, 34)
+#undef UMMA_DEFINE
+
+// RS form (A fragment a[0..3] in registers), N in {32, 64}
+template <int N>
+__device__ __forceinline__ void mma_rs(float *d, const float *a, uint64_t b_desc, bool accumulate);
+template <>
+__device__ __forceinline__ void mma_rs<32>(float *d, const float *a, uint64_t b_desc, bool accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1;\n\t}\n"
+                 : UMMA_D16(0)
+                 : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])),
+                   "l"(b_desc), "r"((uint32_t)accumulate));
+}
+template <>
+__device__ __forceinline__ void mma_rs<64>(float *d, const float *a, uint64_t b_desc, bool accumulate) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+                 "%24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}\n"
+                 : UMMA_D32(0)
+                 : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])),
+                   "l"(b_desc), "r"((uint32_t)accumulate));
+}
+#undef UMMA_D32
+#undef UMMA_D16
+#undef UMMA_D8
+#undef UMMA_D4
+
+// 3xTF32, SS form: d[64 x N] (+)= A[64 x K] * B[N x K]^T; executed by every thread of ONE warpgroup, which must have
+// fenced its shared-memory writes (fence_async_smem + barrier) before.  *_exact: the operand is exactly representable in
+// TF32 (0/1 indicators), its lo tile is not needed.  Descriptors are built once; a K step of 8 only adds (2*lbo)>>4 to the
+// 14-bit start-address field.  The caller commits and waits (wg_commit / wg_wait).
+template <int N>
+__device__ __forceinline__ void gemm3(float *d, Tile a_hi, Tile a_lo, Tile b_hi, Tile b_lo, int K, bool accumulate_first,
+                                      bool a_exact = false, bool b_exact = false) {
     uint64_t ah = a_hi.desc(0), al = a_lo.desc(0), bh = b_hi.desc(0), bl = b_lo.desc(0);
     const uint64_t da = (uint64_t)((2 * a_hi.lbo) >> 4), db = (uint64_t)((2 * b_hi.lbo) >> 4);
     bool acc = accumulate_first;
+    wg_fence();
     for (int ks = 0; ks < (K >> 3); ks++) {
-        if (!a_exact) { mma_tf32(tmem_d, al, bh, idesc, acc); acc = true; }
-        if (!b_exact) { mma_tf32(tmem_d, ah, bl, idesc, acc); acc = true; }
-        mma_tf32(tmem_d, ah, bh, idesc, acc);
+        if (!a_exact) { Mma<N>::ss(d, al, bh, acc); acc = true; }   // small terms first
+        if (!b_exact) { Mma<N>::ss(d, ah, bl, acc); acc = true; }
+        Mma<N>::ss(d, ah, bh, acc);
         acc = true;
         ah += da; al += da; bh += db; bl += db;
     }
 }
 
-// 3xTF32 with A (hi / lo) in tensor memory: a_hi / a_lo are TMEM column addresses of [M lanes][K columns]
-__device__ __forceinline__ void gemm3_ts(uint32_t tmem_d, uint32_t a_hi, uint32_t a_lo, Tile b_hi, Tile b_lo, int M, int N,
-                                         int K, bool accumulate_first) {
-    const uint32_t idesc = make_idesc_tf32(M, N);
+// 3xTF32, RS form: a_hi / a_lo hold this thread's A fragments of (at most) KSTEPS K steps (4 registers each).  The registers
+// must not be written again before the products have been waited for.
+template <int N, int KSTEPS>
+__device__ __forceinline__ void gemm3_rs(float *d, const float *a_hi, const float *a_lo, Tile b_hi, Tile b_lo, bool accumulate_first,
+                                         int ksteps = KSTEPS) {
     uint64_t bh = b_hi.desc(0), bl = b_lo.desc(0);
     const uint64_t db = (uint64_t)((2 * b_hi.lbo) >> 4);
-    bool acc = accumulate_first;
-    for (int ks = 0; ks < (K >> 3); ks++) {
-        mma_tf32_ts(tmem_d, a_lo + ks * 8, bh, idesc, acc);
-        mma_tf32_ts(tmem_d, a_hi + ks * 8, bl, idesc, true);
-        mma_tf32_ts(tmem_d, a_hi + ks * 8, bh, idesc, true);
-        acc = true;
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < KSTEPS; ks++) {
+        if (ks >= ksteps) break;
+        mma_rs<N>(d, a_lo + 4 * ks, bh, accumulate_first || ks > 0);
+        mma_rs<N>(d, a_hi + 4 * ks, bl, true);
+        mma_rs<N>(d, a_hi + 4 * ks, bh, true);
         bh += db; bl += db;
     }
 }
 
-// 3xTF32 product of one [M x K] A tile pair and one [N x K] B tile pair into a TMEM accumulator.
-// Issued by ONE thread.  a_hi/a_lo/b_hi/b_lo: shared addresses of the tiles.
-__device__ __forceinline__ void gemm_3xtf32(uint32_t tmem_d, uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
-                                            uint32_t b_lo, int M, int N, int K, bool accumulate_first) {
-    const uint32_t idesc = make_idesc_tf32(M, N);
-    const int sbo = tile_sbo(K);
-    bool acc = accumulate_first;
-    for (int k = 0; k < K; k += 8) {
-        const uint32_t o = (uint32_t)(k >> 2) * LBO;
-        const uint64_t ah = make_desc(a_hi + o, sbo), al = make_desc(a_lo + o, sbo);
-        const uint64_t bh = make_desc(b_hi + o, sbo), bl = make_desc(b_lo + o, sbo);
-        mma_tf32(tmem_d, al, bh, idesc, acc);   // small terms first
-        mma_tf32(tmem_d, ah, bl, idesc, true);
-        mma_tf32(tmem_d, ah, bh, idesc, true);
-        acc = true;
-    }
-}
-
-// ---- TMEM management ----------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t *smem_result, uint32_t ncols) {  // one full warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // the allocating warp
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void fence_before_thread_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void fence_after_thread_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// make generic-proxy shared-memory writes visible to the tensor core (async proxy)
-__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// ---- mbarrier (completion of committed MMAs) -------------------------------------
+// ---- mbarrier (completion of TMA bulk copies) -------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mma_commit(uint64_t *bar) {  // arrives on `bar` when all prior MMAs of this thread finish
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
 }
 // Bounded spin: a wait that cannot complete (protocol bug, lost TMA transaction) ends the kernel with a trap and a
 // message instead of hanging the device — over a second of polling, orders of magnitude beyond any legitimate wait.
@@ -223,54 +213,5 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         }
     } while (!done);
 }
-
-// ---- accumulator read-back: this warp's 32 lanes (rows) x 32 consecutive fp32 columns -------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float *v) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
-}
-
-// registers -> tensor memory: this warp's 32 lanes (rows) x 32 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float *v) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-          "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])),
-          "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])),
-          "r"(__float_as_uint(v[11])), "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])),
-          "r"(__float_as_uint(v[15])), "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])),
-          "r"(__float_as_uint(v[19])), "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])),
-          "r"(__float_as_uint(v[23])), "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])),
-          "r"(__float_as_uint(v[27])), "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])),
-          "r"(__float_as_uint(v[31]))
-        : "memory");
-}
-// registers -> tensor memory: this warp's 32 lanes (rows) x 16 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const float *v) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-          "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])),
-          "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])),
-          "r"(__float_as_uint(v[11])), "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])),
-          "r"(__float_as_uint(v[15]))
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 }  // namespace umma

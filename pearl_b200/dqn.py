@@ -99,7 +99,7 @@ class _B200DQNMixin:
         return flat
 
     def _bind(self, need_batch: int) -> None:
-        # `list(module.parameters())` walks the module tree (12 us): with 144 learners per group.learn() that is 2 ms of host
+        # `list(module.parameters())` walks the module tree (12 us): with a hundred learners per group.learn() that is milliseconds of host
         # time ahead of the launch.  The Parameter objects of a module only change if the module itself is replaced.
         if self.__dict__.get("_params_of") is not self._Q:   # via __dict__: as an nn.Module attribute `_Q` would be registered twice
             self.__dict__["_params_of"], self.__dict__["_params"] = self._Q, list(self._Q.parameters())

@@ -35,7 +35,7 @@ def gae_and_lambda_returns(values: torch.Tensor, last_next_value: float, reward:
 
 class B200ProximalPolicyOptimization:
     """The learner side of Pearl's ProximalPolicyOptimization (pearl/policy_learners/sequential_decision_making/
-    ppo.py:96-293) for discrete actions on a B200.  `learn(replay_buffer)` = `preprocess_replay_buffer` (state values,
+    ppo.py:96-293) for discrete actions on an H100.  `learn(replay_buffer)` = `preprocess_replay_buffer` (state values,
     taken-action probabilities, GAE and lambda returns over the whole rollout) followed by `training_rounds` x
     (sample -> clipped-surrogate actor step -> state-value critic step), all in CUDA through `prl_ppo_*`
     (include/pearl_b200.h).  Same constructor argument names and reporting keys (`actor_loss`, `critic_loss`) as the

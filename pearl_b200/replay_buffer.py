@@ -295,7 +295,7 @@ class B200ReplayBuffer(ReplayBuffer):
         """Snapshot of the buffer: the stored records in FIFO order (oldest first, raw record words as the kernels keep
         them), the layout needed to re-create the storage, and the sampler's MT19937 stream.  The reference never
         serialises replay-buffer contents (the buffer is not a Module; `PearlAgent.compare` only checks its type,
-        pearl_agent.py:313-318) — this is what makes a B200 training job resumable."""
+        pearl_agent.py:313-318) — this is what makes a GPU training job resumable."""
         if self._shard:
             raise NotImplementedError("snapshot a sharded buffer shard by shard with set_shard cleared")
         n = self.local_len()
@@ -334,7 +334,7 @@ class B200ReplayBuffer(ReplayBuffer):
 
     def load_offline_data(self, transitions, max_number_actions_if_discrete: Optional[int] = None, chunk: int = 65536) -> int:
         """The reference's `get_offline_data_in_buffer` (utils/functional_utils/train_and_eval/
-        offline_learning_and_evaluation.py:39-137) for a B200 buffer: `transitions` is the iterable of dicts a `.pt` offline
+        offline_learning_and_evaluation.py:39-137) for a device-resident buffer: `transitions` is the iterable of dicts a `.pt` offline
         data file holds (`observation, action, reward, next_observation, curr_available_actions, next_available_actions,
         done`); they are packed into the device ring `chunk` at a time instead of one Python push each.  Discrete action
         sets must be the full `range(max_number_actions)` (a `Discrete(n)` space or a DiscreteActionSpace of all ids), as in

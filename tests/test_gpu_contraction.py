@@ -1,5 +1,5 @@
 """The actor-critic learners' contraction (pearl_b200/csrc/gemm.cuh, gemm_tc.cu) against fp64 products: the three kinds the
-learners use (nn.Linear forward, backward-data, backward-weight + bias gradient), on the tcgen05 tiles (3xTF32) and on the
+learners use (nn.Linear forward, backward-data, backward-weight + bias gradient), on the tensor-core tiles (wgmma, 3xTF32) and on the
 SIMT tiles, with every feature of the operand descriptor: two concatenated sources (state || action), stacked networks
 (twin critics), ones column, ReLU / mask / accumulate epilogues, ragged sizes.
 
@@ -13,7 +13,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-ENGINES = [0, 64, 32, 164, 132]   # SIMT tiles; tcgen05 with both operands in shared memory; tcgen05 with A in tensor memory
+ENGINES = [0, 64, 32, 164, 132]   # SIMT tiles; wgmma with both operands in shared memory; wgmma with A in registers
 
 
 def _p(t):

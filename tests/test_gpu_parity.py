@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): the CUDA path, called through the C ABI via the
+"""GPU parity tests (H100): the CUDA path, called through the C ABI via the
 pearl_b200 plugins, against (a) golden fixtures recorded from the reference,
 (b) the CPU oracle on the same seeded inputs, (c) size-independent properties
 at BASELINE.json's full sizes.
@@ -314,7 +314,7 @@ def test_empty_buffer_learn_returns_empty_report():
 def test_full_size_cfg2_against_oracle_on_the_sampled_batches(engine):
     """obs=128, A=16, [64,64], B=256 on a 1e6-transition buffer (set branch of random.sample): the learner's own
     sampled indices (bit-exact vs the C oracle) select the batches the torch oracle replays.  Both engines: the
-    cooperative fp32 SIMT kernel and the one-SM tcgen05 (3xTF32) kernel."""
+    cooperative fp32 SIMT kernel and the one-SM wgmma (3xTF32) kernel."""
     pearl_b200, c_oracle, OracleDQN, _, _ = _imports()
     n, obs, A, B, rounds = 1_000_000, 128, 16, 256, 12
     g = torch.Generator(device="cuda").manual_seed(4321)
@@ -366,7 +366,7 @@ def test_full_size_cfg2_against_oracle_on_the_sampled_batches(engine):
 
 # --------------------------------------------------------------------------- tensor-core engine
 def test_tc_engine_matches_reference_golden_cfg2():
-    """The one-SM tcgen05 learner (3xTF32) on the cfg2-shaped fixture: same indices, q, y, loss,
+    """The one-SM wgmma learner (3xTF32) on the cfg2-shaped fixture: same indices, q, y, loss,
     parameters, target parameters and AdamW state as the recorded reference run, 1e-4."""
     name = "dqn_cfg2_pool"
     fx, cfg, data, buf, learner = build_from_fixture(name)
@@ -393,20 +393,17 @@ def test_tc_engine_matches_reference_golden_cfg2():
     assert_close(st["max_exp_avg_sq"].cpu().numpy(), fx["max_exp_avg_sq"], "tc max_exp_avg_sq", atol=1e-9)
 
 
-def test_learner_group_equals_individual_simt_learners():
-    """B200LearnerGroup (one launch, one SM per learner, tensor cores) vs the same learners trained one
-    by one with the fp32 SIMT kernel: identical index streams, parameters within 1e-4; dynamic action
-    sets and obs < 128 included."""
+def _group_vs_simt(obs, A, B, dynamic=True, adamw_outliers=False):
     pearl_b200, _, _, _, make_transitions = _imports()
-    obs, A, B, n, rounds, L = 40, 8, 128, 2000, 25, 5
+    n, rounds, L = 2000, 25, 5
     groups = {}
     for engine in ("simt", "tc"):
         learners, bufs = [], []
         for i in range(L):
-            d = make_transitions(n, obs, A, seed=300 + i, dynamic=(i % 2 == 1))
+            d = make_transitions(n, obs, A, seed=300 + i, dynamic=(dynamic and i % 2 == 1))
             buf = pearl_b200.B200ReplayBuffer(n, rng="device", dynamic_action_space=True)
             kw = {}
-            if i % 2 == 1:
+            if dynamic and i % 2 == 1:
                 kw = dict(next_available_ids=torch.from_numpy(d["next_avail_ids"].astype(np.uint8)),
                           next_available_count=torch.from_numpy(d["next_avail_n"].astype(np.int32)))
             buf.push_batch(*(torch.from_numpy(d[k]) for k in ("state", "action", "reward", "next_state", "terminated", "truncated")),
@@ -427,8 +424,26 @@ def test_learner_group_equals_individual_simt_learners():
         ls, lt = groups["simt"][0][i], groups["tc"][0][i]
         assert np.array_equal(groups["simt"][1][i].get_rng_state(), groups["tc"][1][i].get_rng_state())
         assert_close(np.asarray(groups["tc"][2][i]["loss"]), np.asarray(groups["simt"][2][i]["loss"]), f"group loss {i}")
-        assert_close(lt.flat_parameters.cpu().numpy(), ls.flat_parameters.cpu().numpy(), f"group params {i}")
-        assert_close(lt.flat_target_parameters.cpu().numpy(), ls.flat_target_parameters.cpu().numpy(), f"group target {i}")
+        close = (lambda g, w, what: assert_close_adamw(g, w, what, 1e-3, rounds)) if adamw_outliers else assert_close
+        close(lt.flat_parameters.cpu().numpy(), ls.flat_parameters.cpu().numpy(), f"group params {i}")
+        close(lt.flat_target_parameters.cpu().numpy(), ls.flat_target_parameters.cpu().numpy(), f"group target {i}")
+
+
+def test_learner_group_equals_individual_simt_learners():
+    """B200LearnerGroup (one launch, one SM per learner, tensor cores) vs the same learners trained one
+    by one with the fp32 SIMT kernel: identical index streams, parameters within 1e-4; dynamic action
+    sets and obs < 128 included."""
+    _group_vs_simt(40, 8, 128)
+
+
+@pytest.mark.parametrize("obs", [72, 96])
+def test_learner_group_with_a_partial_second_k_pass(obs):
+    """64 < obs < 128: layer 1 takes a second K pass shorter than 64 and the second warpgroup's share of dW1s is
+    narrower than 64 columns (8 at obs 72, 32 at obs 96); two row tiles (batch 256).  Full action sets: with dynamic sets
+    of 16 actions some first-step gradients are ~1e-7, where AdamW's eps makes the step depend on fp32 summation order,
+    and 25 free-running rounds amplify that beyond an elementwise 1e-4; the dynamic path does not depend on obs and is
+    covered at obs 40 above.  Parameters: elementwise 1e-4 with the bounded AdamW outliers of tests/_tol.py."""
+    _group_vs_simt(obs, 16, 256, dynamic=False, adamw_outliers=True)
 
 
 def test_tc_group_chunked_launch_is_bit_identical_to_short_calls():

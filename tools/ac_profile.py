@@ -1,5 +1,5 @@
 """Developer tool: a few SAC (configs[2] shape) and PPO (configs[3] shape) rounds with plain stream launches, for
-`ncu --metrics gpu__time_duration.sum` launch lists (profiles/r2_launches_sac_ppo.csv); plus a TD3 round and the GAE pass of
+`ncu --metrics gpu__time_duration.sum` launch lists; plus a TD3 round and the GAE pass of
 the HBM-side table (16M transitions, episodes of 500)."""
 import os
 import sys

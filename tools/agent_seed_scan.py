@@ -1,4 +1,4 @@
-"""Developer tool (CPU only, needs /root/reference): how sensitive is the PearlAgent parity loop of tests/pearl_agent_worker.py to the
+"""Developer tool (CPU only, needs /root/reference): how sensitive is the PearlAgent parity loop of tools/pearl_agent_check.py to the
 initial weights?  For seeds [argv1, argv2) the REFERENCE agent is driven three times - unperturbed and with the initial Q
 weights perturbed by 2e-7 relative - and the largest relative difference of the reported losses is printed for DeepQLearning
 and DoubleDQN.  Quiet seeds stay at ~5e-7; chaotic ones (AdamW sign flips on near-zero gradients) reach 1e-4 .. 3e-3."""

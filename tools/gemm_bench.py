@@ -1,4 +1,4 @@
-"""Developer tool: time the learners' contraction shapes on the SIMT tiles and on the tcgen05 tiles (CUDA events around
+"""Developer tool: time the learners' contraction shapes on the SIMT tiles and on the wgmma tiles (CUDA events around
 replays of a CUDA graph of 20 launches, so the figure is the device-side issue-to-issue time — what the CUDA-graph
 replay of a learner round sees).  python tools/gemm_bench.py [reps]"""
 import ctypes as C

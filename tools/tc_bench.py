@@ -5,7 +5,7 @@ import torch, ctypes as C
 import pearl_b200
 from pearl_b200 import _lib
 from bench import Space, OBS, N_ACT, HIDDEN, BATCH
-R = int(sys.argv[1]) if len(sys.argv) > 1 else 144
+R = int(sys.argv[1]) if len(sys.argv) > 1 else 64
 rounds = int(sys.argv[2]) if len(sys.argv) > 2 else 256
 cap = int(sys.argv[3]) if len(sys.argv) > 3 else 100_000
 dev = torch.device("cuda", 0)
@@ -38,9 +38,14 @@ _lib.check(ls[0]._libh.prl_dqn_set_profile(ls[0]._handle, C.c_void_p(st.data_ptr
 grp.learn()
 torch.cuda.synchronize()
 s = st.cpu()[4:].double()
-names = ["row scalars + soft upd", "load target weights", "target layer 1 (2 tiles)", "all-actions (32 tiles)", "load online weights",
-         "online layer 1", "tile0: fwd L2 + dZ2 + dH1", "rest (weight grads t0, tile1 all)", "AdamW"]
+# stamps written by k_dqn_tc: 0 round start, 1 row scalars + soft update done, 2 target tiles loaded, 3 phase T done,
+# 4 online tiles + W2^T ready, 5 tile 0 layer 1 done, 6 tile 0 forward / dZ2 / dH1 done, 8 weight gradients done, 9 AdamW done
+names = ["row scalars + soft upd", "load target weights", "phase T (layer 1 + all actions)", "load online weights + W2^T",
+         "tile 0: online layer 1", "tile 0: fwd L2 + dZ2 + dH1", None, "rest (weight grads, other tiles)", "AdamW"]
 tot = (s[1:, 0] - s[:-1, 0]).mean()
 print(f"{tot:.0f} clk/round (CTA {os.environ.get('PRL_TC_PROF_CTA', '0')} with {R} learners resident)")
 for i, n in enumerate(names):
-    print(f"  {n:36s} {(s[:, i+1]-s[:, i]).mean():10.0f} clk")
+    if n is not None:
+        j = 8 if i == 7 else i + 1      # stamp 7 is not written: "rest" runs from stamp 6 to stamp 8
+        k = 6 if i == 7 else i
+        print(f"  {n:36s} {(s[:, j]-s[:, k]).mean():10.0f} clk")
