@@ -1,0 +1,148 @@
+"""oracle/dqn_fp64.py — one DQN gradient step in float64, with an error scale for every quantity.
+
+TEST INFRASTRUCTURE ONLY (like the rest of oracle/).  The network is the [obs + A] -> h1 -> h2 -> 1 ReLU MLP of
+VanillaQValueNetwork in torch parameter order: W1 [h1, obs + A] (state columns, then one-hot action columns), b1,
+W2 [h2, h1], b2, W3 [1, h2], b3.  One step of DeepQLearning.learn_batch on a batch:
+
+    q_i = Q(s_i, a_i)
+    y_i = max over the available a' of Q_target(s'_i, a') * gamma * (1 - terminated_i) + r_i   (unavailable: -inf;
+          `truncated` plays no part, as in the reference)
+    loss = mean((q - y)^2), and its gradient with respect to the seven parameter blocks.
+
+Everything is written as explicit formulas, not autograd, so that the SAME code applied to |.| of every operand gives
+the error scale of each result: the sum of |a||b| over every product that contributed to it, carried through the chain
+(the natural scale of a rounding error in a chain of dot products).  ReLU is the identity on non-negative values and
+the ReLU derivatives are the masks of the value pass, so they need no special case.  The one change is the loss
+derivative: |dq_i| becomes |dq_i| + (2 / B) (scale(q_i) + scale(y_i)), so that a row with q ~ y is judged by the
+rounding noise of q - y and not by its own tiny value.
+"""
+from __future__ import annotations
+
+import torch
+
+BLOCKS = ("dW1s", "dW1a", "db1", "dW2", "db2", "dW3", "db3")
+
+
+def unflatten(flat: torch.Tensor, obs: int, n_actions: int, hidden=(64, 64)) -> tuple:
+    """(W1, b1, W2, b2, W3, b3) as float64 views of a flat torch-order parameter vector."""
+    h1, h2 = hidden
+    D = obs + n_actions
+    shapes = [(h1, D), (h1,), (h2, h1), (h2,), (1, h2), (1,)]
+    flat = flat.to(torch.float64)
+    out, off = [], 0
+    for s in shapes:
+        n = 1
+        for x in s:
+            n *= x
+        out.append(flat[off:off + n].view(s))
+        off += n
+    assert off == flat.numel(), "parameter count does not match the network shape"
+    return tuple(out)
+
+
+def _forward(net, state, onehot):
+    """Z1, Z2 and Q for rows (state [n, obs], onehot [n, A])."""
+    W1, b1, W2, b2, W3, b3 = net
+    obs = state.shape[1]
+    z1 = state @ W1[:, :obs].T + onehot @ W1[:, obs:].T + b1
+    h1 = z1.clamp_min(0)
+    z2 = h1 @ W2.T + b2
+    h2 = z2.clamp_min(0)
+    return z1, h1, z2, h2, h2 @ W3[0] + b3[0]
+
+
+def _target(net, next_state, avail_ids, avail_n, gamma, terminated, reward):
+    """y per row: the max over the first avail_n[i] entries of avail_ids[i] of Q_target(s'_i, .), then the TD target."""
+    B, A = avail_ids.shape
+    eye = torch.eye(A, dtype=next_state.dtype, device=next_state.device)
+    onehot = eye[avail_ids.reshape(-1)]                                        # [B * A, A]
+    s = next_state.repeat_interleave(A, dim=0)
+    v = _forward(net, s, onehot)[4].view(B, A)
+    slot = torch.arange(A, device=v.device).view(1, A)
+    v = v.masked_fill(slot >= avail_n.view(B, 1), float("-inf"))
+    return v.max(1)[0] * gamma * (1.0 - terminated) + reward
+
+
+def _backward(net, state, onehot, m1, m2, h1, h2, dq) -> dict:
+    W1, b1, W2, b2, W3, b3 = net
+    obs = state.shape[1]
+    dz2 = dq[:, None] * W3[0][None, :] * m2
+    dz1 = (dz2 @ W2) * m1
+    return dict(dW1s=dz1.T @ state, dW1a=dz1.T @ onehot, db1=dz1.sum(0), dW2=dz2.T @ h1, db2=dz2.sum(0),
+                dW3=(dq @ h2).view(1, -1), db3=dq.sum().view(1))
+
+
+def dqn_step(w, wt, batch: dict, obs: int, n_actions: int, gamma: float, hidden=(64, 64)) -> tuple:
+    """One DQN step in float64.  `w`, `wt`: flat online / target parameters.  `batch`: state [B, obs], action [B] ids,
+    reward [B], terminated [B], next_state [B, obs], avail_ids [B, A] (ids of the available next actions first),
+    avail_n [B] (how many are available).  Returns (value, scale): two dicts with q, y, z1, z2 [B, h], mae (the
+    reported loss, mean |q - y|), loss (mean (q - y)^2), grad (flat, torch order) and the seven blocks of BLOCKS."""
+    f64 = lambda x: torch.as_tensor(x).to(torch.float64)
+    state, next_state = f64(batch["state"]), f64(batch["next_state"])
+    reward, term = f64(batch["reward"]), f64(batch["terminated"])
+    action = torch.as_tensor(batch["action"]).long().to(state.device)
+    avail_ids = torch.as_tensor(batch["avail_ids"]).long().to(state.device)
+    avail_n = torch.as_tensor(batch["avail_n"]).long().to(state.device)
+    B = state.shape[0]
+    onehot = torch.eye(n_actions, dtype=torch.float64, device=state.device)[action]
+    net, net_t = unflatten(w, obs, n_actions, hidden), unflatten(wt, obs, n_actions, hidden)
+    absnet, absnet_t = tuple(p.abs() for p in net), tuple(p.abs() for p in net_t)
+
+    z1, h1, z2, h2, q = _forward(net, state, onehot)
+    y = _target(net_t, next_state, avail_ids, avail_n, gamma, term, reward)
+    m1, m2 = (z1 > 0).to(torch.float64), (z2 > 0).to(torch.float64)
+    sz1, sh1, sz2, sh2, sq = _forward(absnet, state.abs(), onehot)
+    sy = _target(absnet_t, next_state.abs(), avail_ids, avail_n, gamma, term, reward.abs())
+
+    dq = (q - y) * (2.0 / B)
+    sdq = dq.abs() + (2.0 / B) * (sq + sy)
+    g = _backward(net, state, onehot, m1, m2, h1, h2, dq)
+    sg = _backward(absnet, state.abs(), onehot, m1, m2, sh1, sh2, sdq)
+
+    def pack(d, q, y, z1, z2, mae, loss):
+        out = dict(d, q=q, y=y, z1=z1, z2=z2, mae=mae, loss=loss)
+        out["grad"] = torch.cat([torch.cat([d["dW1s"], d["dW1a"]], 1).reshape(-1), d["db1"], d["dW2"].reshape(-1),
+                                 d["db2"], d["dW3"].reshape(-1), d["db3"]])
+        return out
+
+    value = pack(g, q, y, z1, z2, (q - y).abs().mean(), ((q - y) ** 2).mean())
+    scale = pack(sg, sq, sy, sz1, sz2, (sq + sy).mean(), (2 * (q - y).abs() * (sq + sy)).mean())
+    return value, scale
+
+
+def relu_margin(w, state, action, obs: int, n_actions: int, hidden=(64, 64)) -> torch.Tensor:
+    """Per row: the smallest |pre-activation| / scale over both hidden layers of the network `w` at (state, action).  A
+    row whose margin exceeds a kernel's relative rounding error has the same ReLU derivatives in the kernel as here."""
+    state = torch.as_tensor(state).to(torch.float64)
+    onehot = torch.eye(n_actions, dtype=torch.float64)[torch.as_tensor(action).long()]
+    net = unflatten(torch.as_tensor(w).cpu(), obs, n_actions, hidden)
+    z1, _, z2, _, _ = _forward(net, state, onehot)
+    s1, _, s2, _, _ = _forward(tuple(p.abs() for p in net), state.abs(), onehot)
+    return torch.minimum((z1.abs() / s1).min(1)[0], (z2.abs() / s2).min(1)[0])
+
+
+def err_over_scale(got, want, scale) -> torch.Tensor:
+    """|got - want| / scale elementwise; an element of scale 0 (say a dead hidden unit's gradient) must be exact: 0 if it
+    is, inf if not."""
+    diff = (torch.as_tensor(got).to(torch.float64) - want).abs()
+    return torch.where(scale > 0, diff / scale.clamp_min(1e-300), torch.where(diff > 0, float("inf"), 0.0))
+
+
+def block_slices(obs: int, n_actions: int, hidden=(64, 64)) -> dict:
+    """Where each gradient block lives in the flat torch-order vector: name -> (offset, rows, cols, column offset,
+    row pitch) so that element (r, c) of the block is flat[offset + r * pitch + col0 + c]."""
+    h1, h2 = hidden
+    D = obs + n_actions
+    o_b1 = h1 * D
+    o_W2 = o_b1 + h1
+    o_b2 = o_W2 + h2 * h1
+    o_W3 = o_b2 + h2
+    o_b3 = o_W3 + h2
+    return dict(dW1s=(0, h1, obs, 0, D), dW1a=(0, h1, n_actions, obs, D), db1=(o_b1, 1, h1, 0, h1),
+                dW2=(o_W2, h2, h1, 0, h1), db2=(o_b2, 1, h2, 0, h2), dW3=(o_W3, 1, h2, 0, h2), db3=(o_b3, 1, 1, 0, 1))
+
+
+def block_view(flat: torch.Tensor, name: str, obs: int, n_actions: int, hidden=(64, 64)) -> torch.Tensor:
+    """Block `name` of a flat torch-order vector as a [rows, cols] tensor."""
+    off, rows, cols, col0, pitch = block_slices(obs, n_actions, hidden)[name]
+    return flat[off:off + rows * pitch].view(rows, pitch)[:, col0:col0 + cols]

@@ -786,6 +786,8 @@ extern "C" int prl_dqn_learn_multi(prl_dqn *const *dqns, prl_buf *const *bufs, i
         prl_dqn *q = dqns[i];
         prl_buf *b = bufs[i];
         PRL_REQUIRE(q && b, "null learner / buffer");
+        // a shard's sampler draws global slots in [0, capacity * world); the learner indexes its local records with them
+        PRL_REQUIRE(b->shard_world <= 1, "buffer %d is one shard of a multi-GPU buffer: the tensor-core learner samples local buffers only", i);
         const prl_dqn_cfg &ci = q->cfg;
         PRL_REQUIRE(ci.obs_dim == c.obs_dim && ci.n_actions == c.n_actions && ci.hidden1 == c.hidden1 &&
                         ci.hidden2 == c.hidden2 && ci.double_dqn == c.double_dqn &&

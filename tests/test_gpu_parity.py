@@ -448,15 +448,21 @@ def test_learner_group_with_a_partial_second_k_pass(obs):
 
 def test_tc_group_chunked_launch_is_bit_identical_to_short_calls():
     """One `group.learn()` of 80 rounds (index streams produced in chunks on a side stream, a 32-round and a
-    48-round learner launch; inside a launch the target network's small vectors stay cached in shared memory
-    between soft updates and the target tiles are updated in tile order) vs the same learners driven by calls
-    of at most 20 rounds: same arithmetic in the same order, so losses, parameters, target parameters and AdamW
-    state must be bit-identical — any state carried wrongly across a round or launch boundary shows up here.
-    Soft target updates (freq 4) fall on both sides of the boundaries."""
+    48-round learner launch) and one of 300 rounds (four chunks: 32 rounds, then three launches of about 89); inside a
+    launch the target network's small vectors stay cached in shared memory between soft updates and the target tiles
+    are updated in tile order.  Each is compared with the same learners driven by calls of at most 20 / 50 rounds (one
+    chunk each): same arithmetic in the same order, so losses, parameters, target parameters and AdamW state must be
+    bit-identical — any state carried wrongly across a round or launch boundary shows up here.  Soft target updates
+    (freq 4) fall on both sides of the boundaries."""
+    for rounds, short in ((80, 20), (300, 50)):
+        _chunked_vs_short_calls(rounds, short)
+
+
+def _chunked_vs_short_calls(rounds, short):
     pearl_b200, _, _, _, make_transitions = _imports()
-    obs, A, B, n, rounds, L = 128, 16, 256, 3000, 80, 3
+    obs, A, B, n, L = 128, 16, 256, 3000, 3
     out = {}
-    for per_call in (rounds, 20):
+    for per_call in (rounds, short):
         learners, bufs = [], []
         for i in range(L):
             d = make_transitions(n, obs, A, seed=700 + i)
@@ -473,9 +479,9 @@ def test_tc_group_chunked_launch_is_bit_identical_to_short_calls():
         reps = pearl_b200.B200LearnerGroup(learners, bufs).learn()
         out[per_call] = (learners, bufs, reps)
     for i in range(L):
-        la, lb = out[rounds][0][i], out[20][0][i]
-        assert np.array_equal(out[rounds][1][i].get_rng_state(), out[20][1][i].get_rng_state())
-        assert out[rounds][2][i]["loss"] == out[20][2][i]["loss"]
+        la, lb = out[rounds][0][i], out[short][0][i]
+        assert np.array_equal(out[rounds][1][i].get_rng_state(), out[short][1][i].get_rng_state())
+        assert out[rounds][2][i]["loss"] == out[short][2][i]["loss"]
         assert torch.equal(la.flat_parameters, lb.flat_parameters)
         assert torch.equal(la.flat_target_parameters, lb.flat_target_parameters)
         sa, sb = la.adam_state(), lb.adam_state()

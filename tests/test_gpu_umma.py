@@ -29,7 +29,7 @@ def test_umma_3xtf32_matches_fp64(n, k):
 
 
 @pytest.mark.parametrize("m,n,k,lbo", [(128, 64, 64, 144), (64, 64, 64, 128), (64, 64, 64, 144), (64, 128, 64, 144),
-                                         (64, 32, 64, 144), (128, 64, 128, 128), (64, 8, 128, 144)])
+                                         (64, 32, 64, 144), (128, 64, 128, 128), (64, 8, 128, 144), (64, 16, 64, 144)])
 def test_umma_m64_and_padded_chunk_pitch(m, n, k, lbo):
     """M = 64 / 128, N down to 8 and operand tiles with a 144-byte chunk pitch (the layout the
     backward pass uses for transposed tiles so that scattered column writes are bank-conflict free)."""
