@@ -372,6 +372,46 @@ int prl_sac_learn(prl_sac *sac, prl_buf *buf, int rounds, int batch, const float
 int prl_sac_set_graph(prl_sac *sac, int enable);
 int64_t prl_sac_last_launches(const prl_sac *sac);
 
+/* ---- discrete Soft Actor-Critic ----------------------------------------------------------------
+ * Replaces SoftActorCritic.learn_batch (policy_learners/sequential_decision_making/soft_actor_critic.py:
+ * learn_batch, _actor_loss, _critic_loss, _get_next_state_expected_values on actor_critic_base.py:309-366)
+ * driven by PolicyLearner.learn (policy_learner.py:162-204) over a discrete-action ring: per round sample ->
+ * actor step (VanillaActorNetwork softmax against min(Q1, Q2) of every action, the pre-step coefficient) ->
+ * critic step with the updated actor and the critic target (twin MSE, critic_utils.py) -> soft target update
+ * (tau every round) -> entropy step (torch.optim.Adam on log alpha, with the actor-step probabilities).
+ * Two AdamW(amsgrad) states (actor, both critics).  Flat layouts (fp32, row-major [out][in]):
+ *   actor : W1[h1][obs] b1 W2[h2][h1] b2 W3[A][h2] b3
+ *   critic: TWO consecutive copies (q1 then q2) of W1[c1][obs+A] b1 W2[c2][c1] b2 W3[1][c2] b3 (one-hot action)
+ * target_entropy = -scale * log(1 / A) as the reference computes it; entropy_lr / entropy_eps are the entropy
+ * optimizer's (the critic lr at construction, 1e-4).  Sharded and continuous-action buffers are rejected (EINVAL). */
+typedef struct prl_sacd_cfg {
+    int32_t obs_dim, n_actions, actor_h1, actor_h2, critic_h1, critic_h2;
+    int32_t autotune;     /* entropy_autotune */
+    int32_t max_batch, max_rounds;
+    double actor_lr, critic_lr, beta1, beta2, eps, weight_decay, gamma, tau;
+    double target_entropy, entropy_lr, entropy_eps;
+} prl_sacd_cfg;
+typedef struct prl_sacd prl_sacd;
+int64_t prl_sacd_actor_param_count(const prl_sacd_cfg *cfg);
+int64_t prl_sacd_critic_param_count(const prl_sacd_cfg *cfg);   /* ONE critic */
+int64_t prl_sacd_workspace_bytes(const prl_sacd_cfg *cfg);
+/* Device memory owned by the caller: actor vectors f32[actor_param_count], critic vectors f32[2 * critic_param_count],
+ * log_alpha3 = {log_alpha, exp_avg, exp_avg_sq} (torch.optim.Adam state), alpha1 = the entropy coefficient in use. */
+int prl_sacd_create(prl_sacd **out, const prl_sacd_cfg *cfg, float *actor_w, float *actor_m, float *actor_v,
+                    float *actor_vmax, float *critic_w, float *critic_m, float *critic_v, float *critic_vmax,
+                    float *critic_target_w, float *log_alpha3, float *alpha1, int64_t adam_step, void *workspace);
+int prl_sacd_destroy(prl_sacd *sacd);
+int64_t prl_sacd_adam_step(const prl_sacd *sacd);
+/* New actor / critic AdamW learning rates from the next learn on (an lr scheduler's step, e.g. the ExponentialLR
+ * that SoftActorCritic.reset steps).  Every lr-dependent scalar travels in the per-call block: no re-capture. */
+int prl_sacd_set_lr(prl_sacd *sacd, double actor_lr, double critic_lr);
+/* out_*_loss: device f32[rounds] (entropy: the entropy optimizer's loss, as the reference reports it);
+ * out_logical_dev (optional) i32[rounds][batch] = sampled indices */
+int prl_sacd_learn(prl_sacd *sacd, prl_buf *buf, int rounds, int batch, float *out_actor_loss_dev,
+                   float *out_critic_loss_dev, float *out_entropy_loss_dev, int32_t *out_logical_dev, void *stream);
+int prl_sacd_set_graph(prl_sacd *sacd, int enable);
+int64_t prl_sacd_last_launches(const prl_sacd *sacd);
+
 /* ---- TD3 / DDPG ----------------------------------------------------------------------------------
  * Replaces TD3.learn_batch (policy_learners/sequential_decision_making/td3.py:106-202) and, with
  * actor_update_freq = 1 and no noise, DeepDeterministicPolicyGradient (ddpg.py:105-157 on

@@ -1,6 +1,7 @@
 """Actor-critic plugins that SUBCLASS the reference classes (SURVEY.md §8 rows a1 / a14-a16, f3):
 
     B200ContinuousSoftActorCritic   (ContinuousSoftActorCritic, soft_actor_critic_continuous.py:42-231)
+    B200SoftActorCritic             (SoftActorCritic, soft_actor_critic.py: discrete actions)
     B200ProximalPolicyOptimization  (ProximalPolicyOptimization, ppo.py:96-293)
     B200TD3 / B200DeepDeterministicPolicyGradient  (td3.py:43-202, ddpg.py:41-157)
 
@@ -9,7 +10,7 @@ constructor runs unchanged (same arguments, same networks, same optimizers, same
 `pearl.pearl_agent.PearlAgent` accepts them as they are, `act()` / `reset()` / `compare()` / `state_dict()` are the
 reference's own code.  On the first `learn()` (after PearlAgent moved the learner to its CUDA device) the parameters of
 `_actor`, `_critic` (and their targets) are re-pointed at views into the flat fp32 vectors of the CUDA learner
-(`pearl_b200.sac / ppo / td3`), and `optimizer.state` at views into its flat AdamW vectors: the kernels and torch see the
+(`pearl_b200.sac / sac_discrete / ppo / td3`), and `optimizer.state` at views into its flat AdamW vectors: the kernels and torch see the
 same memory, nothing is copied per call, `get_extra_state` / `set_extra_state` (actor_critic_base.py:411-428) checkpoint
 the live state, and a state loaded with `load_state_dict` is picked up on the next `learn()`.
 
@@ -24,11 +25,13 @@ import torch
 
 from .ppo import B200ProximalPolicyOptimization as PpoCore
 from .sac import B200ContinuousSoftActorCritic as SacCore
+from .sac_discrete import B200SoftActorCritic as SacdCore
 from .td3 import B200DeepDeterministicPolicyGradient as DdpgCore
 from .td3 import B200TD3 as Td3Core
 
 try:  # pragma: no cover - depends on the environment
     from pearl.policy_learners.sequential_decision_making.ddpg import DeepDeterministicPolicyGradient as _RefDDPG
+    from pearl.policy_learners.sequential_decision_making.soft_actor_critic import SoftActorCritic as _RefSACD
     from pearl.policy_learners.sequential_decision_making.ppo import ProximalPolicyOptimization as _RefPPO
     from pearl.policy_learners.sequential_decision_making.soft_actor_critic_continuous import (
         ContinuousSoftActorCritic as _RefSAC,
@@ -49,6 +52,17 @@ def _adamw_lr(opt: torch.optim.Optimizer, what: str) -> float:
         raise NotImplementedError(f"{what}: the fused update implements torch.optim.AdamW(amsgrad=True) with default "
                                   "betas / eps / weight_decay in one parameter group")
     return float(g["lr"])
+
+
+def _adam_lr_eps(opt: torch.optim.Optimizer) -> tuple:
+    """(lr, eps) of the discrete SAC entropy optimizer, which must be torch.optim.Adam without weight decay or amsgrad
+    and with default betas (soft_actor_critic.py constructs Adam(lr=critic lr, eps=1e-4))."""
+    g = opt.param_groups[0] if type(opt) is torch.optim.Adam and len(opt.param_groups) == 1 else None
+    if (g is None or g.get("amsgrad", False) or g.get("maximize", False) or float(g.get("weight_decay", 0.0)) != 0.0
+            or tuple(g["betas"]) != (0.9, 0.999)):
+        raise NotImplementedError("entropy optimizer: the CUDA learner implements torch.optim.Adam (no weight decay, no amsgrad, "
+                                  "default betas) in one parameter group")
+    return float(g["lr"]), float(g["eps"])
 
 
 def _shapes(module: torch.nn.Module) -> list:
@@ -133,6 +147,13 @@ class _B200ActorCriticMixin:
     def _bind_extras(self, core) -> None:   # idempotent: runs on every learn()
         pass
 
+    def _apply_learning_rates(self, core, lrs: tuple) -> None:
+        """New (actor, critic) learning rates: by default the C handle is re-created with them at the current AdamW step
+        counts (moments and parameters live in the core's vectors)."""
+        steps = self._core_steps(core)
+        core._actor_learning_rate, core._critic_learning_rate = lrs
+        self._restart_core(core, steps)
+
     # ---- binding
     def _device_of_parameters(self) -> torch.device:
         dev = next(self._actor.parameters()).device
@@ -156,9 +177,7 @@ class _B200ActorCriticMixin:
         # handle is re-created with the new rates at the current AdamW step counts (moments and parameters live in our vectors)
         lrs = (_adamw_lr(self._actor_optimizer, "actor optimizer"), _adamw_lr(self._critic_optimizer, "critic optimizer"))
         if lrs != (core._actor_learning_rate, core._critic_learning_rate):
-            steps = self._core_steps(core)
-            core._actor_learning_rate, core._critic_learning_rate = lrs
-            self._restart_core(core, steps)
+            self._apply_learning_rates(core, lrs)
         triples = self._optimizer_triples(core)
         if not all(_is_bound(o, m, s3) for o, m, s3 in triples):
             cur = self._core_steps(core)
@@ -265,6 +284,86 @@ if HAVE_REFERENCE:
             if self._entropy_autotune:
                 _set_steps(self._entropy_optimizer, self._core_steps(core)[0])
 
+    class B200SoftActorCritic(_B200ActorCriticMixin, _RefSACD):
+        """Drop-in for `pearl...soft_actor_critic.SoftActorCritic` (discrete actions): VanillaActorNetwork and
+        TwinCritic(VanillaQValueNetwork) with two hidden layers each, one-hot action representation.  The actor lr that
+        `reset()`'s ExponentialLR changes every episode reaches the CUDA learner through `prl_sacd_set_lr`: same handle,
+        same captured graph.  Current action sets are not stored by B200ReplayBuffer: the actor loss always runs over
+        every action."""
+
+        def _make_core(self, device):
+            sa, sc = _shapes(self._actor), _shapes(self._critic)
+            nets = (type(self._actor).__name__, type(self._critic).__name__,
+                    type(getattr(self._critic, "_critic_1", None)).__name__, type(getattr(self._critic, "_critic_2", None)).__name__)
+            if nets != ("VanillaActorNetwork", "TwinCritic", "VanillaQValueNetwork", "VanillaQValueNetwork") or len(sa) != 6 or len(sc) != 12:
+                raise NotImplementedError("the CUDA discrete SAC learner is built for VanillaActorNetwork + TwinCritic(VanillaQValueNetwork) "
+                                          "with two hidden layers each")
+            obs, h1, h2, n_act = _mlp3(sa, "actor")
+            dq, c1, c2, one = _mlp3(sc[:6], "critic")
+            arm = getattr(self, "_action_representation_module", None) or getattr(self, "action_representation_module", None)
+            if type(arm).__name__ != "OneHotActionTensorRepresentationModule":
+                raise NotImplementedError("the CUDA discrete SAC learner folds a one-hot action representation into the critic")
+            if dq != obs + n_act or one != 1 or sc[6:] != sc[:6]:
+                raise NotImplementedError("unexpected discrete SAC network shapes")
+            core = SacdCore(state_dim=obs, n_actions=n_act, actor_hidden_dims=[h1, h2], critic_hidden_dims=[c1, c2],
+                            actor_learning_rate=_adamw_lr(self._actor_optimizer, "actor optimizer"),
+                            critic_learning_rate=_adamw_lr(self._critic_optimizer, "critic optimizer"),
+                            critic_soft_update_tau=float(self._critic_soft_update_tau), discount_factor=float(self._discount_factor),
+                            training_rounds=int(self._training_rounds), batch_size=int(self._batch_size),
+                            entropy_coef=float(self._entropy_coef), entropy_autotune=bool(self._entropy_autotune), device=device,
+                            **self._b200_opts)
+            if self._entropy_autotune:
+                core._target_entropy = float(self._target_entropy)
+                core._entropy_learning_rate, core._entropy_eps = _adam_lr_eps(self._entropy_optimizer)
+            return core
+
+        def _module_pairs(self, core):
+            return [(self._actor, core.actor_params), (self._critic, core.critic_params), (self._critic_target, core.critic_target_params)]
+
+        def _core_steps(self, core):
+            s = int(core._lib.prl_sacd_adam_step(core._handle)) if core._handle.value else int(core._adam_step)
+            return (s, s)
+
+        def _restart_core(self, core, steps):
+            if steps[0] != steps[1]:
+                raise NotImplementedError("discrete SAC steps its actor and critics once per round: one AdamW step count")
+            if core._handle.value:
+                core._lib.prl_sacd_destroy(core._handle)
+                core._handle = C.c_void_p(0)
+            core._adam_step = int(steps[0])
+
+        def _apply_learning_rates(self, core, lrs):
+            core.set_learning_rates(*lrs)
+
+        def _bind_extras(self, core):
+            """`_entropy_coef` (buffer, shape kept) is a view of the core's coefficient; with autotune, `_log_entropy`
+            (Parameter) and the entropy optimizer's Adam state are the [log alpha | exp_avg | exp_avg_sq] block of the
+            core.  A state loaded into the entropy optimizer since the last call is imported."""
+            coef = core._entropy_coef
+            if self._entropy_coef.data_ptr() != coef.data_ptr():
+                coef.copy_(self._entropy_coef.detach().reshape(1).to(coef))
+                self._entropy_coef = coef.view(self._entropy_coef.shape)
+            if not self._entropy_autotune:
+                return
+            hp = _adam_lr_eps(self._entropy_optimizer)
+            if hp != (core._entropy_learning_rate, core._entropy_eps):      # fixed in the handle's configuration
+                core._entropy_learning_rate, core._entropy_eps = hp
+                self._restart_core(core, self._core_steps(core))
+            blk, p, st = core._log_entropy, self._log_entropy, self._entropy_optimizer.state
+            if p.data_ptr() != blk.data_ptr():
+                blk[0:1].copy_(p.detach().reshape(1).to(blk))
+                p.data = blk[0:1]
+            if p in st and "exp_avg" in st[p] and st[p]["exp_avg"].data_ptr() == blk[1:2].data_ptr():
+                return
+            if p in st and "exp_avg" in st[p]:
+                blk[1:2].copy_(st[p]["exp_avg"].reshape(1))
+                blk[2:3].copy_(st[p]["exp_avg_sq"].reshape(1))
+            st[p] = dict(step=torch.tensor(float(self._core_steps(core)[0])), exp_avg=blk[1:2], exp_avg_sq=blk[2:3])
+
+        def _after_learn(self, core):
+            if self._entropy_autotune:
+                _set_steps(self._entropy_optimizer, self._core_steps(core)[0])
+
     class B200ProximalPolicyOptimization(_B200ActorCriticMixin, _RefPPO):
         """Drop-in for `pearl...ppo.ProximalPolicyOptimization` (discrete actions, as the reference's `_actor_loss`)."""
 
@@ -357,6 +456,7 @@ if HAVE_REFERENCE:
 
 else:
     B200ContinuousSoftActorCritic = SacCore
+    B200SoftActorCritic = SacdCore
     B200ProximalPolicyOptimization = PpoCore
     B200TD3 = Td3Core
     B200DeepDeterministicPolicyGradient = DdpgCore

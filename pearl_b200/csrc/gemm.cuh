@@ -270,6 +270,19 @@ static __global__ void k_head_bwd(int B, int H, const float *__restrict__ dq, co
     dc2[o] = (c2[o] > 0.f) ? dq[z * B + m] * __ldg(w3 + z * w_net_stride + j) : 0.f;
 }
 
+// one row of softmax(logits) as torch computes it: p_k = exp(l_k - max) / sum.  The row's max and sum are computed once;
+// p_k is evaluated where it is needed (the same arithmetic every time, no per-thread arrays)
+struct RowSoftmax {
+    const float *l; float mx, s;
+    __device__ __forceinline__ RowSoftmax(const float *logit, int A) : l(logit) {
+        mx = l[0];
+        for (int k = 1; k < A; k++) mx = fmaxf(mx, l[k]);
+        s = 0.f;
+        for (int k = 0; k < A; k++) s += expf(l[k] - mx);
+    }
+    __device__ __forceinline__ float operator()(int k) const { return expf(l[k] - mx) / s; }
+};
+
 struct AdamHp { float decay, omb1, beta2, omb2, eps; };
 __device__ __forceinline__ float adamw1(float w, float &m, float &v, float &x, float g, const AdamHp &h, float step_size, float bc2s) {
     float p = __fmul_rn(w, h.decay);
@@ -279,13 +292,16 @@ __device__ __forceinline__ float adamw1(float w, float &m, float &v, float &x, f
     const float denom = __fadd_rn(__fdiv_rn(__fsqrt_rn(x), bc2s), h.eps);
     return __fadd_rn(p, __fdiv_rn(__fmul_rn(-step_size, m), denom));
 }
-// AdamW(amsgrad) over a flat vector; optional soft update of a target vector with the NEW parameters
+// AdamW(amsgrad) over a flat vector; optional soft update of a target vector with the NEW parameters.
+// decay (optional): device copy of 1 - lr * weight_decay that overrides h.decay, so that a learning-rate change reaches a
+// captured graph through its per-call block
 static __global__ void k_adamw(int n, float *__restrict__ w, float *__restrict__ m, float *__restrict__ v, float *__restrict__ vmax,
                         const float *__restrict__ grad, AdamHp h, const float2 *__restrict__ scal, const int *__restrict__ round_idx,
-                        float *__restrict__ target, float tau, float omtau) {
+                        float *__restrict__ target, float tau, float omtau, const float *__restrict__ decay = nullptr) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float2 sc = scal[*round_idx];
+    if (decay) h.decay = *decay;
     float mm = m[i], vv = v[i], xx = vmax[i];
     const float p = adamw1(w[i], mm, vv, xx, grad[i], h, sc.x, sc.y);
     w[i] = p; m[i] = mm; v[i] = vv; vmax[i] = xx;

@@ -268,12 +268,8 @@ __global__ void k_ppo_last_next_state(const uint32_t *__restrict__ records, prl_
 __global__ void k_ppo_taken_prob(int rows, int A, const float *__restrict__ logits, const int32_t *__restrict__ act, float *__restrict__ out) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= rows) return;
-    const float *l = logits + (size_t)b * A;
-    float mx = l[0];
-    for (int j = 1; j < A; j++) mx = fmaxf(mx, l[j]);
-    float sum = 0.f;
-    for (int j = 0; j < A; j++) sum += expf(l[j] - mx);
-    out[b] = expf(l[act[b]] - mx) / sum;
+    const RowSoftmax sm(logits + (size_t)b * A, A);
+    out[b] = sm(act[b]);
 }
 // batch rows of one round
 __global__ void k_ppo_gather(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, const PpoCall *__restrict__ call,
@@ -297,13 +293,9 @@ __global__ void k_ppo_actor_loss(int B, int A, const float *__restrict__ logits,
     __shared__ float red[256], red2[256];
     float loss = 0.f, psum = 0.f;
     for (int b = threadIdx.x; b < B; b += blockDim.x) {
-        const float *l = logits + (size_t)b * A;
-        float mx = l[0];
-        for (int j = 1; j < A; j++) mx = fmaxf(mx, l[j]);
-        float sum = 0.f;
-        for (int j = 0; j < A; j++) sum += expf(l[j] - mx);
+        const RowSoftmax sm(logits + (size_t)b * A, A);
         const int a = act[b];
-        const float ap = expf(l[a] - mx) / sum;
+        const float ap = sm(a);
         const float r = ap / old[b], g = gae[b];
         const float lo = 1.f - eps_clip, hi = 1.f + eps_clip;
         const float clip = fminf(fmaxf(r, lo), hi);
@@ -315,7 +307,7 @@ __global__ void k_ppo_actor_loss(int B, int A, const float *__restrict__ logits,
         const float dr = -g * (w1 + w2 * inside);
         const float dap = dr / old[b];
         for (int j = 0; j < A; j++) {
-            const float pj = expf(l[j] - mx) / sum;
+            const float pj = sm(j);
             dlogits[(size_t)b * A + j] = dap * ap * ((j == a ? 1.f : 0.f) - pj);
         }
         ap_buf[b] = ap;
