@@ -446,6 +446,55 @@ int prl_td3_learn(prl_td3 *td3, prl_buf *buf, int rounds, int batch, int64_t tra
 int prl_td3_set_graph(prl_td3 *td3, int enable);
 int64_t prl_td3_last_launches(const prl_td3 *td3);
 
+/* ---- Implicit Q-Learning (offline actor-critic) ----------------------------------------------------
+ * Replaces ImplicitQLearning.learn_batch (policy_learners/sequential_decision_making/implicit_q_learning.py:159-302),
+ * driven by PolicyLearner.learn (prl_iql_learn: sample -> round, `rounds` times) or called on a caller's batch
+ * (prl_iql_learn_batch: one round; offline_learning() drives the agent this way).  Per round, every loss from the
+ * parameters before the round: value loss mean(w u^2), u = tq - V(s), w = expectile if u > 0 else 1 - expectile;
+ * twin critic loss against r + gamma (1 - terminated) V(s') (critic_utils.py:170-203); advantage-weighted actor loss with
+ * adv = min(exp((tq - V(s)) temperature), advantage_clamp); tq is q1 or q2 of the critic TARGET at (s, a), picked by the
+ * round's two bits.  Then the value, critic and actor AdamW(amsgrad) steps (one shared step count) and the soft update of
+ * the critic targets.  Discrete (n_actions > 0, act_dim = 0): VanillaActorNetwork, L = -mean(adv log softmax[a]), one-hot
+ * critic input.  Continuous (act_dim > 0, n_actions = 0): VanillaContinuousActorNetwork (tanh scaled to [low, high]),
+ * L = mean(adv mean_d (mu - a)^2).  Flat layouts (fp32, row-major [out][in]):
+ *   actor : W1[h1][obs] b1 W2[h2][h1] b2 W3[N][h2] b3        (N = n_actions or act_dim)
+ *   critic: TWO consecutive copies (q1 then q2) of W1[c1][obs+N] b1 W2[c2][c1] b2 W3[1][c2] b3
+ *   value : W1[v1][obs] b1 W2[v2][v1] b2 W3[1][v2] b3
+ * bits_dev: device i32[rounds][2] = the round's torch.randint(0, 2) draws (value loss first, then actor loss).
+ * Sharded buffers, buffers of the other action kind or other dimensions, and batch / rounds above the configured
+ * maxima are rejected (EINVAL) before any launch. */
+typedef struct prl_iql_cfg {
+    int32_t obs_dim, n_actions, act_dim, actor_h1, actor_h2, critic_h1, critic_h2, value_h1, value_h2;
+    int32_t max_batch, max_rounds;
+    double actor_lr, critic_lr, value_lr, beta1, beta2, eps, weight_decay, gamma, tau;
+    double expectile, temperature, advantage_clamp;
+} prl_iql_cfg;
+typedef struct prl_iql prl_iql;
+int64_t prl_iql_actor_param_count(const prl_iql_cfg *cfg);
+int64_t prl_iql_critic_param_count(const prl_iql_cfg *cfg);   /* ONE critic */
+int64_t prl_iql_value_param_count(const prl_iql_cfg *cfg);
+int64_t prl_iql_workspace_bytes(const prl_iql_cfg *cfg);
+/* Device memory owned by the caller: actor vectors f32[actor_param_count], critic vectors f32[2 * critic_param_count],
+ * value vectors f32[value_param_count]; low/high f32[act_dim] (continuous only, may be null when discrete). */
+int prl_iql_create(prl_iql **out, const prl_iql_cfg *cfg, float *actor_w, float *actor_m, float *actor_v,
+                   float *actor_vmax, float *critic_w, float *critic_m, float *critic_v, float *critic_vmax,
+                   float *critic_target_w, float *value_w, float *value_m, float *value_v, float *value_vmax,
+                   const float *low_dev, const float *high_dev, int64_t adam_step, void *workspace);
+int prl_iql_destroy(prl_iql *iql);
+int64_t prl_iql_adam_step(const prl_iql *iql);
+/* New AdamW learning rates from the next call on; every lr-dependent scalar travels in the per-call block: no re-capture. */
+int prl_iql_set_lr(prl_iql *iql, double actor_lr, double critic_lr, double value_lr);
+/* out_*_loss: device f32[rounds]; out_logical_dev (optional) i32[rounds][batch] = sampled indices */
+int prl_iql_learn(prl_iql *iql, prl_buf *buf, int rounds, int batch, const int32_t *bits_dev, float *out_value_loss_dev,
+                  float *out_critic_loss_dev, float *out_actor_loss_dev, int32_t *out_logical_dev, void *stream);
+/* One round on a dense device batch: state / next_state f32[batch][obs], action f32[batch][act_dim] (continuous) or
+ * action_id i32[batch] (discrete), reward f32[batch], terminated u8[batch]; out_*_loss: device f32[1]. */
+int prl_iql_learn_batch(prl_iql *iql, int batch, const float *state, const float *action, const int32_t *action_id,
+                        const float *reward, const float *next_state, const uint8_t *terminated, const int32_t *bits_dev,
+                        float *out_value_loss_dev, float *out_critic_loss_dev, float *out_actor_loss_dev, void *stream);
+int prl_iql_set_graph(prl_iql *iql, int enable);
+int64_t prl_iql_last_launches(const prl_iql *iql);
+
 /* ---- PPO learner ------------------------------------------------------------------------------
  * Replaces ProximalPolicyOptimization.learn (policy_learners/sequential_decision_making/ppo.py:195-293):
  * prl_ppo_preprocess = preprocess_replay_buffer (state values, taken-action probabilities under the current

@@ -57,6 +57,15 @@ class Td3Cfg(C.Structure):
                 ("actor_tau", C.c_double), ("critic_tau", C.c_double), ("noise_clip", C.c_double)]
 
 
+class IqlCfg(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("act_dim", C.c_int32), ("actor_h1", C.c_int32),
+                ("actor_h2", C.c_int32), ("critic_h1", C.c_int32), ("critic_h2", C.c_int32), ("value_h1", C.c_int32),
+                ("value_h2", C.c_int32), ("max_batch", C.c_int32), ("max_rounds", C.c_int32), ("actor_lr", C.c_double),
+                ("critic_lr", C.c_double), ("value_lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double),
+                ("eps", C.c_double), ("weight_decay", C.c_double), ("gamma", C.c_double), ("tau", C.c_double),
+                ("expectile", C.c_double), ("temperature", C.c_double), ("advantage_clamp", C.c_double)]
+
+
 class PpoCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("actor_h1", C.c_int32), ("actor_h2", C.c_int32),
                 ("critic_h1", C.c_int32), ("critic_h2", C.c_int32), ("max_batch", C.c_int32), ("max_rounds", C.c_int32),
@@ -153,6 +162,18 @@ _SIGNATURES = {
     "prl_td3_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, _P, _P, _P, _P, _P]),
     "prl_td3_set_graph": (C.c_int, [_P, C.c_int]),
     "prl_td3_last_launches": (C.c_int64, [_P]),
+    "prl_iql_actor_param_count": (C.c_int64, [C.POINTER(IqlCfg)]),
+    "prl_iql_critic_param_count": (C.c_int64, [C.POINTER(IqlCfg)]),
+    "prl_iql_value_param_count": (C.c_int64, [C.POINTER(IqlCfg)]),
+    "prl_iql_workspace_bytes": (C.c_int64, [C.POINTER(IqlCfg)]),
+    "prl_iql_create": (C.c_int, [C.POINTER(_P), C.POINTER(IqlCfg)] + [_P] * 15 + [C.c_int64, _P]),
+    "prl_iql_destroy": (C.c_int, [_P]),
+    "prl_iql_adam_step": (C.c_int64, [_P]),
+    "prl_iql_set_lr": (C.c_int, [_P, C.c_double, C.c_double, C.c_double]),
+    "prl_iql_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P]),
+    "prl_iql_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 10 + [_P]),
+    "prl_iql_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_iql_last_launches": (C.c_int64, [_P]),
     "prl_ppo_actor_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_critic_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_workspace_bytes": (C.c_int64, [C.POINTER(PpoCfg)]),

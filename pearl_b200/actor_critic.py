@@ -4,6 +4,7 @@
     B200SoftActorCritic             (SoftActorCritic, soft_actor_critic.py: discrete actions)
     B200ProximalPolicyOptimization  (ProximalPolicyOptimization, ppo.py:96-293)
     B200TD3 / B200DeepDeterministicPolicyGradient  (td3.py:43-202, ddpg.py:41-157)
+    B200ImplicitQLearning           (ImplicitQLearning, implicit_q_learning.py: offline RL; learn_batch runs on the GPU too)
 
 When facebookresearch/Pearl is importable these are the reference classes with `learn()` replaced: the reference
 constructor runs unchanged (same arguments, same networks, same optimizers, same exploration module), so
@@ -23,6 +24,7 @@ from typing import Any
 
 import torch
 
+from .iql import B200ImplicitQLearning as IqlCore
 from .ppo import B200ProximalPolicyOptimization as PpoCore
 from .sac import B200ContinuousSoftActorCritic as SacCore
 from .sac_discrete import B200SoftActorCritic as SacdCore
@@ -41,6 +43,13 @@ try:  # pragma: no cover - depends on the environment
     HAVE_REFERENCE = True
 except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
     HAVE_REFERENCE = False
+
+try:  # pragma: no cover - depends on the environment; kept apart so the classes above do not depend on it
+    from pearl.policy_learners.sequential_decision_making.implicit_q_learning import ImplicitQLearning as _RefIQL
+
+    HAVE_REFERENCE_IQL = True
+except Exception:
+    HAVE_REFERENCE_IQL = False
 
 
 def _adamw_lr(opt: torch.optim.Optimizer, what: str) -> float:
@@ -460,3 +469,97 @@ else:
     B200ProximalPolicyOptimization = PpoCore
     B200TD3 = Td3Core
     B200DeepDeterministicPolicyGradient = DdpgCore
+
+
+def _iql_core_kwargs(pl) -> dict:
+    """Checks that a reference ImplicitQLearning is the configuration the CUDA learner implements and returns the core's
+    network and action-space arguments; raises NotImplementedError otherwise."""
+    name = lambda m: type(m).__name__  # noqa: E731
+    actor, critic, value = pl._actor, pl._critic, pl._value_network
+    continuous = bool(pl._is_action_continuous)
+    if name(actor) != ("VanillaContinuousActorNetwork" if continuous else "VanillaActorNetwork"):
+        raise NotImplementedError(f"the CUDA IQL learner is built for VanillaActorNetwork (discrete actions) or VanillaContinuousActorNetwork "
+                                  f"(continuous actions), not {name(actor)} with {'continuous' if continuous else 'discrete'} actions")
+    if (name(critic), name(getattr(critic, "_critic_1", None)), name(getattr(critic, "_critic_2", None))) != \
+            ("TwinCritic", "VanillaQValueNetwork", "VanillaQValueNetwork") or name(value) != "VanillaValueNetwork":
+        raise NotImplementedError("the CUDA IQL learner is built for TwinCritic(VanillaQValueNetwork) and VanillaValueNetwork")
+    if name(getattr(pl, "_history_summarization_module", None)) != "IdentityHistorySummarizationModule":
+        raise NotImplementedError("the CUDA IQL learner reads states as they are stored: IdentityHistorySummarizationModule only")
+    arm = getattr(pl, "_action_representation_module", None) or getattr(pl, "action_representation_module", None)
+    if name(arm) != ("IdentityActionRepresentationModule" if continuous else "OneHotActionTensorRepresentationModule"):
+        raise NotImplementedError("the CUDA IQL learner takes a one-hot action representation (discrete) or the identity (continuous)")
+    sa, sc, sv = _shapes(actor), _shapes(critic), _shapes(value)
+    if len(sa) != 6 or len(sc) != 12 or len(sv) != 6:
+        raise NotImplementedError("the CUDA IQL learner is built for two hidden layers in the actor, each critic and the value net")
+    obs, h1, h2, n_out = _mlp3(sa, "actor")
+    dq, c1, c2, one = _mlp3(sc[:6], "critic")
+    ov, v1, v2, onev = _mlp3(sv, "value network")
+    if dq != obs + n_out or one != 1 or sc[6:] != sc[:6] or ov != obs or onev != 1:
+        raise NotImplementedError("unexpected IQL network shapes")
+    kw = dict(state_dim=obs, actor_hidden_dims=[h1, h2], critic_hidden_dims=[c1, c2], value_critic_hidden_dims=[v1, v2])
+    if continuous:
+        space = getattr(actor, "_action_space", None) or pl._action_space     # the box the actor scales its output to
+        kw.update(low=space.low, high=space.high)
+    else:
+        kw.update(n_actions=n_out)
+    return kw
+
+
+if HAVE_REFERENCE_IQL:
+
+    class B200ImplicitQLearning(_B200ActorCriticMixin, _RefIQL):
+        """Drop-in for `pearl...implicit_q_learning.ImplicitQLearning`: VanillaActorNetwork (discrete) or
+        VanillaContinuousActorNetwork (continuous), TwinCritic(VanillaQValueNetwork), VanillaValueNetwork, two hidden layers
+        each, AdamW(amsgrad) for all three.  `_value_network` and its optimizer's state are views into the CUDA learner like
+        the actor and critics.  A change of any of the three learning rates goes through `prl_iql_set_lr` (same handle, same
+        graphs).  `learn_batch` runs on the GPU too, so `PearlAgent.learn_batch` and `offline_learning()` do."""
+
+        def _make_core(self, device):
+            kw = _iql_core_kwargs(self)
+            return IqlCore(actor_learning_rate=_adamw_lr(self._actor_optimizer, "actor optimizer"),
+                           critic_learning_rate=_adamw_lr(self._critic_optimizer, "critic optimizer"),
+                           value_critic_learning_rate=_adamw_lr(self._value_network_optimizer, "value optimizer"),
+                           critic_soft_update_tau=float(self._critic_soft_update_tau), discount_factor=float(self._discount_factor),
+                           training_rounds=int(self._training_rounds), batch_size=int(self._batch_size),
+                           expectile=float(self._expectile),
+                           temperature_advantage_weighted_regression=float(self._temperature_advantage_weighted_regression),
+                           advantage_clamp=float(self._advantage_clamp), device=device, **kw, **self._b200_opts)
+
+        def _module_pairs(self, core):
+            return [(self._actor, core.actor_params), (self._critic, core.critic_params), (self._critic_target, core.critic_target_params),
+                    (self._value_network, core.value_params)]
+
+        def _optimizer_triples(self, core):
+            return super()._optimizer_triples(core) + [(self._value_network_optimizer, self._value_network, core._value_state)]
+
+        def _core_steps(self, core):
+            s = int(core._lib.prl_iql_adam_step(core._handle)) if core._handle.value else int(core._adam_step)
+            return (s, s, s)
+
+        def _restart_core(self, core, steps):
+            if len(set(steps)) != 1:
+                raise NotImplementedError("IQL steps its actor, critics and value net once per round: one AdamW step count")
+            if core._handle.value:
+                core._lib.prl_iql_destroy(core._handle)
+                core._handle = C.c_void_p(0)
+            core._adam_step = int(steps[0])
+
+        def _apply_learning_rates(self, core, lrs):
+            core.set_learning_rates(*lrs, core._value_learning_rate)
+
+        def _bind_extras(self, core):
+            vlr = _adamw_lr(self._value_network_optimizer, "value optimizer")
+            if vlr != core._value_learning_rate:
+                core.set_learning_rates(core._actor_learning_rate, core._critic_learning_rate, vlr)
+
+        def learn_batch(self, batch) -> dict:
+            """ImplicitQLearning.learn_batch on the GPU (the batch as preprocess_batch leaves it: one-hot or continuous
+            actions).  Like the reference it does not advance the training-step count."""
+            core = self._ensure_core()
+            report = core.learn_batch(batch)
+            for (opt, _, _), step in zip(self._optimizer_triples(core), self._core_steps(core)):
+                _set_steps(opt, step)
+            return report
+
+else:
+    B200ImplicitQLearning = IqlCore
