@@ -495,6 +495,53 @@ int prl_iql_learn_batch(prl_iql *iql, int batch, const float *state, const float
 int prl_iql_set_graph(prl_iql *iql, int enable);
 int64_t prl_iql_last_launches(const prl_iql *iql);
 
+/* ---- Quantile Regression DQN -------------------------------------------------------------------------
+ * Replaces QuantileRegressionDeepTDLearning.learn_batch (policy_learners/sequential_decision_making/
+ * quantile_regression_deep_td_learning.py) with QuantileRegressionDeepQLearning._get_next_state_quantiles
+ * (quantile_regression_deep_q_learning.py), the QuantileQValueNetwork (neural_networks/sequential_decision_making/
+ * q_value_networks.py: mlp_block(state || one-hot(action)) -> N quantiles) and the risk metrics of
+ * safety_modules/risk_sensitive_safety_modules.py, driven by PolicyLearner.learn (prl_qrdqn_learn: sample -> round,
+ * `rounds` times) or called on a caller's batch (prl_qrdqn_learn_batch: one round).  Per round:
+ *   theta_i(s, a) of the online net; theta'_j(s', k) of the target net for every next-action slot k;
+ *   rho_k = mean_j theta'_j - beta sum_j w_j (theta'_j - mean)^2, w_j = (j+1)/N - j/N in fp32, -inf on masked slots;
+ *   g = first argmax; T_j = theta'_j(s', g) gamma (1 - terminated) + r;
+ *   L = mean over (b, i) of sum_j |tau^_i - 1{u < 0}| huber(u), u = T_j - theta_i, tau^_i = (i/N + (i+1)/N) / 2, kappa = 1;
+ *   one AdamW(amsgrad) step; then, when (training_steps + 1) % target_update_freq == 0 with training_steps the count the
+ *   reference's learn_batch sees, the soft update target = tau * online + (1 - tau) * target with the NEW parameters.
+ *   Reported loss: mean over (b, i) of |theta_i - T_i|.
+ * beta = 0 is RiskNeutralSafetyModule, beta > 0 QuantileNetworkMeanVarianceSafetyModule(beta).  1 <= num_quantiles <= 256,
+ * 1 <= n_actions <= 255.  Flat layout (fp32, row-major [out][in]): W1[h1][obs + A] b1 W2[h2][h1] b2 W3[N][h2] b3.
+ * Sharded buffers, continuous-action buffers, buffers of other obs_dim / n_actions, and batch / rounds above the
+ * configured maxima are rejected (EINVAL) before any launch. */
+typedef struct prl_qrdqn_cfg {
+    int32_t obs_dim, n_actions, hidden1, hidden2, num_quantiles, target_update_freq;
+    int32_t max_batch, max_rounds;
+    double lr, beta1, beta2, eps, weight_decay, gamma, tau;
+} prl_qrdqn_cfg;
+typedef struct prl_qrdqn prl_qrdqn;
+int64_t prl_qrdqn_param_count(const prl_qrdqn_cfg *cfg);
+int64_t prl_qrdqn_workspace_bytes(const prl_qrdqn_cfg *cfg);
+/* Device memory owned by the caller: f32[param_count] each (online, target, AdamW exp_avg / exp_avg_sq / max_exp_avg_sq). */
+int prl_qrdqn_create(prl_qrdqn **out, const prl_qrdqn_cfg *cfg, float *q_w, float *q_m, float *q_v, float *q_vmax,
+                     float *q_target_w, int64_t adam_step, void *workspace);
+int prl_qrdqn_destroy(prl_qrdqn *qr);
+int64_t prl_qrdqn_adam_step(const prl_qrdqn *qr);
+/* New AdamW learning rate from the next call on; every lr-dependent scalar travels in the per-call block: no re-capture. */
+int prl_qrdqn_set_lr(prl_qrdqn *qr, double lr);
+/* training_steps = the learner's count before the call (PolicyLearner.learn increments it before each round);
+ * out_loss_dev: device f32[rounds]; out_logical_dev (optional) i32[rounds][batch] = sampled indices */
+int prl_qrdqn_learn(prl_qrdqn *qr, prl_buf *buf, int rounds, int batch, int64_t training_steps, double beta,
+                    float *out_loss_dev, int32_t *out_logical_dev, void *stream);
+/* One round on a dense device batch: state / next_state f32[batch][obs], action_id i32[batch], reward f32[batch],
+ * terminated u8[batch], next_ids i32[batch][n_actions] (slot k holds an action id) and next_count i32[batch] (slots at
+ * and beyond it are unavailable), both null when every action is available; training_steps = the count learn_batch sees
+ * (agent.learn_batch does not advance it); out_loss_dev: device f32[1]. */
+int prl_qrdqn_learn_batch(prl_qrdqn *qr, int batch, const float *state, const int32_t *action_id, const float *reward,
+                          const float *next_state, const uint8_t *terminated, const int32_t *next_ids,
+                          const int32_t *next_count, int64_t training_steps, double beta, float *out_loss_dev, void *stream);
+int prl_qrdqn_set_graph(prl_qrdqn *qr, int enable);
+int64_t prl_qrdqn_last_launches(const prl_qrdqn *qr);
+
 /* ---- PPO learner ------------------------------------------------------------------------------
  * Replaces ProximalPolicyOptimization.learn (policy_learners/sequential_decision_making/ppo.py:195-293):
  * prl_ppo_preprocess = preprocess_replay_buffer (state values, taken-action probabilities under the current

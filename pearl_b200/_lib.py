@@ -66,6 +66,13 @@ class IqlCfg(C.Structure):
                 ("expectile", C.c_double), ("temperature", C.c_double), ("advantage_clamp", C.c_double)]
 
 
+class QrdqnCfg(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden1", C.c_int32), ("hidden2", C.c_int32),
+                ("num_quantiles", C.c_int32), ("target_update_freq", C.c_int32), ("max_batch", C.c_int32),
+                ("max_rounds", C.c_int32), ("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double),
+                ("eps", C.c_double), ("weight_decay", C.c_double), ("gamma", C.c_double), ("tau", C.c_double)]
+
+
 class PpoCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("actor_h1", C.c_int32), ("actor_h2", C.c_int32),
                 ("critic_h1", C.c_int32), ("critic_h2", C.c_int32), ("max_batch", C.c_int32), ("max_rounds", C.c_int32),
@@ -174,6 +181,16 @@ _SIGNATURES = {
     "prl_iql_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 10 + [_P]),
     "prl_iql_set_graph": (C.c_int, [_P, C.c_int]),
     "prl_iql_last_launches": (C.c_int64, [_P]),
+    "prl_qrdqn_param_count": (C.c_int64, [C.POINTER(QrdqnCfg)]),
+    "prl_qrdqn_workspace_bytes": (C.c_int64, [C.POINTER(QrdqnCfg)]),
+    "prl_qrdqn_create": (C.c_int, [C.POINTER(_P), C.POINTER(QrdqnCfg)] + [_P] * 5 + [C.c_int64, _P]),
+    "prl_qrdqn_destroy": (C.c_int, [_P]),
+    "prl_qrdqn_adam_step": (C.c_int64, [_P]),
+    "prl_qrdqn_set_lr": (C.c_int, [_P, C.c_double]),
+    "prl_qrdqn_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, C.c_double, _P, _P, _P]),
+    "prl_qrdqn_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 7 + [C.c_int64, C.c_double, _P, _P]),
+    "prl_qrdqn_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_qrdqn_last_launches": (C.c_int64, [_P]),
     "prl_ppo_actor_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_critic_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_workspace_bytes": (C.c_int64, [C.POINTER(PpoCfg)]),

@@ -5,6 +5,8 @@
     B200ProximalPolicyOptimization  (ProximalPolicyOptimization, ppo.py:96-293)
     B200TD3 / B200DeepDeterministicPolicyGradient  (td3.py:43-202, ddpg.py:41-157)
     B200ImplicitQLearning           (ImplicitQLearning, implicit_q_learning.py: offline RL; learn_batch runs on the GPU too)
+    B200QuantileRegressionDeepQLearning  (QuantileRegressionDeepQLearning, QR-DQN; not an actor-critic, but bound the same
+                                    way: `_Q`, `_Q_target` and the optimizer state are views; learn_batch runs on the GPU too)
 
 When facebookresearch/Pearl is importable these are the reference classes with `learn()` replaced: the reference
 constructor runs unchanged (same arguments, same networks, same optimizers, same exploration module), so
@@ -26,6 +28,7 @@ import torch
 
 from .iql import B200ImplicitQLearning as IqlCore
 from .ppo import B200ProximalPolicyOptimization as PpoCore
+from .qrdqn import B200QuantileRegressionDeepQLearning as QrdqnCore
 from .sac import B200ContinuousSoftActorCritic as SacCore
 from .sac_discrete import B200SoftActorCritic as SacdCore
 from .td3 import B200DeepDeterministicPolicyGradient as DdpgCore
@@ -50,6 +53,15 @@ try:  # pragma: no cover - depends on the environment; kept apart so the classes
     HAVE_REFERENCE_IQL = True
 except Exception:
     HAVE_REFERENCE_IQL = False
+
+try:  # pragma: no cover - depends on the environment; kept apart so the classes above do not depend on it
+    from pearl.policy_learners.sequential_decision_making.quantile_regression_deep_q_learning import (
+        QuantileRegressionDeepQLearning as _RefQRDQN,
+    )
+
+    HAVE_REFERENCE_QRDQN = True
+except Exception:
+    HAVE_REFERENCE_QRDQN = False
 
 
 def _adamw_lr(opt: torch.optim.Optimizer, what: str) -> float:
@@ -563,3 +575,120 @@ if HAVE_REFERENCE_IQL:
 
 else:
     B200ImplicitQLearning = IqlCore
+
+
+def _qrdqn_adamw_lr(opt: torch.optim.Optimizer) -> float:
+    """`_adamw_lr` for the QR-DQN optimizer, whose extra parameter groups (the one
+    set_history_summarization_module adds for the identity module) must be empty."""
+    groups = opt.param_groups if isinstance(opt, torch.optim.AdamW) else []
+    if not groups or any(len(g["params"]) for g in groups[1:]):
+        raise NotImplementedError("optimizer: the fused update implements torch.optim.AdamW(amsgrad=True) over the quantile "
+                                  "network alone")
+    g = groups[0]
+    if (not g.get("amsgrad", False) or g.get("maximize", False) or tuple(g["betas"]) != (0.9, 0.999) or float(g["eps"]) != 1e-8
+            or float(g["weight_decay"]) != 0.01):
+        raise NotImplementedError("optimizer: the fused update implements torch.optim.AdamW(amsgrad=True) with default "
+                                  "betas / eps / weight_decay")
+    return float(g["lr"])
+
+
+def _qrdqn_beta(safety_module) -> float:
+    """Variance weight of the risk metric: 0 for RiskNeutralSafetyModule (PearlAgent's default for distributional
+    learners) or no safety module, `_beta` for QuantileNetworkMeanVarianceSafetyModule."""
+    name = type(safety_module).__name__
+    if safety_module is None or name == "RiskNeutralSafetyModule":
+        return 0.0
+    if name == "QuantileNetworkMeanVarianceSafetyModule":
+        return float(safety_module._beta)
+    raise NotImplementedError(f"the CUDA QR-DQN learner implements RiskNeutralSafetyModule and "
+                              f"QuantileNetworkMeanVarianceSafetyModule, not {name}")
+
+
+def _qrdqn_core_kwargs(pl) -> dict:
+    """Checks that a reference QuantileRegressionDeepQLearning is the configuration the CUDA learner implements and
+    returns the core's network arguments; raises NotImplementedError otherwise."""
+    name = lambda m: type(m).__name__  # noqa: E731
+    q = pl._Q
+    if name(q) != "QuantileQValueNetwork":
+        raise NotImplementedError(f"the CUDA QR-DQN learner is built for QuantileQValueNetwork, not {name(q)}")
+    if any(isinstance(m, torch.nn.LayerNorm) for m in q.modules()):
+        raise NotImplementedError("the CUDA QR-DQN learner is built for QuantileQValueNetwork without use_layer_norm")
+    if name(getattr(pl, "_history_summarization_module", None)) != "IdentityHistorySummarizationModule":
+        raise NotImplementedError("the CUDA QR-DQN learner reads states as they are stored: IdentityHistorySummarizationModule only")
+    arm = getattr(pl, "_action_representation_module", None) or getattr(pl, "action_representation_module", None)
+    if name(arm) != "OneHotActionTensorRepresentationModule":
+        raise NotImplementedError("the CUDA QR-DQN learner folds a one-hot action representation into the quantile network")
+    sq = _shapes(q)
+    if len(sq) != 6:
+        raise NotImplementedError("the CUDA QR-DQN learner is built for a quantile network with two hidden layers")
+    din, h1, h2, n_q = _mlp3(sq, "quantile network")
+    obs, A = int(q.state_dim), int(pl._action_space.n)
+    if din != obs + A or int(q.action_dim) != A or n_q != int(q.num_quantiles):
+        raise NotImplementedError("unexpected QR-DQN network shapes")
+    _qrdqn_beta(getattr(pl, "safety_module", None))
+    return dict(state_dim=obs, n_actions=A, hidden_dims=[h1, h2], num_quantiles=n_q)
+
+
+if HAVE_REFERENCE_QRDQN:
+
+    class B200QuantileRegressionDeepQLearning(_RefQRDQN):
+        """Drop-in for `pearl...quantile_regression_deep_q_learning.QuantileRegressionDeepQLearning`:
+        QuantileQValueNetwork with two hidden layers, one-hot actions, AdamW(amsgrad).  On the first `learn()` /
+        `learn_batch()` (after PearlAgent moved the learner to its CUDA device) `_Q`, `_Q_target` and the optimizer's
+        state become views into the CUDA learner's flat vectors; a checkpoint loaded with `load_state_dict` is picked up on
+        the next call.  The risk coefficient is read from `self.safety_module` and the learning rate from
+        `param_groups[0]` on every call (neither re-creates the handle).  `act()` is the reference's own code."""
+
+        def __init__(self, *args: Any, max_rounds_per_call: int = 1024, seed: int | None = None, **kwargs: Any) -> None:
+            super().__init__(*args, **kwargs)
+            self._b200_opts = dict(max_rounds_per_call=max_rounds_per_call, seed=seed)
+            self._b200 = None
+
+        def _ensure_core(self):
+            dev = next(self._Q.parameters()).device
+            if dev.type != "cuda":
+                raise RuntimeError(f"{type(self).__name__}: parameters are on {dev}; move the learner to a CUDA device "
+                                   "(PearlAgent(device_id=0) does this) - pearl_b200 has no CPU path")
+            core = self._b200
+            if core is None or core._device != dev:
+                core = QrdqnCore(learning_rate=_qrdqn_adamw_lr(self._optimizer), discount_factor=float(self._discount_factor),
+                                 training_rounds=int(self._training_rounds), batch_size=int(self._batch_size),
+                                 target_update_freq=int(self._target_update_freq), soft_update_tau=float(self._soft_update_tau),
+                                 device=dev, **_qrdqn_core_kwargs(self), **self._b200_opts)
+                self._b200 = core
+            if not (_is_adopted(self._Q, core.params) and _is_adopted(self._Q_target, core.target_params)):
+                _adopt(self._Q, core.params)
+                _adopt(self._Q_target, core.target_params)
+            lr = _qrdqn_adamw_lr(self._optimizer)
+            if lr != core._learning_rate:
+                core.set_learning_rate(lr)
+            if not _is_bound(self._optimizer, self._Q, core._state):
+                cur = core._current_adam_step()
+                step = _bind_optimizer(self._optimizer, self._Q, core._state, cur)
+                if step != cur:
+                    core._restart(step)
+            core._variance_weighting_coefficient = _qrdqn_beta(getattr(self, "safety_module", None))
+            core._training_rounds, core._batch_size = int(self._training_rounds), int(self._batch_size)
+            core._training_steps = int(self._training_steps)
+            return core
+
+        def learn(self, replay_buffer) -> dict:
+            """PolicyLearner.learn on the GPU (`training_rounds` rounds from a B200ReplayBuffer)."""
+            if len(replay_buffer) == 0:
+                return {}
+            core = self._ensure_core()
+            report = core.learn(replay_buffer)
+            self._training_steps = int(core._training_steps)
+            _set_steps(self._optimizer, core._current_adam_step())
+            return report
+
+        def learn_batch(self, batch) -> dict:
+            """QuantileRegressionDeepTDLearning.learn_batch on the GPU (the batch as preprocess_batch leaves it).  Like the
+            reference it does not advance the training-step count."""
+            core = self._ensure_core()
+            report = core.learn_batch(batch)
+            _set_steps(self._optimizer, core._current_adam_step())
+            return report
+
+else:
+    B200QuantileRegressionDeepQLearning = QrdqnCore

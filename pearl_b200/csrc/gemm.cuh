@@ -1,4 +1,4 @@
-// gemm.cuh — the one tiled fp32 contraction kernel the actor-critic learners (sac.cu, ppo.cu) are built from.
+// gemm.cuh — the one tiled fp32 contraction kernel the actor-critic learners (sac.cu, ppo.cu, ...) and qrdqn.cu are built from.
 //   C[i][j] = sum_c A(i, c) * B(j, c)        i < Mo, j < No, c < Kc
 // covers nn.Linear forward (y = act(x W^T + b)), backward-data (dx = dy W, optionally masked by the ReLU of
 // the layer below and accumulated) and backward-weight (dW = dy^T x, the bias gradient as an implicit
@@ -270,6 +270,45 @@ static __global__ void k_head_bwd(int B, int H, const float *__restrict__ dq, co
     dc2[o] = (c2[o] > 0.f) ? dq[z * B + m] * __ldg(w3 + z * w_net_stride + j) : 0.f;
 }
 
+// The one-hot fold: a network whose input is state || one-hot(action id) computes its layer-1 state product once per row
+// (P = state W1[:, :obs]^T + b1) and adds the column W1[:, obs + id] of the action.  Per blockIdx.z, one of several stacked
+// networks (net_stride apart).
+// layer 1 at the taken action: c1[z][b][j] = relu(P[z][b][j] + W1[z][j][obs + a_b])      (w1a = W1 + obs)
+static __global__ void k_fold(int B, int C1, const float *__restrict__ P, const float *__restrict__ w1a, int ld, long long net_stride,
+                              const int *__restrict__ act, float *__restrict__ c1) {
+    const int z = blockIdx.z, e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= B * C1) return;
+    const int b = e / C1, j = e - b * C1;
+    const size_t o = (size_t)z * B * C1 + e;
+    c1[o] = fmaxf(P[o] + __ldg(w1a + z * net_stride + (size_t)j * ld + act[b]), 0.f);
+}
+
+// layer 1 for every (row, slot): c1[z][b*A + k][j] = relu(P[z][b][j] + W1[z][j][obs + id]), id = ids[b][k], or k when ids
+// is null (every action)
+static __global__ void k_fold_expand(int B, int A, int C1, const float *__restrict__ P, const float *__restrict__ w1a, int ld,
+                                     long long net_stride, const int *__restrict__ ids, float *__restrict__ c1) {
+    const int z = blockIdx.z;
+    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (long long)B * A * C1) return;
+    const int row = (int)(e / C1), j = (int)(e - (long long)row * C1), b = row / A, k = row - b * A;
+    const int id = ids ? ids[row] : k;
+    const float v = P[(size_t)z * B * C1 + (size_t)b * C1 + j] + __ldg(w1a + z * net_stride + (size_t)j * ld + id);
+    c1[(size_t)z * B * A * C1 + e] = fmaxf(v, 0.f);
+}
+
+// gradient of the one-hot columns of W1 (the fold backwards): dW1[z][j][obs + k] = sum over rows b with a_b = k of dc1[z][b][j],
+// rows in ascending order
+static __global__ void k_fold_w1a_grad(int B, int A, int C1, const int *__restrict__ act, const float *__restrict__ dc1,
+                                       float *__restrict__ gw1, int ld, long long net_stride) {
+    const int z = blockIdx.z, e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= C1 * A) return;
+    const int k = e / C1, j = e - k * C1;
+    float s = 0.f;
+    for (int b = 0; b < B; b++)
+        if (act[b] == k) s += dc1[((size_t)z * B + b) * C1 + j];
+    gw1[z * net_stride + (size_t)j * ld + k] = s;
+}
+
 // one row of softmax(logits) as torch computes it: p_k = exp(l_k - max) / sum.  The row's max and sum are computed once;
 // p_k is evaluated where it is needed (the same arithmetic every time, no per-thread arrays)
 struct RowSoftmax {
@@ -295,9 +334,11 @@ __device__ __forceinline__ float adamw1(float w, float &m, float &v, float &x, f
 // AdamW(amsgrad) over a flat vector; optional soft update of a target vector with the NEW parameters.
 // decay (optional): device copy of 1 - lr * weight_decay that overrides h.decay, so that a learning-rate change reaches a
 // captured graph through its per-call block
+// target_on (optional): per-round flags; the soft update runs only in rounds whose flag is non-zero
 static __global__ void k_adamw(int n, float *__restrict__ w, float *__restrict__ m, float *__restrict__ v, float *__restrict__ vmax,
                         const float *__restrict__ grad, AdamHp h, const float2 *__restrict__ scal, const int *__restrict__ round_idx,
-                        float *__restrict__ target, float tau, float omtau, const float *__restrict__ decay = nullptr) {
+                        float *__restrict__ target, float tau, float omtau, const float *__restrict__ decay = nullptr,
+                        const int *__restrict__ target_on = nullptr) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float2 sc = scal[*round_idx];
@@ -305,7 +346,7 @@ static __global__ void k_adamw(int n, float *__restrict__ w, float *__restrict__
     float mm = m[i], vv = v[i], xx = vmax[i];
     const float p = adamw1(w[i], mm, vv, xx, grad[i], h, sc.x, sc.y);
     w[i] = p; m[i] = mm; v[i] = vv; vmax[i] = xx;
-    if (target) target[i] = __fadd_rn(__fmul_rn(tau, p), __fmul_rn(omtau, target[i]));
+    if (target && (!target_on || target_on[*round_idx])) target[i] = __fadd_rn(__fmul_rn(tau, p), __fmul_rn(omtau, target[i]));
 }
 inline AdamHp adam_hp(double lr, double beta1, double beta2, double eps, double weight_decay) {
     return AdamHp{(float)(1.0 - lr * weight_decay), (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps};

@@ -72,16 +72,6 @@ __global__ void k_iql_load(const uint32_t *__restrict__ records, prl_buf_layout 
     }
 }
 
-// layer 1 of both critics at the taken action (the one-hot fold): c1[z][b][j] = relu(P[z][b][j] + W1[z][j][obs + a_b])
-__global__ void k_iql_fold(int B, int C1, const float *__restrict__ P, const float *__restrict__ w1a, int ld, long long net_stride,
-                           const int *__restrict__ act, float *__restrict__ c1) {
-    const int z = blockIdx.z, e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= B * C1) return;
-    const int b = e / C1, j = e - b * C1;
-    const size_t o = (size_t)z * B * C1 + e;
-    c1[o] = fmaxf(P[o] + __ldg(w1a + z * net_stride + (size_t)j * ld + act[b]), 0.f);
-}
-
 // The three losses of one round and the gradients they send into their networks (implicit_q_learning.py:159-286).
 //   value : u = tq_v - V(s), w = expectile if u > 0 else 1 - expectile; L = mean(w u^2); dV = -2 w u / B
 //   critic: y = V(s') gamma (1 - terminated) + r; L = (mean (q1 - y)^2 + mean (q2 - y)^2) / 2; dq_z = (q_z - y) / B
@@ -147,18 +137,6 @@ __global__ void __launch_bounds__(256) k_iql_losses(int B, int n_out, int discre
         call->out_critic[rnd] = red[1][0] * ib * 0.5f;
         call->out_actor[rnd] = red[2][0] * ib;
     }
-}
-
-// gradient of the one-hot columns of W1 (the fold backwards): dW1[z][j][obs + k] = sum over rows b with a_b = k of dc1[z][b][j]
-__global__ void k_iql_w1a_grad(int B, int A, int C1, const int *__restrict__ act, const float *__restrict__ dc1, float *__restrict__ gw1,
-                               int ld, long long net_stride) {
-    const int z = blockIdx.z, e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= C1 * A) return;
-    const int k = e / C1, j = e - k * C1;
-    float s = 0.f;
-    for (int b = 0; b < B; b++)
-        if (act[b] == k) s += dc1[((size_t)z * B + b) * C1 + j];
-    gw1[z * net_stride + (size_t)j * ld + k] = s;
 }
 
 __global__ void k_iql_bump(int *round_idx) { *round_idx += 1; }
@@ -361,7 +339,7 @@ static int iql_round(prl_iql *s, prl_buf *buf, int B, cudaStream_t st) {
     auto critic_sa = [&](const float *net, float *c1, float *c2, float *q) {
         if (disc) {
             L.fwd(mat(S, O), B, net + s->cW1, D, Pc, net + s->cb1, Pc, C1, O, false, s->P, C1, sC1, 2);
-            k_iql_fold<<<dim3((B * C1 + eb - 1) / eb, 1, 2), eb, 0, st>>>(B, C1, s->P, net + s->cW1 + O, D, Pc, s->act, c1);
+            k_fold<<<dim3((B * C1 + eb - 1) / eb, 1, 2), eb, 0, st>>>(B, C1, s->P, net + s->cW1 + O, D, Pc, s->act, c1);
             small++;
         } else {
             L.fwd(mat2(S, O, O, s->Act, N), B, net + s->cW1, D, Pc, net + s->cb1, Pc, C1, D, true, c1, C1, sC1, 2);
@@ -406,7 +384,7 @@ static int iql_round(prl_iql *s, prl_buf *buf, int B, cudaStream_t st) {
         L.bwd_x(s->dc2, C2, sC2, B, C2, cw + s->cW2, C1, Pc, 0, C1, s->dc1, C1, sC1, s->c1, C1, sC1, false, 2);
         if (disc) {
             L.bwd_w(s->dc1, C1, sC1, B, C1, mat(S, O), O, gc + s->cW1, D, Pc, gc + s->cb1, Pc, 2);   // state columns + b1
-            k_iql_w1a_grad<<<dim3((C1 * N + eb - 1) / eb, 1, 2), eb, 0, st>>>(B, N, C1, s->act, s->dc1, gc + s->cW1 + O, D, Pc);
+            k_fold_w1a_grad<<<dim3((C1 * N + eb - 1) / eb, 1, 2), eb, 0, st>>>(B, N, C1, s->act, s->dc1, gc + s->cW1 + O, D, Pc);
             small++;
         } else {
             L.bwd_w(s->dc1, C1, sC1, B, C1, mat2(S, O, O, s->Act, N), D, gc + s->cW1, D, Pc, gc + s->cb1, Pc, 2);

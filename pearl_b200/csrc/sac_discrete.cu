@@ -57,19 +57,6 @@ __global__ void k_sacd_gather(const uint32_t *__restrict__ records, prl_buf_layo
     }
 }
 
-// layer 1 of both critics for every (row, slot): c1[z][b*A + k][j] = relu(P[z][b][j] + W1[z][j][obs + id]),
-// P = state product + b1; id = ids[b][k], or k when ids is null (every action)
-__global__ void k_sacd_expand(int B, int A, int C1, const float *__restrict__ P, const float *__restrict__ w1a, int ld, long long net_stride,
-                              const int *__restrict__ ids, float *__restrict__ c1) {
-    const int z = blockIdx.z;
-    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= (long long)B * A * C1) return;
-    const int row = (int)(e / C1), j = (int)(e - (long long)row * C1), b = row / A, k = row - b * A;
-    const int id = ids ? ids[row] : k;
-    const float v = P[(size_t)z * B * C1 + (size_t)b * C1 + j] + __ldg(w1a + z * net_stride + (size_t)j * ld + id);
-    c1[(size_t)z * B * A * C1 + e] = fmaxf(v, 0.f);
-}
-
 // rows of the taken action: c1a[z][b] = c1[z][b*A + a_b] (and c2a, qa); the online critic does not change between the
 // actor step and the critic step, so Q(s, a) and its activations are those of the all-action pass
 __global__ void k_sacd_pick(int B, int A, int C1, int C2, const int *__restrict__ act, const float *__restrict__ c1, const float *__restrict__ c2,
@@ -157,18 +144,6 @@ __global__ void __launch_bounds__(256) k_sacd_critic_loss(int B, const float *__
     __syncthreads();
     for (int o = 128; o; o >>= 1) { if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o]; __syncthreads(); }
     if (threadIdx.x == 0) call->out_critic[*round_idx] = red[0] * ib * 0.5f;
-}
-
-// gradient of the one-hot columns of W1 (the fold backwards): dW1[z][j][obs + k] = sum over rows b with a_b = k of dc1[z][b][j]
-__global__ void k_sacd_w1a_grad(int B, int A, int C1, const int *__restrict__ act, const float *__restrict__ dc1, float *__restrict__ gw1,
-                                int ld, long long net_stride) {
-    const int z = blockIdx.z, e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= C1 * A) return;
-    const int k = e / C1, j = e - k * C1;
-    float s = 0.f;
-    for (int b = 0; b < B; b++)
-        if (act[b] == k) s += dc1[((size_t)z * B + b) * C1 + j];
-    gw1[z * net_stride + (size_t)j * ld + k] = s;
 }
 
 // entropy step (soft_actor_critic.py learn_batch): H = -mean_b sum_k pi log(pi + 1e-8) of the actor-step probabilities;
@@ -378,7 +353,7 @@ static int sacd_round(prl_sacd *s, prl_buf *buf, int B, cudaStream_t st) {
     auto critic_all = [&](const float *net, const float *X, const int *ids) {   // q[z][b*A + k], both critics (blockIdx.z)
         L.fwd(mat(X, O), B, net + s->cW1, D, Pc, net + s->cb1, Pc, C1, O, false, s->P, C1, sP, 2);
         dim3 ge((unsigned)(((long long)BA * C1 + eb - 1) / eb), 1, 2);
-        k_sacd_expand<<<ge, eb, 0, st>>>(B, A, C1, s->P, net + s->cW1 + O, D, Pc, ids, s->c1);
+        k_fold_expand<<<ge, eb, 0, st>>>(B, A, C1, s->P, net + s->cW1 + O, D, Pc, ids, s->c1);
         L.fwd(mat(s->c1, C1, sC1), BA, net + s->cW2, C1, Pc, net + s->cb2, Pc, C2, C1, true, s->c2, C2, sC2, 2);
         L.fwd(mat(s->c2, C2, sC2), BA, net + s->cW3, C2, Pc, net + s->cb3, Pc, 1, C2, false, s->q, 1, BA, 2);
         small++;
@@ -414,7 +389,7 @@ static int sacd_round(prl_sacd *s, prl_buf *buf, int B, cudaStream_t st) {
         L.bwd_w(s->dc2, C2, sA2, B, C2, mat(s->c1a, C1, sA1), C1, gc + s->cW2, C1, Pc, gc + s->cb2, Pc, 2);
         L.bwd_x(s->dc2, C2, sA2, B, C2, cw + s->cW2, C1, Pc, 0, C1, s->dc1, C1, sA1, s->c1a, C1, sA1, false, 2);
         L.bwd_w(s->dc1, C1, sA1, B, C1, mat(s->S, O), O, gc + s->cW1, D, Pc, gc + s->cb1, Pc, 2);   // state columns + b1
-        k_sacd_w1a_grad<<<dim3((C1 * A + eb - 1) / eb, 1, 2), eb, 0, st>>>(B, A, C1, s->act, s->dc1, gc + s->cW1 + O, D, Pc);
+        k_fold_w1a_grad<<<dim3((C1 * A + eb - 1) / eb, 1, 2), eb, 0, st>>>(B, A, C1, s->act, s->dc1, gc + s->cW1 + O, D, Pc);
         const int n2p = 2 * s->Pc;
         k_adamw<<<(n2p + eb - 1) / eb, eb, 0, st>>>(n2p, s->critic, s->critic_m, s->critic_v, s->critic_x, gc, h, s->scal_c, s->round_idx,
                                                   s->critic_t, (float)c.tau, (float)(1.0 - c.tau), &s->call->decay_c);
