@@ -10,16 +10,16 @@
 //
 // Per gradient step (256 threads = two warpgroups; warpgroup h owns the 64 batch rows 128 i + 64 h .. of row tile i,
 // a thread the elements of those rows that the wgmma accumulator layout gives it, umma.cuh):
-//   layer 1  T1 = X W1s^T: the rows are gathered into shared memory by cp.async (K chunks of 64) and read back
-//            as register A fragments (RS form); B = the W1 tile.
+//   layer 1  T1 = X W1s^T: the rows are gathered into shared memory by cp.async (K chunks of 64, double-buffered, the
+//            first chunk issued ahead of time) and read back as register A fragments (RS form); B = the W1 tile.
 //   phase T  target net: per action slot one 64 x 64 x 64 product whose A operand relu(T1 + W1a[:,a] + b1) is
 //            built in registers from the layer-1 accumulator and never leaves them; running max over the slots.
 //   phase O  online net forward the same way, loss gradient, dZ2, dH1 = dZ2 W2 (B operand = W2^T tile), all on
 //            register operands; then the weight gradients as products over the batch dimension:
 //            dW2 = dZ2^T H1, dW1s = dZ1^T S, and [db | dW1a] = dZ^T E with E = [1 | onehot(action)];
 //            their operands are explicitly transposed tiles written with a 144-byte chunk pitch
-//            (bank-conflict-free column scatter), 64 batch rows per pass, the two warpgroups taking
-//            different output columns.  Their accumulators stay in registers for the whole step.
+//            (bank-conflict-free column scatter), 64 batch rows per pass, the two warpgroups issuing the same
+//            products on equal shares of the output columns.  Their accumulators stay in registers for the whole step.
 //   AdamW    gradients registers -> shared staging, then one coalesced 16-byte sweep over the flat parameter
 //            vector (parameters / moments in L2) that also writes the operand-layout weight tiles.
 //
@@ -30,6 +30,14 @@
 // which an accumulator's columns feed the next product's register A operand.  The target network's small vectors are
 // cached in shared memory between soft updates, AdamW walks one flat list with two groups of loads in flight, the soft
 // target update is applied to the tiles in tile order.
+//
+// Each 3xTF32 product is one chain of wgmma with a single wait at its end, and that only holds while ptxas can pipeline
+// the kernel's wgmma: ONE obstacle anywhere in the kernel makes it wait after every wgmma of the kernel.  What must
+// stay true: no function call in the kernel (not even printf, C7510); no wgmma under
+// a branch, including a runtime step count or a branch on the warpgroup index (both warpgroups issue the same products,
+// C7520), and no conditional load feeding an A fragment; and each chain fits in the registers together with everything
+// live across it (C7511 / C7512), which is why H1 and dZ2 wait in shared memory while dH1 is formed and the learner
+// descriptor and the dW3 partial sums live in shared memory.  tests/test_dqn_tc_sass.py checks the SASS.
 #include <math.h>
 #include <stdarg.h>
 #include <stdlib.h>
@@ -96,6 +104,9 @@ struct Misc {
     float redw[8][HID];
     float redmae[8], reddb3[8];
     unsigned long long bar[3];   // 0: target tiles; 1: online W1 tiles; 2: online W2 tiles
+    // kept here rather than in registers: the wgmma chains need the registers (section 3.1 of DESIGN.md)
+    TcLearner L;                 // this CTA's learner, per-round arrays shifted to the launch's first round
+    float dw3[16][NTH];          // per-thread dW3 partial sums, carried across the row tiles
 };
 
 __device__ __forceinline__ void cp_async16_zfill_tc(void *smem_dst, const void *gmem_src, int src_bytes) {
@@ -118,17 +129,24 @@ __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.pr
 using umma::tf32_lo;
 
 // Operand-layout copies of one network's matrices in global memory (floats):
-//   [W1 hi: 64 x obs][W1 lo][W2 hi: 64 x 64][W2 lo]      (the shared-memory images, tile by tile; the W2 tiles with their
+//   [W1 hi: 64 x k1][W1 lo][W2 hi: 64 x 64][W2 lo]      (the shared-memory images, tile by tile; the W2 tiles with their
 //   K axis in umma::kperm order; the W2^T tiles of the online network are transposed out of the W2 tiles in shared memory)
+// The W1 tiles have K = k1 = obs rounded up to a multiple of 64, the columns from obs on are zero: every layer-1 K chunk is
+// a full 8-step product (no runtime step count inside a wgmma chain), and the padding adds exact zeros to the sums.
 struct NetTiles { float *w1hi, *w1lo, *w2; };   // w2: the 2 x 4096-float block W2 hi | W2 lo
-__host__ __device__ inline int net_tile_floats(int obs) { return 128 * obs + 2 * HID * HID; }
-__device__ __forceinline__ NetTiles net_tiles(float *base, int obs) { return NetTiles{base, base + 64 * obs, base + 128 * obs}; }
+__host__ __device__ inline int k1_cols(int obs) { return (obs + 63) & ~63; }
+__host__ __device__ inline int net_tile_floats(int obs) { return 128 * k1_cols(obs) + 2 * HID * HID; }
+__device__ __forceinline__ NetTiles net_tiles(float *base, int obs) {
+    const int k1 = k1_cols(obs);
+    return NetTiles{base, base + 64 * k1, base + 128 * k1};
+}
 // all tiles of one network from its flat parameter vector (kernel prologue, soft target update)
 __device__ void rebuild_tiles(const float *__restrict__ net, const Dims &d, const NetTiles &t, int tid) {
-    for (int e = tid; e < HID * d.obs; e += NTH) {
-        const int j = e / d.obs, k = e - j * d.obs;
-        const float x = __ldcg(net + d.oW1 + (size_t)j * d.D + k);
-        const int idx = umma::tile_index(j, k, d.obs);
+    const int k1 = k1_cols(d.obs);
+    for (int e = tid; e < HID * k1; e += NTH) {
+        const int j = e / k1, k = e - j * k1;
+        const float x = k < d.obs ? __ldcg(net + d.oW1 + (size_t)j * d.D + k) : 0.f;
+        const int idx = umma::tile_index(j, k, k1);
         t.w1hi[idx] = x; t.w1lo[idx] = tf32_lo(x);
     }
     for (int e = tid; e < HID * HID; e += NTH) {
@@ -179,25 +197,34 @@ __device__ __forceinline__ float adam_math(float w, float &m, float &v, float &x
 }
 
 // t1[64 x 64] = X[rows row0 .. row0 + 64) W1s^T for this warpgroup, X = state (online) or next_state (target).  The rows
-// arrive by coalesced 16-byte cp.async (16 lanes per row) in a staging buffer [64 rows][64 floats] whose 16-byte chunk c
+// arrive by coalesced 16-byte cp.async (16 lanes per row) in staging buffers [64 rows][64 floats] whose 16-byte chunk c
 // of row r sits at chunk position c ^ (r & 7), which makes the fragment reads below (8 rows x 4 consecutive k per warp
-// and load) conflict free; 64 columns of K per pass.
+// and load) conflict free; 64 columns of K per chunk.  Each warpgroup has two buffers, K chunk kc goes to buffer kc & 1:
+// chunk kc + 1 is in flight while chunk kc is multiplied, and chunk 0 of a block is issued by the caller (l1_issue)
+// ahead of layer1_block, as early as its buffer is free.
+__device__ __forceinline__ void l1_issue(const TcArgs &a, const TcLearner &L, const Misc &mi, char *smem, int field_off, int row0, int kc) {
+    const int m = threadIdx.x & 127, g = threadIdx.x >> 7;
+    float *sbuf = reinterpret_cast<float *>(smem + REG2 + g * 2 * SBUF + (kc & 1) * SBUF);
+#pragma unroll 4
+    for (int i = 0; i < 8; i++) {
+        const int item = i * 128 + m, rr = item >> 4, c = item & 15, k = kc * 64 + c * 4;
+        const float *src = reinterpret_cast<const float *>(L.records + (size_t)mi.slot[row0 + rr] * a.lay.record_words) + field_off + k;
+        const int nb = k < a.d.obs ? 16 : 0;
+        cp_async16_zfill_tc(sbuf + rr * 64 + ((c ^ (rr & 7)) << 2), nb ? src : reinterpret_cast<const float *>(L.records), nb);
+    }
+    cp_async_commit();
+}
 __device__ __forceinline__ void layer1_block(const TcArgs &a, const TcLearner &L, const Misc &mi, char *smem, int field_off, int row0,
                                              float (&t1)[32]) {
-    const int m = threadIdx.x & 127, g = threadIdx.x >> 7, t = threadIdx.x & 3;
-    const umma::Tile B_hi = umma::make_tile(smem + REG1, a.d.obs, 128), B_lo = umma::make_tile(smem + REG1 + HALF, a.d.obs, 128);
-    float *sbuf = reinterpret_cast<float *>(smem + REG2 + g * SBUF);
-    for (int kc = 0; kc * 64 < a.d.obs; kc++) {
-#pragma unroll 4
-        for (int i = 0; i < 8; i++) {
-            const int item = i * 128 + m, rr = item >> 4, c = item & 15, k = kc * 64 + c * 4;
-            const float *src = reinterpret_cast<const float *>(L.records + (size_t)mi.slot[row0 + rr] * a.lay.record_words) + field_off + k;
-            const int nb = k < a.d.obs ? 16 : 0;
-            cp_async16_zfill_tc(sbuf + rr * 64 + ((c ^ (rr & 7)) << 2), nb ? src : reinterpret_cast<const float *>(L.records), nb);
-        }
-        cp_async_commit();
-        cp_async_wait<0>();
+    const int g = threadIdx.x >> 7, t = threadIdx.x & 3;
+    const int k1 = k1_cols(a.d.obs);
+    const umma::Tile B_hi = umma::make_tile(smem + REG1, k1, 128), B_lo = umma::make_tile(smem + REG1 + HALF, k1, 128);
+    for (int kc = 0; kc * 64 < k1; kc++) {
+        if ((kc + 1) * 64 < k1) l1_issue(a, L, mi, smem, field_off, row0, kc + 1);
+        else cp_async_commit();          // empty group: the wait below always leaves exactly the newest group in flight
+        cp_async_wait<1>();
         group_sync(g);
+        const float *sbuf = reinterpret_cast<const float *>(smem + REG2 + g * 2 * SBUF + (kc & 1) * SBUF);
         float hi[32], lo[32];
 #pragma unroll
         for (int ks = 0; ks < 8; ks++)
@@ -208,11 +235,10 @@ __device__ __forceinline__ void layer1_block(const TcArgs &a, const TcLearner &L
                     const int r = umma::acc_row(p), k = 8 * ks + t + 4 * q;
                     umma::split_tf32(sbuf[r * 64 + (((k >> 2) ^ (r & 7)) << 2) + (k & 3)], hi[4 * ks + 2 * q + p], lo[4 * ks + 2 * q + p]);
                 }
-        const int keff = min(64, a.d.obs - kc * 64);
-        umma::gemm3_rs<HID, 8>(t1, hi, lo, B_hi.shifted(kc * 2048), B_lo.shifted(kc * 2048), kc > 0, keff >> 3);
+        group_sync(g);   // the buffer is free for chunk kc + 2 (or chunk 0 of the next block)
+        umma::gemm3_rs<HID, 8>(t1, hi, lo, B_hi.shifted(kc * 2048), B_lo.shifted(kc * 2048), kc > 0);
         umma::wg_commit();
         umma::wg_wait<0>();
-        group_sync(g);   // the staging buffer is free for the next pass
     }
 }
 
@@ -226,6 +252,14 @@ __device__ __forceinline__ void acc_to_frag(const float (&v)[32], float (&hi)[32
             for (int e = 0; e < 2; e++) umma::split_tf32(v[4 * j + 2 * p + e], hi[4 * j + 2 * e + p], lo[4 * j + 2 * e + p]);
 }
 
+// A shared-memory load the compiler may not hoist out of a loop: the small vectors (w3, b2, ...) are the same in every
+// action slot / row tile, and keeping them in registers across the loop costs the registers the wgmma chains need.
+__device__ __forceinline__ float2 lds2(const float *p) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(umma::smem_u32(p)));
+    return v;
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -236,29 +270,31 @@ __device__ __forceinline__ float quad_sum(float v) {
     return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// d[64 x n] (+)= A B^T over 64 batch rows, n in {8, 16, 32, 64}
-__device__ __forceinline__ void gemm3_n(int n, float *d, umma::Tile ah, umma::Tile al, umma::Tile bh, umma::Tile bl, bool accumulate) {
-    if (n == 64) umma::gemm3<64>(d, ah, al, bh, bl, 64, accumulate);
-    else if (n == 32) umma::gemm3<32>(d, ah, al, bh, bl, 64, accumulate);
-    else if (n == 16) umma::gemm3<16>(d, ah, al, bh, bl, 64, accumulate);
-    else umma::gemm3<8>(d, ah, al, bh, bl, 64, accumulate);
-}
-__host__ __device__ inline int pow2_cols(int n) { return n > 32 ? 64 : n > 16 ? 32 : n > 8 ? 16 : 8; }
+// dW1s columns per warpgroup: the two warpgroups take equal shares [0, NW) and [NW, 2 NW) of the obs columns
+__host__ __device__ inline int dw1_share(int obs) { return obs > 64 ? 64 : obs > 32 ? 32 : obs > 16 ? 16 : 8; }
 
+__device__ const uint8_t kIota[16] = {0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15};
+
+template <int NW>
 __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     extern __shared__ __align__(1024) char smem[];
     Misc &mi = *reinterpret_cast<Misc *>(smem + MISC_OFF);
-    TcLearner L = a.learners[blockIdx.x];
-    if (a.round0) {   // a later chunk of the same call: shift every per-round array once
-        L.slots += (size_t)a.round0 * a.B;
-        L.scal += a.round0;
-        L.out_mae += a.round0;
-        if (L.out_q) L.out_q += (size_t)a.round0 * a.B;
-        if (L.out_y) L.out_y += (size_t)a.round0 * a.B;
-        L.steps0 += a.round0;
-    }
-    const Dims &d = a.d;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if (tid == 0) {
+        TcLearner L = a.learners[blockIdx.x];
+        if (a.round0) {   // a later chunk of the same call: shift every per-round array once
+            L.slots += (size_t)a.round0 * a.B;
+            L.scal += a.round0;
+            L.out_mae += a.round0;
+            if (L.out_q) L.out_q += (size_t)a.round0 * a.B;
+            if (L.out_y) L.out_y += (size_t)a.round0 * a.B;
+            L.steps0 += a.round0;
+        }
+        mi.L = L;
+    }
+    __syncthreads();
+    const TcLearner &L = mi.L;
+    const Dims &d = a.d;
     const int h = tid >> 7, t4 = tid & 3;
     const int ntiles = a.B >> 7;
     const int W = a.lay.record_words;
@@ -274,12 +310,14 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     if (tid == 0)
         for (int i = 0; i < 3; i++) umma::mbar_init(bar + i, 1);
     // the operand-layout tiles follow the flat parameters (which the host may have changed between calls)
-    const NetTiles To = net_tiles(L.tiles, d.obs), Tt = net_tiles(L.tiles + net_tile_floats(d.obs), d.obs);
-    rebuild_tiles(L.w, d, To, tid);
-    rebuild_tiles(L.wt, d, Tt, tid);
+    auto To = [&] { return net_tiles(L.tiles, d.obs); };
+    auto Tt = [&] { return net_tiles(L.tiles + net_tile_floats(d.obs), d.obs); };
+    rebuild_tiles(L.w, d, To(), tid);
+    rebuild_tiles(L.wt, d, Tt(), tid);
     fence_proxy_async_all();
     __syncthreads();
-    const uint32_t w1_bytes = 64u * d.obs * 4, w2_bytes = 2u * HID * HID * 4;
+    const int k1 = k1_cols(d.obs);
+    const uint32_t w1_bytes = 64u * k1 * 4, w2_bytes = 2u * HID * HID * 4;
     // B-operand tiles of one network by TMA: W1 hi / lo into region 1, the W2 block into region 3
     auto tma_w1 = [&](const NetTiles &t, uint64_t *b) {
         mbar_expect_tx(b, 2 * w1_bytes);
@@ -293,9 +331,6 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     uint32_t par_w1 = 0;   // phase parity of bar[1] (one completion per row tile)
     const umma::Tile W2_hi = umma::make_tile(smem + REG3, 64, 128), W2_lo = umma::make_tile(smem + REG3 + 16384, 64, 128);
     const umma::Tile W2T_hi = umma::make_tile(smem + REG3 + 32768, 64, 128), W2T_lo = umma::make_tile(smem + REG3 + 49152, 64, 128);
-    // weight-gradient products: warpgroup 0 accumulates dW2 (g1) and columns [0, 64) of dW1s (g2), warpgroup 1
-    // [db2 | .] (g1[0..16)), [db1 | dW1a] (g1[16..32)) and columns [64, obs) of dW1s (g2)
-    const int n_dw1 = h == 0 ? pow2_cols(min(d.obs, 64)) : (d.obs > 64 ? pow2_cols(d.obs - 64) : 0);
 
     for (int round = 0; round < a.rounds; round++) {
         TC_STAMP(0);
@@ -331,8 +366,8 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                     *reinterpret_cast<float4 *>(tg_lo + i) = make_float4(tf32_lo(r.x), tf32_lo(r.y), tf32_lo(r.z), tf32_lo(r.w));
                 }
             };
-            update_tile(To.w1hi, Tt.w1hi, Tt.w1lo, HID * d.obs);
-            update_tile(To.w2, Tt.w2, Tt.w2 + HID * HID, HID * HID);
+            update_tile(To().w1hi, Tt().w1hi, Tt().w1lo, HID * k1);
+            update_tile(To().w2, Tt().w2, Tt().w2 + HID * HID, HID * HID);
             fence_proxy_async_all();
         }
         __syncthreads();
@@ -341,10 +376,11 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
         TC_STAMP(1);
         if (tid == 0) {   // target tiles: three TMA bulk copies (regions 1 and 3 are free: every product of the last round was waited for)
             mbar_expect_tx(bar + 0, 2 * w1_bytes + w2_bytes);
-            bulk_g2s(smem + REG1, Tt.w1hi, w1_bytes, bar + 0);
-            bulk_g2s(smem + REG1 + HALF, Tt.w1lo, w1_bytes, bar + 0);
-            bulk_g2s(smem + REG3, Tt.w2, w2_bytes, bar + 0);
+            bulk_g2s(smem + REG1, Tt().w1hi, w1_bytes, bar + 0);
+            bulk_g2s(smem + REG1 + HALF, Tt().w1lo, w1_bytes, bar + 0);
+            bulk_g2s(smem + REG3, Tt().w2, w2_bytes, bar + 0);
         }
+        l1_issue(a, L, mi, smem, a.lay.off_next_state, h * 64, 0);
         if (soft_upd || round == 0) load_smalls(L.wt, d, mi.sm[1]);   // the target's small vectors only change at a soft update
         umma::mbar_wait(bar + 0, round & 1);
         __syncthreads();
@@ -353,6 +389,9 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             const int row0 = i * 128 + h * 64;
             float t1[32];
             layer1_block(a, L, mi, smem, a.lay.off_next_state, row0, t1);
+            // chunk 0 of the next layer-1 block (the next row tile, or phase O's first) loads during the action loop
+            if (i + 1 < ntiles) l1_issue(a, L, mi, smem, a.lay.off_next_state, row0 + 128, 0);
+            else l1_issue(a, L, mi, smem, a.lay.off_state, h * 64, 0);
             const int rows[2] = {row0 + rA, row0 + rB};
             int cnt[2];
             const uint8_t *ids[2];
@@ -360,17 +399,18 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
 #pragma unroll
             for (int p = 0; p < 2; p++) {
                 cnt[p] = mi.cnt[rows[p]];
-                ids[p] = reinterpret_cast<const uint8_t *>(L.records + (size_t)mi.slot[rows[p]] * W + a.lay.off_avail);
+                ids[p] = (L.buf_flags & PRL_BUF_DYNAMIC_ACTIONS) ? reinterpret_cast<const uint8_t *>(L.records + (size_t)mi.slot[rows[p]] * W + a.lay.off_avail)
+                                                                : kIota;
             }
             for (int act = 0; act < d.A; act++) {
                 float hi[32], lo[32], acc[32];
 #pragma unroll
                 for (int p = 0; p < 2; p++) {
-                    int id = act;
-                    if ((L.buf_flags & PRL_BUF_DYNAMIC_ACTIONS) && act < cnt[p]) id = ids[p][act];
+                    // a select, not a branch: a conditional load here made ptxas serialise the kernel's wgmma (C7520)
+                    const int id_l = ids[p][act], id = act < cnt[p] ? id_l : act;
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
-                        const float2 wv = *reinterpret_cast<const float2 *>(&mi.sm[1].watb[id][8 * j + 2 * t4]);
+                        const float2 wv = lds2(&mi.sm[1].watb[id][8 * j + 2 * t4]);
                         umma::split_tf32(fmaxf(t1[4 * j + 2 * p] + wv.x, 0.f), hi[4 * j + p], lo[4 * j + p]);
                         umma::split_tf32(fmaxf(t1[4 * j + 2 * p + 1] + wv.y, 0.f), hi[4 * j + 2 + p], lo[4 * j + 2 + p]);
                     }
@@ -381,8 +421,8 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 float q[2] = {0.f, 0.f};
 #pragma unroll
                 for (int j = 0; j < 8; j++) {
-                    const float2 w3v = *reinterpret_cast<const float2 *>(&mi.sm[1].w3[8 * j + 2 * t4]);
-                    const float2 b2v = *reinterpret_cast<const float2 *>(&mi.sm[1].b2[8 * j + 2 * t4]);
+                    const float2 w3v = lds2(&mi.sm[1].w3[8 * j + 2 * t4]);
+                    const float2 b2v = lds2(&mi.sm[1].b2[8 * j + 2 * t4]);
 #pragma unroll
                     for (int p = 0; p < 2; p++) {
                         q[p] = fmaf(w3v.x, fmaxf(acc[4 * j + 2 * p] + b2v.x, 0.f), q[p]);
@@ -405,7 +445,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
 
         // ================= phase O: online forward, loss, backward =================
         TC_STAMP(3);
-        if (tid == 0) { tma_w1(To, bar + 1); tma_w2(To, bar + 2); }
+        if (tid == 0) { tma_w1(To(), bar + 1); tma_w2(To(), bar + 2); }
         load_smalls(L.w, d, mi.sm[0]);
         umma::mbar_wait(bar + 2, round & 1);
         {   // W2^T tiles (B operand of dH1 = dZ2 W2, contraction over W2's rows) out of the W2 tiles
@@ -418,20 +458,24 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             umma::fence_async_smem();
         }
         TC_STAMP(4);
-        float dw3[16], g1[32], g2[32];
+        // weight-gradient accumulators; both warpgroups issue the same products on different output columns:
+        // gw2 = dW2 columns [32 h, 32 h + 32), gb2 = [db2 | .] (column 0 of dZ2^T E, the same on both warpgroups),
+        // gw1 = dW1s columns [NW h, NW h + NW), gba = [db1 | dW1a] columns [16 h, 16 h + 16) (0 = bias, 1 + k = action k)
+        float gw2[16], gb2[4], gw1[NW / 2], gba[8];
         float mae_acc = 0.f, db3_acc = 0.f;
-#pragma unroll
-        for (int c = 0; c < 16; c++) dw3[c] = 0.f;
         float *arena = reinterpret_cast<float *>(smem);
         const umma::Tile TA_hi = umma::make_tile(smem + AR_A_HI, 64, TL), TA_lo = umma::make_tile(smem + AR_A_LO, 64, TL);
         const umma::Tile TB_hi = umma::make_tile(smem + AR_B_HI, 64, TL), TB_lo = umma::make_tile(smem + AR_B_LO, 64, TL);
         const umma::Tile TE = umma::make_tile(smem + AR_E, 64, TL);
         for (int i = 0; i < ntiles; i++) {
-            if (i > 0 && tid == 0) tma_w1(To, bar + 1);   // the arena of the last tile overwrote region 1
+            const int row0 = i * 128 + h * 64;
+            if (i > 0) {   // the arena of the last tile overwrote regions 1 and 2 (tile 0's first chunk was issued in phase T)
+                if (tid == 0) tma_w1(To(), bar + 1);
+                l1_issue(a, L, mi, smem, a.lay.off_state, row0, 0);
+            }
             umma::mbar_wait(bar + 1, par_w1);
             par_w1 ^= 1;
             __syncthreads();   // also: the W2^T tiles are complete
-            const int row0 = i * 128 + h * 64;
             const int rows[2] = {row0 + rA, row0 + rB};
             float h1[32], z[32], hi[32], lo[32];
             layer1_block(a, L, mi, smem, a.lay.off_state, row0, h1);
@@ -442,11 +486,17 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 ai[p] = mi.act[rows[p]];
 #pragma unroll
                 for (int j = 0; j < 8; j++) {
-                    const float2 wv = *reinterpret_cast<const float2 *>(&mi.sm[0].watb[ai[p]][8 * j + 2 * t4]);
+                    const float2 wv = lds2(&mi.sm[0].watb[ai[p]][8 * j + 2 * t4]);
                     h1[4 * j + 2 * p] = fmaxf(h1[4 * j + 2 * p] + wv.x, 0.f);
                     h1[4 * j + 2 * p + 1] = fmaxf(h1[4 * j + 2 * p + 1] + wv.y, 0.f);
                 }
             }
+            // H1 and dZ2 wait in this warpgroup's (free) staging buffers while dZ2 and dH1 are formed: values that stay live
+            // across a wgmma chain besides its own operands cost the registers the chain needs, and ptxas serialises every
+            // wgmma of the kernel when a chain does not fit (C7511)
+            float *h1s = reinterpret_cast<float *>(smem + REG2 + h * 2 * SBUF) + (tid & 127);
+#pragma unroll
+            for (int c = 0; c < 32; c++) h1s[c * 128] = h1[c];
             acc_to_frag(h1, hi, lo);
             umma::gemm3_rs<HID, 8>(z, hi, lo, W2_hi, W2_lo, false);
             umma::wg_commit();
@@ -454,8 +504,8 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             float part[2] = {0.f, 0.f}, dq[2];
 #pragma unroll
             for (int j = 0; j < 8; j++) {
-                const float2 w3v = *reinterpret_cast<const float2 *>(&mi.sm[0].w3[8 * j + 2 * t4]);
-                const float2 b2v = *reinterpret_cast<const float2 *>(&mi.sm[0].b2[8 * j + 2 * t4]);
+                const float2 w3v = lds2(&mi.sm[0].w3[8 * j + 2 * t4]);
+                const float2 b2v = lds2(&mi.sm[0].b2[8 * j + 2 * t4]);
 #pragma unroll
                 for (int p = 0; p < 2; p++) {
                     z[4 * j + 2 * p] = fmaxf(z[4 * j + 2 * p] + b2v.x, 0.f);
@@ -479,9 +529,9 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             // dW3 partial sums over this thread's two rows, then dZ2 in place of h2
 #pragma unroll
             for (int j = 0; j < 8; j++) {
-                const float2 w3v = *reinterpret_cast<const float2 *>(&mi.sm[0].w3[8 * j + 2 * t4]);
-                dw3[2 * j] += dq[0] * z[4 * j] + dq[1] * z[4 * j + 2];
-                dw3[2 * j + 1] += dq[0] * z[4 * j + 1] + dq[1] * z[4 * j + 3];
+                const float2 w3v = lds2(&mi.sm[0].w3[8 * j + 2 * t4]);
+                mi.dw3[2 * j][tid] = (i == 0 ? 0.f : mi.dw3[2 * j][tid]) + (dq[0] * z[4 * j] + dq[1] * z[4 * j + 2]);
+                mi.dw3[2 * j + 1][tid] = (i == 0 ? 0.f : mi.dw3[2 * j + 1][tid]) + (dq[0] * z[4 * j + 1] + dq[1] * z[4 * j + 3]);
 #pragma unroll
                 for (int p = 0; p < 2; p++) {
                     z[4 * j + 2 * p] = z[4 * j + 2 * p] > 0.f ? dq[p] * w3v.x : 0.f;
@@ -489,12 +539,18 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 }
             }
             float dz1[32];
+#pragma unroll
+            for (int c = 0; c < 32; c++) h1s[(32 + c) * 128] = z[c];   // dZ2 waits there too
             acc_to_frag(z, hi, lo);
             umma::gemm3_rs<HID, 8>(dz1, hi, lo, W2T_hi, W2T_lo, false);   // dH1 = dZ2 W2
             umma::wg_commit();
             umma::wg_wait<0>();
 #pragma unroll
-            for (int c = 0; c < 32; c++) dz1[c] = (h1[c] > 0.f) ? dz1[c] : 0.f;
+            for (int c = 0; c < 32; c++) {
+                h1[c] = h1s[c * 128];
+                z[c] = h1s[(32 + c) * 128];
+                dz1[c] = (h1[c] > 0.f) ? dz1[c] : 0.f;
+            }
             if (i == 0) TC_STAMP(6);
 
             // ---- weight gradients: contractions over the batch rows, 64 rows (one warpgroup's block) per pass
@@ -523,8 +579,8 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 }
                 umma::fence_async_smem();
                 __syncthreads();
-                if (h == 0) umma::gemm3<64>(g1, TA_hi, TA_lo, TB_hi, TB_lo, 64, !first);
-                else umma::gemm3<32>(g1, TA_hi, TA_lo, TE, TE, 64, !first, false, true);
+                umma::gemm3<32>(gw2, TA_hi, TA_lo, TB_hi.rows_from(32 * h), TB_lo.rows_from(32 * h), 64, !first);
+                umma::gemm3<8>(gb2, TA_hi, TA_lo, TE, TE, 64, !first, false, true);
                 umma::wg_commit();
                 // S^T: every warp reads whole state rows of this half coalesced (lane = k) and scatters them into column rq of
                 // the transposed tile; the first four rows are requested BEFORE waiting for the dW2 product
@@ -569,8 +625,8 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 st_rows_scatter(4);
                 umma::fence_async_smem();
                 __syncthreads();
-                if (n_dw1) gemm3_n(n_dw1, g2, TA_hi, TA_lo, TB_hi.rows_from(64 * h), TB_lo.rows_from(64 * h), !first);
-                if (h == 1) umma::gemm3<32>(g1 + 16, TA_hi, TA_lo, TE, TE, 64, !first, false, true);
+                umma::gemm3<NW>(gw1, TA_hi, TA_lo, TB_hi.rows_from(NW * h), TB_lo.rows_from(NW * h), 64, !first);
+                umma::gemm3<16>(gba, TA_hi, TA_lo, TE.rows_from(16 * h), TE.rows_from(16 * h), 64, !first, false, true);
                 umma::wg_commit();
                 umma::wg_wait<0>();
             }
@@ -583,7 +639,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
         // column sums of dW3 over the warp's rows: lanes with equal lane % 4 hold the same columns
 #pragma unroll
         for (int c = 0; c < 16; c++) {
-            float v = dw3[c];
+            float v = mi.dw3[c][tid];
             v += __shfl_xor_sync(0xffffffffu, v, 4);
             v += __shfl_xor_sync(0xffffffffu, v, 8);
             v += __shfl_xor_sync(0xffffffffu, v, 16);
@@ -603,17 +659,26 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             for (int p = 0; p < 2; p++) {
                 const int j = p ? rB : rA;                             // the gradient's row = hidden unit
 #pragma unroll
-                for (int jb = 0; jb < 8; jb++)
+                for (int jb = 0; jb < 4; jb++)
 #pragma unroll
                     for (int e = 0; e < 2; e++) {
-                        const int c = 8 * jb + 2 * t4 + e, k = 64 * h + c;
-                        if (h == 0) gs_w2[j * 65 + c] = g1[4 * jb + 2 * p + e];
-                        if (c < n_dw1 && k < d.obs) gs_w1[j * pitch1 + k] = g2[4 * jb + 2 * p + e];
-                        if (h == 1 && jb < 4) {                        // [db | dW1a] columns: 0 = bias, 1 + k = action k
-                            if (c == 0) { gs_b2[j] = g1[4 * jb + 2 * p + e]; gs_b1[j] = g1[16 + 4 * jb + 2 * p + e]; }
-                            else if (c - 1 < d.A) gs_w1[j * pitch1 + d.obs + c - 1] = g1[16 + 4 * jb + 2 * p + e];
+                        const int c = 8 * jb + 2 * t4 + e, x = 4 * jb + 2 * p + e;
+                        gs_w2[j * 65 + 32 * h + c] = gw2[x];
+                        if (jb < NW / 8 && NW * h + c < d.obs) gs_w1[j * pitch1 + NW * h + c] = gw1[x];
+                        if (jb < 2) {
+                            const int ce = 16 * h + c;
+                            if (ce == 0) gs_b1[j] = gba[x];
+                            else if (ce - 1 < d.A) gs_w1[j * pitch1 + d.obs + ce - 1] = gba[x];
                         }
                     }
+#pragma unroll
+                for (int jb = 4; jb < NW / 8; jb++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const int k = NW * h + 8 * jb + 2 * t4 + e;
+                        if (k < d.obs) gs_w1[j * pitch1 + k] = gw1[4 * jb + 2 * p + e];
+                    }
+                if (h == 0 && t4 == 0) gs_b2[j] = gb2[2 * p];
             }
             __syncthreads();
             // 2) AdamW over the flat parameter vector, all 256 threads, fully coalesced 16-byte accesses.  The sweep is bound by
@@ -682,16 +747,16 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                             // the same values in the operand-layout tiles (hi = the value, lo = residual)
                             if (is_w1) {
                                 if (c < d.obs) {
-                                    const int ti = umma::tile_index(row, c, d.obs);
-                                    *reinterpret_cast<float4 *>(To.w1hi + ti) = w;
-                                    *reinterpret_cast<float4 *>(To.w1lo + ti) = make_float4(tf32_lo(w.x), tf32_lo(w.y), tf32_lo(w.z), tf32_lo(w.w));
+                                    const int ti = umma::tile_index(row, c, k1);
+                                    *reinterpret_cast<float4 *>(To().w1hi + ti) = w;
+                                    *reinterpret_cast<float4 *>(To().w1lo + ti) = make_float4(tf32_lo(w.x), tf32_lo(w.y), tf32_lo(w.z), tf32_lo(w.w));
                                 }
                             } else {   // kperm order: columns c, c + 2 and c + 1, c + 3 are neighbours
                                 const int te = umma::tile_index(row, umma::kperm(c), HID), to = umma::tile_index(row, umma::kperm(c + 1), HID);
-                                *reinterpret_cast<float2 *>(To.w2 + te) = make_float2(w.x, w.z);
-                                *reinterpret_cast<float2 *>(To.w2 + to) = make_float2(w.y, w.w);
-                                *reinterpret_cast<float2 *>(To.w2 + 4096 + te) = make_float2(tf32_lo(w.x), tf32_lo(w.z));
-                                *reinterpret_cast<float2 *>(To.w2 + 4096 + to) = make_float2(tf32_lo(w.y), tf32_lo(w.w));
+                                *reinterpret_cast<float2 *>(To().w2 + te) = make_float2(w.x, w.z);
+                                *reinterpret_cast<float2 *>(To().w2 + to) = make_float2(w.y, w.w);
+                                *reinterpret_cast<float2 *>(To().w2 + 4096 + te) = make_float2(tf32_lo(w.x), tf32_lo(w.z));
+                                *reinterpret_cast<float2 *>(To().w2 + 4096 + to) = make_float2(tf32_lo(w.y), tf32_lo(w.w));
                             }
                         }
                     }
@@ -711,7 +776,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                     L.m[i] = mm; L.v[i] = vv; L.vmax[i] = xx;
                 }
                 __syncthreads();
-                rebuild_tiles(L.w, d, To, tid);         // unaligned shapes (D % 4 != 0): tiles from the flat vector
+                rebuild_tiles(L.w, d, To(), tid);         // unaligned shapes (D % 4 != 0): tiles from the flat vector
             }
             fence_proxy_async_all();                    // the tile writes are read by TMA in the next round
             if (si >= 0) {
@@ -848,7 +913,9 @@ extern "C" int prl_dqn_learn_multi(prl_dqn *const *dqns, prl_buf *const *bufs, i
     { static const int c = [] { const char *e = getenv("PRL_TC_PROF_CTA"); return e ? atoi(e) : 0; }(); a.prof_cta = c; }
     const size_t smem = MISC_OFF + sizeof(Misc);
     PRL_REQUIRE(smem <= (size_t)q0->max_smem, "tensor-core learner needs %zu B of shared memory", smem);
-    PRL_CUDA(cudaFuncSetAttribute(k_dqn_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const int nw = dw1_share(c.obs_dim);
+    void (*const kern)(TcArgs) = nw == 64 ? k_dqn_tc<64> : nw == 32 ? k_dqn_tc<32> : nw == 16 ? k_dqn_tc<16> : k_dqn_tc<8>;
+    PRL_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 
     // The index streams are produced in chunks of rounds: chunk 0 ahead of the first learner launch, chunk c + 1 on a
     // side stream WHILE the learners run chunk c (one learner CTA fills an SM, so the producers of the next chunk run
@@ -879,7 +946,7 @@ extern "C" int prl_dqn_learn_multi(prl_dqn *const *dqns, prl_buf *const *bufs, i
         const int r0 = chunk_begin(cix), r1 = chunk_begin(cix + 1);
         if (cix > 0) PRL_CUDA(cudaStreamWaitEvent(stream, ev_idx[cix], 0));
         a.round0 = r0; a.rounds = r1 - r0;
-        k_dqn_tc<<<count, NTH, smem, stream>>>(a);
+        kern<<<count, NTH, smem, stream>>>(a);
         PRL_CUDA(cudaGetLastError());
         if (cix + 1 < nchunks) {
             const int n0 = r1, n1 = chunk_begin(cix + 2);

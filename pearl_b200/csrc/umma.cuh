@@ -168,7 +168,8 @@ __device__ __forceinline__ void gemm3(float *d, Tile a_hi, Tile a_lo, Tile b_hi,
 }
 
 // 3xTF32, RS form: a_hi / a_lo hold this thread's A fragments of (at most) KSTEPS K steps (4 registers each).  The registers
-// must not be written again before the products have been waited for.
+// must not be written again before the products have been waited for.  A runtime ksteps < KSTEPS puts a branch into the
+// chain, and ptxas then serialises every wgmma of the kernel: pipelined kernels leave it at KSTEPS.
 template <int N, int KSTEPS>
 __device__ __forceinline__ void gemm3_rs(float *d, const float *a_hi, const float *a_lo, Tile b_hi, Tile b_lo, bool accumulate_first,
                                          int ksteps = KSTEPS) {
@@ -190,8 +191,9 @@ __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// Bounded spin: a wait that cannot complete (protocol bug, lost TMA transaction) ends the kernel with a trap and a
-// message instead of hanging the device — over a second of polling, orders of magnitude beyond any legitimate wait.
+// Bounded spin: a wait that cannot complete (protocol bug, lost TMA transaction) ends the kernel with a trap instead of
+// hanging the device — over a second of polling, orders of magnitude beyond any legitimate wait.  No printf here: a
+// function call anywhere in a kernel makes ptxas serialise every wgmma of that kernel (warning C7510).
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
     const uint32_t a = smem_u32(bar);
     uint32_t done;
@@ -207,8 +209,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         if (!done) {
             if (t0 == 0) t0 = clock64();
             if (clock64() - t0 < 3000000000ll) continue;   // ~1.5 s of SM clocks
-            printf("pearl_b200: mbarrier wait timed out: block %d thread %d barrier@%u parity %u\n", (int)blockIdx.x,
-                   (int)threadIdx.x, a, parity);
             __trap();
         }
     } while (!done);
