@@ -7,17 +7,24 @@ W2 [h2, h1], b2, W3 [1, h2], b3.  One step of DeepQLearning.learn_batch on a bat
     q_i = Q(s_i, a_i)
     y_i = max over the available a' of Q_target(s'_i, a') * gamma * (1 - terminated_i) + r_i   (unavailable: -inf;
           `truncated` plays no part, as in the reference)
-    loss = mean((q - y)^2), and its gradient with respect to the seven parameter blocks.
+    DoubleDQN: y_i = Q_target(s'_i, a*_i) * gamma * (1 - terminated_i) + r_i, a*_i = the first arg-max over the
+          available slots of the ONLINE Q(s'_i, .)
+    loss = mean(w_i (q_i - y_i)^2) (w = 1 without importance weights), and its gradient with respect to the seven
+          parameter blocks.
 
 Everything is written as explicit formulas, not autograd, so that the SAME code applied to |.| of every operand gives
 the error scale of each result: the sum of |a||b| over every product that contributed to it, carried through the chain
 (the natural scale of a rounding error in a chain of dot products).  ReLU is the identity on non-negative values and
 the ReLU derivatives are the masks of the value pass, so they need no special case.  The one change is the loss
-derivative: |dq_i| becomes |dq_i| + (2 / B) (scale(q_i) + scale(y_i)), so that a row with q ~ y is judged by the
-rounding noise of q - y and not by its own tiny value.
+derivative: |dq_i| becomes w_i (|q_i - y_i| + scale(q_i) + scale(y_i)) 2 / B, so that a row with q ~ y is judged by
+the rounding noise of q - y and not by its own tiny value.  The arg-max of DoubleDQN is not continuous: a row whose
+top two online values are closer than a kernel's rounding (next_action_gap) has to be left out of a comparison.
+
+make_data and check are the data builder and the elementwise comparison of the GPU shape tests.
 """
 from __future__ import annotations
 
+import numpy as np
 import torch
 
 BLOCKS = ("dW1s", "dW1a", "db1", "dW2", "db2", "dW3", "db3")
@@ -51,16 +58,32 @@ def _forward(net, state, onehot):
     return z1, h1, z2, h2, h2 @ W3[0] + b3[0]
 
 
-def _target(net, next_state, avail_ids, avail_n, gamma, terminated, reward):
-    """y per row: the max over the first avail_n[i] entries of avail_ids[i] of Q_target(s'_i, .), then the TD target."""
+def _next_q(net, next_state, avail_ids, avail_n):
+    """Q(s'_i, avail_ids[i, k]) for every slot k of every row, -inf at the slots k >= avail_n[i]."""
     B, A = avail_ids.shape
     eye = torch.eye(A, dtype=next_state.dtype, device=next_state.device)
     onehot = eye[avail_ids.reshape(-1)]                                        # [B * A, A]
     s = next_state.repeat_interleave(A, dim=0)
     v = _forward(net, s, onehot)[4].view(B, A)
     slot = torch.arange(A, device=v.device).view(1, A)
-    v = v.masked_fill(slot >= avail_n.view(B, 1), float("-inf"))
-    return v.max(1)[0] * gamma * (1.0 - terminated) + reward
+    return v.masked_fill(slot >= avail_n.view(B, 1), float("-inf"))
+
+
+def _target(net, next_state, avail_ids, avail_n, gamma, terminated, reward, a_star=None):
+    """y per row: the max over the first avail_n[i] entries of avail_ids[i] of Q_target(s'_i, .), then the TD target;
+    with `a_star` (DoubleDQN's chosen action id per row) Q_target(s'_i, a_star[i]) instead of the max."""
+    if a_star is None:
+        v = _next_q(net, next_state, avail_ids, avail_n).max(1)[0]
+    else:
+        eye = torch.eye(avail_ids.shape[1], dtype=next_state.dtype, device=next_state.device)
+        v = _forward(net, next_state, eye[a_star])[4]
+    return v * gamma * (1.0 - terminated) + reward
+
+
+def _double_action(net, next_state, avail_ids, avail_n):
+    """DoubleDQN's a*: the action id at the first arg-max slot of the online Q(s', .) over the available slots."""
+    slot = _next_q(net, next_state, avail_ids, avail_n).max(1)[1]
+    return avail_ids.gather(1, slot.view(-1, 1)).view(-1)
 
 
 def _backward(net, state, onehot, m1, m2, h1, h2, dq) -> dict:
@@ -72,30 +95,36 @@ def _backward(net, state, onehot, m1, m2, h1, h2, dq) -> dict:
                 dW3=(dq @ h2).view(1, -1), db3=dq.sum().view(1))
 
 
-def dqn_step(w, wt, batch: dict, obs: int, n_actions: int, gamma: float, hidden=(64, 64)) -> tuple:
+def dqn_step(w, wt, batch: dict, obs: int, n_actions: int, gamma: float, hidden=(64, 64), double: bool = False,
+             weight=None) -> tuple:
     """One DQN step in float64.  `w`, `wt`: flat online / target parameters.  `batch`: state [B, obs], action [B] ids,
     reward [B], terminated [B], next_state [B, obs], avail_ids [B, A] (ids of the available next actions first),
-    avail_n [B] (how many are available).  Returns (value, scale): two dicts with q, y, z1, z2 [B, h], mae (the
-    reported loss, mean |q - y|), loss (mean (q - y)^2), grad (flat, torch order) and the seven blocks of BLOCKS."""
-    f64 = lambda x: torch.as_tensor(x).to(torch.float64)
+    avail_n [B] (how many are available).  `double`: DoubleDQN's target.  `weight` [B]: importance weights of a
+    prioritized draw (dq_i and its scale are multiplied by w_i; mae stays the unweighted mean |q - y|).  Runs on the
+    device of `w`.  Returns (value, scale): two dicts with q, y, z1, z2 [B, h], mae (the reported loss, mean |q - y|),
+    loss (mean w (q - y)^2), grad (flat, torch order) and the seven blocks of BLOCKS."""
+    dev = torch.as_tensor(w).device
+    f64 = lambda x: torch.as_tensor(x).to(device=dev, dtype=torch.float64)
     state, next_state = f64(batch["state"]), f64(batch["next_state"])
     reward, term = f64(batch["reward"]), f64(batch["terminated"])
-    action = torch.as_tensor(batch["action"]).long().to(state.device)
-    avail_ids = torch.as_tensor(batch["avail_ids"]).long().to(state.device)
-    avail_n = torch.as_tensor(batch["avail_n"]).long().to(state.device)
+    action = torch.as_tensor(batch["action"]).long().to(dev)
+    avail_ids = torch.as_tensor(batch["avail_ids"]).long().to(dev)
+    avail_n = torch.as_tensor(batch["avail_n"]).long().to(dev)
     B = state.shape[0]
-    onehot = torch.eye(n_actions, dtype=torch.float64, device=state.device)[action]
-    net, net_t = unflatten(w, obs, n_actions, hidden), unflatten(wt, obs, n_actions, hidden)
+    onehot = torch.eye(n_actions, dtype=torch.float64, device=dev)[action]
+    net, net_t = unflatten(f64(w), obs, n_actions, hidden), unflatten(f64(wt), obs, n_actions, hidden)
     absnet, absnet_t = tuple(p.abs() for p in net), tuple(p.abs() for p in net_t)
+    a_star = _double_action(net, next_state, avail_ids, avail_n) if double else None
 
     z1, h1, z2, h2, q = _forward(net, state, onehot)
-    y = _target(net_t, next_state, avail_ids, avail_n, gamma, term, reward)
+    y = _target(net_t, next_state, avail_ids, avail_n, gamma, term, reward, a_star)
     m1, m2 = (z1 > 0).to(torch.float64), (z2 > 0).to(torch.float64)
     sz1, sh1, sz2, sh2, sq = _forward(absnet, state.abs(), onehot)
-    sy = _target(absnet_t, next_state.abs(), avail_ids, avail_n, gamma, term, reward.abs())
+    sy = _target(absnet_t, next_state.abs(), avail_ids, avail_n, gamma, term, reward.abs(), a_star)
 
-    dq = (q - y) * (2.0 / B)
-    sdq = dq.abs() + (2.0 / B) * (sq + sy)
+    wgt = torch.ones(B, dtype=torch.float64, device=dev) if weight is None else f64(weight)
+    dq = wgt * (q - y) * (2.0 / B)
+    sdq = wgt * ((q - y).abs() + sq + sy) * (2.0 / B)
     g = _backward(net, state, onehot, m1, m2, h1, h2, dq)
     sg = _backward(absnet, state.abs(), onehot, m1, m2, sh1, sh2, sdq)
 
@@ -105,20 +134,41 @@ def dqn_step(w, wt, batch: dict, obs: int, n_actions: int, gamma: float, hidden=
                                  d["db2"], d["dW3"].reshape(-1), d["db3"]])
         return out
 
-    value = pack(g, q, y, z1, z2, (q - y).abs().mean(), ((q - y) ** 2).mean())
-    scale = pack(sg, sq, sy, sz1, sz2, (sq + sy).mean(), (2 * (q - y).abs() * (sq + sy)).mean())
+    value = pack(g, q, y, z1, z2, (q - y).abs().mean(), (wgt * (q - y) ** 2).mean())
+    scale = pack(sg, sq, sy, sz1, sz2, (sq + sy).mean(), (2 * wgt * (q - y).abs() * (sq + sy)).mean())
     return value, scale
 
 
 def relu_margin(w, state, action, obs: int, n_actions: int, hidden=(64, 64)) -> torch.Tensor:
     """Per row: the smallest |pre-activation| / scale over both hidden layers of the network `w` at (state, action).  A
-    row whose margin exceeds a kernel's relative rounding error has the same ReLU derivatives in the kernel as here."""
-    state = torch.as_tensor(state).to(torch.float64)
-    onehot = torch.eye(n_actions, dtype=torch.float64)[torch.as_tensor(action).long()]
-    net = unflatten(torch.as_tensor(w).cpu(), obs, n_actions, hidden)
+    row whose margin exceeds a kernel's relative rounding error has the same ReLU derivatives in the kernel as here.
+    Runs on the device of `w`; returns a CPU tensor."""
+    w = torch.as_tensor(w)
+    state = torch.as_tensor(state).to(device=w.device, dtype=torch.float64)
+    onehot = torch.eye(n_actions, dtype=torch.float64, device=w.device)[torch.as_tensor(action).long().to(w.device)]
+    net = unflatten(w, obs, n_actions, hidden)
     z1, _, z2, _, _ = _forward(net, state, onehot)
     s1, _, s2, _, _ = _forward(tuple(p.abs() for p in net), state.abs(), onehot)
-    return torch.minimum((z1.abs() / s1).min(1)[0], (z2.abs() / s2).min(1)[0])
+    return torch.minimum((z1.abs() / s1).min(1)[0], (z2.abs() / s2).min(1)[0]).cpu()
+
+
+def next_action_gap(w, next_state, avail_ids, avail_n, obs: int, n_actions: int, hidden=(64, 64)) -> torch.Tensor:
+    """Per row: (top-1 - top-2) of the online Q(s', .) of the network `w` over the available slots, over the sum of the
+    two values' error scales; inf where only one action is available.  A DoubleDQN row whose gap exceeds a kernel's
+    relative rounding error picks the same a* in the kernel as here.  Runs on the device of `w`; returns a CPU tensor."""
+    w = torch.as_tensor(w)
+    dev = w.device
+    next_state = torch.as_tensor(next_state).to(device=dev, dtype=torch.float64)
+    avail_ids = torch.as_tensor(avail_ids).long().to(dev)
+    avail_n = torch.as_tensor(avail_n).long().to(dev)
+    if n_actions < 2:
+        return torch.full((next_state.shape[0],), float("inf"), dtype=torch.float64)
+    net = unflatten(w, obs, n_actions, hidden)
+    v = _next_q(net, next_state, avail_ids, avail_n)
+    sv = _next_q(tuple(p.abs() for p in net), next_state.abs(), avail_ids, avail_n)
+    top, slot = v.topk(2, dim=1)
+    gap = (top[:, 0] - top[:, 1]) / (sv.gather(1, slot).sum(1))
+    return torch.where(avail_n > 1, gap, float("inf")).cpu()
 
 
 def err_over_scale(got, want, scale) -> torch.Tensor:
@@ -146,3 +196,67 @@ def block_view(flat: torch.Tensor, name: str, obs: int, n_actions: int, hidden=(
     """Block `name` of a flat torch-order vector as a [rows, cols] tensor."""
     off, rows, cols, col0, pitch = block_slices(obs, n_actions, hidden)[name]
     return flat[off:off + rows * pitch].view(rows, pitch)[:, col0:col0 + cols]
+
+
+def make_data(w, obs: int, n_actions: int, B: int, seed: int, dynamic: bool, margin: float, hidden=(64, 64),
+              double: bool = False) -> dict:
+    """2 B + 16 transitions (host tensors, push order) for a shape test of a learner with online parameters `w`:
+    about 20 % terminal, some truncated, random actions, full or (`dynamic`) random next-action sets.  A row is kept
+    only if every online pre-activation clears `margin` of its scale (relu_margin) and, for DoubleDQN, the online
+    next-action gap clears it too (next_action_gap), so a kernel's rounding cannot flip a ReLU derivative or a*.
+    Candidates are drawn in batches of 3 (2 B + 16) until enough rows are kept; the fp64 filters run on the device of
+    `w`."""
+    from oracle.synth import make_transitions
+    n = 2 * B + 16
+    keys = ("state", "action", "reward", "next_state", "terminated", "truncated", "next_avail_ids", "next_avail_n")
+    kept = {k: [] for k in keys}
+    have = 0
+    for attempt in range(20):
+        s = seed + 1000003 * attempt
+        d = make_transitions(3 * n, obs, n_actions, seed=s, dynamic=dynamic, p_term=0.2)
+        rng = np.random.default_rng(s)
+        d["action"] = rng.integers(0, n_actions, 3 * n)
+        d["truncated"] = rng.random(3 * n) < 0.1
+        if not dynamic:
+            d["next_avail_ids"] = np.tile(np.arange(n_actions), (3 * n, 1))
+            d["next_avail_n"] = np.full(3 * n, n_actions)
+        ok = relu_margin(w, d["state"], d["action"], obs, n_actions, hidden) >= margin
+        if double:
+            ok &= next_action_gap(w, d["next_state"], d["next_avail_ids"], d["next_avail_n"], obs, n_actions,
+                                  hidden) >= margin
+        keep = np.flatnonzero(ok.numpy())[:n - have]
+        for k in keys:
+            kept[k].append(d[k][keep])
+        have += keep.size
+        if have == n:
+            break
+    assert have == n, "too few rows clear the margin"
+    cat = {k: torch.from_numpy(np.concatenate(v)) for k, v in kept.items()}
+    return dict(state=cat["state"], action=cat["action"], reward=cat["reward"], next_state=cat["next_state"],
+                terminated=cat["terminated"], truncated=cat["truncated"], avail_ids=cat["next_avail_ids"],
+                avail_n=cat["next_avail_n"])
+
+
+def check(what, got, want, scale, worst: dict, bound: float) -> None:
+    """|got - want| <= bound * scale elementwise (got: a kernel's values, want / scale: fp64 value and error scale).
+    Records the largest err / scale in worst[what]; raises AssertionError naming the first element that exceeds it."""
+    want, scale = want.cpu(), scale.cpu()
+    got = torch.as_tensor(got).detach().cpu().to(torch.float64).reshape(want.shape)
+    r = err_over_scale(got, want, scale)
+    m = float(r.max()) if r.numel() else 0.0
+    worst[what] = max(worst.get(what, 0.0), m)
+    if not m <= bound:
+        pos = np.unravel_index(int(r.argmax()), tuple(r.shape)) if r.dim() else ()
+        raise AssertionError(f"{what}{tuple(int(i) for i in pos)}: kernel {float(got[pos]):.9e}, fp64 "
+                             f"{float(want[pos]):.9e}, |err| = {m:.2e} x scale {float(scale[pos]):.3e} > {bound:g}")
+
+
+def q_values(w, state, obs: int, n_actions: int, hidden=(64, 64)) -> tuple:
+    """(Q(s_i, a), its error scale) for every row and action id, [n, A] each, on the device of `w`."""
+    w = torch.as_tensor(w)
+    state = torch.as_tensor(state).to(device=w.device, dtype=torch.float64)
+    n = state.shape[0]
+    ids = torch.arange(n_actions, device=w.device).repeat(n, 1)
+    cnt = torch.full((n,), n_actions, device=w.device)
+    net = unflatten(w, obs, n_actions, hidden)
+    return (_next_q(net, state, ids, cnt), _next_q(tuple(p.abs() for p in net), state.abs(), ids, cnt))

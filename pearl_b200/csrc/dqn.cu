@@ -871,6 +871,13 @@ extern "C" int prl_dqn_create(prl_dqn **out, const prl_dqn_cfg *cfg, float *w, f
     cudaError_t e = cudaGetDevice(&dev);
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&q->sm_count, cudaDevAttrMultiProcessorCount, dev);
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&q->max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    // the opt-in limit covers static + dynamic shared memory: k_dqn_learn's sampler CTA keeps its MT19937 state in
+    // static shared memory, so a plan has to fit in what is left (or cudaFuncSetAttribute refuses the launch)
+    cudaFuncAttributes fa;
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_dqn_learn);
+    if (e == cudaSuccess) q->learn_smem = q->max_smem - (int)fa.sharedSizeBytes;
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_q_values);
+    if (e == cudaSuccess) q->qv_smem = q->max_smem - (int)fa.sharedSizeBytes;
     for (int i = 0; i < 2 && e == cudaSuccess; i++) {
         e = cudaHostAlloc((void **)&q->scal_host[i], (size_t)cfg->max_rounds * 8, cudaHostAllocDefault);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&q->scal_done[i], cudaEventDisableTiming);
@@ -1023,10 +1030,10 @@ static int choose_tiling(const prl_dqn *q, int B, int W, int *R_out, int *mch_ou
     Plan pl;
     for (;; mch /= 2) {
         pl = make_plan(d, R, W, mch);
-        if ((int64_t)pl.total * 4 <= q->max_smem) break;
+        if ((int64_t)pl.total * 4 <= q->learn_smem) break;
         if (mch <= 4)
             return fail(PRL_EUNSUPPORTED, "network/batch tile does not fit shared memory (%lld B needed, %d B available)",
-                        (long long)pl.total * 4, q->max_smem);
+                        (long long)pl.total * 4, q->learn_smem);
     }
     *R_out = R; *mch_out = mch; *plan_out = pl;
     return PRL_OK;
@@ -1125,7 +1132,7 @@ static int launch_learn(prl_dqn *q, const uint32_t *records, const prl_buf_layou
         a.mt_state = sample_from->mt_state;
         a.fused_sampler = 1;
         if (sbytes > smem) smem = sbytes;
-        PRL_REQUIRE(smem <= (size_t)q->max_smem, "sampler tables do not fit shared memory");
+        PRL_REQUIRE(smem <= (size_t)q->learn_smem, "sampler tables do not fit shared memory");
     }
     PRL_CUDA(cudaFuncSetAttribute(k_dqn_learn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     void *args[] = {(void *)&a};
@@ -1219,7 +1226,7 @@ extern "C" int prl_dqn_q_values(prl_dqn *q, int n, const float *state, int targe
     Plan pl;
     for (;; mch /= 2) {
         pl = make_plan(d, R, W, mch);
-        if ((int64_t)pl.total * 4 <= q->max_smem) break;
+        if ((int64_t)pl.total * 4 <= q->qv_smem) break;
         if (mch <= 4) return fail(PRL_EUNSUPPORTED, "network does not fit shared memory");
     }
     const size_t smem = (size_t)pl.total * 4;

@@ -67,6 +67,7 @@ struct prl_dqn {
     cudaEvent_t scal_done[2];
     int scal_next;
     int sm_count, max_smem;
+    int learn_smem, qv_smem;  // dynamic shared memory k_dqn_learn / k_q_values may use: max_smem minus their static part
     int last_launches, last_ctas, last_rows;
     // optional device timing of the persistent kernel (bench / roofline)
     int timing;

@@ -73,24 +73,9 @@ def _learner(obs, A, B, seed, *, freq=1000, tau=0.5, rounds=1, per_call=4096, cl
 
 def _data(learner, obs, A, B, seed, dynamic):
     """About 2 B transitions whose online pre-activations all clear MARGIN (host tensors, push order)."""
-    from oracle.dqn_fp64 import relu_margin
+    from oracle.dqn_fp64 import make_data
     from oracle.pearl_oracle import flat
-    from oracle.synth import make_transitions
-    n = 2 * B + 16
-    d = make_transitions(3 * n, obs, A, seed=seed, dynamic=dynamic, p_term=0.2)
-    rng = np.random.default_rng(seed)
-    d["action"] = rng.integers(0, A, 3 * n)
-    d["truncated"] = rng.random(3 * n) < 0.1
-    if not dynamic:
-        d["next_avail_ids"] = np.tile(np.arange(A), (3 * n, 1))
-        d["next_avail_n"] = np.full(3 * n, A)
-    ok = relu_margin(flat(learner._Q).cpu(), d["state"], d["action"], obs, A) >= MARGIN
-    keep = np.flatnonzero(ok.numpy())[:n]
-    assert keep.size == n, "too few rows clear the ReLU margin"
-    return dict(state=torch.from_numpy(d["state"][keep]), action=torch.from_numpy(d["action"][keep]),
-                reward=torch.from_numpy(d["reward"][keep]), next_state=torch.from_numpy(d["next_state"][keep]),
-                terminated=torch.from_numpy(d["terminated"][keep]), truncated=torch.from_numpy(d["truncated"][keep]),
-                avail_ids=torch.from_numpy(d["next_avail_ids"][keep]), avail_n=torch.from_numpy(d["next_avail_n"][keep]))
+    return make_data(flat(learner._Q).cpu(), obs, A, B, seed, dynamic, MARGIN)
 
 
 def _buffer(data, A, seed, dynamic, dynamic_layout=None):
@@ -115,16 +100,8 @@ def _setup(obs, A, B, **kw):
 
 
 def _check(what, got, want, scale, worst):
-    """|got - want| <= C * scale elementwise; names the first element that is not."""
-    from oracle.dqn_fp64 import err_over_scale
-    got = got.detach().cpu().to(torch.float64).reshape(want.shape)
-    r = err_over_scale(got, want, scale)
-    m = float(r.max())
-    worst[what] = max(worst.get(what, 0.0), m)
-    if not m <= C:
-        pos = np.unravel_index(int(r.argmax()), tuple(r.shape)) if r.dim() else ()
-        pytest.fail(f"{what}{tuple(int(i) for i in pos)}: kernel {float(got[pos]):.9e}, fp64 {float(want[pos]):.9e}, "
-                    f"|err| = {m:.2e} x scale {float(scale[pos]):.3e} > {C:g}")
+    from oracle.dqn_fp64 import check
+    check(what, got, want, scale, worst, C)
 
 
 # --------------------------------------------------------------------------- a. one-step gradient, whole class
