@@ -151,7 +151,7 @@ except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
             self._training_steps = 0
             self._learning_rate, self._discount_factor = learning_rate, discount_factor
             self._target_update_freq, self._soft_update_tau = target_update_freq, soft_update_tau
-            self._is_conservative = is_conservative
+            self._is_conservative, self._conservative_alpha = is_conservative, conservative_alpha
             self._is_action_continuous = False
             self.on_policy = False
             self.exploration_module = exploration_module

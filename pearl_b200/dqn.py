@@ -25,6 +25,7 @@ from typing import Any
 import torch
 
 from . import _lib
+from . import cql as _cql
 from ._compat import _RefDeepQLearning, _RefDoubleDQN, TransitionBatch
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
 
@@ -51,8 +52,7 @@ class _B200DQNMixin:
         if engine not in ("auto", "simt", "tc"):
             raise ValueError("engine must be 'auto', 'simt' or 'tc'")
         self._engine = engine
-        if getattr(self, "_is_conservative", False):
-            raise NotImplementedError("conservative (CQL) updates are outside the fused path")
+        self._conservative = bool(getattr(self, "_is_conservative", False))   # conservative (CQL) rounds: prl_cql_* (cql.py)
         arm = self.action_representation_module
         if type(arm).__name__ != "OneHotActionTensorRepresentationModule":
             raise NotImplementedError("the fused Q network assumes a one-hot action representation")
@@ -64,6 +64,9 @@ class _B200DQNMixin:
             raise NotImplementedError("unexpected Q-network shape")
         self._max_rounds = int(max_rounds_per_call)
         self._rows_per_cta = int(rows_per_cta)
+        if self._conservative:
+            _cql.check_config(self, engine)
+            self.use_cuda_graph = True          # False: plain stream launches (profilers)
         self._handle = C.c_void_p(0)
         self._bound_ptr = None
         self._bound_batch = 0
@@ -73,10 +76,14 @@ class _B200DQNMixin:
     def __del__(self):
         try:
             if getattr(self, "_handle", None) and self._handle.value:
-                self._libh.prl_dqn_destroy(self._handle)
+                self._c("destroy")(self._handle)
                 self._handle = C.c_void_p(0)
         except Exception:
             pass
+
+    def _c(self, name: str):
+        """C entry point `name` of the learner this instance binds: prl_cql_* when conservative, prl_dqn_* otherwise."""
+        return getattr(self._libh, ("prl_cql_" if self._conservative else "prl_dqn_") + name)
 
     def _adam_hparams(self) -> dict:
         opt = self._optimizer
@@ -119,8 +126,8 @@ class _B200DQNMixin:
             if "exp_avg" not in st0 or st0["exp_avg"].data_ptr() == self._flat["m"].data_ptr():
                 # the optimizer still shows our flat vectors (no load_state_dict in between): carry them over
                 old_state = {k: v.clone() for k, v in self._flat.items() if k in ("m", "v", "vmax")}
-                old_step = int(self._libh.prl_dqn_adam_step(self._handle))
-            self._libh.prl_dqn_destroy(self._handle)
+                old_step = int(self._c("adam_step")(self._handle))
+            self._c("destroy")(self._handle)
             self._handle = C.c_void_p(0)
         self._libh = _lib.init(device.index if device.index is not None else torch.cuda.current_device())
         hp = self._adam_hparams()
@@ -138,21 +145,21 @@ class _B200DQNMixin:
         else:
             m, v, vmax = (torch.zeros(P, dtype=torch.float32, device=device) for _ in range(3))
         self._bound_batch = max(int(need_batch), int(self._batch_size) if self._batch_size > 0 else 0, 1)
-        cfg = _lib.DqnCfg(
+        cfg = _cql.make_cfg(self, hp, self._bound_batch) if self._conservative else _lib.DqnCfg(
             obs_dim=self._obs_dim, n_actions=self._n_actions, hidden1=self._hidden[0], hidden2=self._hidden[1],
             double_dqn=int(self._double), target_update_freq=int(self._target_update_freq),
             max_batch=self._bound_batch, max_rounds=self._max_rounds, rows_per_cta=self._rows_per_cta,
             lr=hp["lr"], beta1=hp["beta1"], beta2=hp["beta2"], eps=hp["eps"],
             weight_decay=hp["weight_decay"], gamma=float(self._discount_factor),
             tau=float(self._soft_update_tau))
-        if int(self._libh.prl_dqn_param_count(C.byref(cfg))) != P:
+        if int(self._c("param_count")(C.byref(cfg))) != P:
             raise RuntimeError("parameter count mismatch between the module and the fused kernel")
-        ws_bytes = int(self._libh.prl_dqn_workspace_bytes(C.byref(cfg)))
+        ws_bytes = int(self._c("workspace_bytes")(C.byref(cfg)))
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
         handle = C.c_void_p(0)
         with torch.cuda.device(device):
-            _lib.check(self._libh.prl_dqn_create(C.byref(handle), C.byref(cfg), _lib.ptr(w), _lib.ptr(wt),
-                                                 _lib.ptr(m), _lib.ptr(v), _lib.ptr(vmax), step, _lib.ptr(ws)))
+            _lib.check(self._c("create")(C.byref(handle), C.byref(cfg), _lib.ptr(w), _lib.ptr(wt),
+                                         _lib.ptr(m), _lib.ptr(v), _lib.ptr(vmax), step, _lib.ptr(ws)))
         self._handle, self._cfg = handle, cfg
         if getattr(self, "_comm", None) is not None:
             _lib.check(self._libh.prl_dqn_set_comm(self._handle, self._comm.handle))
@@ -172,7 +179,7 @@ class _B200DQNMixin:
                 self._bound_ptr = None          # betas / eps / weight decay changed: full re-bind with the new config
                 self._bind(self._bound_batch)
                 return
-            _lib.check(self._libh.prl_dqn_set_lr(self._handle, hp["lr"]))
+            _lib.check(self._c("set_lr")(self._handle, hp["lr"]))
             self._bound_hp = hp
         st = self._optimizer.state
         m = self._flat["m"]
@@ -183,7 +190,7 @@ class _B200DQNMixin:
             if len(st) == 0:                    # state dropped (fresh optimizer): restart the moments
                 for k in ("m", "v", "vmax"):
                     self._flat[k].zero_()
-                _lib.check(self._libh.prl_dqn_set_adam_step(self._handle, 0))
+                _lib.check(self._c("set_adam_step")(self._handle, 0))
                 self._expose_state(params, 0)
             return
         dev = m.device
@@ -193,7 +200,7 @@ class _B200DQNMixin:
         self._flat["v"].copy_(cat("exp_avg_sq"))
         self._flat["vmax"].copy_(cat("max_exp_avg_sq") if has_max else cat("exp_avg_sq"))
         step = int(float(st[p0]["step"]))
-        _lib.check(self._libh.prl_dqn_set_adam_step(self._handle, step))
+        _lib.check(self._c("set_adam_step")(self._handle, step))
         self._expose_state(params, step)
 
     def _expose_state(self, params, step: int) -> None:
@@ -212,7 +219,7 @@ class _B200DQNMixin:
             off += n
 
     def _sync_step_tensors(self) -> None:
-        step = float(self._libh.prl_dqn_adam_step(self._handle))
+        step = float(self._c("adam_step")(self._handle))
         for st in self._step_tensors:
             st.fill_(step)
 
@@ -230,9 +237,11 @@ class _B200DQNMixin:
     def adam_state(self) -> dict:
         self._bind(1)
         return dict(exp_avg=self._flat["m"], exp_avg_sq=self._flat["v"], max_exp_avg_sq=self._flat["vmax"],
-                    step=int(self._libh.prl_dqn_adam_step(self._handle)))
+                    step=int(self._c("adam_step")(self._handle)))
 
     def launch_info(self) -> dict:
+        if self._conservative:
+            return dict(launches=int(self._libh.prl_cql_last_launches(self._handle)))
         a, b, c = C.c_int32(0), C.c_int32(0), C.c_int32(0)
         self._libh.prl_dqn_last_launch_info(self._handle, C.byref(a), C.byref(b), C.byref(c))
         return dict(launches=a.value, ctas=b.value, rows_per_cta=c.value)
@@ -242,11 +251,15 @@ class _B200DQNMixin:
         `learn(B200ReplayBuffer)` then applies the mean gradient of all ranks' batches, exchanged
         inside the kernel.  All ranks must call learn() with the same number of rounds and start
         from identical parameters."""
+        if self._conservative:
+            raise NotImplementedError("conservative (CQL) updates run on one GPU: set_communicator is not supported")
         self._bind(1)
         self._comm = comm
         _lib.check(self._libh.prl_dqn_set_comm(self._handle, comm.handle if comm is not None else None))
 
     def set_kernel_timing(self, enable: bool = True) -> None:
+        if self._conservative:
+            raise NotImplementedError("kernel timing belongs to the fused DQN kernel; time conservative rounds with CUDA events")
         self._bind(1)
         _lib.check(self._libh.prl_dqn_set_timing(self._handle, int(enable)))
 
@@ -274,6 +287,8 @@ class _B200DQNMixin:
                     for k, v in self.learn_batch(self.preprocess_batch(batch)).items():
                         report.setdefault(k, []).append(v)
             return report
+        if self._conservative:
+            return _cql.learn(self, replay_buffer, bs, rounds, trace)
         self._bind(bs)
         dev = self._device
         if replay_buffer.device != dev:
@@ -361,6 +376,8 @@ class _B200DQNMixin:
     def learn_batch(self, batch) -> dict:
         """`DeepTDLearning.learn_batch` on a caller-supplied batch (raw ids, or the one-hot
         tensors the reference's preprocess_batch produces)."""
+        if self._conservative:
+            return _cql.learn_batch(self, batch)
         B = len(batch)
         self._bind(B)
         dev = self._device
@@ -389,6 +406,8 @@ class _B200DQNMixin:
     # ------------------------------------------------------------------ act
     def q_values(self, states: torch.Tensor, target: bool = False) -> torch.Tensor:
         """Q(s, a) for every action id: [n, obs] -> [n, n_actions]."""
+        if self._conservative:
+            return _cql.q_values(self, states, target)
         self._bind(1)
         dev = self._device
         s = states.to(device=dev, dtype=torch.float32).reshape(-1, self._obs_dim).contiguous()
@@ -421,6 +440,8 @@ class B200LearnerGroup:
     def __init__(self, learners, buffers) -> None:
         if len(learners) != len(buffers) or not learners:
             raise ValueError("need one replay buffer per learner")
+        if any(getattr(l, "_conservative", False) for l in learners):
+            raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no conservative (CQL) update")
         self.learners, self.buffers = list(learners), list(buffers)
 
     def learn(self) -> list:
