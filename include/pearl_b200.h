@@ -596,6 +596,64 @@ int prl_cql_q_values(prl_cql *cql, int n, const float *state, int target, float 
 int prl_cql_set_graph(prl_cql *cql, int enable);
 int64_t prl_cql_last_launches(const prl_cql *cql);
 
+/* ---- dueling DQN / DoubleDQN --------------------------------------------------------------------
+ * Replaces DuelingQValueNetwork.get_q_values (neural_networks/sequential_decision_making/q_value_networks.py:352-510),
+ * DeepTDLearning.forward / loss / learn_batch (policy_learners/sequential_decision_making/deep_td_learning.py:269-360) and
+ * DeepQLearning / DoubleDQN.get_next_state_values (deep_q_learning.py:130-167, double_dqn.py:29-57), driven by
+ * PolicyLearner.learn (prl_duel_learn: sample -> round, `rounds` times) or called on a caller's batch (prl_duel_learn_batch:
+ * one round, PearlAgent.learn_batch).  The network: state_arch obs -> state_h1 -> state_h2 -> feature_dim (no ReLU on the
+ * feature), value_arch feature_dim -> value_h1 -> value_h2 -> 1, advantage_arch (feature || one-hot action) -> adv_h1 ->
+ * adv_h2 -> 1; Q(s, a) = fl(fl(V(s) + Adv(s, a)) - mean of Adv(s, .) over a set that depends on the caller:
+ *   online q: the A current slots, padding (id 0) included; the query action alone when learn_batch gets no current ids;
+ *   DQN target: max over the available next slots, the mean over all A next slots (unavailable ones with their ids);
+ *   DoubleDQN target: a* = first argmax over the available next slots of the online Q (mean over all A next slots), then
+ *   V' = fl(fl(V_t(s') + Adv_t(s', a*)) - Adv_t(s', a*)) (the target net called with the single query a*).
+ * Per round: when (training_steps + 1) % target_update_freq == 0, FIRST target = tau * online + (1 - tau) * target;
+ * y = V' gamma (1 - terminated) + r; L = mean (q - y)^2; one AdamW(amsgrad) step.  Reported loss: mean |q - y|.
+ * 1 <= n_actions <= 255.  Flat layout (fp32, row-major [out][in], torch's parameter order): state_arch W1 b1 W2 b2 W3 b3,
+ * value_arch W1 b1 W2 b2 W3 b3, advantage_arch W1 b1 W2 b2 W3 b3.  Sharded buffers, continuous-action buffers, buffers of
+ * other obs_dim / n_actions, and batch / rounds above the configured maxima are rejected (EINVAL) before any launch. */
+typedef struct prl_duel_cfg {
+    int32_t obs_dim, n_actions, feature_dim;   /* feature_dim: output width of state_arch (hidden_dims[-1]) */
+    int32_t state_h1, state_h2, value_h1, value_h2, adv_h1, adv_h2;
+    int32_t double_dqn;            /* 0: DeepQLearning, 1: DoubleDQN */
+    int32_t target_update_freq, max_batch, max_rounds;
+    double lr, beta1, beta2, eps, weight_decay, gamma, tau;
+} prl_duel_cfg;
+typedef struct prl_duel prl_duel;
+int64_t prl_duel_param_count(const prl_duel_cfg *cfg);
+int64_t prl_duel_workspace_bytes(const prl_duel_cfg *cfg);
+/* w, w_target, exp_avg, exp_avg_sq, max_exp_avg_sq: device f32[param_count] owned by the caller (the argument order of
+ * prl_dqn_create); adam_step: optimizer steps already taken (torch's `step`). */
+int prl_duel_create(prl_duel **out, const prl_duel_cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq,
+                    float *max_exp_avg_sq, int64_t adam_step, void *workspace_dev);
+int prl_duel_destroy(prl_duel *duel);
+int64_t prl_duel_adam_step(const prl_duel *duel);
+int prl_duel_set_adam_step(prl_duel *duel, int64_t step);
+/* New AdamW learning rate from the next call on; every lr-dependent scalar travels in the per-call block: no re-capture. */
+int prl_duel_set_lr(prl_duel *duel, double lr);
+/* training_steps = the learner's count before the call (PolicyLearner.learn increments it before each round);
+ * out_loss_dev: device f32[rounds]; out_logical_dev (optional) i32[rounds][batch] = sampled indices.  The ring stores no
+ * current action sets: the online mean runs over every action, as B200ReplayBuffer.sample reports the set. */
+int prl_duel_learn(prl_duel *duel, prl_buf *buf, int rounds, int batch, int64_t training_steps, float *out_loss_dev,
+                   int32_t *out_logical_dev, void *stream);
+/* One round on a dense device batch: state / next_state f32[batch][obs], action_id i32[batch], reward f32[batch],
+ * terminated u8[batch]; curr_ids i32[batch][n_actions] (slot k of the current set, padding included), null = the online
+ * mean runs over the query action alone; next_ids i32[batch][n_actions] (every slot, unavailable ones included: they
+ * enter the mean with these ids), null = slot k holds k; next_unavailable u8[batch][n_actions] (1 = unavailable), null =
+ * every slot available; training_steps = the count learn_batch sees (agent.learn_batch does not advance it);
+ * out_loss_dev: device f32[1]. */
+int prl_duel_learn_batch(prl_duel *duel, int batch, const float *state, const int32_t *action_id, const float *reward,
+                         const float *next_state, const uint8_t *terminated, const int32_t *curr_ids, const int32_t *next_ids,
+                         const uint8_t *next_unavailable, int64_t training_steps, float *out_loss_dev, void *stream);
+/* Q(s, .) over an id set (DeepTDLearning.act, deep_td_learning.py:200-254): device state f32[n][obs_dim], ids
+ * i32[n][K] (null: every action, K = n_actions) -> out_q f32[n][K], the advantage mean over the row's K ids; online
+ * (target = 0) or target network.  1 <= K <= n_actions + 1. */
+int prl_duel_q_values(prl_duel *duel, int n, const float *state, const int32_t *ids, int K, int target, float *out_q_dev,
+                      void *stream);
+int prl_duel_set_graph(prl_duel *duel, int enable);
+int64_t prl_duel_last_launches(const prl_duel *duel);
+
 /* ---- PPO learner ------------------------------------------------------------------------------
  * Replaces ProximalPolicyOptimization.learn (policy_learners/sequential_decision_making/ppo.py:195-293):
  * prl_ppo_preprocess = preprocess_replay_buffer (state values, taken-action probabilities under the current

@@ -6,7 +6,7 @@
 Hand-written CUDA in libpearlb200.so (C ABI: include/pearl_b200.h), called through
 ctypes; PyTorch only allocates memory and provides streams.  No CPU fallback.
 """
-from ._compat import HAVE_PEARL, OneHotActionTensorRepresentationModule, TransitionBatch  # noqa: F401
+from ._compat import HAVE_PEARL, DuelingQValueNetwork, OneHotActionTensorRepresentationModule, TransitionBatch  # noqa: F401
 from .dqn import B200DeepQLearning, B200DoubleDQN, B200LearnerGroup  # noqa: F401
 from .replay_buffer import B200ReplayBuffer  # noqa: F401
 from .per import B200PrioritizedReplayBuffer  # noqa: F401
@@ -22,4 +22,4 @@ from .dist import B200Communicator, all_gather_bytes, shard_owner  # noqa: F401
 __all__ = ["B200ReplayBuffer", "B200DeepQLearning", "B200DoubleDQN", "TransitionBatch",
            "OneHotActionTensorRepresentationModule", "HAVE_PEARL", "B200Communicator", "B200LearnerGroup", "B200PrioritizedReplayBuffer", "gae_and_lambda_returns", "B200ContinuousSoftActorCritic", "B200SoftActorCritic", "B200ProximalPolicyOptimization",
            "B200TD3", "B200DeepDeterministicPolicyGradient", "B200HindsightExperienceReplayBuffer", "B200ImplicitQLearning",
-           "B200QuantileRegressionDeepQLearning"]
+           "B200QuantileRegressionDeepQLearning", "DuelingQValueNetwork"]

@@ -23,6 +23,7 @@ try:  # pragma: no cover - depends on the environment
     from pearl.policy_learners.sequential_decision_making.deep_q_learning import (
         DeepQLearning as _RefDeepQLearning,
     )
+    from pearl.neural_networks.sequential_decision_making.q_value_networks import DuelingQValueNetwork
     from pearl.policy_learners.sequential_decision_making.double_dqn import DoubleDQN as _RefDoubleDQN
     from pearl.replay_buffers.replay_buffer import ReplayBuffer
     from pearl.replay_buffers.transition import TransitionBatch
@@ -123,13 +124,42 @@ except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
         """Same module tree (hence state_dict keys) as VanillaQValueNetwork built by
         mlp_block: `_model.{i}.0` = Linear (pearl/neural_networks/common/utils.py:75-152)."""
 
-        def __init__(self, state_dim: int, action_dim: int, hidden_dims) -> None:
+        def __init__(self, state_dim: int, action_dim: int, hidden_dims, output_dim: int = 1) -> None:
             super().__init__()
-            dims = [state_dim + action_dim] + list(hidden_dims) + [1]
+            dims = [state_dim + action_dim] + list(hidden_dims) + [output_dim]
             layers = [nn.Sequential(nn.Linear(dims[i], dims[i + 1]), nn.ReLU()) for i in range(len(dims) - 2)]
             layers.append(nn.Sequential(nn.Linear(dims[-2], dims[-1])))
             self._model = nn.Sequential(*layers)
             self._state_dim, self._action_dim = state_dim, action_dim
+
+    class _ValueMLP(nn.Module):
+        """Same module tree as VanillaValueNetwork: `_model` = mlp_block (Linear+ReLU per hidden layer, then Linear)."""
+
+        def __init__(self, input_dim: int, hidden_dims, output_dim: int) -> None:
+            super().__init__()
+            self._model = _QNet(input_dim, 0, hidden_dims, output_dim)._model
+
+    class DuelingQValueNetwork(nn.Module):
+        """Same constructor, module tree and state_dict keys as DuelingQValueNetwork
+        (pearl/neural_networks/sequential_decision_making/q_value_networks.py:352-400): `{state,value,advantage}_arch`."""
+
+        def __init__(self, state_dim: int, action_dim: int, hidden_dims, output_dim: int = 1, value_hidden_dims=None,
+                     advantage_hidden_dims=None, state_hidden_dims=None) -> None:
+            super().__init__()
+            self._state_dim, self._action_dim = state_dim, action_dim
+            F = hidden_dims[-1]
+            self.state_arch = _ValueMLP(state_dim, hidden_dims if state_hidden_dims is None else state_hidden_dims, F)
+            self.value_arch = _ValueMLP(F, hidden_dims if value_hidden_dims is None else value_hidden_dims, output_dim)
+            self.advantage_arch = _ValueMLP(F + action_dim, hidden_dims if advantage_hidden_dims is None else advantage_hidden_dims,
+                                            output_dim)
+
+        @property
+        def state_dim(self) -> int:
+            return self._state_dim
+
+        @property
+        def action_dim(self) -> int:
+            return self._action_dim
 
     class _RefDeepQLearning(nn.Module):
         """Attribute-compatible stand-in for DeepQLearning's constructor
@@ -156,8 +186,13 @@ except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
             self.on_policy = False
             self.exploration_module = exploration_module
             self._action_representation_module = action_representation_module
-            self._Q = network_instance if network_instance is not None else _QNet(
-                state_dim, action_representation_module.representation_dim, hidden_dims)
+            A = action_representation_module.representation_dim
+            if network_instance is not None:
+                self._Q = network_instance
+            elif network_type is DuelingQValueNetwork:   # deep_td_learning.py make_specified_network
+                self._Q = DuelingQValueNetwork(state_dim=state_dim, action_dim=A, hidden_dims=hidden_dims, output_dim=1)
+            else:
+                self._Q = _QNet(state_dim, A, hidden_dims)
             self._Q_target = copy.deepcopy(self._Q)
             self._optimizer = optimizer if optimizer is not None else torch.optim.AdamW(
                 self._Q.parameters(), lr=learning_rate, amsgrad=True)

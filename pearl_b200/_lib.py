@@ -80,6 +80,14 @@ class CqlCfg(C.Structure):
                 ("eps", C.c_double), ("weight_decay", C.c_double), ("gamma", C.c_double), ("tau", C.c_double)]
 
 
+class DuelCfg(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("feature_dim", C.c_int32), ("state_h1", C.c_int32),
+                ("state_h2", C.c_int32), ("value_h1", C.c_int32), ("value_h2", C.c_int32), ("adv_h1", C.c_int32),
+                ("adv_h2", C.c_int32), ("double_dqn", C.c_int32), ("target_update_freq", C.c_int32), ("max_batch", C.c_int32),
+                ("max_rounds", C.c_int32), ("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double),
+                ("eps", C.c_double), ("weight_decay", C.c_double), ("gamma", C.c_double), ("tau", C.c_double)]
+
+
 class PpoCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("actor_h1", C.c_int32), ("actor_h2", C.c_int32),
                 ("critic_h1", C.c_int32), ("critic_h2", C.c_int32), ("max_batch", C.c_int32), ("max_rounds", C.c_int32),
@@ -210,6 +218,18 @@ _SIGNATURES = {
     "prl_cql_q_values": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
     "prl_cql_set_graph": (C.c_int, [_P, C.c_int]),
     "prl_cql_last_launches": (C.c_int64, [_P]),
+    "prl_duel_param_count": (C.c_int64, [C.POINTER(DuelCfg)]),
+    "prl_duel_workspace_bytes": (C.c_int64, [C.POINTER(DuelCfg)]),
+    "prl_duel_create": (C.c_int, [C.POINTER(_P), C.POINTER(DuelCfg), _P, _P, _P, _P, _P, C.c_int64, _P]),
+    "prl_duel_destroy": (C.c_int, [_P]),
+    "prl_duel_adam_step": (C.c_int64, [_P]),
+    "prl_duel_set_adam_step": (C.c_int, [_P, C.c_int64]),
+    "prl_duel_set_lr": (C.c_int, [_P, C.c_double]),
+    "prl_duel_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, _P, _P, _P]),
+    "prl_duel_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 8 + [C.c_int64, _P, _P]),
+    "prl_duel_q_values": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P]),
+    "prl_duel_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_duel_last_launches": (C.c_int64, [_P]),
     "prl_ppo_actor_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_critic_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_workspace_bytes": (C.c_int64, [C.POINTER(PpoCfg)]),

@@ -97,15 +97,6 @@ __global__ void k_cql_load(const uint32_t *__restrict__ records, prl_buf_layout 
     }
 }
 
-// update_target_network at the start of a flagged round (deep_td_learning.py forward): t = tau * w + (1 - tau) * t with
-// the current online parameters
-__global__ void k_cql_soft_update(int n, const float *__restrict__ w, float *__restrict__ t, float tau, float omtau,
-                                  const int *__restrict__ target_on, const int *__restrict__ round_idx) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n || !target_on[*round_idx]) return;
-    t[i] = __fadd_rn(__fmul_rn(tau, w[i]), __fmul_rn(omtau, t[i]));
-}
-
 // Bellman target, loss gradients and |q - y|.  One warp per row b; lane l handles slots l, l + 32, ...
 //   DQN:        V = max over available next slots of Q'(s', .)
 //   DoubleDQN:  g = first argmax over available next slots of Q(s', .), V = Q'(s', g)
@@ -156,35 +147,6 @@ __global__ void __launch_bounds__(128) k_cql_target(int B, int A, int dbl, const
         const float e = __fsub_rn(l[A], y);
         d[A] = __fmul_rn(__fdiv_rn(2.f, fB), e);
         rowabs[b] = fabsf(e);
-    }
-}
-
-// layer-1 gradient of a row's state product: dh[b][j] = sum over the row's S slots of dc1[b * S + k][j], k ascending
-__global__ void k_cql_rowsum(int B, int S, int H, const float *__restrict__ dc1, float *__restrict__ dh) {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= B * H) return;
-    const int b = e / H, j = e - b * H;
-    const float *p = dc1 + (size_t)b * S * H + j;
-    float s = 0.f;
-    for (int k = 0; k < S; k++) s += p[(size_t)k * H];
-    dh[e] = s;
-}
-
-// reported loss: mean over rows of |q - y| (rows in a fixed tree order), then the round counter advances
-__global__ void __launch_bounds__(256) k_cql_report(int B, const float *__restrict__ rowabs, const CqlCall *__restrict__ call,
-                                                    int *__restrict__ round_idx) {
-    __shared__ float red[256];
-    float s = 0.f;
-    for (int b = threadIdx.x; b < B; b += blockDim.x) s += rowabs[b];
-    red[threadIdx.x] = s;
-    __syncthreads();
-    for (int o = 128; o; o >>= 1) {
-        if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) {
-        call->out_loss[*round_idx] = red[0] / (float)B;
-        *round_idx += 1;
     }
 }
 
@@ -355,8 +317,8 @@ static int cql_round(prl_cql *s, prl_buf *buf, int B, cudaStream_t st) {
     k_cql_load<<<(B * 32 + eb - 1) / eb, eb, 0, st>>>(buf ? buf->records : nullptr, buf ? buf->lay : prl_buf_layout{}, O, A, dynamic,
                                                      s->call, s->round_idx, B, s->S, s->S2, s->R, s->T, s->cnt, s->ids, s->cids);
     // ---------------- target update first, with the current online parameters (flagged rounds only)
-    k_cql_soft_update<<<(s->P + eb - 1) / eb, eb, 0, st>>>(s->P, s->q, s->q_t, (float)c.tau, (float)(1.0 - c.tau), s->target_on,
-                                                           s->round_idx);
+    k_soft_update_flagged<<<(s->P + eb - 1) / eb, eb, 0, st>>>(s->P, s->q, s->q_t, (float)c.tau, (float)(1.0 - c.tau), s->target_on,
+                                                               s->round_idx);
     small += 2;
     // ---------------- online net over the A current slots and the taken action (kept for the backward pass)
     L.fwd(mat(s->S, O), B, w + s->W1, D, 0, w + s->b1, 0, H1, O, false, s->P1, H1, 0);
@@ -383,14 +345,14 @@ static int cql_round(prl_cql *s, prl_buf *buf, int B, cudaStream_t st) {
     k_head_bwd<<<(BA1 * H2 + eb - 1) / eb, eb, 0, st>>>(BA1, H2, s->dq, w + s->W3, 0, s->c2, s->dc2);
     L.bwd_w(s->dc2, H2, 0, BA1, H2, mat(s->c1, H1), H1, g + s->W2, H1, 0, g + s->b2, 0);
     L.bwd_x(s->dc2, H2, 0, BA1, H2, w + s->W2, H1, 0, 0, H1, s->dc1, H1, 0, s->c1, H1, 0, false);
-    k_cql_rowsum<<<(B * H1 + eb - 1) / eb, eb, 0, st>>>(B, A + 1, H1, s->dc1, s->dh1);
+    k_slot_rowsum<<<(B * H1 + eb - 1) / eb, eb, 0, st>>>(B, A + 1, H1, s->dc1, s->dh1);
     L.bwd_w(s->dh1, H1, 0, B, H1, mat(s->S, O), O, g + s->W1, D, 0, g + s->b1, 0);                   // state columns + b1
     k_fold_w1a_grad<<<(H1 * A + eb - 1) / eb, eb, 0, st>>>(BA1, A, H1, s->cids, s->dc1, g + s->W1 + O, D, 0);
     small += 3;
     // ---------------- AdamW(amsgrad); the target was updated at the start of the round
     k_adamw<<<(s->P + eb - 1) / eb, eb, 0, st>>>(s->P, s->q, s->q_m, s->q_v, s->q_x, g, h, s->scal, s->round_idx, nullptr, 0.f, 0.f,
                                                 &s->call->decay);
-    k_cql_report<<<1, 256, 0, st>>>(B, s->rowabs, s->call, s->round_idx);
+    k_round_report<<<1, 256, 0, st>>>(B, s->rowabs, s->call, s->round_idx);
     small += 2;
     s->launches_per_round = L.count + small;
     return PRL_OK;

@@ -309,6 +309,49 @@ static __global__ void k_fold_w1a_grad(int B, int A, int C1, const int *__restri
     gw1[z * net_stride + (size_t)j * ld + k] = s;
 }
 
+// ------------------------------------------------------------------ pieces shared by the one-round DQN-family learners
+// (cql.cu, dueling.cu): a round whose online net runs over S slots per row, captured into a CUDA graph
+
+// layer-1 gradient of a row's state product: dh[b][j] = sum over the row's S slots of dc1[b * S + k][j], k ascending
+static __global__ void k_slot_rowsum(int B, int S, int H, const float *__restrict__ dc1, float *__restrict__ dh) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= B * H) return;
+    const int b = e / H, j = e - b * H;
+    const float *p = dc1 + (size_t)b * S * H + j;
+    float s = 0.f;
+    for (int k = 0; k < S; k++) s += p[(size_t)k * H];
+    dh[e] = s;
+}
+
+// update_target_network at the start of a flagged round (deep_td_learning.py forward): t = tau * w + (1 - tau) * t with
+// the current online parameters
+static __global__ void k_soft_update_flagged(int n, const float *__restrict__ w, float *__restrict__ t, float tau, float omtau,
+                                             const int *__restrict__ target_on, const int *__restrict__ round_idx) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || !target_on[*round_idx]) return;
+    t[i] = __fadd_rn(__fmul_rn(tau, w[i]), __fmul_rn(omtau, t[i]));
+}
+
+// reported loss: mean over rows of |q - y| (rows in a fixed tree order) into call->out_loss[round], then the round counter
+// advances.  Call: the learner's per-call block (a struct with `float *out_loss`)
+template <class Call>
+__global__ void __launch_bounds__(256) k_round_report(int B, const float *__restrict__ rowabs, const Call *__restrict__ call,
+                                                      int *__restrict__ round_idx) {
+    __shared__ float red[256];
+    float s = 0.f;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) s += rowabs[b];
+    red[threadIdx.x] = s;
+    __syncthreads();
+    for (int o = 128; o; o >>= 1) {
+        if (threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        call->out_loss[*round_idx] = red[0] / (float)B;
+        *round_idx += 1;
+    }
+}
+
 // one row of softmax(logits) as torch computes it: p_k = exp(l_k - max) / sum.  The row's max and sum are computed once;
 // p_k is evaluated where it is needed (the same arithmetic every time, no per-thread arrays)
 struct RowSoftmax {

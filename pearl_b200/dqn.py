@@ -26,6 +26,7 @@ import torch
 
 from . import _lib
 from . import cql as _cql
+from . import dueling as _duel
 from ._compat import _RefDeepQLearning, _RefDoubleDQN, TransitionBatch
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
 
@@ -57,15 +58,22 @@ class _B200DQNMixin:
         if type(arm).__name__ != "OneHotActionTensorRepresentationModule":
             raise NotImplementedError("the fused Q network assumes a one-hot action representation")
         self._n_actions = int(arm.max_number_actions)
-        lin = _linears(self._Q)
-        self._obs_dim = lin[0].in_features - self._n_actions
-        self._hidden = (lin[0].out_features, lin[1].out_features)
-        if lin[1].in_features != self._hidden[0] or lin[2].in_features != self._hidden[1] or lin[2].out_features != 1:
-            raise NotImplementedError("unexpected Q-network shape")
+        self._dueling = _duel.is_dueling(self._Q)       # DuelingQValueNetwork: prl_duel_* (dueling.py)
+        if self._dueling:
+            self._obs_dim, self._duel_dims = _duel.shape_of(self._Q, self._n_actions)
+        else:
+            lin = _linears(self._Q)
+            self._obs_dim = lin[0].in_features - self._n_actions
+            self._hidden = (lin[0].out_features, lin[1].out_features)
+            if lin[1].in_features != self._hidden[0] or lin[2].in_features != self._hidden[1] or lin[2].out_features != 1:
+                raise NotImplementedError("unexpected Q-network shape")
         self._max_rounds = int(max_rounds_per_call)
         self._rows_per_cta = int(rows_per_cta)
-        if self._conservative:
+        if self._dueling:
+            _duel.check_config(self, engine)
+        elif self._conservative:
             _cql.check_config(self, engine)
+        if self._dueling or self._conservative:
             self.use_cuda_graph = True          # False: plain stream launches (profilers)
         self._handle = C.c_void_p(0)
         self._bound_ptr = None
@@ -82,8 +90,10 @@ class _B200DQNMixin:
             pass
 
     def _c(self, name: str):
-        """C entry point `name` of the learner this instance binds: prl_cql_* when conservative, prl_dqn_* otherwise."""
-        return getattr(self._libh, ("prl_cql_" if self._conservative else "prl_dqn_") + name)
+        """C entry point `name` of the learner this instance binds: prl_duel_* for a dueling Q network, prl_cql_* when
+        conservative, prl_dqn_* otherwise."""
+        prefix = "prl_duel_" if self._dueling else "prl_cql_" if self._conservative else "prl_dqn_"
+        return getattr(self._libh, prefix + name)
 
     def _adam_hparams(self) -> dict:
         opt = self._optimizer
@@ -145,7 +155,8 @@ class _B200DQNMixin:
         else:
             m, v, vmax = (torch.zeros(P, dtype=torch.float32, device=device) for _ in range(3))
         self._bound_batch = max(int(need_batch), int(self._batch_size) if self._batch_size > 0 else 0, 1)
-        cfg = _cql.make_cfg(self, hp, self._bound_batch) if self._conservative else _lib.DqnCfg(
+        cfg = _duel.make_cfg(self, hp, self._bound_batch) if self._dueling else \
+            _cql.make_cfg(self, hp, self._bound_batch) if self._conservative else _lib.DqnCfg(
             obs_dim=self._obs_dim, n_actions=self._n_actions, hidden1=self._hidden[0], hidden2=self._hidden[1],
             double_dqn=int(self._double), target_update_freq=int(self._target_update_freq),
             max_batch=self._bound_batch, max_rounds=self._max_rounds, rows_per_cta=self._rows_per_cta,
@@ -240,8 +251,8 @@ class _B200DQNMixin:
                     step=int(self._c("adam_step")(self._handle)))
 
     def launch_info(self) -> dict:
-        if self._conservative:
-            return dict(launches=int(self._libh.prl_cql_last_launches(self._handle)))
+        if self._dueling or self._conservative:
+            return dict(launches=int(self._c("last_launches")(self._handle)))
         a, b, c = C.c_int32(0), C.c_int32(0), C.c_int32(0)
         self._libh.prl_dqn_last_launch_info(self._handle, C.byref(a), C.byref(b), C.byref(c))
         return dict(launches=a.value, ctas=b.value, rows_per_cta=c.value)
@@ -251,15 +262,16 @@ class _B200DQNMixin:
         `learn(B200ReplayBuffer)` then applies the mean gradient of all ranks' batches, exchanged
         inside the kernel.  All ranks must call learn() with the same number of rounds and start
         from identical parameters."""
-        if self._conservative:
-            raise NotImplementedError("conservative (CQL) updates run on one GPU: set_communicator is not supported")
+        if self._dueling or self._conservative:
+            raise NotImplementedError("dueling and conservative (CQL) updates run on one GPU: set_communicator is not supported")
         self._bind(1)
         self._comm = comm
         _lib.check(self._libh.prl_dqn_set_comm(self._handle, comm.handle if comm is not None else None))
 
     def set_kernel_timing(self, enable: bool = True) -> None:
-        if self._conservative:
-            raise NotImplementedError("kernel timing belongs to the fused DQN kernel; time conservative rounds with CUDA events")
+        if self._dueling or self._conservative:
+            raise NotImplementedError("kernel timing belongs to the fused DQN kernel; time dueling and conservative rounds with "
+                                      "CUDA events")
         self._bind(1)
         _lib.check(self._libh.prl_dqn_set_timing(self._handle, int(enable)))
 
@@ -287,6 +299,8 @@ class _B200DQNMixin:
                     for k, v in self.learn_batch(self.preprocess_batch(batch)).items():
                         report.setdefault(k, []).append(v)
             return report
+        if self._dueling:
+            return _duel.learn(self, replay_buffer, bs, rounds, trace)
         if self._conservative:
             return _cql.learn(self, replay_buffer, bs, rounds, trace)
         self._bind(bs)
@@ -376,6 +390,8 @@ class _B200DQNMixin:
     def learn_batch(self, batch) -> dict:
         """`DeepTDLearning.learn_batch` on a caller-supplied batch (raw ids, or the one-hot
         tensors the reference's preprocess_batch produces)."""
+        if self._dueling:
+            return _duel.learn_batch(self, batch)
         if self._conservative:
             return _cql.learn_batch(self, batch)
         B = len(batch)
@@ -406,6 +422,8 @@ class _B200DQNMixin:
     # ------------------------------------------------------------------ act
     def q_values(self, states: torch.Tensor, target: bool = False) -> torch.Tensor:
         """Q(s, a) for every action id: [n, obs] -> [n, n_actions]."""
+        if self._dueling:
+            return _duel.q_values(self, states, target)
         if self._conservative:
             return _cql.q_values(self, states, target)
         self._bind(1)
@@ -419,10 +437,14 @@ class _B200DQNMixin:
         return out
 
     def act(self, subjective_state, available_action_space, exploit: bool = False):
-        """`DeepTDLearning.act` (deep_td_learning.py:200-254)."""
-        qs = self.q_values(torch.as_tensor(subjective_state).reshape(1, -1))[0]
-        ids = available_action_space.actions_batch.reshape(available_action_space.n, -1)[:, 0].long().to(qs.device)
-        q_avail = qs[ids]
+        """`DeepTDLearning.act` (deep_td_learning.py:200-254).  A dueling network's advantage mean runs over the available
+        actions only, as get_q_values does with the available set as its query."""
+        ids = available_action_space.actions_batch.reshape(available_action_space.n, -1)[:, 0].long()
+        if self._dueling:
+            q_avail = _duel.q_values(self, torch.as_tensor(subjective_state).reshape(1, -1), False, ids.view(1, -1))[0]
+        else:
+            qs = self.q_values(torch.as_tensor(subjective_state).reshape(1, -1))[0]
+            q_avail = qs[ids.to(qs.device)]
         best = int(torch.argmax(q_avail))
         exploit_action = available_action_space.actions[best]
         if exploit or self.exploration_module is None:
@@ -442,6 +464,8 @@ class B200LearnerGroup:
             raise ValueError("need one replay buffer per learner")
         if any(getattr(l, "_conservative", False) for l in learners):
             raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no conservative (CQL) update")
+        if any(getattr(l, "_dueling", False) for l in learners):
+            raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no dueling network")
         self.learners, self.buffers = list(learners), list(buffers)
 
     def learn(self) -> list:
