@@ -556,7 +556,9 @@ int64_t prl_qrdqn_last_launches(const prl_qrdqn *qr);
  *   + Q(s_b, c_b[1])]: the reference gathers the current-action values with the ONE-HOT action, so its second term reads
  *   columns 0 and 1, not the taken action; c_b[k] are the current slots including padding (id 0);
  *   one AdamW(amsgrad) step.  Reported loss: mean_b |q_b - y_b| (the Bellman error only).
- * 2 <= n_actions <= 255 (A = 1 makes the reference's gather index out of range).  Flat layout (fp32, row-major [out][in]):
+ * 2 <= n_actions <= 255 (A = 1 makes the reference's gather index out of range); max_batch (n_actions + 1)
+ * max(hidden1, hidden2) < 2^31 (32-bit element offsets of the slot rows; param_count / workspace_bytes return -1 and
+ * create returns EINVAL beyond it).  Flat layout (fp32, row-major [out][in]):
  * W1[h1][obs + A] b1 W2[h2][h1] b2 W3[1][h2] b3, as prl_dqn.  Sharded buffers, continuous-action buffers, buffers of
  * other obs_dim / n_actions, and batch / rounds above the configured maxima are rejected (EINVAL) before any launch. */
 typedef struct prl_cql_cfg {
@@ -610,7 +612,9 @@ int64_t prl_cql_last_launches(const prl_cql *cql);
  *   V' = fl(fl(V_t(s') + Adv_t(s', a*)) - Adv_t(s', a*)) (the target net called with the single query a*).
  * Per round: when (training_steps + 1) % target_update_freq == 0, FIRST target = tau * online + (1 - tau) * target;
  * y = V' gamma (1 - terminated) + r; L = mean (q - y)^2; one AdamW(amsgrad) step.  Reported loss: mean |q - y|.
- * 1 <= n_actions <= 255.  Flat layout (fp32, row-major [out][in], torch's parameter order): state_arch W1 b1 W2 b2 W3 b3,
+ * 1 <= n_actions <= 255; max_batch (n_actions + 1) max(adv_h1, adv_h2) < 2^31 (32-bit element offsets of the slot rows;
+ * param_count / workspace_bytes return -1 and create returns EINVAL beyond it).  Flat layout (fp32, row-major [out][in],
+ * torch's parameter order): state_arch W1 b1 W2 b2 W3 b3,
  * value_arch W1 b1 W2 b2 W3 b3, advantage_arch W1 b1 W2 b2 W3 b3.  Sharded buffers, continuous-action buffers, buffers of
  * other obs_dim / n_actions, and batch / rounds above the configured maxima are rejected (EINVAL) before any launch. */
 typedef struct prl_duel_cfg {

@@ -20,7 +20,9 @@ derivative: |dq_i| becomes w_i (|q_i - y_i| + scale(q_i) + scale(y_i)) 2 / B, so
 the rounding noise of q - y and not by its own tiny value.  The arg-max of DoubleDQN is not continuous: a row whose
 top two online values are closer than a kernel's rounding (next_action_gap) has to be left out of a comparison.
 
-make_data and check are the data builder and the elementwise comparison of the GPU shape tests.
+cql_step is the same step for the conservative learner (csrc/cql.cu): the online pass over A + 1 slots per row and the
+CQL term's slot gradients.  make_data and check are the data builder and the elementwise comparison of the GPU shape
+tests.
 """
 from __future__ import annotations
 
@@ -139,17 +141,80 @@ def dqn_step(w, wt, batch: dict, obs: int, n_actions: int, gamma: float, hidden=
     return value, scale
 
 
+def cql_step(w, wt, batch: dict, obs: int, n_actions: int, gamma: float, alpha: float, hidden=(64, 64),
+             double: bool = False, curr_ids=None) -> tuple:
+    """One conservative (CQL) DQN step in float64 (csrc/cql.cu, oracle/cql_oracle.py), on the batch of dqn_step.  The
+    online pass runs over A + 1 slots per row: the A current slots (curr_ids [B, A], padding with id 0 taking part;
+    None: slot k holds k) and, as slot A, the taken action.  y as in dqn_step.  Slot gradients of mean (q - y)^2 +
+    alpha cql (the reference's CQL term, whose second part reads columns 0 and 1 of the current-slot values):
+        taken slot:     2 / B (q - y)
+        current slot k: alpha (softmax_k / B - n_k / (B A)),   n_0 = A - 1, n_1 = 1, n_k = 0 otherwise
+    The backward pass runs over the B (A + 1) slot rows: the state columns and b1 see each row's sum over its slots, the
+    action columns are scattered by slot id.  The |.| rule does not apply to exp: the scale of a current slot's gradient is
+    alpha (p_k (s_k + sum_j p_j s_j + 1) / B + n_k / (B A)) with s the scale of the logits (an error e_j of logit j moves
+    p_k by p_k (e_k - sum_j p_j e_j); the trailing p_k / B covers the rounding of expf and of the division).  Returns
+    (value, scale) as dqn_step, with q_all [B, A + 1] (the slot values) in place of z1 / z2."""
+    dev = torch.as_tensor(w).device
+    f64 = lambda x: torch.as_tensor(x).to(device=dev, dtype=torch.float64)  # noqa: E731
+    state, next_state = f64(batch["state"]), f64(batch["next_state"])
+    reward, term = f64(batch["reward"]), f64(batch["terminated"])
+    action = torch.as_tensor(batch["action"]).long().to(dev)
+    avail_ids = torch.as_tensor(batch["avail_ids"]).long().to(dev)
+    avail_n = torch.as_tensor(batch["avail_n"]).long().to(dev)
+    B, A = state.shape[0], n_actions
+    curr = (torch.arange(A, device=dev).repeat(B, 1) if curr_ids is None
+            else torch.as_tensor(curr_ids).long().to(dev).view(B, A))
+    cids = torch.cat([curr, action.view(B, 1)], 1)                                     # [B, A + 1]
+    onehot = torch.eye(A, dtype=torch.float64, device=dev)[cids.reshape(-1)]
+    xs = state.repeat_interleave(A + 1, dim=0)
+    net, net_t = unflatten(f64(w), obs, A, hidden), unflatten(f64(wt), obs, A, hidden)
+    absnet, absnet_t = tuple(p.abs() for p in net), tuple(p.abs() for p in net_t)
+    a_star = _double_action(net, next_state, avail_ids, avail_n) if double else None
+
+    z1, h1, z2, h2, q_all = _forward(net, xs, onehot)
+    m1, m2 = (z1 > 0).to(torch.float64), (z2 > 0).to(torch.float64)
+    _, sh1, _, sh2, sq_all = _forward(absnet, xs.abs(), onehot)
+    q_all, sq_all = q_all.view(B, A + 1), sq_all.view(B, A + 1)
+    q, sq = q_all[:, A], sq_all[:, A]
+    y = _target(net_t, next_state, avail_ids, avail_n, gamma, term, reward, a_star)
+    sy = _target(absnet_t, next_state.abs(), avail_ids, avail_n, gamma, term, reward.abs(), a_star)
+
+    n_k = torch.zeros(A, dtype=torch.float64, device=dev)
+    n_k[0], n_k[1] = A - 1, 1
+    p = torch.softmax(q_all[:, :A], dim=1)
+    s = sq_all[:, :A]
+    dq = torch.cat([alpha * (p / B - n_k / (B * A)), ((q - y) * (2.0 / B)).view(B, 1)], 1)
+    sdq = torch.cat([alpha * (p * (s + (p * s).sum(1, keepdim=True) + 1.0) / B + n_k / (B * A)),
+                     (((q - y).abs() + sq + sy) * (2.0 / B)).view(B, 1)], 1)
+    g = _backward(net, xs, onehot, m1, m2, h1, h2, dq.reshape(-1))
+    sg = _backward(absnet, xs.abs(), onehot, m1, m2, sh1, sh2, sdq.reshape(-1))
+
+    def pack(d, q, y, q_all, mae):
+        out = dict(d, q=q, y=y, q_all=q_all, mae=mae)
+        out["grad"] = torch.cat([torch.cat([d["dW1s"], d["dW1a"]], 1).reshape(-1), d["db1"], d["dW2"].reshape(-1),
+                                 d["db2"], d["dW3"].reshape(-1), d["db3"]])
+        return out
+
+    return pack(g, q, y, q_all, (q - y).abs().mean()), pack(sg, sq, sy, sq_all, (sq + sy).mean())
+
+
 def relu_margin(w, state, action, obs: int, n_actions: int, hidden=(64, 64)) -> torch.Tensor:
-    """Per row: the smallest |pre-activation| / scale over both hidden layers of the network `w` at (state, action).  A
-    row whose margin exceeds a kernel's relative rounding error has the same ReLU derivatives in the kernel as here.
-    Runs on the device of `w`; returns a CPU tensor."""
+    """Per row: the smallest |pre-activation| / scale over both hidden layers of the network `w` at (state, action).
+    `action`: [B] ids, or a [B, S] matrix of slot ids (a learner whose online pass evaluates S slots per row): then the
+    smallest over every slot of the row.  A row whose margin exceeds a kernel's relative rounding error has the same ReLU
+    derivatives in the kernel as here.  Runs on the device of `w`; returns a CPU tensor."""
     w = torch.as_tensor(w)
     state = torch.as_tensor(state).to(device=w.device, dtype=torch.float64)
-    onehot = torch.eye(n_actions, dtype=torch.float64, device=w.device)[torch.as_tensor(action).long().to(w.device)]
+    ids = torch.as_tensor(action).long().to(w.device)
+    ids = ids.view(-1, 1) if ids.dim() == 1 else ids
+    B, S = ids.shape
+    onehot = torch.eye(n_actions, dtype=torch.float64, device=w.device)[ids.reshape(-1)]
+    state = state.repeat_interleave(S, dim=0)
     net = unflatten(w, obs, n_actions, hidden)
     z1, _, z2, _, _ = _forward(net, state, onehot)
     s1, _, s2, _, _ = _forward(tuple(p.abs() for p in net), state.abs(), onehot)
-    return torch.minimum((z1.abs() / s1).min(1)[0], (z2.abs() / s2).min(1)[0]).cpu()
+    m = torch.minimum((z1.abs() / s1).min(1)[0], (z2.abs() / s2).min(1)[0])
+    return m.view(B, S).min(1)[0].cpu()
 
 
 def next_action_gap(w, next_state, avail_ids, avail_n, obs: int, n_actions: int, hidden=(64, 64)) -> torch.Tensor:
@@ -199,14 +264,22 @@ def block_view(flat: torch.Tensor, name: str, obs: int, n_actions: int, hidden=(
 
 
 def make_data(w, obs: int, n_actions: int, B: int, seed: int, dynamic: bool, margin: float, hidden=(64, 64),
-              double: bool = False) -> dict:
+              double: bool = False, all_slots: bool = False, margin_fn=None, gap_fn=None) -> dict:
     """2 B + 16 transitions (host tensors, push order) for a shape test of a learner with online parameters `w`:
     about 20 % terminal, some truncated, random actions, full or (`dynamic`) random next-action sets.  A row is kept
     only if every online pre-activation clears `margin` of its scale (relu_margin) and, for DoubleDQN, the online
     next-action gap clears it too (next_action_gap), so a kernel's rounding cannot flip a ReLU derivative or a*.
+    `all_slots`: the online pass evaluates every action id as well as the taken one (the A + 1 slots of the conservative
+    and dueling learners; any current set drawn from those ids is then covered too), so the margin is taken over the
+    [B, A + 1] slot matrix.  `margin_fn(w, state, slot_ids)` / `gap_fn(w, next_state, ids, n)` replace relu_margin /
+    next_action_gap for another network (defaults: the VanillaQValueNetwork of `obs`, `n_actions`, `hidden`).
     Candidates are drawn in batches of 3 (2 B + 16) until enough rows are kept; the fp64 filters run on the device of
     `w`."""
     from oracle.synth import make_transitions
+    if margin_fn is None:
+        margin_fn = lambda w, s, a: relu_margin(w, s, a, obs, n_actions, hidden)  # noqa: E731
+    if gap_fn is None:
+        gap_fn = lambda w, s, ids, n: next_action_gap(w, s, ids, n, obs, n_actions, hidden)  # noqa: E731
     n = 2 * B + 16
     keys = ("state", "action", "reward", "next_state", "terminated", "truncated", "next_avail_ids", "next_avail_n")
     kept = {k: [] for k in keys}
@@ -220,10 +293,12 @@ def make_data(w, obs: int, n_actions: int, B: int, seed: int, dynamic: bool, mar
         if not dynamic:
             d["next_avail_ids"] = np.tile(np.arange(n_actions), (3 * n, 1))
             d["next_avail_n"] = np.full(3 * n, n_actions)
-        ok = relu_margin(w, d["state"], d["action"], obs, n_actions, hidden) >= margin
+        slots = d["action"]
+        if all_slots:
+            slots = np.concatenate([np.tile(np.arange(n_actions), (3 * n, 1)), d["action"].reshape(-1, 1)], 1)
+        ok = margin_fn(w, d["state"], slots) >= margin
         if double:
-            ok &= next_action_gap(w, d["next_state"], d["next_avail_ids"], d["next_avail_n"], obs, n_actions,
-                                  hidden) >= margin
+            ok &= gap_fn(w, d["next_state"], d["next_avail_ids"], d["next_avail_n"]) >= margin
         keep = np.flatnonzero(ok.numpy())[:n - have]
         for k in keys:
             kept[k].append(d[k][keep])

@@ -203,6 +203,11 @@ static int cql_check(const prl_cql_cfg *c) {
                 "n_actions must be in [2, %d]: the reference's CQL term gathers column 1 of the current-action values", kMaxA);
     PRL_REQUIRE(c->target_update_freq > 0, "target_update_freq must be positive");
     PRL_REQUIRE(c->max_batch > 0 && c->max_rounds > 0, "max_batch / max_rounds must be positive");
+    // the online pass over B (A + 1) slot rows indexes its activations (and the tensor-core operand rows) with 32-bit ints
+    const int64_t slot_elems = (int64_t)c->max_batch * (c->n_actions + 1) * (c->hidden1 > c->hidden2 ? c->hidden1 : c->hidden2);
+    PRL_REQUIRE(slot_elems < ((int64_t)1 << 31),
+                "max_batch * (n_actions + 1) * max(hidden1, hidden2) = %lld must stay below 2^31 (32-bit element offsets)",
+                (long long)slot_elems);
     return PRL_OK;
 }
 
@@ -342,7 +347,7 @@ static int cql_round(prl_cql *s, prl_buf *buf, int B, cudaStream_t st) {
     small++;
     // ---------------- backward through the online net over B*(A+1) rows
     L.bwd_w(s->dq, 1, 0, BA1, 1, mat(s->c2, H2), H2, g + s->W3, H2, 0, g + s->b3, 0);
-    k_head_bwd<<<(BA1 * H2 + eb - 1) / eb, eb, 0, st>>>(BA1, H2, s->dq, w + s->W3, 0, s->c2, s->dc2);
+    k_head_bwd<<<(unsigned)(((long long)BA1 * H2 + eb - 1) / eb), eb, 0, st>>>(BA1, H2, s->dq, w + s->W3, 0, s->c2, s->dc2);
     L.bwd_w(s->dc2, H2, 0, BA1, H2, mat(s->c1, H1), H1, g + s->W2, H1, 0, g + s->b2, 0);
     L.bwd_x(s->dc2, H2, 0, BA1, H2, w + s->W2, H1, 0, 0, H1, s->dc1, H1, 0, s->c1, H1, 0, false);
     k_slot_rowsum<<<(B * H1 + eb - 1) / eb, eb, 0, st>>>(B, A + 1, H1, s->dc1, s->dh1);

@@ -248,6 +248,11 @@ static int duel_check(const prl_duel_cfg *c) {
     PRL_REQUIRE(c->n_actions >= 1 && c->n_actions <= kMaxA, "n_actions must be in [1, %d]: next-action ids are stored as bytes", kMaxA);
     PRL_REQUIRE(c->target_update_freq > 0, "target_update_freq must be positive");
     PRL_REQUIRE(c->max_batch > 0 && c->max_rounds > 0, "max_batch / max_rounds must be positive");
+    // the advantage net over B (A + 1) slot rows indexes its activations (and the tensor-core operand rows) with 32-bit ints
+    const int64_t slot_elems = (int64_t)c->max_batch * (c->n_actions + 1) * (c->adv_h1 > c->adv_h2 ? c->adv_h1 : c->adv_h2);
+    PRL_REQUIRE(slot_elems < ((int64_t)1 << 31),
+                "max_batch * (n_actions + 1) * max(adv_h1, adv_h2) = %lld must stay below 2^31 (32-bit element offsets)",
+                (long long)slot_elems);
     return PRL_OK;
 }
 
@@ -409,7 +414,7 @@ static int duel_round(prl_duel *s, prl_buf *buf, int B, cudaStream_t st) {
     small++;
     // ---------------- advantage net backward over B*(A+1) rows; the slots' layer-1 gradients summed per row
     L.bwd_w(s->dAdv, 1, 0, BA1, 1, mat(on.a2, ad.h2), ad.h2, g + ad.W3, ad.h2, 0, g + ad.b3, 0);
-    k_head_bwd<<<(BA1 * ad.h2 + eb - 1) / eb, eb, 0, st>>>(BA1, ad.h2, s->dAdv, w + ad.W3, 0, on.a2, s->da2);
+    k_head_bwd<<<(unsigned)(((long long)BA1 * ad.h2 + eb - 1) / eb), eb, 0, st>>>(BA1, ad.h2, s->dAdv, w + ad.W3, 0, on.a2, s->da2);
     L.bwd_w(s->da2, ad.h2, 0, BA1, ad.h2, mat(on.a1, ad.h1), ad.h1, g + ad.W2, ad.h1, 0, g + ad.b2, 0);
     L.bwd_x(s->da2, ad.h2, 0, BA1, ad.h2, w + ad.W2, ad.h1, 0, 0, ad.h1, s->da1, ad.h1, 0, on.a1, ad.h1, 0, false);
     k_slot_rowsum<<<(B * ad.h1 + eb - 1) / eb, eb, 0, st>>>(B, A + 1, ad.h1, s->da1, s->dPa);

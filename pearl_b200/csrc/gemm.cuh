@@ -259,13 +259,14 @@ struct GemmLauncher {
 };
 
 // ------------------------------------------------------------------ pieces shared by the actor-critic learners
-// dC2[z][m][j] = dq[z][m] * W3[z][j] * (c2 > 0)      (backward through the scalar head)
+// dC2[z][m][j] = dq[z][m] * W3[z][j] * (c2 > 0)      (backward through the scalar head).  B * H < 2^31; the thread index is
+// unsigned so that the last block of such a launch does not wrap
 static __global__ void k_head_bwd(int B, int H, const float *__restrict__ dq, const float *__restrict__ w3, long long w_net_stride,
                            const float *__restrict__ c2, float *__restrict__ dc2) {
     const int z = blockIdx.z;
-    const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= B * H) return;
-    const int m = e / H, j = e - m * H;
+    const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (unsigned)(B * H)) return;
+    const int e = (int)t, m = e / H, j = e - m * H;
     const size_t o = (size_t)z * B * H + e;
     dc2[o] = (c2[o] > 0.f) ? dq[z * B + m] * __ldg(w3 + z * w_net_stride + j) : 0.f;
 }

@@ -130,6 +130,21 @@ class _B200DQNMixin:
                 and need_batch <= self._bound_batch):
             self._refresh_optimizer_binding(params)
             return
+        # the configuration is checked before anything is released or allocated: a refused shape leaves the bound handle as it was
+        self._libh = _lib.init(device.index if device.index is not None else torch.cuda.current_device())
+        hp = self._adam_hparams()
+        bound_batch = max(int(need_batch), int(self._batch_size) if self._batch_size > 0 else 0, 1)
+        cfg = _duel.make_cfg(self, hp, bound_batch) if self._dueling else \
+            _cql.make_cfg(self, hp, bound_batch) if self._conservative else _lib.DqnCfg(
+            obs_dim=self._obs_dim, n_actions=self._n_actions, hidden1=self._hidden[0], hidden2=self._hidden[1],
+            double_dqn=int(self._double), target_update_freq=int(self._target_update_freq),
+            max_batch=bound_batch, max_rounds=self._max_rounds, rows_per_cta=self._rows_per_cta,
+            lr=hp["lr"], beta1=hp["beta1"], beta2=hp["beta2"], eps=hp["eps"],
+            weight_decay=hp["weight_decay"], gamma=float(self._discount_factor),
+            tau=float(self._soft_update_tau))
+        P_cfg = int(self._c("param_count")(C.byref(cfg)))
+        if P_cfg < 0:
+            raise ValueError(_lib.last_error())
         old_state = None
         if self._handle.value:
             st0 = self._optimizer.state.get(params[0], {})
@@ -139,8 +154,6 @@ class _B200DQNMixin:
                 old_step = int(self._c("adam_step")(self._handle))
             self._c("destroy")(self._handle)
             self._handle = C.c_void_p(0)
-        self._libh = _lib.init(device.index if device.index is not None else torch.cuda.current_device())
-        hp = self._adam_hparams()
         w = self._flatten(self._Q, device)
         wt = self._flatten(self._Q_target, device)
         P = w.numel()
@@ -154,16 +167,8 @@ class _B200DQNMixin:
             step = int(float(opt_state[params[0]]["step"]))
         else:
             m, v, vmax = (torch.zeros(P, dtype=torch.float32, device=device) for _ in range(3))
-        self._bound_batch = max(int(need_batch), int(self._batch_size) if self._batch_size > 0 else 0, 1)
-        cfg = _duel.make_cfg(self, hp, self._bound_batch) if self._dueling else \
-            _cql.make_cfg(self, hp, self._bound_batch) if self._conservative else _lib.DqnCfg(
-            obs_dim=self._obs_dim, n_actions=self._n_actions, hidden1=self._hidden[0], hidden2=self._hidden[1],
-            double_dqn=int(self._double), target_update_freq=int(self._target_update_freq),
-            max_batch=self._bound_batch, max_rounds=self._max_rounds, rows_per_cta=self._rows_per_cta,
-            lr=hp["lr"], beta1=hp["beta1"], beta2=hp["beta2"], eps=hp["eps"],
-            weight_decay=hp["weight_decay"], gamma=float(self._discount_factor),
-            tau=float(self._soft_update_tau))
-        if int(self._c("param_count")(C.byref(cfg))) != P:
+        self._bound_batch = bound_batch
+        if P_cfg != P:
             raise RuntimeError("parameter count mismatch between the module and the fused kernel")
         ws_bytes = int(self._c("workspace_bytes")(C.byref(cfg)))
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)

@@ -61,6 +61,29 @@ def test_param_count_matches_torch_module():
     assert lib.prl_dqn_workspace_bytes(ctypes.byref(cfg)) > 0
 
 
+def test_slot_expanded_learners_refuse_shapes_past_32_bit_offsets():
+    """The conservative and dueling learners index their B (A + 1) slot rows with 32-bit element offsets: a shape with
+    max_batch (n_actions + 1) max(slot-expanded width) >= 2^31 is refused by param_count / workspace_bytes (and so by
+    create) with a message naming the limit; one row less is accepted.  Host arithmetic only, nothing is allocated."""
+    from pearl_b200 import _lib
+    lib = _lib.load()
+    # 8192 * 256 * 1024 = 2^31: batch 8192, 255 actions, width 1024 (about 32 GB of workspace)
+    for B, ok in ((8191, True), (8192, False)):
+        cql = _lib.CqlCfg(obs_dim=4, n_actions=255, hidden1=1024, hidden2=7, target_update_freq=10, max_batch=B, max_rounds=1)
+        duel = _lib.DuelCfg(obs_dim=4, n_actions=255, feature_dim=3, state_h1=5, state_h2=5, value_h1=5, value_h2=5,
+                            adv_h1=7, adv_h2=1024, target_update_freq=10, max_batch=B, max_rounds=1)
+        for fn, cfg in ((lib.prl_cql_param_count, cql), (lib.prl_cql_workspace_bytes, cql),
+                        (lib.prl_duel_param_count, duel), (lib.prl_duel_workspace_bytes, duel)):
+            got = fn(ctypes.byref(cfg))
+            if ok:
+                assert got > 0, _lib.last_error()
+            else:
+                assert got == -1 and "2^31" in _lib.last_error()
+    ws = lib.prl_cql_workspace_bytes(ctypes.byref(_lib.CqlCfg(obs_dim=4, n_actions=255, hidden1=1024, hidden2=7,
+                                                              target_update_freq=10, max_batch=8191, max_rounds=1)))
+    assert ws > 2 * 8191 * 256 * 1024 * 4      # c1 and dc1 alone
+
+
 def test_no_cpu_fallback():
     import torch
     if torch.cuda.is_available():
