@@ -27,6 +27,7 @@
 #include <new>
 
 #include "common.cuh"
+#include "dqn_family.cuh"
 #include "gemm.cuh"
 
 using namespace prl;
@@ -153,38 +154,17 @@ __global__ void __launch_bounds__(128) k_cql_target(int B, int A, int dbl, const
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_cql {
+struct prl_cql : DqnRounds<prl_cql, CqlCall> {
+    static constexpr const char *kFn = "prl_cql", *kName = "CQL";
     prl_cql_cfg cfg;
     int P;
     int W1, b1, W2, b2, W3, b3;
     float *q, *q_t, *q_m, *q_v, *q_x;
-    int64_t adam_step;
     // workspace
     float *S, *S2, *R, *T, *P1, *c1, *c2, *qa, *P1t, *c1t, *c2t, *qt, *qn, *dq, *rowabs, *dc2, *dc1, *dh1, *grad;
     int *cnt, *ids, *cids;
-    int32_t *slots, *logical;
-    float2 *scal;
-    int *target_on;
-    CqlCall *call;
-    int *round_idx;
-    size_t tail_bytes;
-    bool use_graph;
-    cudaGraphExec_t graph_exec[2];            // [0] rounds from a replay buffer, [1] learn_batch on a dense batch
-    int graph_batch[2];
-    const uint32_t *graph_buf;
-    int graph_dynamic;
-    int launches_per_round;
-    char *tail_host[2];
-    cudaEvent_t tail_done[2];
-    int tail_next;
-    int64_t last_launches;
+    static int round(prl_cql *s, prl_buf *buf, int B, cudaStream_t st);
 };
-
-static int64_t al64(int64_t x) { return (x + 255) / 256 * 256; }
-
-// per-call tail of the workspace: scal float2[MR] | target_on int32[MR] | call (8-byte aligned) | round_idx
-static size_t cql_call_offset(int MR) { return ((size_t)MR * 12 + 7) / 8 * 8; }
-static size_t cql_tail_bytes(int MR) { return cql_call_offset(MR) + sizeof(CqlCall) + 4; }
 
 static void cql_layout(prl_cql *s) {
     const prl_cql_cfg &c = s->cfg;
@@ -217,27 +197,24 @@ extern "C" int64_t prl_cql_param_count(const prl_cql_cfg *c) {
     return t.P;
 }
 
-struct CqlWs { int64_t off[32]; int64_t total; };
-static CqlWs cql_ws(const prl_cql_cfg *c, int P) {
-    CqlWs w; int64_t o = 0; int k = 0;
-    const int64_t B = c->max_batch, O = c->obs_dim, A = c->n_actions, BA = B * A, BA1 = B * (A + 1);
-    const int64_t H1 = c->hidden1, H2 = c->hidden2;
-    auto add = [&](int64_t words) { w.off[k++] = o; o = al64(o + words * 4); };
-    add(B * O); add(B * O); add(B); add(B);                                   // S S2 R T
-    add(B * H1); add(BA1 * H1); add(BA1 * H2); add(BA1);                      // P1 c1 c2 qa     (online, A + 1 slots per row)
-    add(B * H1); add(BA * H1); add(BA * H2); add(BA); add(BA);                // P1t c1t c2t qt qn (next slots)
-    add(BA1); add(B);                                                         // dq rowabs
-    add(BA1 * H2); add(BA1 * H1); add(B * H1); add(P);                        // dc2 dc1 dh1 grad
-    add(B); add(BA); add(BA1);                                                // cnt ids cids (int32)
-    add((int64_t)c->max_rounds * B); add((int64_t)c->max_rounds * B);        // slots logical (int32)
-    add(((int64_t)cql_tail_bytes(c->max_rounds) + 3) / 4);                    // scal | target_on | call | round_idx
-    w.total = o;
-    return w;
+// the workspace, in order; base == null: only its size
+static int64_t cql_carve(prl_cql *s, void *base) {
+    const prl_cql_cfg &c = s->cfg;
+    const int64_t B = c.max_batch, O = c.obs_dim, A = c.n_actions, BA = B * A, BA1 = B * (A + 1), H1 = c.hidden1, H2 = c.hidden2;
+    Carve w{(char *)base};
+    w(s->S, B * O); w(s->S2, B * O); w(s->R, B); w(s->T, B);
+    w(s->P1, B * H1); w(s->c1, BA1 * H1); w(s->c2, BA1 * H2); w(s->qa, BA1);                 // online, A + 1 slots per row
+    w(s->P1t, B * H1); w(s->c1t, BA * H1); w(s->c2t, BA * H2); w(s->qt, BA); w(s->qn, BA);   // next slots
+    w(s->dq, BA1); w(s->rowabs, B);
+    w(s->dc2, BA1 * H2); w(s->dc1, BA1 * H1); w(s->dh1, B * H1); w(s->grad, s->P);
+    w(s->cnt, B); w(s->ids, BA); w(s->cids, BA1);
+    s->carve_tail(w, c.max_rounds, B);
+    return w.bytes;
 }
 extern "C" int64_t prl_cql_workspace_bytes(const prl_cql_cfg *c) {
     if (cql_check(c)) return -1;
     prl_cql t; t.cfg = *c; cql_layout(&t);
-    return cql_ws(c, t.P).total;
+    return cql_carve(&t, nullptr);
 }
 
 extern "C" int prl_cql_create(prl_cql **out, const prl_cql_cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq,
@@ -251,64 +228,18 @@ extern "C" int prl_cql_create(prl_cql **out, const prl_cql_cfg *cfg, float *w, f
     cql_layout(s);
     s->q = w; s->q_t = w_target; s->q_m = exp_avg; s->q_v = exp_avg_sq; s->q_x = max_exp_avg_sq;
     s->adam_step = adam_step;
-    CqlWs ws = cql_ws(cfg, s->P);
-    char *b = (char *)workspace;
-    float **f[] = {&s->S, &s->S2, &s->R, &s->T, &s->P1, &s->c1, &s->c2, &s->qa, &s->P1t, &s->c1t, &s->c2t, &s->qt, &s->qn,
-                   &s->dq, &s->rowabs, &s->dc2, &s->dc1, &s->dh1, &s->grad};
-    int k = 0;
-    for (auto p : f) *p = (float *)(b + ws.off[k++]);
-    s->cnt = (int *)(b + ws.off[k++]); s->ids = (int *)(b + ws.off[k++]); s->cids = (int *)(b + ws.off[k++]);
-    s->slots = (int32_t *)(b + ws.off[k++]); s->logical = (int32_t *)(b + ws.off[k++]);
-    char *tail = b + ws.off[k++];
-    const int MR = cfg->max_rounds;
-    s->scal = (float2 *)tail;
-    s->target_on = (int *)(tail + (size_t)MR * 8);
-    s->call = (CqlCall *)(tail + cql_call_offset(MR));
-    s->round_idx = (int *)(s->call + 1);
-    s->tail_bytes = cql_tail_bytes(MR);
-    s->tail_next = 0; s->use_graph = true; s->graph_exec[0] = s->graph_exec[1] = nullptr; s->graph_batch[0] = s->graph_batch[1] = 0;
-    s->graph_buf = nullptr; s->graph_dynamic = -1; s->last_launches = 0; s->launches_per_round = 0;
-    cudaError_t e = cudaSuccess;
-    int made = 0;   // pinned buffer / event pairs fully created
-    s->tail_host[0] = s->tail_host[1] = nullptr;
-    for (int i = 0; i < 2 && e == cudaSuccess; i++) {
-        e = cudaHostAlloc((void **)&s->tail_host[i], s->tail_bytes, cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->tail_done[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) made++;
-    }
-    if (e != cudaSuccess) {
-        for (int i = 0; i < made; i++) { cudaEventDestroy(s->tail_done[i]); cudaFreeHost(s->tail_host[i]); }
-        if (made < 2 && s->tail_host[made]) cudaFreeHost(s->tail_host[made]);   // its event was not created
-        delete s;
-        return fail(PRL_ECUDA, "prl_cql_create: %s", cudaGetErrorString(e));
-    }
-    *out = s;
-    return PRL_OK;
+    cql_carve(s, workspace);
+    return prl_cql::open(s, out);
 }
-extern "C" int prl_cql_destroy(prl_cql *s) {
-    if (!s) return PRL_OK;
-    for (int i = 0; i < 2; i++) { cudaEventSynchronize(s->tail_done[i]); cudaEventDestroy(s->tail_done[i]); cudaFreeHost(s->tail_host[i]); }
-    for (int i = 0; i < 2; i++) if (s->graph_exec[i]) cudaGraphExecDestroy(s->graph_exec[i]);
-    delete s;
-    return PRL_OK;
-}
-extern "C" int64_t prl_cql_adam_step(const prl_cql *s) { return s ? s->adam_step : -1; }
-extern "C" int prl_cql_set_adam_step(prl_cql *s, int64_t step) {
-    PRL_REQUIRE(s, "null handle");
-    PRL_REQUIRE(step >= 0, "the AdamW step count must be non-negative");
-    s->adam_step = step;
-    return PRL_OK;
-}
-
-extern "C" int prl_cql_set_lr(prl_cql *s, double lr) {
-    PRL_REQUIRE(s, "null handle");
-    PRL_REQUIRE(lr >= 0.0, "the learning rate must be non-negative");
-    s->cfg.lr = lr;
-    return PRL_OK;
-}
+extern "C" int prl_cql_destroy(prl_cql *s) { return prl_cql::destroy(s); }
+extern "C" int64_t prl_cql_adam_step(const prl_cql *s) { return prl_cql::adam_step_of(s); }
+extern "C" int prl_cql_set_adam_step(prl_cql *s, int64_t step) { return prl_cql::set_adam_step(s, step); }
+extern "C" int prl_cql_set_lr(prl_cql *s, double lr) { return prl_cql::set_lr(s, lr); }
+extern "C" int prl_cql_set_graph(prl_cql *s, int enable) { return prl_cql::set_graph(s, enable); }
+extern "C" int64_t prl_cql_last_launches(const prl_cql *s) { return prl_cql::last_launches_of(s); }
 
 // one learner round, launched (or captured) on `st`; buf == null: the dense batch of the call block (learn_batch)
-static int cql_round(prl_cql *s, prl_buf *buf, int B, cudaStream_t st) {
+int prl_cql::round(prl_cql *s, prl_buf *buf, int B, cudaStream_t st) {
     const prl_cql_cfg &c = s->cfg;
     const int O = c.obs_dim, A = c.n_actions, D = O + A, H1 = c.hidden1, H2 = c.hidden2, BA = B * A, BA1 = B * (A + 1);
     // the decay factor is overridden by call->decay (k_adamw's decay pointer)
@@ -363,84 +294,11 @@ static int cql_round(prl_cql *s, prl_buf *buf, int B, cudaStream_t st) {
     return PRL_OK;
 }
 
-// per-call block (Adam scalars of every round as torch evaluates them in double, target-update flags, decay, alpha,
-// pointers), uploaded on `st`.  steps0 = the training-step count the reference's learn_batch sees in round 0; round r
-// updates the target first when (steps0 + r + 1) % target_update_freq == 0.
-static int cql_upload(prl_cql *s, int rounds, int64_t steps0, double alpha, float *out_loss, const CqlCall &dense, cudaStream_t st) {
-    const prl_cql_cfg &c = s->cfg;
-    const int sb = s->tail_next; s->tail_next ^= 1;
-    PRL_CUDA(cudaEventSynchronize(s->tail_done[sb]));
-    char *tail = s->tail_host[sb];
-    const int MR = c.max_rounds;
-    float2 *hs = reinterpret_cast<float2 *>(tail);
-    int *on = reinterpret_cast<int *>(tail + (size_t)MR * 8);
-    for (int r = 0; r < rounds; r++) {
-        const double step = (double)(s->adam_step + r + 1);
-        const double bc1 = 1.0 - pow(c.beta1, step), bc2 = 1.0 - pow(c.beta2, step);
-        hs[r] = make_float2((float)(c.lr / bc1), (float)sqrt(bc2));
-        on[r] = (steps0 + r + 1) % c.target_update_freq == 0 ? 1 : 0;
-    }
-    CqlCall *hc = reinterpret_cast<CqlCall *>(tail + cql_call_offset(MR));
-    *hc = dense;
-    hc->slots = s->slots; hc->out_loss = out_loss;
-    hc->decay = (float)(1.0 - c.lr * c.weight_decay);
-    hc->alpha = (float)alpha;
-    *reinterpret_cast<int *>(hc + 1) = 0;
-    PRL_CUDA(cudaMemcpyAsync(s->scal, tail, s->tail_bytes, cudaMemcpyHostToDevice, st));
-    PRL_CUDA(cudaEventRecord(s->tail_done[sb], st));
-    return PRL_OK;
-}
-
-static int cql_run(prl_cql *s, prl_buf *buf, int rounds, int batch, cudaStream_t st) {
-    const int g = buf ? 0 : 1;
-    const int dynamic = (buf && (buf->desc.flags & PRL_BUF_DYNAMIC_ACTIONS)) ? 1 : 0;
-    if (s->use_graph) {
-        if (!s->graph_exec[g] || s->graph_batch[g] != batch || (buf && (s->graph_buf != buf->records || s->graph_dynamic != dynamic))) {
-            if (s->graph_exec[g]) { cudaGraphExecDestroy(s->graph_exec[g]); s->graph_exec[g] = nullptr; }
-            cudaStream_t cs;
-            PRL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-            cudaGraph_t graph = nullptr;
-            cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-            if (e == cudaSuccess) {
-                cql_round(s, buf, batch, cs);
-                e = cudaStreamEndCapture(cs, &graph);
-            }
-            if (e == cudaSuccess) e = cudaGraphInstantiate(&s->graph_exec[g], graph, 0);
-            if (graph) cudaGraphDestroy(graph);
-            cudaStreamDestroy(cs);
-            if (e != cudaSuccess) { s->graph_exec[g] = nullptr; return fail(PRL_ECUDA, "prl_cql: graph capture failed: %s", cudaGetErrorString(e)); }
-            s->graph_batch[g] = batch;
-            if (buf) { s->graph_buf = buf->records; s->graph_dynamic = dynamic; }
-        }
-        for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec[g], st));
-    } else {
-        for (int r = 0; r < rounds; r++) {
-            int rc = cql_round(s, buf, batch, st);
-            if (rc) return rc;
-        }
-    }
-    PRL_CUDA(cudaGetLastError());
-    s->adam_step += rounds;
-    s->last_launches = (int64_t)s->launches_per_round * rounds;
-    return PRL_OK;
-}
-
 extern "C" int prl_cql_learn(prl_cql *s, prl_buf *buf, int rounds, int batch, int64_t training_steps, double alpha, float *out_loss,
                              int32_t *out_logical, void *stream_) {
-    PRL_REQUIRE(s && buf && out_loss, "null argument");
-    const prl_cql_cfg &c = s->cfg;
-    PRL_REQUIRE(rounds > 0 && rounds <= c.max_rounds && batch > 0 && batch <= c.max_batch, "rounds / batch outside the configured maxima");
-    PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.obs_dim == c.obs_dim && buf->desc.n_actions == c.n_actions,
-                "CQL needs a discrete-action buffer with obs_dim = %d and n_actions = %d", c.obs_dim, c.n_actions);
-    PRL_REQUIRE(buf->shard_world <= 1, "the buffer is one shard of a multi-GPU buffer: CQL samples local buffers only");
-    cudaStream_t st = (cudaStream_t)stream_;
-    int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
-    if (rc) return rc;
-    CqlCall dense;
-    memset(&dense, 0, sizeof(dense));
-    rc = cql_upload(s, rounds, training_steps + 1, alpha, out_loss, dense, st);   // PolicyLearner.learn counts the round first
-    if (rc) return rc;
-    return cql_run(s, buf, rounds, batch, st);
+    CqlCall dense{};
+    dense.alpha = (float)alpha;
+    return prl_cql::learn(s, buf, rounds, batch, training_steps, out_loss, out_logical, dense, stream_);
 }
 
 extern "C" int prl_cql_learn_batch(prl_cql *s, int batch, const float *state, const int32_t *action_id, const float *reward,
@@ -448,15 +306,11 @@ extern "C" int prl_cql_learn_batch(prl_cql *s, int batch, const float *state, co
                                    const int32_t *next_ids, const int32_t *next_count, int64_t training_steps, double alpha,
                                    float *out_loss, void *stream_) {
     PRL_REQUIRE(s && state && action_id && reward && next_state && terminated && out_loss, "null argument");
-    PRL_REQUIRE(batch > 0 && batch <= s->cfg.max_batch, "batch outside the configured maximum");
-    cudaStream_t st = (cudaStream_t)stream_;
-    CqlCall dense;
-    memset(&dense, 0, sizeof(dense));
+    CqlCall dense{};
     dense.d_state = state; dense.d_next_state = next_state; dense.d_reward = reward; dense.d_action_id = action_id;
     dense.d_curr_ids = curr_ids; dense.d_next_ids = next_ids; dense.d_next_cnt = next_count; dense.d_term = terminated;
-    int rc = cql_upload(s, 1, training_steps, alpha, out_loss, dense, st);
-    if (rc) return rc;
-    return cql_run(s, nullptr, 1, batch, st);
+    dense.alpha = (float)alpha;
+    return prl_cql::learn_batch(s, batch, training_steps, out_loss, dense, stream_);
 }
 
 // Q(s, a) for every action: the online forward of the round on n rows (chunks of max_batch rows through the workspace)
@@ -477,10 +331,3 @@ extern "C" int prl_cql_q_values(prl_cql *s, int n, const float *state, int targe
     PRL_CUDA(cudaGetLastError());
     return PRL_OK;
 }
-
-extern "C" int prl_cql_set_graph(prl_cql *s, int enable) {
-    PRL_REQUIRE(s, "null handle");
-    s->use_graph = enable != 0;
-    return PRL_OK;
-}
-extern "C" int64_t prl_cql_last_launches(const prl_cql *s) { return s ? s->last_launches : -1; }

@@ -865,8 +865,6 @@ extern "C" int prl_dqn_create(prl_dqn **out, const prl_dqn_cfg *cfg, float *w, f
     q->td = (float *)(base + ws.td);
     q->tc_tiles = prl_tc_tile_floats(cfg) ? (float *)(base + ws.tc_tiles) : nullptr;
     q->tmp_lay = tmp_layout(cfg);
-    q->scal_next = 0;
-    q->scal_host[0] = q->scal_host[1] = nullptr;
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&q->sm_count, cudaDevAttrMultiProcessorCount, dev);
@@ -878,10 +876,7 @@ extern "C" int prl_dqn_create(prl_dqn **out, const prl_dqn_cfg *cfg, float *w, f
     if (e == cudaSuccess) q->learn_smem = q->max_smem - (int)fa.sharedSizeBytes;
     if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, k_q_values);
     if (e == cudaSuccess) q->qv_smem = q->max_smem - (int)fa.sharedSizeBytes;
-    for (int i = 0; i < 2 && e == cudaSuccess; i++) {
-        e = cudaHostAlloc((void **)&q->scal_host[i], (size_t)cfg->max_rounds * 8, cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&q->scal_done[i], cudaEventDisableTiming);
-    }
+    if (e == cudaSuccess) e = q->stage.open((size_t)cfg->max_rounds * 8);
     if (e != cudaSuccess) {
         delete q;
         return fail(PRL_ECUDA, "prl_dqn_create: %s", cudaGetErrorString(e));
@@ -897,12 +892,7 @@ extern "C" int prl_dqn_create(prl_dqn **out, const prl_dqn_cfg *cfg, float *w, f
 
 extern "C" int prl_dqn_destroy(prl_dqn *q) {
     if (!q) return PRL_OK;
-    for (int i = 0; i < 2; i++)
-        if (q->scal_host[i]) {
-            cudaEventSynchronize(q->scal_done[i]);
-            cudaEventDestroy(q->scal_done[i]);
-            cudaFreeHost(q->scal_host[i]);
-        }
+    q->stage.close();
     if (q->t0) { cudaEventDestroy(q->t0); cudaEventDestroy(q->t1); }
     delete q;
     return PRL_OK;
@@ -1042,17 +1032,11 @@ static int choose_tiling(const prl_dqn *q, int B, int W, int *R_out, int *mch_ou
 // per-round optimizer scalars exactly as torch evaluates them (Python floats -> fp32)
 int prl_dqn_stage_scalars(prl_dqn *q, int rounds, cudaStream_t stream) {
     const prl_dqn_cfg &c = q->cfg;
-    const int sb = q->scal_next;
-    q->scal_next ^= 1;
-    PRL_CUDA(cudaEventSynchronize(q->scal_done[sb]));
-    for (int r = 0; r < rounds; r++) {
-        const double step = (double)(q->adam_step + r + 1);
-        const double bc1 = 1.0 - pow(c.beta1, step), bc2 = 1.0 - pow(c.beta2, step);
-        q->scal_host[sb][r] = make_float2((float)(c.lr / bc1), (float)sqrt(bc2));
-    }
-    PRL_CUDA(cudaMemcpyAsync(q->scal_dev, q->scal_host[sb], (size_t)rounds * 8, cudaMemcpyHostToDevice, stream));
-    PRL_CUDA(cudaEventRecord(q->scal_done[sb], stream));
-    return PRL_OK;
+    float2 *hs;
+    int rc = q->stage.wait(&hs);
+    if (rc) return rc;
+    for (int r = 0; r < rounds; r++) hs[r] = adam_scal(c.lr, c.beta1, c.beta2, q->adam_step + r + 1);
+    return q->stage.send(q->scal_dev, (size_t)rounds * 8, stream);
 }
 
 static int launch_learn(prl_dqn *q, const uint32_t *records, const prl_buf_layout &lay, int buf_flags,

@@ -2,6 +2,7 @@
 // one-SM-per-learner kernel (dqn_tc.cu).
 #pragma once
 #include "common.cuh"
+#include "host_runtime.cuh"
 
 namespace prl {
 
@@ -62,10 +63,7 @@ struct prl_dqn {
     float *tc_tiles;          // operand-layout weight tiles of the tensor-core learner (dqn_tc.cu), or null
     int32_t *tmp_slots;
     prl_buf_layout tmp_lay;
-    // pinned per-round optimizer scalars, double buffered
-    float2 *scal_host[2];
-    cudaEvent_t scal_done[2];
-    int scal_next;
+    prl::Stage stage;         // pinned per-round optimizer scalars
     int sm_count, max_smem;
     int learn_smem, qv_smem;  // dynamic shared memory k_dqn_learn / k_q_values may use: max_smem minus their static part
     int last_launches, last_ctas, last_rows;

@@ -32,6 +32,7 @@
 #include <new>
 
 #include "common.cuh"
+#include "dqn_family.cuh"
 #include "gemm.cuh"
 
 using namespace prl;
@@ -189,41 +190,20 @@ struct DuelMlp { int W1, b1, W2, b2, W3, b3, in, h1, h2, out; };
 // activations of one forward pass on m rows with K advantage slots per row
 struct DuelAct { float *t1, *t2, *f, *v1, *v2, *V, *Pa, *a1, *a2, *adv; };
 
-struct prl_duel {
+struct prl_duel : DqnRounds<prl_duel, DuelCall> {
+    static constexpr const char *kFn = "prl_duel", *kName = "dueling DQN";
     prl_duel_cfg cfg;
     int P;
     DuelMlp st, va, ad;
     float *q, *q_t, *q_m, *q_v, *q_x;
-    int64_t adam_step;
     // workspace
     float *S, *S2, *R, *T;
     DuelAct on, nx;                           // online pass (kept for the backward pass); next-state pass scratch
     float *Vt, *At, *Vn, *An;                 // next-state V / advantages of the target and (DoubleDQN) online net
     float *dV, *dAdv, *rowabs, *da2, *da1, *dPa, *dv2, *dv1, *df, *dt2, *dt1, *grad;
     int *ids, *un, *cids;
-    int32_t *slots, *logical;
-    float2 *scal;
-    int *target_on;
-    DuelCall *call;
-    int *round_idx;
-    size_t tail_bytes;
-    bool use_graph;
-    cudaGraphExec_t graph_exec[2];            // [0] rounds from a replay buffer, [1] learn_batch on a dense batch
-    int graph_batch[2];
-    const uint32_t *graph_buf;
-    int graph_dynamic;
-    int launches_per_round;
-    char *tail_host[2];
-    cudaEvent_t tail_done[2];
-    int tail_next;
-    int64_t last_launches;
+    static int round(prl_duel *s, prl_buf *buf, int B, cudaStream_t st);
 };
-
-static int64_t al64(int64_t x) { return (x + 255) / 256 * 256; }
-
-// per-call tail of the workspace: scal float2[MR] | target_on int32[MR] | call (8-byte aligned) | round_idx
-static size_t duel_call_offset(int MR) { return ((size_t)MR * 12 + 7) / 8 * 8; }
-static size_t duel_tail_bytes(int MR) { return duel_call_offset(MR) + sizeof(DuelCall) + 4; }
 
 static void mlp_at(DuelMlp &m, int &o, int in, int h1, int h2, int out) {
     m.in = in; m.h1 = h1; m.h2 = h2; m.out = out;
@@ -262,32 +242,31 @@ extern "C" int64_t prl_duel_param_count(const prl_duel_cfg *c) {
     return t.P;
 }
 
-struct DuelWs { int64_t off[48]; int64_t total; };
-static DuelWs duel_ws(const prl_duel_cfg *c, int P) {
-    DuelWs w; int64_t o = 0; int k = 0;
-    const int64_t B = c->max_batch, O = c->obs_dim, A = c->n_actions, F = c->feature_dim, BA = B * A, BA1 = B * (A + 1);
-    auto add = [&](int64_t words) { w.off[k++] = o; o = al64(o + words * 4); };
-    add(B * O); add(B * O); add(B); add(B);                                               // S S2 R T
-    for (int64_t rows : {BA1, BA}) {                                                      // online pass, next-state pass
-        add(B * c->state_h1); add(B * c->state_h2); add(B * F);                           // t1 t2 f
-        add(B * c->value_h1); add(B * c->value_h2); add(B);                               // v1 v2 V
-        add(B * c->adv_h1); add(rows * c->adv_h1); add(rows * c->adv_h2); add(rows);      // Pa a1 a2 adv
-    }
-    add(B); add(BA); add(B); add(BA);                                                     // Vt At Vn An
-    add(B); add(BA1); add(B);                                                             // dV dAdv rowabs
-    add(BA1 * c->adv_h2); add(BA1 * c->adv_h1); add(B * c->adv_h1);                       // da2 da1 dPa
-    add(B * c->value_h2); add(B * c->value_h1); add(B * F);                               // dv2 dv1 df
-    add(B * c->state_h2); add(B * c->state_h1); add(P);                                   // dt2 dt1 grad
-    add(BA); add(BA); add(BA1);                                                           // ids un cids (int32)
-    add((int64_t)c->max_rounds * B); add((int64_t)c->max_rounds * B);                    // slots logical (int32)
-    add(((int64_t)duel_tail_bytes(c->max_rounds) + 3) / 4);                               // scal | target_on | call | round_idx
-    w.total = o;
-    return w;
+// the workspace, in order; base == null: only its size
+static int64_t duel_carve(prl_duel *s, void *base) {
+    const prl_duel_cfg &c = s->cfg;
+    const int64_t B = c.max_batch, O = c.obs_dim, A = c.n_actions, F = c.feature_dim, BA = B * A, BA1 = B * (A + 1);
+    Carve w{(char *)base};
+    w(s->S, B * O); w(s->S2, B * O); w(s->R, B); w(s->T, B);
+    auto act = [&](DuelAct &a, int64_t rows) {
+        w(a.t1, B * c.state_h1); w(a.t2, B * c.state_h2); w(a.f, B * F);
+        w(a.v1, B * c.value_h1); w(a.v2, B * c.value_h2); w(a.V, B);
+        w(a.Pa, B * c.adv_h1); w(a.a1, rows * c.adv_h1); w(a.a2, rows * c.adv_h2); w(a.adv, rows);
+    };
+    act(s->on, BA1); act(s->nx, BA);                                                     // online pass, next-state pass
+    w(s->Vt, B); w(s->At, BA); w(s->Vn, B); w(s->An, BA);
+    w(s->dV, B); w(s->dAdv, BA1); w(s->rowabs, B);
+    w(s->da2, BA1 * c.adv_h2); w(s->da1, BA1 * c.adv_h1); w(s->dPa, B * c.adv_h1);
+    w(s->dv2, B * c.value_h2); w(s->dv1, B * c.value_h1); w(s->df, B * F);
+    w(s->dt2, B * c.state_h2); w(s->dt1, B * c.state_h1); w(s->grad, s->P);
+    w(s->ids, BA); w(s->un, BA); w(s->cids, BA1);
+    s->carve_tail(w, c.max_rounds, B);
+    return w.bytes;
 }
 extern "C" int64_t prl_duel_workspace_bytes(const prl_duel_cfg *c) {
     if (duel_check(c)) return -1;
     prl_duel t; t.cfg = *c; duel_layout(&t);
-    return duel_ws(c, t.P).total;
+    return duel_carve(&t, nullptr);
 }
 
 extern "C" int prl_duel_create(prl_duel **out, const prl_duel_cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq,
@@ -301,64 +280,15 @@ extern "C" int prl_duel_create(prl_duel **out, const prl_duel_cfg *cfg, float *w
     duel_layout(s);
     s->q = w; s->q_t = w_target; s->q_m = exp_avg; s->q_v = exp_avg_sq; s->q_x = max_exp_avg_sq;
     s->adam_step = adam_step;
-    DuelWs ws = duel_ws(cfg, s->P);
-    char *b = (char *)workspace;
-    float **f[] = {&s->S, &s->S2, &s->R, &s->T,
-                   &s->on.t1, &s->on.t2, &s->on.f, &s->on.v1, &s->on.v2, &s->on.V, &s->on.Pa, &s->on.a1, &s->on.a2, &s->on.adv,
-                   &s->nx.t1, &s->nx.t2, &s->nx.f, &s->nx.v1, &s->nx.v2, &s->nx.V, &s->nx.Pa, &s->nx.a1, &s->nx.a2, &s->nx.adv,
-                   &s->Vt, &s->At, &s->Vn, &s->An, &s->dV, &s->dAdv, &s->rowabs, &s->da2, &s->da1, &s->dPa, &s->dv2, &s->dv1,
-                   &s->df, &s->dt2, &s->dt1, &s->grad};
-    int k = 0;
-    for (auto p : f) *p = (float *)(b + ws.off[k++]);
-    s->ids = (int *)(b + ws.off[k++]); s->un = (int *)(b + ws.off[k++]); s->cids = (int *)(b + ws.off[k++]);
-    s->slots = (int32_t *)(b + ws.off[k++]); s->logical = (int32_t *)(b + ws.off[k++]);
-    char *tail = b + ws.off[k++];
-    const int MR = cfg->max_rounds;
-    s->scal = (float2 *)tail;
-    s->target_on = (int *)(tail + (size_t)MR * 8);
-    s->call = (DuelCall *)(tail + duel_call_offset(MR));
-    s->round_idx = (int *)(s->call + 1);
-    s->tail_bytes = duel_tail_bytes(MR);
-    s->tail_next = 0; s->use_graph = true; s->graph_exec[0] = s->graph_exec[1] = nullptr; s->graph_batch[0] = s->graph_batch[1] = 0;
-    s->graph_buf = nullptr; s->graph_dynamic = -1; s->last_launches = 0; s->launches_per_round = 0;
-    cudaError_t e = cudaSuccess;
-    int made = 0;   // pinned buffer / event pairs fully created
-    s->tail_host[0] = s->tail_host[1] = nullptr;
-    for (int i = 0; i < 2 && e == cudaSuccess; i++) {
-        e = cudaHostAlloc((void **)&s->tail_host[i], s->tail_bytes, cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->tail_done[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) made++;
-    }
-    if (e != cudaSuccess) {
-        for (int i = 0; i < made; i++) { cudaEventDestroy(s->tail_done[i]); cudaFreeHost(s->tail_host[i]); }
-        if (made < 2 && s->tail_host[made]) cudaFreeHost(s->tail_host[made]);   // its event was not created
-        delete s;
-        return fail(PRL_ECUDA, "prl_duel_create: %s", cudaGetErrorString(e));
-    }
-    *out = s;
-    return PRL_OK;
+    duel_carve(s, workspace);
+    return prl_duel::open(s, out);
 }
-extern "C" int prl_duel_destroy(prl_duel *s) {
-    if (!s) return PRL_OK;
-    for (int i = 0; i < 2; i++) { cudaEventSynchronize(s->tail_done[i]); cudaEventDestroy(s->tail_done[i]); cudaFreeHost(s->tail_host[i]); }
-    for (int i = 0; i < 2; i++) if (s->graph_exec[i]) cudaGraphExecDestroy(s->graph_exec[i]);
-    delete s;
-    return PRL_OK;
-}
-extern "C" int64_t prl_duel_adam_step(const prl_duel *s) { return s ? s->adam_step : -1; }
-extern "C" int prl_duel_set_adam_step(prl_duel *s, int64_t step) {
-    PRL_REQUIRE(s, "null handle");
-    PRL_REQUIRE(step >= 0, "the AdamW step count must be non-negative");
-    s->adam_step = step;
-    return PRL_OK;
-}
-
-extern "C" int prl_duel_set_lr(prl_duel *s, double lr) {
-    PRL_REQUIRE(s, "null handle");
-    PRL_REQUIRE(lr >= 0.0, "the learning rate must be non-negative");
-    s->cfg.lr = lr;
-    return PRL_OK;
-}
+extern "C" int prl_duel_destroy(prl_duel *s) { return prl_duel::destroy(s); }
+extern "C" int64_t prl_duel_adam_step(const prl_duel *s) { return prl_duel::adam_step_of(s); }
+extern "C" int prl_duel_set_adam_step(prl_duel *s, int64_t step) { return prl_duel::set_adam_step(s, step); }
+extern "C" int prl_duel_set_lr(prl_duel *s, double lr) { return prl_duel::set_lr(s, lr); }
+extern "C" int prl_duel_set_graph(prl_duel *s, int enable) { return prl_duel::set_graph(s, enable); }
+extern "C" int64_t prl_duel_last_launches(const prl_duel *s) { return prl_duel::last_launches_of(s); }
 
 // the network `net` on m states X: trunk feature, V, and the advantage at K slots per row (ids [m][K]; null: slot k holds
 // k).  The feature part of advantage layer 1 is computed once per row and expanded per slot.  Returns the small launches.
@@ -379,7 +309,7 @@ static int duel_fwd(const prl_duel *s, GemmLauncher &L, const float *net, const 
 }
 
 // one learner round, launched (or captured) on `st`; buf == null: the dense batch of the call block (learn_batch)
-static int duel_round(prl_duel *s, prl_buf *buf, int B, cudaStream_t st) {
+int prl_duel::round(prl_duel *s, prl_buf *buf, int B, cudaStream_t st) {
     const prl_duel_cfg &c = s->cfg;
     const DuelMlp &sa = s->st, &va = s->va, &ad = s->ad;
     const int O = c.obs_dim, A = c.n_actions, F = c.feature_dim, BA1 = B * (A + 1);
@@ -445,83 +375,9 @@ static int duel_round(prl_duel *s, prl_buf *buf, int B, cudaStream_t st) {
     return PRL_OK;
 }
 
-// per-call block (Adam scalars of every round as torch evaluates them in double, target-update flags, decay, the
-// query-alone switch, pointers), uploaded on `st`.  steps0 = the training-step count the reference's learn_batch sees in
-// round 0; round r updates the target first when (steps0 + r + 1) % target_update_freq == 0.
-static int duel_upload(prl_duel *s, int rounds, int64_t steps0, float *out_loss, const DuelCall &dense, cudaStream_t st) {
-    const prl_duel_cfg &c = s->cfg;
-    const int sb = s->tail_next; s->tail_next ^= 1;
-    PRL_CUDA(cudaEventSynchronize(s->tail_done[sb]));
-    char *tail = s->tail_host[sb];
-    const int MR = c.max_rounds;
-    float2 *hs = reinterpret_cast<float2 *>(tail);
-    int *on = reinterpret_cast<int *>(tail + (size_t)MR * 8);
-    for (int r = 0; r < rounds; r++) {
-        const double step = (double)(s->adam_step + r + 1);
-        const double bc1 = 1.0 - pow(c.beta1, step), bc2 = 1.0 - pow(c.beta2, step);
-        hs[r] = make_float2((float)(c.lr / bc1), (float)sqrt(bc2));
-        on[r] = (steps0 + r + 1) % c.target_update_freq == 0 ? 1 : 0;
-    }
-    DuelCall *hc = reinterpret_cast<DuelCall *>(tail + duel_call_offset(MR));
-    *hc = dense;
-    hc->slots = s->slots; hc->out_loss = out_loss;
-    hc->decay = (float)(1.0 - c.lr * c.weight_decay);
-    *reinterpret_cast<int *>(hc + 1) = 0;
-    PRL_CUDA(cudaMemcpyAsync(s->scal, tail, s->tail_bytes, cudaMemcpyHostToDevice, st));
-    PRL_CUDA(cudaEventRecord(s->tail_done[sb], st));
-    return PRL_OK;
-}
-
-static int duel_run(prl_duel *s, prl_buf *buf, int rounds, int batch, cudaStream_t st) {
-    const int g = buf ? 0 : 1;
-    const int dynamic = (buf && (buf->desc.flags & PRL_BUF_DYNAMIC_ACTIONS)) ? 1 : 0;
-    if (s->use_graph) {
-        if (!s->graph_exec[g] || s->graph_batch[g] != batch || (buf && (s->graph_buf != buf->records || s->graph_dynamic != dynamic))) {
-            if (s->graph_exec[g]) { cudaGraphExecDestroy(s->graph_exec[g]); s->graph_exec[g] = nullptr; }
-            cudaStream_t cs;
-            PRL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-            cudaGraph_t graph = nullptr;
-            cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-            if (e == cudaSuccess) {
-                duel_round(s, buf, batch, cs);
-                e = cudaStreamEndCapture(cs, &graph);
-            }
-            if (e == cudaSuccess) e = cudaGraphInstantiate(&s->graph_exec[g], graph, 0);
-            if (graph) cudaGraphDestroy(graph);
-            cudaStreamDestroy(cs);
-            if (e != cudaSuccess) { s->graph_exec[g] = nullptr; return fail(PRL_ECUDA, "prl_duel: graph capture failed: %s", cudaGetErrorString(e)); }
-            s->graph_batch[g] = batch;
-            if (buf) { s->graph_buf = buf->records; s->graph_dynamic = dynamic; }
-        }
-        for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec[g], st));
-    } else {
-        for (int r = 0; r < rounds; r++) {
-            int rc = duel_round(s, buf, batch, st);
-            if (rc) return rc;
-        }
-    }
-    PRL_CUDA(cudaGetLastError());
-    s->adam_step += rounds;
-    s->last_launches = (int64_t)s->launches_per_round * rounds;
-    return PRL_OK;
-}
-
 extern "C" int prl_duel_learn(prl_duel *s, prl_buf *buf, int rounds, int batch, int64_t training_steps, float *out_loss,
                               int32_t *out_logical, void *stream_) {
-    PRL_REQUIRE(s && buf && out_loss, "null argument");
-    const prl_duel_cfg &c = s->cfg;
-    PRL_REQUIRE(rounds > 0 && rounds <= c.max_rounds && batch > 0 && batch <= c.max_batch, "rounds / batch outside the configured maxima");
-    PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.obs_dim == c.obs_dim && buf->desc.n_actions == c.n_actions,
-                "dueling DQN needs a discrete-action buffer with obs_dim = %d and n_actions = %d", c.obs_dim, c.n_actions);
-    PRL_REQUIRE(buf->shard_world <= 1, "the buffer is one shard of a multi-GPU buffer: dueling DQN samples local buffers only");
-    cudaStream_t st = (cudaStream_t)stream_;
-    int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
-    if (rc) return rc;
-    DuelCall dense;
-    memset(&dense, 0, sizeof(dense));
-    rc = duel_upload(s, rounds, training_steps + 1, out_loss, dense, st);   // PolicyLearner.learn counts the round first
-    if (rc) return rc;
-    return duel_run(s, buf, rounds, batch, st);
+    return prl_duel::learn(s, buf, rounds, batch, training_steps, out_loss, out_logical, DuelCall{}, stream_);
 }
 
 extern "C" int prl_duel_learn_batch(prl_duel *s, int batch, const float *state, const int32_t *action_id, const float *reward,
@@ -529,16 +385,11 @@ extern "C" int prl_duel_learn_batch(prl_duel *s, int batch, const float *state, 
                                     const int32_t *next_ids, const uint8_t *next_unavailable, int64_t training_steps,
                                     float *out_loss, void *stream_) {
     PRL_REQUIRE(s && state && action_id && reward && next_state && terminated && out_loss, "null argument");
-    PRL_REQUIRE(batch > 0 && batch <= s->cfg.max_batch, "batch outside the configured maximum");
-    cudaStream_t st = (cudaStream_t)stream_;
-    DuelCall dense;
-    memset(&dense, 0, sizeof(dense));
+    DuelCall dense{};
     dense.d_state = state; dense.d_next_state = next_state; dense.d_reward = reward; dense.d_action_id = action_id;
     dense.d_curr_ids = curr_ids; dense.d_next_ids = next_ids; dense.d_next_unavail = next_unavailable; dense.d_term = terminated;
     dense.query_alone = curr_ids ? 0 : 1;
-    int rc = duel_upload(s, 1, training_steps, out_loss, dense, st);
-    if (rc) return rc;
-    return duel_run(s, nullptr, 1, batch, st);
+    return prl_duel::learn_batch(s, batch, training_steps, out_loss, dense, stream_);
 }
 
 // Q(s, .) over an id set of K slots per row, the mean over that set: the forward of the round on n rows (chunks of
@@ -559,10 +410,3 @@ extern "C" int prl_duel_q_values(prl_duel *s, int n, const float *state, const i
     PRL_CUDA(cudaGetLastError());
     return PRL_OK;
 }
-
-extern "C" int prl_duel_set_graph(prl_duel *s, int enable) {
-    PRL_REQUIRE(s, "null handle");
-    s->use_graph = enable != 0;
-    return PRL_OK;
-}
-extern "C" int64_t prl_duel_last_launches(const prl_duel *s) { return s ? s->last_launches : -1; }

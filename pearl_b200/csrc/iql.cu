@@ -20,6 +20,7 @@
 
 #include "common.cuh"
 #include "gemm.cuh"
+#include "host_runtime.cuh"
 
 using namespace prl;
 
@@ -168,13 +169,9 @@ struct prl_iql {
     int graph_batch[2];
     const uint32_t *graph_buf;
     int launches_per_round;
-    float2 *scal_host[2];
-    cudaEvent_t scal_done[2];
-    int scal_next;
+    Stage stage;
     int64_t last_launches;
 };
-
-static int64_t al64(int64_t x) { return (x + 255) / 256 * 256; }
 
 static bool iql_discrete(const prl_iql_cfg &c) { return c.n_actions > 0; }
 
@@ -226,31 +223,29 @@ extern "C" int64_t prl_iql_value_param_count(const prl_iql_cfg *c) {
     return t.Pv;
 }
 
-struct IqlWs { int64_t off[40]; int64_t total; };
-static IqlWs iql_ws(const prl_iql_cfg *c, int Pa, int Pc, int Pv) {
-    IqlWs w; int64_t o = 0; int k = 0;
-    const int64_t B = c->max_batch, O = c->obs_dim, N = iql_discrete(*c) ? c->n_actions : c->act_dim;
-    const int64_t C1 = c->critic_h1, C2 = c->critic_h2;
-    auto add = [&](int64_t words) { w.off[k++] = o; o = al64(o + words * 4); };
-    add(2 * B * O); add(B * (c->act_dim > 0 ? c->act_dim : 1)); add(B); add(B);                  // S|S' Act R T
-    add(2 * B * c->value_h1); add(2 * B * c->value_h2); add(2 * B);                              // v1 v2 V
-    add(2 * B * C1); add(2 * B * C1); add(2 * B * C2); add(2 * B);                               // P c1t c2t qt
-    add(2 * B * C1); add(2 * B * C2); add(2 * B);                                                // c1 c2 q
-    add(B * c->actor_h1); add(B * c->actor_h2); add(B * N); add(B * N);                          // h1 h2 out dout
-    add(B); add(B * c->value_h2); add(B * c->value_h1);                                          // dV dv2 dv1
-    add(2 * B); add(2 * B * C2); add(2 * B * C1);                                                // dq dc2 dc1
-    add(B * c->actor_h2); add(B * c->actor_h1);                                                  // dh2 dh1
-    add(Pa); add(2 * (int64_t)Pc); add(Pv);                                                      // g_actor g_critic g_value
-    add(B);                                                                                      // act (int32)
-    add((int64_t)c->max_rounds * B); add((int64_t)c->max_rounds * B);                           // slots logical (int32)
-    add(6 * (int64_t)c->max_rounds + 64);                                                        // scal_a | scal_c | scal_v | call | round_idx
-    w.total = o;
-    return w;
+// the workspace, in order; base == null: only its size
+static int64_t iql_carve(prl_iql *s, void *base) {
+    const prl_iql_cfg &c = s->cfg;
+    const int64_t B = c.max_batch, O = c.obs_dim, N = iql_discrete(c) ? c.n_actions : c.act_dim, C1 = c.critic_h1, C2 = c.critic_h2;
+    Carve w{(char *)base};
+    w(s->S, 2 * B * O); w(s->Act, B * (c.act_dim > 0 ? c.act_dim : 1)); w(s->R, B); w(s->T, B);   // S|S' Act R T
+    w(s->v1, 2 * B * c.value_h1); w(s->v2, 2 * B * c.value_h2); w(s->V, 2 * B);
+    w(s->P, 2 * B * C1); w(s->c1t, 2 * B * C1); w(s->c2t, 2 * B * C2); w(s->qt, 2 * B);
+    w(s->c1, 2 * B * C1); w(s->c2, 2 * B * C2); w(s->q, 2 * B);
+    w(s->h1, B * c.actor_h1); w(s->h2, B * c.actor_h2); w(s->out, B * N); w(s->dout, B * N);
+    w(s->dV, B); w(s->dv2, B * c.value_h2); w(s->dv1, B * c.value_h1);
+    w(s->dq, 2 * B); w(s->dc2, 2 * B * C2); w(s->dc1, 2 * B * C1);
+    w(s->dh2, B * c.actor_h2); w(s->dh1, B * c.actor_h1);
+    w(s->g_actor, s->Pa); w(s->g_critic, 2 * (int64_t)s->Pc); w(s->g_value, s->Pv);
+    w(s->act, B);
+    w(s->slots, c.max_rounds * B); w(s->logical, c.max_rounds * B);
+    w(s->scal_a, 3 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | scal_v | call | round_idx
+    return w.bytes;
 }
 extern "C" int64_t prl_iql_workspace_bytes(const prl_iql_cfg *c) {
     if (iql_check(c)) return -1;
     prl_iql t; t.cfg = *c; iql_layout(&t);
-    return iql_ws(c, t.Pa, t.Pc, t.Pv).total;
+    return iql_carve(&t, nullptr);
 }
 
 extern "C" int prl_iql_create(prl_iql **out, const prl_iql_cfg *cfg, float *actor_w, float *actor_m, float *actor_v, float *actor_vmax,
@@ -271,40 +266,20 @@ extern "C" int prl_iql_create(prl_iql **out, const prl_iql_cfg *cfg, float *acto
     s->value = value_w; s->value_m = value_m; s->value_v = value_v; s->value_x = value_vmax;
     s->low = low_dev; s->high = high_dev;
     s->adam_step = adam_step;
-    IqlWs w = iql_ws(cfg, s->Pa, s->Pc, s->Pv);
-    char *b = (char *)workspace;
-    float **f[] = {&s->S, &s->Act, &s->R, &s->T, &s->v1, &s->v2, &s->V, &s->P, &s->c1t, &s->c2t, &s->qt, &s->c1, &s->c2, &s->q, &s->h1,
-                   &s->h2, &s->out, &s->dout, &s->dV, &s->dv2, &s->dv1, &s->dq, &s->dc2, &s->dc1, &s->dh2, &s->dh1, &s->g_actor,
-                   &s->g_critic, &s->g_value};
-    int k = 0;
-    for (auto p : f) *p = (float *)(b + w.off[k++]);
-    s->act = (int *)(b + w.off[k++]);
-    s->slots = (int32_t *)(b + w.off[k++]); s->logical = (int32_t *)(b + w.off[k++]);
-    s->scal_a = (float2 *)(b + w.off[k++]); s->scal_c = s->scal_a + cfg->max_rounds; s->scal_v = s->scal_c + cfg->max_rounds;
+    iql_carve(s, workspace);
+    s->scal_c = s->scal_a + cfg->max_rounds; s->scal_v = s->scal_c + cfg->max_rounds;
     s->call = (IqlCall *)(s->scal_v + cfg->max_rounds); s->round_idx = (int *)(s->call + 1);
     static_assert(sizeof(IqlCall) + 4 <= 64 * 4, "call block fits the reserved tail");
-    s->scal_next = 0; s->use_graph = true; s->graph_exec[0] = s->graph_exec[1] = nullptr; s->graph_batch[0] = s->graph_batch[1] = 0;
+    s->use_graph = true; s->graph_exec[0] = s->graph_exec[1] = nullptr; s->graph_batch[0] = s->graph_batch[1] = 0;
     s->graph_buf = nullptr; s->last_launches = 0; s->launches_per_round = 0;
-    cudaError_t e = cudaSuccess;
-    int made = 0;   // pinned buffer / event pairs fully created
-    s->scal_host[0] = s->scal_host[1] = nullptr;
-    for (int i = 0; i < 2 && e == cudaSuccess; i++) {
-        e = cudaHostAlloc((void **)&s->scal_host[i], (size_t)cfg->max_rounds * 24 + 256, cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->scal_done[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) made++;
-    }
-    if (e != cudaSuccess) {
-        for (int i = 0; i < made; i++) { cudaEventDestroy(s->scal_done[i]); cudaFreeHost(s->scal_host[i]); }
-        if (made < 2 && s->scal_host[made]) cudaFreeHost(s->scal_host[made]);   // its event was not created
-        delete s;
-        return fail(PRL_ECUDA, "prl_iql_create: %s", cudaGetErrorString(e));
-    }
+    cudaError_t e = s->stage.open((size_t)cfg->max_rounds * 24 + 256);
+    if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_iql_create: %s", cudaGetErrorString(e)); }
     *out = s;
     return PRL_OK;
 }
 extern "C" int prl_iql_destroy(prl_iql *s) {
     if (!s) return PRL_OK;
-    for (int i = 0; i < 2; i++) { cudaEventSynchronize(s->scal_done[i]); cudaEventDestroy(s->scal_done[i]); cudaFreeHost(s->scal_host[i]); }
+    s->stage.close();
     for (int i = 0; i < 2; i++) if (s->graph_exec[i]) cudaGraphExecDestroy(s->graph_exec[i]);
     delete s;
     return PRL_OK;
@@ -416,16 +391,14 @@ static int iql_round(prl_iql *s, prl_buf *buf, int B, cudaStream_t st) {
 static int iql_upload(prl_iql *s, int rounds, const int32_t *bits, float *out_value, float *out_critic, float *out_actor, const IqlCall &dense,
                       cudaStream_t st) {
     const prl_iql_cfg &c = s->cfg;
-    const int sb = s->scal_next; s->scal_next ^= 1;
-    PRL_CUDA(cudaEventSynchronize(s->scal_done[sb]));
-    float2 *hs = s->scal_host[sb];
+    float2 *hs;
+    int rc = s->stage.wait(&hs);
+    if (rc) return rc;
     const int MR = c.max_rounds;
     for (int r = 0; r < rounds; r++) {
-        const double step = (double)(s->adam_step + r + 1);
-        const double bc1 = 1.0 - pow(c.beta1, step), bc2 = 1.0 - pow(c.beta2, step);
-        hs[r] = make_float2((float)(c.actor_lr / bc1), (float)sqrt(bc2));
-        hs[MR + r] = make_float2((float)(c.critic_lr / bc1), (float)sqrt(bc2));
-        hs[2 * MR + r] = make_float2((float)(c.value_lr / bc1), (float)sqrt(bc2));
+        hs[r] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->adam_step + r + 1);
+        hs[MR + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->adam_step + r + 1);
+        hs[2 * MR + r] = adam_scal(c.value_lr, c.beta1, c.beta2, s->adam_step + r + 1);
     }
     IqlCall *hc = reinterpret_cast<IqlCall *>(hs + 3 * (size_t)MR);
     *hc = dense;
@@ -435,28 +408,15 @@ static int iql_upload(prl_iql *s, int rounds, const int32_t *bits, float *out_va
     hc->decay_v = (float)(1.0 - c.value_lr * c.weight_decay);
     *reinterpret_cast<int *>(hc + 1) = 0;
     // scal_a | scal_c | scal_v | call | round_idx are contiguous on the device in the same order
-    PRL_CUDA(cudaMemcpyAsync(s->scal_a, hs, 3 * (size_t)MR * 8 + sizeof(IqlCall) + 4, cudaMemcpyHostToDevice, st));
-    PRL_CUDA(cudaEventRecord(s->scal_done[sb], st));
-    return PRL_OK;
+    return s->stage.send(s->scal_a, 3 * (size_t)MR * 8 + sizeof(IqlCall) + 4, st);
 }
 
 static int iql_run(prl_iql *s, prl_buf *buf, int rounds, int batch, cudaStream_t st) {
     const int g = buf ? 0 : 1;
     if (s->use_graph) {
         if (!s->graph_exec[g] || s->graph_batch[g] != batch || (buf && s->graph_buf != buf->records)) {
-            if (s->graph_exec[g]) { cudaGraphExecDestroy(s->graph_exec[g]); s->graph_exec[g] = nullptr; }
-            cudaStream_t cs;
-            PRL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-            cudaGraph_t graph = nullptr;
-            cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-            if (e == cudaSuccess) {
-                iql_round(s, buf, batch, cs);
-                e = cudaStreamEndCapture(cs, &graph);
-            }
-            if (e == cudaSuccess) e = cudaGraphInstantiate(&s->graph_exec[g], graph, 0);
-            if (graph) cudaGraphDestroy(graph);
-            cudaStreamDestroy(cs);
-            if (e != cudaSuccess) { s->graph_exec[g] = nullptr; return fail(PRL_ECUDA, "prl_iql: graph capture failed: %s", cudaGetErrorString(e)); }
+            int rc = capture_graph(&s->graph_exec[g], "prl_iql", [&](cudaStream_t cs) { return iql_round(s, buf, batch, cs); });
+            if (rc) return rc;
             s->graph_batch[g] = batch;
             if (buf) s->graph_buf = buf->records;
         }

@@ -236,6 +236,7 @@ extern "C" int prl_ppo_gae(int n, const float *values_dev, float last_next_value
 #include <new>
 
 #include "gemm.cuh"
+#include "host_runtime.cuh"
 
 namespace {
 
@@ -367,9 +368,7 @@ struct prl_ppo {
     float2 *scal_a, *scal_c;
     PpoCall *call;
     int *round_idx;
-    float2 *scal_host[2];
-    cudaEvent_t scal_done[2];
-    int scal_next;
+    Stage stage;
     bool use_graph;
     cudaGraphExec_t graph_exec;
     int graph_batch;
@@ -416,27 +415,27 @@ extern "C" int64_t prl_ppo_critic_param_count(const prl_ppo_cfg *c) {
     prl_ppo t; t.cfg = *c; ppo_layout(&t);
     return t.Pc;
 }
-struct PpoWs { int64_t off[32]; int64_t total; };
-static PpoWs ppo_ws(const prl_ppo_cfg *c, int Pa, int Pc) {
-    PpoWs w; int64_t o = 0; int k = 0;
-    const int64_t R = c->max_batch > ppo_chunk(c) ? c->max_batch : ppo_chunk(c);   // rows of the widest pass
-    const int64_t hmax1 = c->actor_h1 > c->critic_h1 ? c->actor_h1 : c->critic_h1, hmax2 = c->actor_h2 > c->critic_h2 ? c->actor_h2 : c->critic_h2;
-    auto add = [&](int64_t bytes) { w.off[k++] = o; o = (o + bytes + 255) / 256 * 256; };
-    add(R * c->obs_dim * 4); add(R * hmax1 * 4); add(R * hmax2 * 4); add(R * c->n_actions * 4); add(R * 4);     // S h1 h2 logits v
-    add(R * 4); add(R * 4); add(R * 4); add(R * 4); add(R * c->n_actions * 4);                                       // gae lam old ap dlogits
-    add(R * hmax2 * 4); add(R * hmax1 * 4); add(R * 4); add((int64_t)Pa * 4); add((int64_t)Pc * 4);                // dh2 dh1 dv g_actor g_critic
-    add(c->max_rollout * 4); add(256);                                                                               // reward last_value
-    add(R * 4); add((int64_t)c->max_rounds * c->max_batch * 4); add((int64_t)c->max_rounds * c->max_batch * 4);     // act slots logical
-    add(c->max_rollout); add(c->max_rollout);                                                                        // term trunc
-    add((int64_t)c->max_rounds * 16 + 256);                                                                          // scal_a | scal_c | call | round_idx
-    add((c->max_rollout + 1) * 4);                                                                                   // GAE chain heads + count
-    w.total = o;
-    return w;
+// the workspace, in order; base == null: only its size
+static int64_t ppo_carve(prl_ppo *s, void *base) {
+    const prl_ppo_cfg &c = s->cfg;
+    const int64_t R = c.max_batch > ppo_chunk(&c) ? c.max_batch : ppo_chunk(&c);   // rows of the widest pass
+    const int64_t hmax1 = c.actor_h1 > c.critic_h1 ? c.actor_h1 : c.critic_h1, hmax2 = c.actor_h2 > c.critic_h2 ? c.actor_h2 : c.critic_h2;
+    const int64_t A = c.n_actions, MRB = (int64_t)c.max_rounds * c.max_batch;
+    Carve w{(char *)base};
+    w(s->S, R * c.obs_dim); w(s->h1, R * hmax1); w(s->h2, R * hmax2); w(s->logits, R * A); w(s->v, R);
+    w(s->gae, R); w(s->lam, R); w(s->old, R); w(s->ap, R); w(s->dlogits, R * A);
+    w(s->dh2, R * hmax2); w(s->dh1, R * hmax1); w(s->dv, R); w(s->g_actor, s->Pa); w(s->g_critic, s->Pc);
+    w(s->reward, c.max_rollout); w(s->last_value, 64);
+    w(s->act, R); w(s->slots, MRB); w(s->logical, MRB);
+    w(s->term, c.max_rollout); w(s->trunc, c.max_rollout);
+    w(s->scal_a, 2 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | call | round_idx
+    w(s->gae_heads, c.max_rollout + 1);                                                  // count, then the GAE chain heads
+    return w.bytes;
 }
 extern "C" int64_t prl_ppo_workspace_bytes(const prl_ppo_cfg *c) {
     if (ppo_check(c)) return -1;
     prl_ppo t; t.cfg = *c; ppo_layout(&t);
-    return ppo_ws(c, t.Pa, t.Pc).total;
+    return ppo_carve(&t, nullptr);
 }
 extern "C" int prl_ppo_create(prl_ppo **out, const prl_ppo_cfg *cfg, float *actor_w, float *actor_m, float *actor_v, float *actor_vmax,
                               float *critic_w, float *critic_m, float *critic_v, float *critic_vmax, int64_t adam_step, void *workspace) {
@@ -451,32 +450,20 @@ extern "C" int prl_ppo_create(prl_ppo **out, const prl_ppo_cfg *cfg, float *acto
     s->actor = actor_w; s->actor_m = actor_m; s->actor_v = actor_v; s->actor_x = actor_vmax;
     s->critic = critic_w; s->critic_m = critic_m; s->critic_v = critic_v; s->critic_x = critic_vmax;
     s->adam_step = adam_step;
-    PpoWs w = ppo_ws(cfg, s->Pa, s->Pc);
-    char *b = (char *)workspace;
-    int k = 0;
-    float **f[] = {&s->S, &s->h1, &s->h2, &s->logits, &s->v, &s->gae, &s->lam, &s->old, &s->ap, &s->dlogits, &s->dh2, &s->dh1, &s->dv,
-                   &s->g_actor, &s->g_critic, &s->reward, &s->last_value};
-    for (auto p : f) *p = (float *)(b + w.off[k++]);
-    s->act = (int32_t *)(b + w.off[k++]); s->slots = (int32_t *)(b + w.off[k++]); s->logical = (int32_t *)(b + w.off[k++]);
-    s->term = (uint8_t *)(b + w.off[k++]); s->trunc = (uint8_t *)(b + w.off[k++]);
-    s->scal_a = (float2 *)(b + w.off[k++]); s->scal_c = s->scal_a + cfg->max_rounds;
+    ppo_carve(s, workspace);
+    s->scal_c = s->scal_a + cfg->max_rounds;
     s->call = (PpoCall *)(s->scal_c + cfg->max_rounds); s->round_idx = (int *)(s->call + 1);
-    s->gae_heads = (int *)(b + w.off[k++]);
     static_assert(sizeof(PpoCall) + 4 <= 256, "call block fits the reserved tail");
-    s->scal_next = 0; s->use_graph = true; s->graph_exec = nullptr; s->graph_batch = 0; s->graph_buf = nullptr; s->last_launches = 0;
+    s->use_graph = true; s->graph_exec = nullptr; s->graph_batch = 0; s->graph_buf = nullptr; s->last_launches = 0;
     s->pre_n = 0;
-    cudaError_t e = cudaSuccess;
-    for (int i = 0; i < 2 && e == cudaSuccess; i++) {
-        e = cudaHostAlloc((void **)&s->scal_host[i], (size_t)cfg->max_rounds * 16 + 256, cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->scal_done[i], cudaEventDisableTiming);
-    }
+    cudaError_t e = s->stage.open((size_t)cfg->max_rounds * 16 + 256);
     if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_ppo_create: %s", cudaGetErrorString(e)); }
     *out = s;
     return PRL_OK;
 }
 extern "C" int prl_ppo_destroy(prl_ppo *s) {
     if (!s) return PRL_OK;
-    for (int i = 0; i < 2; i++) { cudaEventSynchronize(s->scal_done[i]); cudaEventDestroy(s->scal_done[i]); cudaFreeHost(s->scal_host[i]); }
+    s->stage.close();
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
     delete s;
     return PRL_OK;
@@ -607,41 +594,31 @@ extern "C" int prl_ppo_learn(prl_ppo *s, prl_buf *buf, int rounds, int batch, co
     cudaStream_t st = (cudaStream_t)stream_;
     int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
     if (rc) return rc;
-    const int sb = s->scal_next; s->scal_next ^= 1;
-    PRL_CUDA(cudaEventSynchronize(s->scal_done[sb]));
-    float2 *hs = s->scal_host[sb];
+    float2 *hs;
+    rc = s->stage.wait(&hs);
+    if (rc) return rc;
     for (int r = 0; r < rounds; r++) {
-        const double step = (double)(s->adam_step + r + 1);
-        const double bc1 = 1.0 - pow(c.beta1, step), bc2 = 1.0 - pow(c.beta2, step);
-        hs[r] = make_float2((float)(c.actor_lr / bc1), (float)sqrt(bc2));
-        hs[c.max_rounds + r] = make_float2((float)(c.critic_lr / bc1), (float)sqrt(bc2));
+        hs[r] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->adam_step + r + 1);
+        hs[c.max_rounds + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->adam_step + r + 1);
     }
     PpoCall *hc = reinterpret_cast<PpoCall *>(hs + 2 * (size_t)c.max_rounds);
     hc->logical = out_logical ? out_logical : s->logical; hc->slots = s->slots; hc->gae = gae_dev; hc->lam_return = lam_return_dev;
     hc->old_probs = action_probs_dev; hc->out_actor = out_actor_loss; hc->out_critic = out_critic_loss;
     *reinterpret_cast<int *>(hc + 1) = 0;
-    PRL_CUDA(cudaMemcpyAsync(s->scal_a, hs, 2 * (size_t)c.max_rounds * 8 + sizeof(PpoCall) + 4, cudaMemcpyHostToDevice, st));
-    PRL_CUDA(cudaEventRecord(s->scal_done[sb], st));
+    rc = s->stage.send(s->scal_a, 2 * (size_t)c.max_rounds * 8 + sizeof(PpoCall) + 4, st);
+    if (rc) return rc;
     if (s->use_graph) {
         if (!s->graph_exec || s->graph_batch != batch || s->graph_buf != buf->records) {
-            if (s->graph_exec) { cudaGraphExecDestroy(s->graph_exec); s->graph_exec = nullptr; }
-            cudaStream_t cs;
-            PRL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-            cudaGraph_t graph = nullptr;
-            cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-            if (e == cudaSuccess) {
-                ppo_round(s, buf, batch, cs);
-                e = cudaStreamEndCapture(cs, &graph);
-            }
-            if (e == cudaSuccess) e = cudaGraphInstantiate(&s->graph_exec, graph, 0);
-            if (graph) cudaGraphDestroy(graph);
-            cudaStreamDestroy(cs);
-            if (e != cudaSuccess) { s->graph_exec = nullptr; return fail(PRL_ECUDA, "prl_ppo_learn: graph capture failed: %s", cudaGetErrorString(e)); }
+            rc = capture_graph(&s->graph_exec, "prl_ppo_learn", [&](cudaStream_t cs) { return ppo_round(s, buf, batch, cs); });
+            if (rc) return rc;
             s->graph_batch = batch; s->graph_buf = buf->records;
         }
         for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec, st));
     } else {
-        for (int r = 0; r < rounds; r++) ppo_round(s, buf, batch, st);
+        for (int r = 0; r < rounds; r++) {
+            rc = ppo_round(s, buf, batch, st);
+            if (rc) return rc;
+        }
     }
     PRL_CUDA(cudaGetLastError());
     s->adam_step += rounds;

@@ -21,6 +21,7 @@
 #include <new>
 
 #include "common.cuh"
+#include "dqn_family.cuh"
 #include "gemm.cuh"
 
 using namespace prl;
@@ -181,38 +182,17 @@ __global__ void __launch_bounds__(256) k_qr_report(int B, int N, const float *__
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_qrdqn {
+struct prl_qrdqn : DqnRounds<prl_qrdqn, QrCall> {
+    static constexpr const char *kFn = "prl_qrdqn", *kName = "QR-DQN";
     prl_qrdqn_cfg cfg;
     int P;
     int W1, b1, W2, b2, W3, b3;
     float *q, *q_m, *q_v, *q_x, *q_t;
-    int64_t adam_step;
     // workspace
     float *S, *S2, *R, *T, *P1, *h1, *h2, *theta, *P1t, *c1t, *c2t, *qt, *tq, *dtheta, *rowabs, *dh2, *dh1, *grad;
     int *act, *cnt, *ids;
-    int32_t *slots, *logical;
-    float2 *scal;
-    int *target_on;
-    QrCall *call;
-    int *round_idx;
-    size_t tail_bytes;
-    bool use_graph;
-    cudaGraphExec_t graph_exec[2];            // [0] rounds from a replay buffer, [1] learn_batch on a dense batch
-    int graph_batch[2];
-    const uint32_t *graph_buf;
-    int graph_dynamic;
-    int launches_per_round;
-    char *tail_host[2];
-    cudaEvent_t tail_done[2];
-    int tail_next;
-    int64_t last_launches;
+    static int round(prl_qrdqn *s, prl_buf *buf, int B, cudaStream_t st);
 };
-
-static int64_t al64(int64_t x) { return (x + 255) / 256 * 256; }
-
-// per-call tail of the workspace: scal float2[MR] | target_on int32[MR] | call (8-byte aligned) | round_idx
-static size_t qr_call_offset(int MR) { return ((size_t)MR * 12 + 7) / 8 * 8; }
-static size_t qr_tail_bytes(int MR) { return qr_call_offset(MR) + sizeof(QrCall) + 4; }
 
 static void qr_layout(prl_qrdqn *s) {
     const prl_qrdqn_cfg &c = s->cfg;
@@ -240,27 +220,24 @@ extern "C" int64_t prl_qrdqn_param_count(const prl_qrdqn_cfg *c) {
     return t.P;
 }
 
-struct QrWs { int64_t off[32]; int64_t total; };
-static QrWs qr_ws(const prl_qrdqn_cfg *c, int P) {
-    QrWs w; int64_t o = 0; int k = 0;
-    const int64_t B = c->max_batch, O = c->obs_dim, A = c->n_actions, N = c->num_quantiles, BA = B * A;
-    const int64_t H1 = c->hidden1, H2 = c->hidden2;
-    auto add = [&](int64_t words) { w.off[k++] = o; o = al64(o + words * 4); };
-    add(B * O); add(B * O); add(B); add(B);                                   // S S2 R T
-    add(B * H1); add(B * H1); add(B * H2); add(B * N);                        // P1 h1 h2 theta      (online, taken action)
-    add(B * H1); add(BA * H1); add(BA * H2); add(BA * N);                     // P1t c1t c2t qt      (target, every slot)
-    add(B * N); add(B * N); add(B);                                           // tq dtheta rowabs
-    add(B * H2); add(B * H1); add(P);                                         // dh2 dh1 grad
-    add(B); add(B); add(BA);                                                  // act cnt ids (int32)
-    add((int64_t)c->max_rounds * B); add((int64_t)c->max_rounds * B);        // slots logical (int32)
-    add(((int64_t)qr_tail_bytes(c->max_rounds) + 3) / 4);                     // scal | target_on | call | round_idx
-    w.total = o;
-    return w;
+// the workspace, in order; base == null: only its size
+static int64_t qr_carve(prl_qrdqn *s, void *base) {
+    const prl_qrdqn_cfg &c = s->cfg;
+    const int64_t B = c.max_batch, O = c.obs_dim, A = c.n_actions, N = c.num_quantiles, BA = B * A, H1 = c.hidden1, H2 = c.hidden2;
+    Carve w{(char *)base};
+    w(s->S, B * O); w(s->S2, B * O); w(s->R, B); w(s->T, B);
+    w(s->P1, B * H1); w(s->h1, B * H1); w(s->h2, B * H2); w(s->theta, B * N);          // online, taken action
+    w(s->P1t, B * H1); w(s->c1t, BA * H1); w(s->c2t, BA * H2); w(s->qt, BA * N);       // target, every slot
+    w(s->tq, B * N); w(s->dtheta, B * N); w(s->rowabs, B);
+    w(s->dh2, B * H2); w(s->dh1, B * H1); w(s->grad, s->P);
+    w(s->act, B); w(s->cnt, B); w(s->ids, BA);
+    s->carve_tail(w, c.max_rounds, B);
+    return w.bytes;
 }
 extern "C" int64_t prl_qrdqn_workspace_bytes(const prl_qrdqn_cfg *c) {
     if (qr_check(c)) return -1;
     prl_qrdqn t; t.cfg = *c; qr_layout(&t);
-    return qr_ws(c, t.P).total;
+    return qr_carve(&t, nullptr);
 }
 
 extern "C" int prl_qrdqn_create(prl_qrdqn **out, const prl_qrdqn_cfg *cfg, float *q_w, float *q_m, float *q_v, float *q_vmax,
@@ -274,58 +251,17 @@ extern "C" int prl_qrdqn_create(prl_qrdqn **out, const prl_qrdqn_cfg *cfg, float
     qr_layout(s);
     s->q = q_w; s->q_m = q_m; s->q_v = q_v; s->q_x = q_vmax; s->q_t = q_target_w;
     s->adam_step = adam_step;
-    QrWs w = qr_ws(cfg, s->P);
-    char *b = (char *)workspace;
-    float **f[] = {&s->S, &s->S2, &s->R, &s->T, &s->P1, &s->h1, &s->h2, &s->theta, &s->P1t, &s->c1t, &s->c2t, &s->qt, &s->tq, &s->dtheta,
-                   &s->rowabs, &s->dh2, &s->dh1, &s->grad};
-    int k = 0;
-    for (auto p : f) *p = (float *)(b + w.off[k++]);
-    s->act = (int *)(b + w.off[k++]); s->cnt = (int *)(b + w.off[k++]); s->ids = (int *)(b + w.off[k++]);
-    s->slots = (int32_t *)(b + w.off[k++]); s->logical = (int32_t *)(b + w.off[k++]);
-    char *tail = b + w.off[k++];
-    const int MR = cfg->max_rounds;
-    s->scal = (float2 *)tail;
-    s->target_on = (int *)(tail + (size_t)MR * 8);
-    s->call = (QrCall *)(tail + qr_call_offset(MR));
-    s->round_idx = (int *)(s->call + 1);
-    s->tail_bytes = qr_tail_bytes(MR);
-    s->tail_next = 0; s->use_graph = true; s->graph_exec[0] = s->graph_exec[1] = nullptr; s->graph_batch[0] = s->graph_batch[1] = 0;
-    s->graph_buf = nullptr; s->graph_dynamic = -1; s->last_launches = 0; s->launches_per_round = 0;
-    cudaError_t e = cudaSuccess;
-    int made = 0;   // pinned buffer / event pairs fully created
-    s->tail_host[0] = s->tail_host[1] = nullptr;
-    for (int i = 0; i < 2 && e == cudaSuccess; i++) {
-        e = cudaHostAlloc((void **)&s->tail_host[i], s->tail_bytes, cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->tail_done[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) made++;
-    }
-    if (e != cudaSuccess) {
-        for (int i = 0; i < made; i++) { cudaEventDestroy(s->tail_done[i]); cudaFreeHost(s->tail_host[i]); }
-        if (made < 2 && s->tail_host[made]) cudaFreeHost(s->tail_host[made]);   // its event was not created
-        delete s;
-        return fail(PRL_ECUDA, "prl_qrdqn_create: %s", cudaGetErrorString(e));
-    }
-    *out = s;
-    return PRL_OK;
+    qr_carve(s, workspace);
+    return prl_qrdqn::open(s, out);
 }
-extern "C" int prl_qrdqn_destroy(prl_qrdqn *s) {
-    if (!s) return PRL_OK;
-    for (int i = 0; i < 2; i++) { cudaEventSynchronize(s->tail_done[i]); cudaEventDestroy(s->tail_done[i]); cudaFreeHost(s->tail_host[i]); }
-    for (int i = 0; i < 2; i++) if (s->graph_exec[i]) cudaGraphExecDestroy(s->graph_exec[i]);
-    delete s;
-    return PRL_OK;
-}
-extern "C" int64_t prl_qrdqn_adam_step(const prl_qrdqn *s) { return s ? s->adam_step : -1; }
-
-extern "C" int prl_qrdqn_set_lr(prl_qrdqn *s, double lr) {
-    PRL_REQUIRE(s, "null handle");
-    PRL_REQUIRE(lr >= 0.0, "the learning rate must be non-negative");
-    s->cfg.lr = lr;
-    return PRL_OK;
-}
+extern "C" int prl_qrdqn_destroy(prl_qrdqn *s) { return prl_qrdqn::destroy(s); }
+extern "C" int64_t prl_qrdqn_adam_step(const prl_qrdqn *s) { return prl_qrdqn::adam_step_of(s); }
+extern "C" int prl_qrdqn_set_lr(prl_qrdqn *s, double lr) { return prl_qrdqn::set_lr(s, lr); }
+extern "C" int prl_qrdqn_set_graph(prl_qrdqn *s, int enable) { return prl_qrdqn::set_graph(s, enable); }
+extern "C" int64_t prl_qrdqn_last_launches(const prl_qrdqn *s) { return prl_qrdqn::last_launches_of(s); }
 
 // one learner round, launched (or captured) on `st`; buf == null: the dense batch of the call block (learn_batch)
-static int qr_round(prl_qrdqn *s, prl_buf *buf, int B, cudaStream_t st) {
+int prl_qrdqn::round(prl_qrdqn *s, prl_buf *buf, int B, cudaStream_t st) {
     const prl_qrdqn_cfg &c = s->cfg;
     const int O = c.obs_dim, A = c.n_actions, D = O + A, N = c.num_quantiles, H1 = c.hidden1, H2 = c.hidden2, BA = B * A;
     // the decay factor is overridden by call->decay (k_adamw's decay pointer)
@@ -372,104 +308,20 @@ static int qr_round(prl_qrdqn *s, prl_buf *buf, int B, cudaStream_t st) {
     return PRL_OK;
 }
 
-// per-call block (Adam scalars of every round as torch evaluates them in double, target-update flags, decay, beta,
-// pointers), uploaded on `st`.  steps0 = the training-step count the reference's learn_batch sees in round 0; round r
-// updates the target when (steps0 + r + 1) % target_update_freq == 0.
-static int qr_upload(prl_qrdqn *s, int rounds, int64_t steps0, double beta, float *out_loss, const QrCall &dense, cudaStream_t st) {
-    const prl_qrdqn_cfg &c = s->cfg;
-    const int sb = s->tail_next; s->tail_next ^= 1;
-    PRL_CUDA(cudaEventSynchronize(s->tail_done[sb]));
-    char *tail = s->tail_host[sb];
-    const int MR = c.max_rounds;
-    float2 *hs = reinterpret_cast<float2 *>(tail);
-    int *on = reinterpret_cast<int *>(tail + (size_t)MR * 8);
-    for (int r = 0; r < rounds; r++) {
-        const double step = (double)(s->adam_step + r + 1);
-        const double bc1 = 1.0 - pow(c.beta1, step), bc2 = 1.0 - pow(c.beta2, step);
-        hs[r] = make_float2((float)(c.lr / bc1), (float)sqrt(bc2));
-        on[r] = (steps0 + r + 1) % c.target_update_freq == 0 ? 1 : 0;
-    }
-    QrCall *hc = reinterpret_cast<QrCall *>(tail + qr_call_offset(MR));
-    *hc = dense;
-    hc->slots = s->slots; hc->out_loss = out_loss;
-    hc->decay = (float)(1.0 - c.lr * c.weight_decay);
-    hc->beta = (float)beta;
-    *reinterpret_cast<int *>(hc + 1) = 0;
-    PRL_CUDA(cudaMemcpyAsync(s->scal, tail, s->tail_bytes, cudaMemcpyHostToDevice, st));
-    PRL_CUDA(cudaEventRecord(s->tail_done[sb], st));
-    return PRL_OK;
-}
-
-static int qr_run(prl_qrdqn *s, prl_buf *buf, int rounds, int batch, cudaStream_t st) {
-    const int g = buf ? 0 : 1;
-    const int dynamic = (buf && (buf->desc.flags & PRL_BUF_DYNAMIC_ACTIONS)) ? 1 : 0;
-    if (s->use_graph) {
-        if (!s->graph_exec[g] || s->graph_batch[g] != batch || (buf && (s->graph_buf != buf->records || s->graph_dynamic != dynamic))) {
-            if (s->graph_exec[g]) { cudaGraphExecDestroy(s->graph_exec[g]); s->graph_exec[g] = nullptr; }
-            cudaStream_t cs;
-            PRL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-            cudaGraph_t graph = nullptr;
-            cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-            if (e == cudaSuccess) {
-                qr_round(s, buf, batch, cs);
-                e = cudaStreamEndCapture(cs, &graph);
-            }
-            if (e == cudaSuccess) e = cudaGraphInstantiate(&s->graph_exec[g], graph, 0);
-            if (graph) cudaGraphDestroy(graph);
-            cudaStreamDestroy(cs);
-            if (e != cudaSuccess) { s->graph_exec[g] = nullptr; return fail(PRL_ECUDA, "prl_qrdqn: graph capture failed: %s", cudaGetErrorString(e)); }
-            s->graph_batch[g] = batch;
-            if (buf) { s->graph_buf = buf->records; s->graph_dynamic = dynamic; }
-        }
-        for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec[g], st));
-    } else {
-        for (int r = 0; r < rounds; r++) {
-            int rc = qr_round(s, buf, batch, st);
-            if (rc) return rc;
-        }
-    }
-    PRL_CUDA(cudaGetLastError());
-    s->adam_step += rounds;
-    s->last_launches = (int64_t)s->launches_per_round * rounds;
-    return PRL_OK;
-}
-
 extern "C" int prl_qrdqn_learn(prl_qrdqn *s, prl_buf *buf, int rounds, int batch, int64_t training_steps, double beta, float *out_loss,
                                int32_t *out_logical, void *stream_) {
-    PRL_REQUIRE(s && buf && out_loss, "null argument");
-    const prl_qrdqn_cfg &c = s->cfg;
-    PRL_REQUIRE(rounds > 0 && rounds <= c.max_rounds && batch > 0 && batch <= c.max_batch, "rounds / batch outside the configured maxima");
-    PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.obs_dim == c.obs_dim && buf->desc.n_actions == c.n_actions,
-                "QR-DQN needs a discrete-action buffer with obs_dim = %d and n_actions = %d", c.obs_dim, c.n_actions);
-    PRL_REQUIRE(buf->shard_world <= 1, "the buffer is one shard of a multi-GPU buffer: QR-DQN samples local buffers only");
-    cudaStream_t st = (cudaStream_t)stream_;
-    int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
-    if (rc) return rc;
-    QrCall dense;
-    memset(&dense, 0, sizeof(dense));
-    rc = qr_upload(s, rounds, training_steps + 1, beta, out_loss, dense, st);   // PolicyLearner.learn counts the round first
-    if (rc) return rc;
-    return qr_run(s, buf, rounds, batch, st);
+    QrCall dense{};
+    dense.beta = (float)beta;
+    return prl_qrdqn::learn(s, buf, rounds, batch, training_steps, out_loss, out_logical, dense, stream_);
 }
 
 extern "C" int prl_qrdqn_learn_batch(prl_qrdqn *s, int batch, const float *state, const int32_t *action_id, const float *reward,
                                      const float *next_state, const uint8_t *terminated, const int32_t *next_ids,
                                      const int32_t *next_count, int64_t training_steps, double beta, float *out_loss, void *stream_) {
     PRL_REQUIRE(s && state && action_id && reward && next_state && terminated && out_loss, "null argument");
-    PRL_REQUIRE(batch > 0 && batch <= s->cfg.max_batch, "batch outside the configured maximum");
-    cudaStream_t st = (cudaStream_t)stream_;
-    QrCall dense;
-    memset(&dense, 0, sizeof(dense));
+    QrCall dense{};
     dense.d_state = state; dense.d_next_state = next_state; dense.d_reward = reward; dense.d_action_id = action_id;
     dense.d_next_ids = next_ids; dense.d_next_cnt = next_count; dense.d_term = terminated;
-    int rc = qr_upload(s, 1, training_steps, beta, out_loss, dense, st);
-    if (rc) return rc;
-    return qr_run(s, nullptr, 1, batch, st);
+    dense.beta = (float)beta;
+    return prl_qrdqn::learn_batch(s, batch, training_steps, out_loss, dense, stream_);
 }
-
-extern "C" int prl_qrdqn_set_graph(prl_qrdqn *s, int enable) {
-    PRL_REQUIRE(s, "null handle");
-    s->use_graph = enable != 0;
-    return PRL_OK;
-}
-extern "C" int64_t prl_qrdqn_last_launches(const prl_qrdqn *s) { return s ? s->last_launches : -1; }

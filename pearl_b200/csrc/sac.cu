@@ -19,6 +19,7 @@
 
 #include "common.cuh"
 #include "gemm.cuh"
+#include "host_runtime.cuh"
 
 using namespace prl;
 
@@ -193,13 +194,9 @@ struct prl_sac {
     int graph_batch;
     const uint32_t *graph_buf;
     int launches_per_round;
-    float2 *scal_host[2];
-    cudaEvent_t scal_done[2];
-    int scal_next;
+    Stage stage;
     int64_t last_launches;
 };
-
-static int64_t al64(int64_t x) { return (x + 255) / 256 * 256; }
 
 static void sac_layout(prl_sac *s) {
     const prl_sac_cfg &c = s->cfg;
@@ -236,27 +233,26 @@ extern "C" int64_t prl_sac_critic_param_count(const prl_sac_cfg *c) {   // ONE c
     return t.Pc;
 }
 
-struct SacWs { int64_t off[40]; int64_t total; };
-static SacWs sac_ws(const prl_sac_cfg *c, int Pa, int Pc) {
-    SacWs w; int64_t o = 0; int k = 0;
-    const int64_t B = c->max_batch, A = c->act_dim, O = c->obs_dim;
-    auto add = [&](int64_t floats) { w.off[k++] = o; o = al64(o + floats * 4); };
-    add(B * O); add(B * A); add(B); add(B * O); add(B);                                  // S A R S2 T
-    add(B * c->actor_h1); add(B * c->actor_h2); add(B * A); add(B * A);                   // h1 h2 mean z
-    add(B * A); add(B * A); add(B * A); add(B); add(B);                                  // act_s na sd logp logp2
-    add(2 * B * c->critic_h1); add(2 * B * c->critic_h2); add(2 * B); add(2 * B);         // c1 c2 q qt
-    add(2 * B); add(2 * B * c->critic_h2); add(2 * B * c->critic_h1); add(2 * B * A);     // dq dc2 dc1 da
-    add(B * A); add(B * A); add(B * c->actor_h2); add(B * c->actor_h1); add(B);          // dmean dz dh2 dh1 y
-    add(Pa); add(2 * (int64_t)Pc);                                                        // g_actor g_critic
-    add((int64_t)c->max_rounds * B); add((int64_t)c->max_rounds * B);                    // slots logical (int32)
-    add(4 * (int64_t)c->max_rounds + 64);                                                 // scal_a | scal_c | call | round_idx
-    w.total = o;
-    return w;
+// the workspace, in order; base == null: only its size
+static int64_t sac_carve(prl_sac *s, void *base) {
+    const prl_sac_cfg &c = s->cfg;
+    const int64_t B = c.max_batch, A = c.act_dim, O = c.obs_dim;
+    Carve w{(char *)base};
+    w(s->S, B * O); w(s->A, B * A); w(s->R, B); w(s->S2, B * O); w(s->T, B);
+    w(s->h1, B * c.actor_h1); w(s->h2, B * c.actor_h2); w(s->mean, B * A); w(s->z, B * A);
+    w(s->act_s, B * A); w(s->na, B * A); w(s->sd, B * A); w(s->logp, B); w(s->logp2, B);
+    w(s->c1, 2 * B * c.critic_h1); w(s->c2, 2 * B * c.critic_h2); w(s->q, 2 * B); w(s->qt, 2 * B);
+    w(s->dq, 2 * B); w(s->dc2, 2 * B * c.critic_h2); w(s->dc1, 2 * B * c.critic_h1); w(s->da, 2 * B * A);
+    w(s->dmean, B * A); w(s->dz, B * A); w(s->dh2, B * c.actor_h2); w(s->dh1, B * c.actor_h1); w(s->y, B);
+    w(s->g_actor, s->Pa); w(s->g_critic, 2 * (int64_t)s->Pc);
+    w(s->slots, c.max_rounds * B); w(s->logical, c.max_rounds * B);
+    w(s->scal_a, 2 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | call | round_idx
+    return w.bytes;
 }
 extern "C" int64_t prl_sac_workspace_bytes(const prl_sac_cfg *c) {
     if (sac_check(c)) return -1;
     prl_sac t; t.cfg = *c; sac_layout(&t);
-    return sac_ws(c, t.Pa, t.Pc).total;
+    return sac_carve(&t, nullptr);
 }
 
 extern "C" int prl_sac_create(prl_sac **out, const prl_sac_cfg *cfg, float *actor_w, float *actor_m, float *actor_v, float *actor_vmax,
@@ -275,30 +271,19 @@ extern "C" int prl_sac_create(prl_sac **out, const prl_sac_cfg *cfg, float *acto
     s->critic = critic_w; s->critic_m = critic_m; s->critic_v = critic_v; s->critic_x = critic_vmax; s->critic_t = critic_target_w;
     s->log_alpha = log_alpha4; s->alpha = alpha1; s->low = low_dev; s->high = high_dev;
     s->adam_step = adam_step;
-    SacWs w = sac_ws(cfg, s->Pa, s->Pc);
-    char *b = (char *)workspace;
-    float **f[] = {&s->S, &s->A, &s->R, &s->S2, &s->T, &s->h1, &s->h2, &s->mean, &s->z, &s->act_s, &s->na, &s->sd, &s->logp, &s->logp2,
-                   &s->c1, &s->c2, &s->q, &s->qt, &s->dq, &s->dc2, &s->dc1, &s->da, &s->dmean, &s->dz, &s->dh2, &s->dh1, &s->y,
-                   &s->g_actor, &s->g_critic};
-    int k = 0;
-    for (auto p : f) *p = (float *)(b + w.off[k++]);
-    s->slots = (int32_t *)(b + w.off[k++]); s->logical = (int32_t *)(b + w.off[k++]);
-    s->scal_a = (float2 *)(b + w.off[k++]); s->scal_c = s->scal_a + cfg->max_rounds;
+    sac_carve(s, workspace);
+    s->scal_c = s->scal_a + cfg->max_rounds;
     s->call = (SacCall *)(s->scal_c + cfg->max_rounds); s->round_idx = (int *)(s->call + 1);
-    s->scal_next = 0; s->use_graph = true; s->graph_exec = nullptr; s->graph_batch = 0; s->graph_buf = nullptr; s->last_launches = 0;
+    s->use_graph = true; s->graph_exec = nullptr; s->graph_batch = 0; s->graph_buf = nullptr; s->last_launches = 0;
     static_assert(sizeof(SacCall) + 4 <= 64 * 4, "call block fits the reserved tail");
-    cudaError_t e = cudaSuccess;
-    for (int i = 0; i < 2 && e == cudaSuccess; i++) {
-        e = cudaHostAlloc((void **)&s->scal_host[i], (size_t)cfg->max_rounds * 16 + 256, cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->scal_done[i], cudaEventDisableTiming);
-    }
+    cudaError_t e = s->stage.open((size_t)cfg->max_rounds * 16 + 256);
     if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_sac_create: %s", cudaGetErrorString(e)); }
     *out = s;
     return PRL_OK;
 }
 extern "C" int prl_sac_destroy(prl_sac *s) {
     if (!s) return PRL_OK;
-    for (int i = 0; i < 2; i++) { cudaEventSynchronize(s->scal_done[i]); cudaEventDestroy(s->scal_done[i]); cudaFreeHost(s->scal_host[i]); }
+    s->stage.close();
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
     delete s;
     return PRL_OK;
@@ -392,38 +377,25 @@ extern "C" int prl_sac_learn(prl_sac *s, prl_buf *buf, int rounds, int batch, co
     int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
     if (rc) return rc;
     // per-call block: AdamW scalars of every round (actor lr / critic lr, as torch evaluates them in double) + pointers
-    const int sb = s->scal_next; s->scal_next ^= 1;
-    PRL_CUDA(cudaEventSynchronize(s->scal_done[sb]));
-    float2 *hs = s->scal_host[sb];
+    float2 *hs;
+    rc = s->stage.wait(&hs);
+    if (rc) return rc;
     for (int r = 0; r < rounds; r++) {
-        const double step = (double)(s->adam_step + r + 1);
-        const double bc1 = 1.0 - pow(c.beta1, step), bc2 = 1.0 - pow(c.beta2, step);
-        hs[r] = make_float2((float)(c.actor_lr / bc1), (float)sqrt(bc2));
-        hs[c.max_rounds + r] = make_float2((float)(c.critic_lr / bc1), (float)sqrt(bc2));
+        hs[r] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->adam_step + r + 1);
+        hs[c.max_rounds + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->adam_step + r + 1);
     }
     SacCall *hc = reinterpret_cast<SacCall *>(hs + 2 * (size_t)c.max_rounds);
     hc->noise = noise_dev; hc->slots = s->slots; hc->out_actor = out_actor_loss; hc->out_critic = out_critic_loss; hc->out_entropy = out_entropy_loss;
     int *hround = reinterpret_cast<int *>(hc + 1);
     *hround = 0;
     // scal_a | scal_c | call | round_idx are contiguous on the device in the same order
-    PRL_CUDA(cudaMemcpyAsync(s->scal_a, hs, 2 * (size_t)c.max_rounds * 8 + sizeof(SacCall) + 4, cudaMemcpyHostToDevice, st));
-    PRL_CUDA(cudaEventRecord(s->scal_done[sb], st));
+    rc = s->stage.send(s->scal_a, 2 * (size_t)c.max_rounds * 8 + sizeof(SacCall) + 4, st);
+    if (rc) return rc;
 
     if (s->use_graph) {
         if (!s->graph_exec || s->graph_batch != batch || s->graph_buf != buf->records) {
-            if (s->graph_exec) { cudaGraphExecDestroy(s->graph_exec); s->graph_exec = nullptr; }
-            cudaStream_t cs;
-            PRL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-            cudaGraph_t graph = nullptr;
-            cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-            if (e == cudaSuccess) {
-                sac_round(s, buf, batch, cs);
-                e = cudaStreamEndCapture(cs, &graph);
-            }
-            if (e == cudaSuccess) e = cudaGraphInstantiate(&s->graph_exec, graph, 0);
-            if (graph) cudaGraphDestroy(graph);
-            cudaStreamDestroy(cs);
-            if (e != cudaSuccess) { s->graph_exec = nullptr; return fail(PRL_ECUDA, "prl_sac_learn: graph capture failed: %s", cudaGetErrorString(e)); }
+            rc = capture_graph(&s->graph_exec, "prl_sac_learn", [&](cudaStream_t cs) { return sac_round(s, buf, batch, cs); });
+            if (rc) return rc;
             s->graph_batch = batch; s->graph_buf = buf->records;
         }
         for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec, st));

@@ -20,6 +20,7 @@
 
 #include "common.cuh"
 #include "gemm.cuh"
+#include "host_runtime.cuh"
 
 using namespace prl;
 
@@ -203,13 +204,9 @@ struct prl_sacd {
     int graph_batch;
     const uint32_t *graph_buf;
     int launches_per_round;
-    float2 *scal_host[2];
-    cudaEvent_t scal_done[2];
-    int scal_next;
+    Stage stage;
     int64_t last_launches;
 };
-
-static int64_t al64(int64_t x) { return (x + 255) / 256 * 256; }
 
 static void sacd_layout(prl_sacd *s) {
     const prl_sacd_cfg &c = s->cfg;
@@ -245,28 +242,27 @@ extern "C" int64_t prl_sacd_critic_param_count(const prl_sacd_cfg *c) {
     return t.Pc;
 }
 
-struct SacdWs { int64_t off[40]; int64_t total; };
-static SacdWs sacd_ws(const prl_sacd_cfg *c, int Pa, int Pc) {
-    SacdWs w; int64_t o = 0; int k = 0;
-    const int64_t B = c->max_batch, A = c->n_actions, O = c->obs_dim, BA = B * A;
-    auto add = [&](int64_t words) { w.off[k++] = o; o = al64(o + words * 4); };
-    add(B * O); add(B * O); add(B); add(B);                                                      // S S2 R T
-    add(B * c->actor_h1); add(B * c->actor_h2); add(BA); add(BA); add(B);                        // h1 h2 logits dlogit ent
-    add(B * c->actor_h2); add(B * c->actor_h1);                                                  // dh2 dh1
-    add(2 * B * c->critic_h1); add(2 * BA * c->critic_h1); add(2 * BA * c->critic_h2); add(2 * BA);   // P c1 c2 q
-    add(2 * B * c->critic_h1); add(2 * B * c->critic_h2); add(2 * B);                           // c1a c2a dq
-    add(2 * B * c->critic_h2); add(2 * B * c->critic_h1); add(B); add(2 * B);                    // dc2 dc1 y qa
-    add(Pa); add(2 * (int64_t)Pc);                                                               // g_actor g_critic
-    add(B); add(B); add(BA);                                                                     // act cnt ids (int32)
-    add((int64_t)c->max_rounds * B); add((int64_t)c->max_rounds * B);                           // slots logical (int32)
-    add(6 * (int64_t)c->max_rounds + 64);                                                        // scal_a | scal_c | scal_e | call | round_idx
-    w.total = o;
-    return w;
+// the workspace, in order; base == null: only its size
+static int64_t sacd_carve(prl_sacd *s, void *base) {
+    const prl_sacd_cfg &c = s->cfg;
+    const int64_t B = c.max_batch, A = c.n_actions, O = c.obs_dim, BA = B * A;
+    Carve w{(char *)base};
+    w(s->S, B * O); w(s->S2, B * O); w(s->R, B); w(s->T, B);
+    w(s->h1, B * c.actor_h1); w(s->h2, B * c.actor_h2); w(s->logits, BA); w(s->dlogit, BA); w(s->ent, B);
+    w(s->dh2, B * c.actor_h2); w(s->dh1, B * c.actor_h1);
+    w(s->P, 2 * B * c.critic_h1); w(s->c1, 2 * BA * c.critic_h1); w(s->c2, 2 * BA * c.critic_h2); w(s->q, 2 * BA);
+    w(s->c1a, 2 * B * c.critic_h1); w(s->c2a, 2 * B * c.critic_h2); w(s->dq, 2 * B);
+    w(s->dc2, 2 * B * c.critic_h2); w(s->dc1, 2 * B * c.critic_h1); w(s->y, B); w(s->qa, 2 * B);
+    w(s->g_actor, s->Pa); w(s->g_critic, 2 * (int64_t)s->Pc);
+    w(s->act, B); w(s->cnt, B); w(s->ids, BA);
+    w(s->slots, c.max_rounds * B); w(s->logical, c.max_rounds * B);
+    w(s->scal_a, 3 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | scal_e | call | round_idx
+    return w.bytes;
 }
 extern "C" int64_t prl_sacd_workspace_bytes(const prl_sacd_cfg *c) {
     if (sacd_check(c)) return -1;
     prl_sacd t; t.cfg = *c; sacd_layout(&t);
-    return sacd_ws(c, t.Pa, t.Pc).total;
+    return sacd_carve(&t, nullptr);
 }
 
 extern "C" int prl_sacd_create(prl_sacd **out, const prl_sacd_cfg *cfg, float *actor_w, float *actor_m, float *actor_v, float *actor_vmax,
@@ -284,39 +280,20 @@ extern "C" int prl_sacd_create(prl_sacd **out, const prl_sacd_cfg *cfg, float *a
     s->critic = critic_w; s->critic_m = critic_m; s->critic_v = critic_v; s->critic_x = critic_vmax; s->critic_t = critic_target_w;
     s->log_alpha = log_alpha3; s->alpha = alpha1;
     s->adam_step = adam_step;
-    SacdWs w = sacd_ws(cfg, s->Pa, s->Pc);
-    char *b = (char *)workspace;
-    float **f[] = {&s->S, &s->S2, &s->R, &s->T, &s->h1, &s->h2, &s->logits, &s->dlogit, &s->ent, &s->dh2, &s->dh1, &s->P, &s->c1, &s->c2,
-                   &s->q, &s->c1a, &s->c2a, &s->dq, &s->dc2, &s->dc1, &s->y, &s->qa, &s->g_actor, &s->g_critic};
-    int k = 0;
-    for (auto p : f) *p = (float *)(b + w.off[k++]);
-    s->act = (int *)(b + w.off[k++]); s->cnt = (int *)(b + w.off[k++]); s->ids = (int *)(b + w.off[k++]);
-    s->slots = (int32_t *)(b + w.off[k++]); s->logical = (int32_t *)(b + w.off[k++]);
-    s->scal_a = (float2 *)(b + w.off[k++]); s->scal_c = s->scal_a + cfg->max_rounds; s->scal_e = s->scal_c + cfg->max_rounds;
+    sacd_carve(s, workspace);
+    s->scal_c = s->scal_a + cfg->max_rounds; s->scal_e = s->scal_c + cfg->max_rounds;
     s->call = (SacdCall *)(s->scal_e + cfg->max_rounds); s->round_idx = (int *)(s->call + 1);
-    s->scal_next = 0; s->use_graph = true; s->graph_exec = nullptr; s->graph_batch = 0; s->graph_buf = nullptr; s->last_launches = 0;
+    s->use_graph = true; s->graph_exec = nullptr; s->graph_batch = 0; s->graph_buf = nullptr; s->last_launches = 0;
     s->launches_per_round = 0;
     static_assert(sizeof(SacdCall) + 4 <= 64 * 4, "call block fits the reserved tail");
-    cudaError_t e = cudaSuccess;
-    int made = 0;   // pinned buffer / event pairs fully created
-    s->scal_host[0] = s->scal_host[1] = nullptr;
-    for (int i = 0; i < 2 && e == cudaSuccess; i++) {
-        e = cudaHostAlloc((void **)&s->scal_host[i], (size_t)cfg->max_rounds * 24 + 256, cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->scal_done[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) made++;
-    }
-    if (e != cudaSuccess) {
-        for (int i = 0; i < made; i++) { cudaEventDestroy(s->scal_done[i]); cudaFreeHost(s->scal_host[i]); }
-        if (made < 2 && s->scal_host[made]) cudaFreeHost(s->scal_host[made]);   // its event was not created
-        delete s;
-        return fail(PRL_ECUDA, "prl_sacd_create: %s", cudaGetErrorString(e));
-    }
+    cudaError_t e = s->stage.open((size_t)cfg->max_rounds * 24 + 256);
+    if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_sacd_create: %s", cudaGetErrorString(e)); }
     *out = s;
     return PRL_OK;
 }
 extern "C" int prl_sacd_destroy(prl_sacd *s) {
     if (!s) return PRL_OK;
-    for (int i = 0; i < 2; i++) { cudaEventSynchronize(s->scal_done[i]); cudaEventDestroy(s->scal_done[i]); cudaFreeHost(s->scal_host[i]); }
+    s->stage.close();
     if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
     delete s;
     return PRL_OK;
@@ -414,16 +391,14 @@ extern "C" int prl_sacd_learn(prl_sacd *s, prl_buf *buf, int rounds, int batch, 
     int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
     if (rc) return rc;
     // per-call block: Adam scalars of every round (as torch evaluates them in double), decay factors, pointers
-    const int sb = s->scal_next; s->scal_next ^= 1;
-    PRL_CUDA(cudaEventSynchronize(s->scal_done[sb]));
-    float2 *hs = s->scal_host[sb];
+    float2 *hs;
+    rc = s->stage.wait(&hs);
+    if (rc) return rc;
     const int MR = c.max_rounds;
     for (int r = 0; r < rounds; r++) {
-        const double step = (double)(s->adam_step + r + 1);
-        const double bc1 = 1.0 - pow(c.beta1, step), bc2 = 1.0 - pow(c.beta2, step);
-        hs[r] = make_float2((float)(c.actor_lr / bc1), (float)sqrt(bc2));
-        hs[MR + r] = make_float2((float)(c.critic_lr / bc1), (float)sqrt(bc2));
-        hs[2 * MR + r] = make_float2((float)(c.entropy_lr / bc1), (float)sqrt(bc2));
+        hs[r] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->adam_step + r + 1);
+        hs[MR + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->adam_step + r + 1);
+        hs[2 * MR + r] = adam_scal(c.entropy_lr, c.beta1, c.beta2, s->adam_step + r + 1);
     }
     SacdCall *hc = reinterpret_cast<SacdCall *>(hs + 3 * (size_t)MR);
     hc->slots = s->slots; hc->out_actor = out_actor_loss; hc->out_critic = out_critic_loss; hc->out_entropy = out_entropy_loss;
@@ -432,24 +407,13 @@ extern "C" int prl_sacd_learn(prl_sacd *s, prl_buf *buf, int rounds, int batch, 
     int *hround = reinterpret_cast<int *>(hc + 1);
     *hround = 0;
     // scal_a | scal_c | scal_e | call | round_idx are contiguous on the device in the same order
-    PRL_CUDA(cudaMemcpyAsync(s->scal_a, hs, 3 * (size_t)MR * 8 + sizeof(SacdCall) + 4, cudaMemcpyHostToDevice, st));
-    PRL_CUDA(cudaEventRecord(s->scal_done[sb], st));
+    rc = s->stage.send(s->scal_a, 3 * (size_t)MR * 8 + sizeof(SacdCall) + 4, st);
+    if (rc) return rc;
 
     if (s->use_graph) {
         if (!s->graph_exec || s->graph_batch != batch || s->graph_buf != buf->records) {
-            if (s->graph_exec) { cudaGraphExecDestroy(s->graph_exec); s->graph_exec = nullptr; }
-            cudaStream_t cs;
-            PRL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-            cudaGraph_t graph = nullptr;
-            cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-            if (e == cudaSuccess) {
-                sacd_round(s, buf, batch, cs);
-                e = cudaStreamEndCapture(cs, &graph);
-            }
-            if (e == cudaSuccess) e = cudaGraphInstantiate(&s->graph_exec, graph, 0);
-            if (graph) cudaGraphDestroy(graph);
-            cudaStreamDestroy(cs);
-            if (e != cudaSuccess) { s->graph_exec = nullptr; return fail(PRL_ECUDA, "prl_sacd_learn: graph capture failed: %s", cudaGetErrorString(e)); }
+            rc = capture_graph(&s->graph_exec, "prl_sacd_learn", [&](cudaStream_t cs) { return sacd_round(s, buf, batch, cs); });
+            if (rc) return rc;
             s->graph_batch = batch; s->graph_buf = buf->records;
         }
         for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec, st));

@@ -16,6 +16,7 @@
 
 #include "common.cuh"
 #include "gemm.cuh"
+#include "host_runtime.cuh"
 
 using namespace prl;
 
@@ -141,13 +142,9 @@ struct prl_td3 {
     int graph_batch;
     const uint32_t *graph_buf;
     int launches_per_round[2];
-    float2 *scal_host[2];
-    cudaEvent_t scal_done[2];
-    int scal_next;
+    Stage stage;
     int64_t last_launches;
 };
-
-static int64_t al64_(int64_t x) { return (x + 255) / 256 * 256; }
 
 static void td3_layout(prl_td3 *s) {
     const prl_td3_cfg &c = s->cfg;
@@ -180,26 +177,25 @@ extern "C" int64_t prl_td3_critic_param_count(const prl_td3_cfg *c) {   // ONE c
     prl_td3 t; t.cfg = *c; td3_layout(&t);
     return t.Pc;
 }
-struct Td3Ws { int64_t off[40]; int64_t total; };
-static Td3Ws td3_ws(const prl_td3_cfg *c, int Pa, int Pc) {
-    Td3Ws w; int64_t o = 0; int k = 0;
-    const int64_t B = c->max_batch, A = c->act_dim, O = c->obs_dim;
-    auto add = [&](int64_t floats) { w.off[k++] = o; o = al64_(o + floats * 4); };
-    add(B * O); add(B * A); add(B); add(B * O); add(B);                                  // S A R S2 T
-    add(B * c->actor_h1); add(B * c->actor_h2); add(B * A); add(B * A); add(B * A);       // h1 h2 pre act_s na
-    add(2 * B * c->critic_h1); add(2 * B * c->critic_h2); add(2 * B); add(2 * B);         // c1 c2 q qt
-    add(2 * B); add(2 * B * c->critic_h2); add(2 * B * c->critic_h1); add(2 * B * A);     // dq dc2 dc1 da
-    add(B * A); add(B * c->actor_h2); add(B * c->actor_h1); add(B);                      // dpre dh2 dh1 y
-    add(Pa); add(2 * (int64_t)Pc); add(4);                                                // g_actor g_critic last_actor_loss
-    add((int64_t)c->max_rounds * B); add((int64_t)c->max_rounds * B);                    // slots logical (int32)
-    add(4 * (int64_t)c->max_rounds + 64);                                                 // scal_a | scal_c | call | round_idx | actor_round_idx
-    w.total = o;
-    return w;
+// the workspace, in order; base == null: only its size
+static int64_t td3_carve(prl_td3 *s, void *base) {
+    const prl_td3_cfg &c = s->cfg;
+    const int64_t B = c.max_batch, A = c.act_dim, O = c.obs_dim;
+    Carve w{(char *)base};
+    w(s->S, B * O); w(s->A, B * A); w(s->R, B); w(s->S2, B * O); w(s->T, B);
+    w(s->h1, B * c.actor_h1); w(s->h2, B * c.actor_h2); w(s->pre, B * A); w(s->act_s, B * A); w(s->na, B * A);
+    w(s->c1, 2 * B * c.critic_h1); w(s->c2, 2 * B * c.critic_h2); w(s->q, 2 * B); w(s->qt, 2 * B);
+    w(s->dq, 2 * B); w(s->dc2, 2 * B * c.critic_h2); w(s->dc1, 2 * B * c.critic_h1); w(s->da, 2 * B * A);
+    w(s->dpre, B * A); w(s->dh2, B * c.actor_h2); w(s->dh1, B * c.actor_h1); w(s->y, B);
+    w(s->g_actor, s->Pa); w(s->g_critic, 2 * (int64_t)s->Pc); w(s->last_actor_loss, 4);
+    w(s->slots, c.max_rounds * B); w(s->logical, c.max_rounds * B);
+    w(s->scal_a, 2 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | call | round_idx | actor_round_idx
+    return w.bytes;
 }
 extern "C" int64_t prl_td3_workspace_bytes(const prl_td3_cfg *c) {
     if (td3_check(c)) return -1;
     prl_td3 t; t.cfg = *c; td3_layout(&t);
-    return td3_ws(c, t.Pa, t.Pc).total;
+    return td3_carve(&t, nullptr);
 }
 
 extern "C" int prl_td3_create(prl_td3 **out, const prl_td3_cfg *cfg, float *actor_w, float *actor_m, float *actor_v, float *actor_vmax,
@@ -218,30 +214,21 @@ extern "C" int prl_td3_create(prl_td3 **out, const prl_td3_cfg *cfg, float *acto
     s->critic = critic_w; s->critic_m = critic_m; s->critic_v = critic_v; s->critic_x = critic_vmax; s->critic_t = critic_target_w;
     s->low = low_dev; s->high = high_dev;
     s->actor_step = actor_adam_step; s->critic_step = critic_adam_step;
-    Td3Ws w = td3_ws(cfg, s->Pa, s->Pc);
-    char *b = (char *)workspace;
-    float **f[] = {&s->S, &s->A, &s->R, &s->S2, &s->T, &s->h1, &s->h2, &s->pre, &s->act_s, &s->na, &s->c1, &s->c2, &s->q, &s->qt, &s->dq,
-                   &s->dc2, &s->dc1, &s->da, &s->dpre, &s->dh2, &s->dh1, &s->y, &s->g_actor, &s->g_critic, &s->last_actor_loss};
-    int k = 0;
-    for (auto p : f) *p = (float *)(b + w.off[k++]);
-    s->slots = (int32_t *)(b + w.off[k++]); s->logical = (int32_t *)(b + w.off[k++]);
-    s->scal_a = (float2 *)(b + w.off[k++]); s->scal_c = s->scal_a + cfg->max_rounds;
+    td3_carve(s, workspace);
+    s->scal_c = s->scal_a + cfg->max_rounds;
     s->call = (Td3Call *)(s->scal_c + cfg->max_rounds); s->round_idx = (int *)(s->call + 1); s->actor_round_idx = s->round_idx + 1;
     static_assert(sizeof(Td3Call) + 8 <= 64 * 4, "call block fits the reserved tail");
-    s->scal_next = 0; s->use_graph = true; s->graph_exec[0] = s->graph_exec[1] = nullptr; s->graph_batch = 0; s->graph_buf = nullptr;
+    s->use_graph = true; s->graph_exec[0] = s->graph_exec[1] = nullptr; s->graph_batch = 0; s->graph_buf = nullptr;
     s->last_launches = 0;
     cudaError_t e = cudaMemset(s->last_actor_loss, 0, 16);
-    for (int i = 0; i < 2 && e == cudaSuccess; i++) {
-        e = cudaHostAlloc((void **)&s->scal_host[i], (size_t)cfg->max_rounds * 16 + 256, cudaHostAllocDefault);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->scal_done[i], cudaEventDisableTiming);
-    }
+    if (e == cudaSuccess) e = s->stage.open((size_t)cfg->max_rounds * 16 + 256);
     if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_td3_create: %s", cudaGetErrorString(e)); }
     *out = s;
     return PRL_OK;
 }
 extern "C" int prl_td3_destroy(prl_td3 *s) {
     if (!s) return PRL_OK;
-    for (int i = 0; i < 2; i++) { cudaEventSynchronize(s->scal_done[i]); cudaEventDestroy(s->scal_done[i]); cudaFreeHost(s->scal_host[i]); }
+    s->stage.close();
     for (int i = 0; i < 2; i++) if (s->graph_exec[i]) cudaGraphExecDestroy(s->graph_exec[i]);
     delete s;
     return PRL_OK;
@@ -342,16 +329,14 @@ extern "C" int prl_td3_learn(prl_td3 *s, prl_buf *buf, int rounds, int batch, in
     // which rounds update the actor: PolicyLearner.learn increments _training_steps before learn_batch (policy_learner.py:183),
     // TD3 tests `_training_steps % actor_update_freq == 0` (td3.py:121)
     auto updates = [&](int r) { return c.actor_update_freq <= 1 || (training_steps0 + r + 1) % c.actor_update_freq == 0; };
-    const int sb = s->scal_next; s->scal_next ^= 1;
-    PRL_CUDA(cudaEventSynchronize(s->scal_done[sb]));
-    float2 *hs = s->scal_host[sb];
+    float2 *hs;
+    rc = s->stage.wait(&hs);
+    if (rc) return rc;
     int n_actor = 0;
     for (int r = 0; r < rounds; r++) {
-        const double cstep = (double)(s->critic_step + r + 1);
-        hs[c.max_rounds + r] = make_float2((float)(c.critic_lr / (1.0 - pow(c.beta1, cstep))), (float)sqrt(1.0 - pow(c.beta2, cstep)));
+        hs[c.max_rounds + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->critic_step + r + 1);
         if (updates(r)) {     // the actor optimizer's own step count: it only advances on update rounds
-            const double astep = (double)(s->actor_step + n_actor + 1);
-            hs[n_actor] = make_float2((float)(c.actor_lr / (1.0 - pow(c.beta1, astep))), (float)sqrt(1.0 - pow(c.beta2, astep)));
+            hs[n_actor] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->actor_step + n_actor + 1);
             n_actor++;
         }
     }
@@ -359,25 +344,14 @@ extern "C" int prl_td3_learn(prl_td3 *s, prl_buf *buf, int rounds, int batch, in
     hc->noise = noise_dev; hc->slots = s->slots; hc->out_actor = out_actor_loss; hc->out_critic = out_critic_loss;
     int *hround = reinterpret_cast<int *>(hc + 1);
     hround[0] = 0; hround[1] = 0;
-    PRL_CUDA(cudaMemcpyAsync(s->scal_a, hs, 2 * (size_t)c.max_rounds * 8 + sizeof(Td3Call) + 8, cudaMemcpyHostToDevice, st));
-    PRL_CUDA(cudaEventRecord(s->scal_done[sb], st));
+    rc = s->stage.send(s->scal_a, 2 * (size_t)c.max_rounds * 8 + sizeof(Td3Call) + 8, st);
+    if (rc) return rc;
 
     if (s->use_graph) {
         if (!s->graph_exec[0] || s->graph_batch != batch || s->graph_buf != buf->records) {
             for (int u = 0; u < 2; u++) {
-                if (s->graph_exec[u]) { cudaGraphExecDestroy(s->graph_exec[u]); s->graph_exec[u] = nullptr; }
-                cudaStream_t cs;
-                PRL_CUDA(cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking));
-                cudaGraph_t graph = nullptr;
-                cudaError_t e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-                if (e == cudaSuccess) {
-                    td3_round(s, buf, batch, u == 1, cs);
-                    e = cudaStreamEndCapture(cs, &graph);
-                }
-                if (e == cudaSuccess) e = cudaGraphInstantiate(&s->graph_exec[u], graph, 0);
-                if (graph) cudaGraphDestroy(graph);
-                cudaStreamDestroy(cs);
-                if (e != cudaSuccess) { s->graph_exec[u] = nullptr; return fail(PRL_ECUDA, "prl_td3_learn: graph capture failed: %s", cudaGetErrorString(e)); }
+                rc = capture_graph(&s->graph_exec[u], "prl_td3_learn", [&](cudaStream_t cs) { return td3_round(s, buf, batch, u == 1, cs); });
+                if (rc) return rc;
             }
             s->graph_batch = batch; s->graph_buf = buf->records;
         }

@@ -27,6 +27,7 @@ import torch
 from . import _lib
 from . import cql as _cql
 from . import dueling as _duel
+from ._batch import action_ids
 from ._compat import _RefDeepQLearning, _RefDoubleDQN, TransitionBatch
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
 
@@ -304,10 +305,8 @@ class _B200DQNMixin:
                     for k, v in self.learn_batch(self.preprocess_batch(batch)).items():
                         report.setdefault(k, []).append(v)
             return report
-        if self._dueling:
-            return _duel.learn(self, replay_buffer, bs, rounds, trace)
-        if self._conservative:
-            return _cql.learn(self, replay_buffer, bs, rounds, trace)
+        if self._dueling or self._conservative:
+            return self._learn_rounds(replay_buffer, bs, rounds, trace)
         self._bind(bs)
         dev = self._device
         if replay_buffer.device != dev:
@@ -349,6 +348,41 @@ class _B200DQNMixin:
             report.update(q=q, y=y, idx=idx)
         return report
 
+    def _learn_rounds(self, replay_buffer, bs: int, rounds: int, trace: bool) -> dict:
+        """learn() of the dueling and conservative (CQL) learners over a B200ReplayBuffer: `rounds` x (sample -> round)
+        through prl_duel_learn / prl_cql_learn (which also takes alpha).  The ring holds no current action sets, so every
+        round uses the full set, as B200ReplayBuffer.sample reports it."""
+        from .per import B200PrioritizedReplayBuffer
+        if isinstance(replay_buffer, B200PrioritizedReplayBuffer):
+            raise NotImplementedError(("dueling DQN samples uniformly" if self._dueling else "conservative (CQL) updates sample "
+                                       "uniformly") + ": a B200PrioritizedReplayBuffer is not supported")
+        self._bind(bs)
+        dev = self._device
+        if replay_buffer.device != dev:
+            raise RuntimeError(f"replay buffer is on {replay_buffer.device}, learner on {dev}")
+        alpha = () if self._dueling else (_cql.alpha(self),)
+        h = self._handle
+        mae = torch.empty(rounds, dtype=torch.float32, device=dev)
+        idx = torch.empty((rounds, bs), dtype=torch.int32, device=dev) if trace else None
+        with torch.cuda.device(dev):
+            stream = _stream_ptr(dev)
+            _lib.check(self._c("set_graph")(h, int(self.use_cuda_graph)))
+            replay_buffer._rng_push()
+            done = 0
+            while done < rounds:
+                r = min(self._max_rounds, rounds - done)
+                off = lambda t, w=1: C.c_void_p(0) if t is None else C.c_void_p(t.data_ptr() + 4 * done * w)  # noqa: E731
+                _lib.check(self._c("learn")(h, replay_buffer.handle, r, bs, int(self._training_steps), *alpha, off(mae),
+                                            off(idx, bs), stream))
+                self._training_steps += r
+                done += r
+            replay_buffer._rng_pull()
+        self._sync_step_tensors()
+        report = {"loss": mae.cpu().tolist()}
+        if trace:
+            report.update(idx=idx, launches=int(self._c("last_launches")(h)))
+        return report
+
     def _learn_prioritized(self, rb, bs: int, rounds: int, trace: bool) -> dict:
         """learn() over a B200PrioritizedReplayBuffer: per round stratified sum-tree draw, importance-weighted
         MSE step, priority update from |q - y| (prl_dqn_learn_per)."""
@@ -384,14 +418,6 @@ class _B200DQNMixin:
             raise NotImplementedError("only the identity history summarization module is fused")
         return batch
 
-    def _action_ids(self, a: torch.Tensor, one_hot_last: bool) -> torch.Tensor:
-        A = self._n_actions
-        if a.is_floating_point() and a.dim() >= 2 and a.shape[-1] == A and one_hot_last and A > 1:
-            return a.argmax(-1)
-        if a.dim() >= 2 and a.shape[-1] == 1:
-            a = a.squeeze(-1)
-        return a.long()
-
     def learn_batch(self, batch) -> dict:
         """`DeepTDLearning.learn_batch` on a caller-supplied batch (raw ids, or the one-hot
         tensors the reference's preprocess_batch produces)."""
@@ -406,11 +432,11 @@ class _B200DQNMixin:
         state, next_state = f32(batch.state), f32(batch.next_state)
         reward = f32(batch.reward.reshape(B))
         term = batch.terminated.reshape(B).to(device=dev, dtype=torch.uint8).contiguous()
-        action = self._action_ids(batch.action.to(dev), batch.action.dim() == 2).reshape(B).contiguous()
+        action = action_ids(batch.action.to(dev), self._n_actions, batch.action.dim() == 2).reshape(B).contiguous()
         avail = mask = None
         if batch.next_available_actions is not None:
             na = batch.next_available_actions.to(dev)
-            avail = self._action_ids(na, na.dim() == 3).reshape(B, self._n_actions).to(torch.float32).contiguous()
+            avail = action_ids(na, self._n_actions, na.dim() == 3).reshape(B, self._n_actions).to(torch.float32).contiguous()
         if batch.next_unavailable_actions_mask is not None:
             mask = batch.next_unavailable_actions_mask.to(device=dev, dtype=torch.uint8).contiguous()
         mae = torch.empty(1, dtype=torch.float32, device=dev)
@@ -429,15 +455,12 @@ class _B200DQNMixin:
         """Q(s, a) for every action id: [n, obs] -> [n, n_actions]."""
         if self._dueling:
             return _duel.q_values(self, states, target)
-        if self._conservative:
-            return _cql.q_values(self, states, target)
         self._bind(1)
         dev = self._device
         s = states.to(device=dev, dtype=torch.float32).reshape(-1, self._obs_dim).contiguous()
         out = torch.empty((s.shape[0], self._n_actions), dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(self._libh.prl_dqn_q_values(self._handle, s.shape[0], _lib.ptr(s), int(target),
-                                                   _lib.ptr(out), _stream_ptr(dev)))
+            _lib.check(self._c("q_values")(self._handle, s.shape[0], _lib.ptr(s), int(target), _lib.ptr(out), _stream_ptr(dev)))
         torch.cuda.current_stream(dev).synchronize()
         return out
 

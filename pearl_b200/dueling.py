@@ -4,18 +4,17 @@
 
 The DQN plugin (dqn.py) keeps its binding: `_Q`, `_Q_target` and the AdamW state are views into the flat vectors it
 allocates, and a checkpoint or lr change is picked up the same way.  When the Q network is a dueling one, the plugin hands
-the flat vectors to a `prl_duel` handle and delegates `learn` (over a B200ReplayBuffer), `learn_batch`, `q_values` and
-`act` to the functions here.  The advantage mean of `get_q_values` runs over the set the reference's caller hands it
-(include/pearl_b200.h): the current slots (padding included) in a round, all next slots (masked ones included) for the
-target, the query alone when a batch has no current sets, and the available actions in `act`.  No CPU fallback."""
+the flat vectors to a `prl_duel` handle: `learn` (over a B200ReplayBuffer) runs through its prl_duel_* entry points,
+`learn_batch`, `q_values` and `act` through the functions here.  The advantage mean of `get_q_values` runs over the set
+the reference's caller hands it (include/pearl_b200.h): the current slots (padding included) in a round, all next slots
+(masked ones included) for the target, the query alone when a batch has no current sets, and the available actions in
+`act`.  No CPU fallback."""
 from __future__ import annotations
-
-import ctypes as C
 
 import torch
 
 from . import _lib
-from .cql import _ids
+from ._batch import checked_ids
 from .replay_buffer import _stream_ptr
 
 _ARCHS = ("state_arch", "value_arch", "advantage_arch")
@@ -64,38 +63,6 @@ def make_cfg(pl, hp: dict, max_batch: int) -> _lib.DuelCfg:
                         gamma=float(pl._discount_factor), tau=float(pl._soft_update_tau))
 
 
-def learn(pl, replay_buffer, bs: int, rounds: int, trace: bool) -> dict:
-    """PolicyLearner.learn over a B200ReplayBuffer: `rounds` x (sample -> round) through prl_duel_learn.  The ring holds no
-    current action sets, so every round's advantage mean runs over every action, as B200ReplayBuffer.sample reports."""
-    from .per import B200PrioritizedReplayBuffer
-    if isinstance(replay_buffer, B200PrioritizedReplayBuffer):
-        raise NotImplementedError("dueling DQN samples uniformly: a B200PrioritizedReplayBuffer is not supported")
-    pl._bind(bs)
-    dev = pl._device
-    if replay_buffer.device != dev:
-        raise RuntimeError(f"replay buffer is on {replay_buffer.device}, learner on {dev}")
-    lib, h = pl._libh, pl._handle
-    mae = torch.empty(rounds, dtype=torch.float32, device=dev)
-    idx = torch.empty((rounds, bs), dtype=torch.int32, device=dev) if trace else None
-    with torch.cuda.device(dev):
-        stream = _stream_ptr(dev)
-        _lib.check(lib.prl_duel_set_graph(h, int(pl.use_cuda_graph)))
-        replay_buffer._rng_push()
-        done = 0
-        while done < rounds:
-            r = min(pl._max_rounds, rounds - done)
-            off = lambda t, w=1: C.c_void_p(0) if t is None else C.c_void_p(t.data_ptr() + 4 * done * w)  # noqa: E731
-            _lib.check(lib.prl_duel_learn(h, replay_buffer.handle, r, bs, int(pl._training_steps), off(mae), off(idx, bs), stream))
-            pl._training_steps += r
-            done += r
-        replay_buffer._rng_pull()
-    pl._sync_step_tensors()
-    report = {"loss": mae.cpu().tolist()}
-    if trace:
-        report.update(idx=idx, launches=int(lib.prl_duel_last_launches(h)))
-    return report
-
-
 def learn_batch(pl, batch) -> dict:
     """`DeepTDLearning.learn_batch` on a caller-supplied batch (raw ids, or the one-hot tensors the reference's
     preprocess_batch produces).  `curr_available_actions` (padding included) sets the online advantage mean; without it the
@@ -111,16 +78,16 @@ def learn_batch(pl, batch) -> dict:
     reward = f32(batch.reward.reshape(B))
     term = batch.terminated.reshape(B).to(device=dev, dtype=torch.uint8).contiguous()
     i32 = lambda t: t.to(torch.int32).contiguous()  # noqa: E731
-    action = i32(_ids(pl, batch.action.to(dev), batch.action.dim() == 2, "batch.action").reshape(B))
+    action = i32(checked_ids(batch.action.to(dev), A, batch.action.dim() == 2, "batch.action").reshape(B))
     cur = nid = mask = None
     ca = getattr(batch, "curr_available_actions", None)
     if ca is not None:
         ca = ca.to(dev)
-        cur = i32(_ids(pl, ca, ca.dim() == 3, "batch.curr_available_actions").reshape(B, A))
+        cur = i32(checked_ids(ca, A, ca.dim() == 3, "batch.curr_available_actions").reshape(B, A))
     na = getattr(batch, "next_available_actions", None)
     if na is not None:
         na = na.to(dev)
-        nid = i32(_ids(pl, na, na.dim() == 3, "batch.next_available_actions").reshape(B, A))
+        nid = i32(checked_ids(na, A, na.dim() == 3, "batch.next_available_actions").reshape(B, A))
     nm = getattr(batch, "next_unavailable_actions_mask", None)
     if nm is not None:
         mask = nm.to(dev).reshape(B, A).to(torch.uint8).contiguous()

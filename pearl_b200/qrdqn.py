@@ -19,6 +19,7 @@ from typing import Any, Iterable, Optional
 import torch
 
 from . import _lib
+from ._batch import available_first, checked_ids
 from .per import B200PrioritizedReplayBuffer
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
 
@@ -177,18 +178,6 @@ class B200QuantileRegressionDeepQLearning:
             trace["launches"] = int(self._lib.prl_qrdqn_last_launches(self._handle))
         return {"loss": losses}
 
-    def _ids(self, a: torch.Tensor, what: str) -> torch.Tensor:
-        """Action ids from one-hot rows (the reference's preprocess_batch) or from raw ids (trailing dimension 1 or none)."""
-        A = self._n_actions
-        if a.is_floating_point() and a.shape[-1] == A and A > 1:
-            a = a.argmax(-1)
-        elif a.shape[-1] == 1:
-            a = a.squeeze(-1)
-        a = a.long()
-        if bool(((a < 0) | (a >= A)).any()):
-            raise ValueError(f"{what}: action ids must lie in [0, {A})")
-        return a
-
     # ------------------------------------------------------------------ QuantileRegressionDeepTDLearning.learn_batch
     def learn_batch(self, batch) -> dict:
         """One round on a caller-supplied batch (state, action, reward, next_state, terminated and, optionally,
@@ -201,17 +190,12 @@ class B200QuantileRegressionDeepQLearning:
         f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
         state, next_state, reward = f32(batch.state), f32(batch.next_state), f32(batch.reward.reshape(B))
         term = batch.terminated.reshape(B).to(device=dev, dtype=torch.uint8).contiguous()
-        aid = self._ids(batch.action.to(dev).reshape(B, -1), "batch.action").to(torch.int32).contiguous()
+        aid = checked_ids(batch.action.to(dev).reshape(B, -1), A, True, "batch.action").to(torch.int32).contiguous()
         nid = cnt = None
         nxt = getattr(batch, "next_available_actions", None)
         if nxt is not None:
-            nid = self._ids(nxt.to(dev).reshape(B, A, -1), "batch.next_available_actions")
-            mask = getattr(batch, "next_unavailable_actions_mask", None)
-            mask = torch.zeros((B, A), dtype=torch.bool, device=dev) if mask is None else mask.to(dev).reshape(B, A).bool()
-            # available slots first, in their order: the first argmax over them is the first argmax with the others at -inf
-            order = torch.sort(mask.to(torch.int8), dim=1, stable=True).indices
-            nid = nid.gather(1, order).to(torch.int32).contiguous()
-            cnt = (~mask).sum(1).to(torch.int32).contiguous()
+            nid = checked_ids(nxt.to(dev).reshape(B, A, -1), A, True, "batch.next_available_actions")
+            nid, cnt = available_first(nid, getattr(batch, "next_unavailable_actions_mask", None))
         out = torch.empty(1, dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
             _lib.check(self._lib.prl_qrdqn_set_graph(self._handle, int(self.use_cuda_graph)))

@@ -84,6 +84,30 @@ def test_slot_expanded_learners_refuse_shapes_past_32_bit_offsets():
     assert ws > 2 * 8191 * 256 * 1024 * 4      # c1 and dc1 alone
 
 
+@pytest.mark.parametrize("max_rounds", [800_000_000, 1 << 30])
+def test_workspace_holds_the_per_round_blocks_of_large_max_rounds(max_rounds):
+    """max_rounds is only required to be positive: for a max_rounds whose per-round byte counts pass 2^31, every
+    learner's workspace still holds its per-round blocks (sampled slots and logical indices, 4 bytes each per row, and the
+    float2 AdamW scalars of each optimizer plus, in the DQN family, the int32 target flags).  Host arithmetic only."""
+    from pearl_b200 import _lib
+    lib = _lib.load()
+    small = dict(max_batch=1, max_rounds=max_rounds)
+    ac = dict(actor_h1=3, actor_h2=3, critic_h1=3, critic_h2=3)
+    cases = [("sac", _lib.SacCfg(obs_dim=2, act_dim=1, **ac, **small), 8 + 2 * 8),
+             ("sacd", _lib.SacdCfg(obs_dim=2, n_actions=2, **ac, **small), 8 + 3 * 8),
+             ("td3", _lib.Td3Cfg(obs_dim=2, act_dim=1, **ac, actor_update_freq=2, **small), 8 + 2 * 8),
+             ("iql", _lib.IqlCfg(obs_dim=2, n_actions=2, **ac, value_h1=3, value_h2=3, **small), 8 + 3 * 8),
+             ("ppo", _lib.PpoCfg(obs_dim=2, n_actions=2, **ac, max_rollout=16, **small), 8 + 2 * 8),
+             ("qrdqn", _lib.QrdqnCfg(obs_dim=2, n_actions=2, hidden1=3, hidden2=3, num_quantiles=2, target_update_freq=1, **small),
+              8 + 8 + 4),
+             ("cql", _lib.CqlCfg(obs_dim=2, n_actions=2, hidden1=3, hidden2=3, target_update_freq=1, **small), 8 + 8 + 4),
+             ("duel", _lib.DuelCfg(obs_dim=2, n_actions=2, feature_dim=3, state_h1=3, state_h2=3, value_h1=3, value_h2=3, adv_h1=3,
+                                   adv_h2=3, target_update_freq=1, **small), 8 + 8 + 4)]
+    for name, cfg, bytes_per_round in cases:
+        ws = getattr(lib, f"prl_{name}_workspace_bytes")(ctypes.byref(cfg))
+        assert ws >= bytes_per_round * max_rounds, (name, ws, _lib.last_error())
+
+
 def test_no_cpu_fallback():
     import torch
     if torch.cuda.is_available():
