@@ -698,6 +698,44 @@ int prl_ppo_learn(prl_ppo *ppo, prl_buf *buf, int rounds, int batch, const float
                   const float *lam_return_dev, const float *action_probs_dev, float *out_actor_loss_dev,
                   float *out_critic_loss_dev, int32_t *out_logical_dev, void *stream);
 
+/* ---- REINFORCE learner (state-value baseline) -------------------------------------------------------
+ * Replaces REINFORCE.learn (policy_learners/sequential_decision_making/reinforce.py:179-208, losses :146-167) on top of
+ * ActorCriticBase.learn_batch (actor_critic_base.py:309-366) and PolicyLearner.learn (policy_learner.py:162-204), with
+ * use_critic=True, VanillaActorNetwork (softmax policy over every action, actor_networks.py:155-176) and
+ * VanillaValueNetwork, two hidden layers each.  prl_reinforce_returns = the return pass: R = critic(next_state of the newest
+ * transition) * (1 - terminated) + the rewards of every stored transition added newest -> oldest in fp32 (no discount, no
+ * episode reset; every transition of the reference holds this one value).  prl_reinforce_learn = rounds x (sample -> actor
+ * step on B * sum_j nlp_j (R - v_j), the reference's B x B broadcast -> critic step on mean((v - R)^2)), two AdamW(amsgrad)
+ * states.  Flat parameter layouts (row-major [out][in]):
+ *   actor : W1[h1][obs] b1 W2[h2][h1] b2 W3[A][h2] b3      critic: W1[c1][obs] b1 W2[c2][c1] b2 W3[1][c2] b3
+ * 1 <= n_actions <= 255.  Continuous-action, mismatched and sharded buffers are rejected (EINVAL) before any launch. */
+typedef struct prl_reinforce_cfg {
+    int32_t obs_dim, n_actions, actor_h1, actor_h2, critic_h1, critic_h2;
+    int32_t max_batch, max_rounds;
+    double actor_lr, critic_lr, beta1, beta2, eps, weight_decay;
+} prl_reinforce_cfg;
+typedef struct prl_reinforce prl_reinforce;
+int64_t prl_reinforce_actor_param_count(const prl_reinforce_cfg *cfg);
+int64_t prl_reinforce_critic_param_count(const prl_reinforce_cfg *cfg);
+int64_t prl_reinforce_workspace_bytes(const prl_reinforce_cfg *cfg);
+int prl_reinforce_create(prl_reinforce **out, const prl_reinforce_cfg *cfg, float *actor_w, float *actor_m, float *actor_v,
+                         float *actor_vmax, float *critic_w, float *critic_m, float *critic_v, float *critic_vmax,
+                         int64_t adam_step, void *workspace);
+int prl_reinforce_destroy(prl_reinforce *rf);
+int64_t prl_reinforce_adam_step(const prl_reinforce *rf);
+/* New actor / critic AdamW learning rates from the next learn on.  Every lr-dependent scalar travels in the per-call
+ * block: no re-capture, same handle. */
+int prl_reinforce_set_lr(prl_reinforce *rf, double actor_lr, double critic_lr);
+int prl_reinforce_set_graph(prl_reinforce *rf, int enable);
+int64_t prl_reinforce_last_launches(const prl_reinforce *rf);
+/* out_return_dev: device f32[2] = {R, the bootstrap term critic(s'_newest) * (1 - terminated)}.  Given the same
+ * bootstrap term, R is bit-identical to the reference's fold. */
+int prl_reinforce_returns(prl_reinforce *rf, prl_buf *buf, float *out_return_dev, void *stream);
+/* return_dev: the array prl_reinforce_returns wrote (R = return_dev[0]); out_*_loss: device f32[rounds];
+ * out_logical_dev (optional) i32[rounds][batch] = sampled indices */
+int prl_reinforce_learn(prl_reinforce *rf, prl_buf *buf, int rounds, int batch, const float *return_dev,
+                        float *out_actor_loss_dev, float *out_critic_loss_dev, int32_t *out_logical_dev, void *stream);
+
 /* Device timing of the persistent learner kernel alone (CUDA events recorded on
  * the launch stream around the kernel); used by bench.py for the roofline line.
  * prl_dqn_last_kernel_ms synchronises on the end event. */

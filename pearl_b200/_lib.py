@@ -96,6 +96,13 @@ class PpoCfg(C.Structure):
                 ("lam", C.c_double), ("epsilon", C.c_double), ("entropy_bonus", C.c_double)]
 
 
+class ReinforceCfg(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("actor_h1", C.c_int32), ("actor_h2", C.c_int32),
+                ("critic_h1", C.c_int32), ("critic_h2", C.c_int32), ("max_batch", C.c_int32), ("max_rounds", C.c_int32),
+                ("actor_lr", C.c_double), ("critic_lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double),
+                ("eps", C.c_double), ("weight_decay", C.c_double)]
+
+
 class DqnCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden1", C.c_int32),
                 ("hidden2", C.c_int32), ("double_dqn", C.c_int32), ("target_update_freq", C.c_int32),
@@ -241,6 +248,17 @@ _SIGNATURES = {
     "prl_ppo_preprocess": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P]),
     "prl_ppo_gae_redo": (C.c_int, [_P, _P, C.c_float, C.c_float, _P, _P, _P]),
     "prl_ppo_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P, _P, _P]),
+    "prl_reinforce_actor_param_count": (C.c_int64, [C.POINTER(ReinforceCfg)]),
+    "prl_reinforce_critic_param_count": (C.c_int64, [C.POINTER(ReinforceCfg)]),
+    "prl_reinforce_workspace_bytes": (C.c_int64, [C.POINTER(ReinforceCfg)]),
+    "prl_reinforce_create": (C.c_int, [C.POINTER(_P), C.POINTER(ReinforceCfg)] + [_P] * 8 + [C.c_int64, _P]),
+    "prl_reinforce_destroy": (C.c_int, [_P]),
+    "prl_reinforce_adam_step": (C.c_int64, [_P]),
+    "prl_reinforce_set_lr": (C.c_int, [_P, C.c_double, C.c_double]),
+    "prl_reinforce_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_reinforce_last_launches": (C.c_int64, [_P]),
+    "prl_reinforce_returns": (C.c_int, [_P, _P, _P, _P]),
+    "prl_reinforce_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "prl_dqn_set_timing": (C.c_int, [_P, C.c_int]),
     "prl_dqn_set_profile": (C.c_int, [_P, _P]),
     "prl_dqn_last_kernel_ms": (C.c_int, [_P, C.POINTER(C.c_float)]),

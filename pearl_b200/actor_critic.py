@@ -3,6 +3,7 @@
     B200ContinuousSoftActorCritic   (ContinuousSoftActorCritic, soft_actor_critic_continuous.py:42-231)
     B200SoftActorCritic             (SoftActorCritic, soft_actor_critic.py: discrete actions)
     B200ProximalPolicyOptimization  (ProximalPolicyOptimization, ppo.py:96-293)
+    B200REINFORCE                   (REINFORCE, reinforce.py: use_critic=True)
     B200TD3 / B200DeepDeterministicPolicyGradient  (td3.py:43-202, ddpg.py:41-157)
     B200ImplicitQLearning           (ImplicitQLearning, implicit_q_learning.py: offline RL; learn_batch runs on the GPU too)
     B200QuantileRegressionDeepQLearning  (QuantileRegressionDeepQLearning, QR-DQN; not an actor-critic, but bound the same
@@ -29,6 +30,7 @@ import torch
 from .iql import B200ImplicitQLearning as IqlCore
 from .ppo import B200ProximalPolicyOptimization as PpoCore
 from .qrdqn import B200QuantileRegressionDeepQLearning as QrdqnCore
+from .reinforce import B200REINFORCE as RfCore
 from .sac import B200ContinuousSoftActorCritic as SacCore
 from .sac_discrete import B200SoftActorCritic as SacdCore
 from .td3 import B200DeepDeterministicPolicyGradient as DdpgCore
@@ -53,6 +55,13 @@ try:  # pragma: no cover - depends on the environment; kept apart so the classes
     HAVE_REFERENCE_IQL = True
 except Exception:
     HAVE_REFERENCE_IQL = False
+
+try:  # pragma: no cover - depends on the environment; kept apart so the classes above do not depend on it
+    from pearl.policy_learners.sequential_decision_making.reinforce import REINFORCE as _RefREINFORCE
+
+    HAVE_REFERENCE_REINFORCE = True
+except Exception:
+    HAVE_REFERENCE_REINFORCE = False
 
 try:  # pragma: no cover - depends on the environment; kept apart so the classes above do not depend on it
     from pearl.policy_learners.sequential_decision_making.quantile_regression_deep_q_learning import (
@@ -575,6 +584,74 @@ if HAVE_REFERENCE_IQL:
 
 else:
     B200ImplicitQLearning = IqlCore
+
+
+def _reinforce_core_kwargs(pl) -> dict:
+    """Checks that a reference REINFORCE is the configuration the CUDA learner implements and returns the core's network
+    arguments; raises NotImplementedError otherwise.  use_critic=False is refused: the reference's learn() evaluates the
+    critic for its bootstrap value and fails without one."""
+    name = lambda m: type(m).__name__  # noqa: E731
+    if not getattr(pl, "_use_critic", False):
+        raise NotImplementedError("the CUDA REINFORCE learner implements use_critic=True (the reference's learn() needs the "
+                                  "critic for its bootstrap value)")
+    actor, critic = pl._actor, pl._critic
+    if name(actor) != "VanillaActorNetwork":
+        raise NotImplementedError(f"the CUDA REINFORCE learner is built for VanillaActorNetwork, not {name(actor)}")
+    if name(critic) != "VanillaValueNetwork":
+        raise NotImplementedError(f"the CUDA REINFORCE learner is built for VanillaValueNetwork, not {name(critic)}")
+    hsm = getattr(pl, "_history_summarization_module", None)
+    if isinstance(hsm, torch.nn.Module) and any(True for _ in hsm.parameters()):
+        raise NotImplementedError("the CUDA REINFORCE learner reads states as they are stored: a history summarization module "
+                                  "without parameters only")
+    arm = getattr(pl, "_action_representation_module", None) or getattr(pl, "action_representation_module", None)
+    if name(arm) != "OneHotActionTensorRepresentationModule":
+        raise NotImplementedError("the CUDA REINFORCE learner takes a one-hot action representation")
+    if hasattr(getattr(pl, "safety_module", None), "lambda_constraint"):
+        raise NotImplementedError("the CUDA REINFORCE learner does not implement the reward-constrained safety module")
+    sa, sc = _shapes(actor), _shapes(critic)
+    if len(sa) != 6 or len(sc) != 6:
+        raise NotImplementedError("the CUDA REINFORCE learner is built for two hidden layers in the actor and in the critic")
+    obs, h1, h2, n_act = _mlp3(sa, "actor")
+    oc, c1, c2, one = _mlp3(sc, "critic")
+    if oc != obs or one != 1:
+        raise NotImplementedError("unexpected REINFORCE network shapes")
+    return dict(state_dim=obs, n_actions=n_act, actor_hidden_dims=[h1, h2], critic_hidden_dims=[c1, c2])
+
+
+if HAVE_REFERENCE_REINFORCE:
+
+    class B200REINFORCE(_B200ActorCriticMixin, _RefREINFORCE):
+        """Drop-in for `pearl...reinforce.REINFORCE` with use_critic=True: VanillaActorNetwork and VanillaValueNetwork with two
+        hidden layers each, one-hot actions, AdamW(amsgrad) for both.  `learn()` runs the return pass and the training rounds
+        on the GPU from a B200ReplayBuffer; a learning-rate change goes through `prl_reinforce_set_lr` (same handle, same
+        captured graph).  `act()` is the reference's own code (PropensityExploration over the live parameters)."""
+
+        def _make_core(self, device):
+            return RfCore(actor_learning_rate=_adamw_lr(self._actor_optimizer, "actor optimizer"),
+                          critic_learning_rate=_adamw_lr(self._critic_optimizer, "critic optimizer"),
+                          discount_factor=float(self._discount_factor), training_rounds=int(self._training_rounds),
+                          batch_size=int(self._batch_size), device=device, **_reinforce_core_kwargs(self), **self._b200_opts)
+
+        def _module_pairs(self, core):
+            return [(self._actor, core.actor_params), (self._critic, core.critic_params)]
+
+        def _core_steps(self, core):
+            s = int(core._lib.prl_reinforce_adam_step(core._handle)) if core._handle.value else int(core._adam_step)
+            return (s, s)
+
+        def _restart_core(self, core, steps):
+            if steps[0] != steps[1]:
+                raise NotImplementedError("REINFORCE steps actor and critic once per round: one AdamW step count")
+            if core._handle.value:
+                core._lib.prl_reinforce_destroy(core._handle)
+                core._handle = C.c_void_p(0)
+            core._adam_step = int(steps[0])
+
+        def _apply_learning_rates(self, core, lrs):
+            core.set_learning_rates(*lrs)
+
+else:
+    B200REINFORCE = RfCore
 
 
 def _qrdqn_adamw_lr(opt: torch.optim.Optimizer) -> float:

@@ -235,7 +235,7 @@ extern "C" int prl_ppo_gae(int n, const float *values_dev, float last_next_value
 
 #include <new>
 
-#include "gemm.cuh"
+#include "ac_nets.cuh"
 #include "host_runtime.cuh"
 
 namespace {
@@ -260,10 +260,6 @@ __global__ void k_ppo_rollout_rows(const uint32_t *__restrict__ records, prl_buf
         const uint32_t f = r[L.off_flags];
         term[i0 + w] = f & 1u; trunc[i0 + w] = (f >> 1) & 1u;
     }
-}
-__global__ void k_ppo_last_next_state(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int64_t slot, float *__restrict__ S) {
-    const uint32_t *r = records + (size_t)slot * L.record_words;
-    for (int p = threadIdx.x; p < obs; p += blockDim.x) S[p] = __uint_as_float(r[L.off_next_state + p]);
 }
 // probability of the taken action under softmax(logits)
 __global__ void k_ppo_taken_prob(int rows, int A, const float *__restrict__ logits, const int32_t *__restrict__ act, float *__restrict__ out) {
@@ -356,8 +352,7 @@ __global__ void k_ppo_cuts(int n, const uint8_t *__restrict__ term, const uint8_
 
 struct prl_ppo {
     prl_ppo_cfg cfg;
-    int Pa, Pc;
-    int aW1, ab1, aW2, ab2, aW3, ab3, cW1, cb1, cW2, cb2, cW3, cb3;
+    Mlp2 an, cn;          // actor (softmax head) and critic (scalar head) layouts
     float *actor, *actor_m, *actor_v, *actor_x, *critic, *critic_m, *critic_v, *critic_x;
     int64_t adam_step;
     // workspace
@@ -394,26 +389,18 @@ static int ppo_check(const prl_ppo_cfg *c) {
 }
 static void ppo_layout(prl_ppo *s) {
     const prl_ppo_cfg &c = s->cfg;
-    int o = 0;
-    s->aW1 = o; o += c.actor_h1 * c.obs_dim; s->ab1 = o; o += c.actor_h1;
-    s->aW2 = o; o += c.actor_h2 * c.actor_h1; s->ab2 = o; o += c.actor_h2;
-    s->aW3 = o; o += c.n_actions * c.actor_h2; s->ab3 = o; o += c.n_actions;
-    s->Pa = o;
-    o = 0;
-    s->cW1 = o; o += c.critic_h1 * c.obs_dim; s->cb1 = o; o += c.critic_h1;
-    s->cW2 = o; o += c.critic_h2 * c.critic_h1; s->cb2 = o; o += c.critic_h2;
-    s->cW3 = o; o += c.critic_h2; s->cb3 = o; o += 1;
-    s->Pc = o;
+    s->an = mlp2(c.obs_dim, c.actor_h1, c.actor_h2, c.n_actions);
+    s->cn = mlp2(c.obs_dim, c.critic_h1, c.critic_h2, 1);
 }
 extern "C" int64_t prl_ppo_actor_param_count(const prl_ppo_cfg *c) {
     if (ppo_check(c)) return -1;
     prl_ppo t; t.cfg = *c; ppo_layout(&t);
-    return t.Pa;
+    return t.an.P;
 }
 extern "C" int64_t prl_ppo_critic_param_count(const prl_ppo_cfg *c) {
     if (ppo_check(c)) return -1;
     prl_ppo t; t.cfg = *c; ppo_layout(&t);
-    return t.Pc;
+    return t.cn.P;
 }
 // the workspace, in order; base == null: only its size
 static int64_t ppo_carve(prl_ppo *s, void *base) {
@@ -424,7 +411,7 @@ static int64_t ppo_carve(prl_ppo *s, void *base) {
     Carve w{(char *)base};
     w(s->S, R * c.obs_dim); w(s->h1, R * hmax1); w(s->h2, R * hmax2); w(s->logits, R * A); w(s->v, R);
     w(s->gae, R); w(s->lam, R); w(s->old, R); w(s->ap, R); w(s->dlogits, R * A);
-    w(s->dh2, R * hmax2); w(s->dh1, R * hmax1); w(s->dv, R); w(s->g_actor, s->Pa); w(s->g_critic, s->Pc);
+    w(s->dh2, R * hmax2); w(s->dh1, R * hmax1); w(s->dv, R); w(s->g_actor, s->an.P); w(s->g_critic, s->cn.P);
     w(s->reward, c.max_rollout); w(s->last_value, 64);
     w(s->act, R); w(s->slots, MRB); w(s->logical, MRB);
     w(s->term, c.max_rollout); w(s->trunc, c.max_rollout);
@@ -477,18 +464,10 @@ extern "C" int prl_ppo_set_graph(prl_ppo *s, int enable) {
 extern "C" int64_t prl_ppo_last_launches(const prl_ppo *s) { return s ? s->last_launches : -1; }
 
 static void ppo_actor_forward(prl_ppo *s, GemmLauncher &L, int rows) {
-    const prl_ppo_cfg &c = s->cfg;
-    const float *aw = s->actor;
-    L.fwd(mat(s->S, c.obs_dim), rows, aw + s->aW1, c.obs_dim, 0, aw + s->ab1, 0, c.actor_h1, c.obs_dim, true, s->h1, c.actor_h1, 0);
-    L.fwd(mat(s->h1, c.actor_h1), rows, aw + s->aW2, c.actor_h1, 0, aw + s->ab2, 0, c.actor_h2, c.actor_h1, true, s->h2, c.actor_h2, 0);
-    L.fwd(mat(s->h2, c.actor_h2), rows, aw + s->aW3, c.actor_h2, 0, aw + s->ab3, 0, c.n_actions, c.actor_h2, false, s->logits, c.n_actions, 0);
+    mlp2_forward(L, s->an, s->actor, s->S, rows, s->h1, s->h2, s->logits);
 }
 static void ppo_critic_forward(prl_ppo *s, GemmLauncher &L, int rows, float *vout) {
-    const prl_ppo_cfg &c = s->cfg;
-    const float *cw = s->critic;
-    L.fwd(mat(s->S, c.obs_dim), rows, cw + s->cW1, c.obs_dim, 0, cw + s->cb1, 0, c.critic_h1, c.obs_dim, true, s->h1, c.critic_h1, 0);
-    L.fwd(mat(s->h1, c.critic_h1), rows, cw + s->cW2, c.critic_h1, 0, cw + s->cb2, 0, c.critic_h2, c.critic_h1, true, s->h2, c.critic_h2, 0);
-    L.fwd(mat(s->h2, c.critic_h2), rows, cw + s->cW3, c.critic_h2, 0, cw + s->cb3, 0, 1, c.critic_h2, false, vout, 1, 0);
+    mlp2_forward(L, s->cn, s->critic, s->S, rows, s->h1, s->h2, vout);
 }
 
 // preprocess_replay_buffer (ppo.py:201-293): state values, taken-action probabilities, GAE and lambda returns of the whole
@@ -518,7 +497,7 @@ extern "C" int prl_ppo_preprocess(prl_ppo *s, prl_buf *buf, float *out_values, f
         ppo_actor_forward(s, L, rows);
         k_ppo_taken_prob<<<(rows + 255) / 256, 256, 0, st>>>(rows, c.n_actions, s->logits, s->act, out_action_probs + i0);
     }
-    k_ppo_last_next_state<<<1, 128, 0, st>>>(buf->records, buf->lay, c.obs_dim, (head + n - 1) % cap, s->S);
+    k_last_next_state<<<1, 128, 0, st>>>(buf->records, buf->lay, c.obs_dim, (head + n - 1) % cap, s->S);
     ppo_critic_forward(s, L, 1, s->last_value);
     {
         const int rc = launch_gae((int)n, out_values, 0.f, s->last_value, 0.f, s->reward, s->term, s->trunc, (float)c.gamma,
@@ -547,36 +526,24 @@ extern "C" int prl_ppo_gae_redo(prl_ppo *s, const float *values_dev, float next_
 
 static int ppo_round(prl_ppo *s, prl_buf *buf, int B, cudaStream_t st) {
     const prl_ppo_cfg &c = s->cfg;
-    const int O = c.obs_dim, A = c.n_actions, H1 = c.actor_h1, H2 = c.actor_h2, C1 = c.critic_h1, C2 = c.critic_h2;
+    const int O = c.obs_dim;
     GemmLauncher L; L.st = st;
     const AdamHp ha = adam_hp(c.actor_lr, c.beta1, c.beta2, c.eps, c.weight_decay), hc = adam_hp(c.critic_lr, c.beta1, c.beta2, c.eps, c.weight_decay);
     const int eb = 256;
     k_ppo_gather<<<(B * 32 + eb - 1) / eb, eb, 0, st>>>(buf->records, buf->lay, O, s->call, s->round_idx, B, s->S, s->act, s->gae, s->lam, s->old);
     // ---------------- actor step
     ppo_actor_forward(s, L, B);
-    k_ppo_actor_loss<<<1, 256, 0, st>>>(B, A, s->logits, s->act, s->gae, s->old, (float)c.epsilon, (float)c.entropy_bonus, s->ap, s->dlogits,
+    k_ppo_actor_loss<<<1, 256, 0, st>>>(B, c.n_actions, s->logits, s->act, s->gae, s->old, (float)c.epsilon, (float)c.entropy_bonus, s->ap, s->dlogits,
                                         s->call, s->round_idx);
-    {
-        const float *aw = s->actor; float *ga = s->g_actor;
-        L.bwd_w(s->dlogits, A, 0, B, A, mat(s->h2, H2), H2, ga + s->aW3, H2, 0, ga + s->ab3, 0);
-        L.bwd_x(s->dlogits, A, 0, B, A, aw + s->aW3, H2, 0, 0, H2, s->dh2, H2, 0, s->h2, H2, 0, false);
-        L.bwd_w(s->dh2, H2, 0, B, H2, mat(s->h1, H1), H1, ga + s->aW2, H1, 0, ga + s->ab2, 0);
-        L.bwd_x(s->dh2, H2, 0, B, H2, aw + s->aW2, H1, 0, 0, H1, s->dh1, H1, 0, s->h1, H1, 0, false);
-        L.bwd_w(s->dh1, H1, 0, B, H1, mat(s->S, O), O, ga + s->aW1, O, 0, ga + s->ab1, 0);
-        k_adamw<<<(s->Pa + eb - 1) / eb, eb, 0, st>>>(s->Pa, s->actor, s->actor_m, s->actor_v, s->actor_x, ga, ha, s->scal_a, s->round_idx, nullptr, 0.f, 0.f);
-    }
+    mlp2_backward(L, s->an, s->actor, s->g_actor, s->dlogits, s->S, s->h1, s->h2, s->dh2, s->dh1, B);
+    k_adamw<<<(s->an.P + eb - 1) / eb, eb, 0, st>>>(s->an.P, s->actor, s->actor_m, s->actor_v, s->actor_x, s->g_actor, ha, s->scal_a, s->round_idx,
+                                                  nullptr, 0.f, 0.f);
     // ---------------- critic step (critic_utils.py:139-167)
     ppo_critic_forward(s, L, B, s->v);
     k_ppo_critic_loss<<<1, 256, 0, st>>>(B, s->v, s->lam, s->dv, s->call, s->round_idx);
-    {
-        const float *cw = s->critic; float *gc = s->g_critic;
-        L.bwd_w(s->dv, 1, 0, B, 1, mat(s->h2, C2), C2, gc + s->cW3, C2, 0, gc + s->cb3, 0);
-        k_head_bwd<<<dim3((B * C2 + eb - 1) / eb, 1, 1), eb, 0, st>>>(B, C2, s->dv, cw + s->cW3, 0, s->h2, s->dh2);
-        L.bwd_w(s->dh2, C2, 0, B, C2, mat(s->h1, C1), C1, gc + s->cW2, C1, 0, gc + s->cb2, 0);
-        L.bwd_x(s->dh2, C2, 0, B, C2, cw + s->cW2, C1, 0, 0, C1, s->dh1, C1, 0, s->h1, C1, 0, false);
-        L.bwd_w(s->dh1, C1, 0, B, C1, mat(s->S, O), O, gc + s->cW1, O, 0, gc + s->cb1, 0);
-        k_adamw<<<(s->Pc + eb - 1) / eb, eb, 0, st>>>(s->Pc, s->critic, s->critic_m, s->critic_v, s->critic_x, gc, hc, s->scal_c, s->round_idx, nullptr, 0.f, 0.f);
-    }
+    mlp2_backward(L, s->cn, s->critic, s->g_critic, s->dv, s->S, s->h1, s->h2, s->dh2, s->dh1, B);   // + one k_head_bwd
+    k_adamw<<<(s->cn.P + eb - 1) / eb, eb, 0, st>>>(s->cn.P, s->critic, s->critic_m, s->critic_v, s->critic_x, s->g_critic, hc, s->scal_c,
+                                                  s->round_idx, nullptr, 0.f, 0.f);
     k_ppo_bump<<<1, 1, 0, st>>>(s->round_idx);
     s->launches_per_round = L.count + 7;
     return PRL_OK;
