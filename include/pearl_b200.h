@@ -59,7 +59,9 @@ int prl_sm_count(void);
  *     [off_action     .. +act_words) action       i32 (discrete) | f32[act_dim]
  *     [off_reward]                   reward       f32
  *     [off_flags]                    bit0 terminated, bit1 truncated,
- *                                    bits 8..23 number of next available actions
+ *                                    bits 8..23 number of next available actions,
+ *                                    bits 24..31 (PRL_BUF_NEXT_ACTION only) the
+ *                                    committed next action id (SARSA)
  *     [off_avail .. ) (PRL_BUF_DYNAMIC_ACTIONS only) n_actions u8 ids of the
  *                     next available actions (padded with 0), as the reference
  *                     pads `next_available_actions` (tensor_based_replay_buffer.py:179-251)
@@ -68,6 +70,7 @@ int prl_sm_count(void);
 #define PRL_BUF_DISCRETE 0x1          /* action is one int32 id in [0, n_actions) */
 #define PRL_BUF_CONTINUOUS 0x2        /* action is act_dim floats */
 #define PRL_BUF_DYNAMIC_ACTIONS 0x4   /* per-transition next-available-action sets */
+#define PRL_BUF_NEXT_ACTION 0x8       /* discrete only: the committed next action id of SARSA in the flags word */
 
 typedef struct prl_buf_desc {
     int64_t capacity;
@@ -136,6 +139,26 @@ int prl_buf_push_device(prl_buf *buf, int64_t n, const float *state, const void 
                         const uint8_t *truncated, const uint8_t *next_avail_ids,
                         const int32_t *next_avail_cnt, void *stream);
 
+/* The pushes of a PRL_BUF_NEXT_ACTION buffer (SARSAReplayBuffer's complete tuples,
+ * replay_buffers/sequential_decision_making/sarsa_replay_buffer.py:29-101): the
+ * arguments of prl_buf_push_host / prl_buf_push_device / prl_buf_push_host_multi
+ * plus next_action int32[n] (multi: [count][n]), ids in [0, n_actions) (host
+ * pushes check them).  A PRL_BUF_NEXT_ACTION buffer refuses the plain entries, a
+ * plain buffer refuses these (PRL_EINVAL): no next action is ever stored as id 0
+ * by omission. */
+int prl_buf_push_host_sarsa(prl_buf *buf, int64_t n, const float *state, const void *action,
+                            const float *reward, const float *next_state, const uint8_t *terminated,
+                            const uint8_t *truncated, const uint8_t *next_avail_ids,
+                            const int32_t *next_avail_cnt, const int32_t *next_action, void *stream);
+int prl_buf_push_device_sarsa(prl_buf *buf, int64_t n, const float *state, const void *action,
+                              const float *reward, const float *next_state, const uint8_t *terminated,
+                              const uint8_t *truncated, const uint8_t *next_avail_ids,
+                              const int32_t *next_avail_cnt, const int32_t *next_action, void *stream);
+int prl_buf_push_host_multi_sarsa(prl_buf *const *bufs, int count, int64_t n, const float *state,
+                                  const void *action, const float *reward, const float *next_state,
+                                  const uint8_t *terminated, const uint8_t *truncated,
+                                  const int32_t *next_action, void *stream);
+
 /* RNG state hand-off with CPython's global `random` module
  * (the reference samples with random.sample, tensor_based_replay_buffer.py:276;
  * state = random.getstate()[1]).  Host pointers, uint32[625].  get synchronises
@@ -164,6 +187,12 @@ int prl_buf_sample_indices(prl_buf *buf, int rounds, int k, int32_t *out_logical
 int prl_buf_gather(const prl_buf *buf, const int32_t *slot_dev, int k, float *state, void *action,
                    float *reward, float *next_state, uint8_t *terminated, uint8_t *truncated,
                    float *next_avail, uint8_t *next_unavail_mask, void *stream);
+
+/* The committed next action of k records of a PRL_BUF_NEXT_ACTION buffer:
+ * out_dev i64[k] (the reference collates next_action as int64); PRL_EINVAL on
+ * any other buffer. */
+int prl_buf_gather_next_action(const prl_buf *buf, const int32_t *slot_dev, int k, int64_t *out_dev,
+                               void *stream);
 
 /* ---- DQN / DoubleDQN learner ---------------------------------------------
  * Replaces DeepTDLearning.learn_batch + DeepQLearning / DoubleDQN
@@ -657,6 +686,54 @@ int prl_duel_q_values(prl_duel *duel, int n, const float *state, const int32_t *
                       void *stream);
 int prl_duel_set_graph(prl_duel *duel, int enable);
 int64_t prl_duel_last_launches(const prl_duel *duel);
+
+/* ---- DeepSARSA ------------------------------------------------------------------------------------
+ * Replaces DeepSARSA.get_next_state_values (policy_learners/sequential_decision_making/deep_sarsa.py:58-75) on
+ * DeepTDLearning.forward / loss / learn_batch (deep_td_learning.py:269-360) with VanillaQValueNetwork.get_q_values
+ * (neural_networks/sequential_decision_making/q_value_networks.py:152-174), driven by PolicyLearner.learn (prl_sarsa_learn:
+ * sample -> round, `rounds` times, over a PRL_BUF_NEXT_ACTION buffer) or called on a caller's batch (prl_sarsa_learn_batch:
+ * one round, PearlAgent.learn_batch).  Per round:
+ *   when (training_steps + 1) % target_update_freq == 0, FIRST target = tau * online + (1 - tau) * target;
+ *   q_b = Q(s_b, a_b); y_b = Q'(s'_b, a'_b) gamma (1 - terminated_b) + r_b with a'_b the committed next action (no max,
+ *   the available sets take no part); L = mean_b (q_b - y_b)^2; one AdamW(amsgrad) step.  Reported loss: mean_b |q_b - y_b|.
+ * 1 <= n_actions <= 255.  Flat layout as prl_dqn: W1[h1][obs + A] b1 W2[h2][h1] b2 W3[1][h2] b3.  Buffers without
+ * PRL_BUF_NEXT_ACTION, sharded, continuous-action or mismatched buffers, and batch / rounds above the configured maxima
+ * are rejected (EINVAL) before any launch.
+ * The round is captured into a CUDA graph per (batch, buffer) and kept in a small cache (least recently used out), so an
+ * on-policy loop whose batch follows the episode length replays the graph of a batch size it has seen. */
+typedef struct prl_sarsa_cfg {
+    int32_t obs_dim, n_actions, hidden1, hidden2;
+    int32_t target_update_freq, max_batch, max_rounds;
+    double lr, beta1, beta2, eps, weight_decay, gamma, tau;
+} prl_sarsa_cfg;
+typedef struct prl_sarsa prl_sarsa;
+int64_t prl_sarsa_param_count(const prl_sarsa_cfg *cfg);
+int64_t prl_sarsa_workspace_bytes(const prl_sarsa_cfg *cfg);
+/* w, w_target, exp_avg, exp_avg_sq, max_exp_avg_sq: device f32[param_count] owned by the caller (the argument order of
+ * prl_dqn_create); adam_step: optimizer steps already taken (torch's `step`). */
+int prl_sarsa_create(prl_sarsa **out, const prl_sarsa_cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq,
+                     float *max_exp_avg_sq, int64_t adam_step, void *workspace_dev);
+int prl_sarsa_destroy(prl_sarsa *sarsa);
+int64_t prl_sarsa_adam_step(const prl_sarsa *sarsa);
+int prl_sarsa_set_adam_step(prl_sarsa *sarsa, int64_t step);
+/* New AdamW learning rate from the next call on; every lr-dependent scalar travels in the per-call block: no re-capture. */
+int prl_sarsa_set_lr(prl_sarsa *sarsa, double lr);
+/* training_steps = the learner's count before the call (PolicyLearner.learn increments it before each round);
+ * out_loss_dev: device f32[rounds]; out_logical_dev (optional) i32[rounds][batch] = sampled indices. */
+int prl_sarsa_learn(prl_sarsa *sarsa, prl_buf *buf, int rounds, int batch, int64_t training_steps, float *out_loss_dev,
+                    int32_t *out_logical_dev, void *stream);
+/* One round on a dense device batch: state / next_state f32[batch][obs], action_id / next_action_id i32[batch] in
+ * [0, n_actions), reward f32[batch], terminated u8[batch]; training_steps = the count learn_batch sees (agent.learn_batch
+ * does not advance it); out_loss_dev: device f32[1]. */
+int prl_sarsa_learn_batch(prl_sarsa *sarsa, int batch, const float *state, const int32_t *action_id, const float *reward,
+                          const float *next_state, const int32_t *next_action_id, const uint8_t *terminated,
+                          int64_t training_steps, float *out_loss_dev, void *stream);
+/* Q(s, a) for every action: device state f32[n][obs_dim] -> out_q f32[n][n_actions], online (target = 0) or target. */
+int prl_sarsa_q_values(prl_sarsa *sarsa, int n, const float *state, int target, float *out_q_dev, void *stream);
+int prl_sarsa_set_graph(prl_sarsa *sarsa, int enable);
+int64_t prl_sarsa_last_launches(const prl_sarsa *sarsa);
+/* CUDA graphs captured by this handle so far (a batch size already in the graph cache adds none). */
+int64_t prl_sarsa_graph_captures(const prl_sarsa *sarsa);
 
 /* ---- PPO learner ------------------------------------------------------------------------------
  * Replaces ProximalPolicyOptimization.learn (policy_learners/sequential_decision_making/ppo.py:195-293):

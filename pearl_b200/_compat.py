@@ -25,6 +25,8 @@ try:  # pragma: no cover - depends on the environment
     )
     from pearl.neural_networks.sequential_decision_making.q_value_networks import DuelingQValueNetwork
     from pearl.policy_learners.sequential_decision_making.double_dqn import DoubleDQN as _RefDoubleDQN
+    from pearl.policy_learners.sequential_decision_making.deep_sarsa import DeepSARSA as _RefDeepSARSA
+    from pearl.policy_learners.exploration_modules.common.epsilon_greedy_exploration import EGreedyExploration
     from pearl.replay_buffers.replay_buffer import ReplayBuffer
     from pearl.replay_buffers.transition import TransitionBatch
 
@@ -221,3 +223,31 @@ except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
 
     class _RefDoubleDQN(_RefDeepQLearning):
         pass
+
+    class EGreedyExploration:
+        """Attribute-compatible stand-in for EGreedyExploration (exploration_modules/common/epsilon_greedy_exploration.py):
+        with probability `curr_epsilon` a uniformly drawn action of the space, else the greedy one."""
+
+        def __init__(self, epsilon: float) -> None:
+            self.curr_epsilon = epsilon
+
+        def act(self, subjective_state, action_space, exploit_action, values=None, action_availability_mask=None,
+                representation=None):
+            import random
+            if random.random() < self.curr_epsilon:
+                return action_space.actions[random.randrange(action_space.n)]
+            return exploit_action
+
+    class _RefDeepSARSA(_RefDeepQLearning):
+        """Attribute-compatible stand-in for DeepSARSA's constructor (deep_sarsa.py:35-56): on-policy, and
+        EGreedyExploration(0.05) unless an exploration module is given, and DeepTDLearning's own defaults (100 training
+        rounds, soft_update_tau 0.1) where DeepQLearning sets others."""
+
+        def __init__(self, state_dim=None, action_space=None, exploration_module=None, action_representation_module=None,
+                     optimizer=None, **kwargs: Any) -> None:
+            kwargs.setdefault("training_rounds", 100)
+            kwargs.setdefault("soft_update_tau", 0.1)
+            super().__init__(state_dim=state_dim, action_space=action_space,
+                             exploration_module=exploration_module if exploration_module is not None else EGreedyExploration(0.05),
+                             action_representation_module=action_representation_module, optimizer=optimizer, **kwargs)
+            self.on_policy = True

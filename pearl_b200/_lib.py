@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libpearlb200.so")
 PRL_BUF_DISCRETE = 0x1
 PRL_BUF_CONTINUOUS = 0x2
 PRL_BUF_DYNAMIC_ACTIONS = 0x4
+PRL_BUF_NEXT_ACTION = 0x8
 PRL_EINVAL = -1
 
 
@@ -88,6 +89,13 @@ class DuelCfg(C.Structure):
                 ("eps", C.c_double), ("weight_decay", C.c_double), ("gamma", C.c_double), ("tau", C.c_double)]
 
 
+class SarsaCfg(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden1", C.c_int32), ("hidden2", C.c_int32),
+                ("target_update_freq", C.c_int32), ("max_batch", C.c_int32), ("max_rounds", C.c_int32), ("lr", C.c_double),
+                ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double), ("weight_decay", C.c_double),
+                ("gamma", C.c_double), ("tau", C.c_double)]
+
+
 class PpoCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("actor_h1", C.c_int32), ("actor_h2", C.c_int32),
                 ("critic_h1", C.c_int32), ("critic_h2", C.c_int32), ("max_batch", C.c_int32), ("max_rounds", C.c_int32),
@@ -130,6 +138,10 @@ _SIGNATURES = {
     "prl_buf_push_host": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "prl_buf_push_host_multi": (C.c_int, [_P, C.c_int, C.c_int64, _P, _P, _P, _P, _P, _P, _P]),
     "prl_buf_push_device": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "prl_buf_push_host_sarsa": (C.c_int, [_P, C.c_int64] + [_P] * 10),
+    "prl_buf_push_device_sarsa": (C.c_int, [_P, C.c_int64] + [_P] * 10),
+    "prl_buf_push_host_multi_sarsa": (C.c_int, [_P, C.c_int, C.c_int64] + [_P] * 8),
+    "prl_buf_gather_next_action": (C.c_int, [_P, _P, C.c_int, _P, _P]),
     "prl_rng_set_state": (C.c_int, [_P, _P, _P]),
     "prl_rng_get_state": (C.c_int, [_P, _P, _P]),
     "prl_rng_seed": (C.c_int, [_P, _P, C.c_int, _P]),
@@ -237,6 +249,19 @@ _SIGNATURES = {
     "prl_duel_q_values": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P]),
     "prl_duel_set_graph": (C.c_int, [_P, C.c_int]),
     "prl_duel_last_launches": (C.c_int64, [_P]),
+    "prl_sarsa_param_count": (C.c_int64, [C.POINTER(SarsaCfg)]),
+    "prl_sarsa_workspace_bytes": (C.c_int64, [C.POINTER(SarsaCfg)]),
+    "prl_sarsa_create": (C.c_int, [C.POINTER(_P), C.POINTER(SarsaCfg), _P, _P, _P, _P, _P, C.c_int64, _P]),
+    "prl_sarsa_destroy": (C.c_int, [_P]),
+    "prl_sarsa_adam_step": (C.c_int64, [_P]),
+    "prl_sarsa_set_adam_step": (C.c_int, [_P, C.c_int64]),
+    "prl_sarsa_set_lr": (C.c_int, [_P, C.c_double]),
+    "prl_sarsa_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, _P, _P, _P]),
+    "prl_sarsa_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 6 + [C.c_int64, _P, _P]),
+    "prl_sarsa_q_values": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
+    "prl_sarsa_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_sarsa_last_launches": (C.c_int64, [_P]),
+    "prl_sarsa_graph_captures": (C.c_int64, [_P]),
     "prl_ppo_actor_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_critic_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_workspace_bytes": (C.c_int64, [C.POINTER(PpoCfg)]),

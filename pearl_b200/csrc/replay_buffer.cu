@@ -61,6 +61,7 @@ extern "C" int prl_buf_layout_of(const prl_buf_desc *d, prl_buf_layout *out) {
     if (disc) PRL_REQUIRE(d->n_actions > 0 && d->n_actions <= 255, "n_actions must be in [1,255]");
     if (cont) PRL_REQUIRE(d->act_dim > 0, "act_dim must be positive");
     if (d->flags & PRL_BUF_DYNAMIC_ACTIONS) PRL_REQUIRE(disc, "dynamic action sets need a discrete space");
+    if (d->flags & PRL_BUF_NEXT_ACTION) PRL_REQUIRE(disc, "a committed next action needs a discrete space");
     const int obs_p = round_up(d->obs_dim, 4);
     prl_buf_layout l;
     l.off_state = 0;
@@ -169,11 +170,24 @@ static int ensure_staging(prl_buf *b) {
     return PRL_OK;
 }
 
+// next_action: the committed next action ids of a PRL_BUF_NEXT_ACTION buffer (the *_sarsa entries), null for every other
+// buffer; a push that would store id 0 for it, or drop it, is refused
+static int check_next_action(const prl_buf *b, const void *next_action) {
+    PRL_REQUIRE(b, "null buffer");
+    if (b->desc.flags & PRL_BUF_NEXT_ACTION)
+        PRL_REQUIRE(next_action, "the buffer stores a committed next action (PRL_BUF_NEXT_ACTION): push with the *_sarsa entries");
+    else
+        PRL_REQUIRE(!next_action, "next actions given for a buffer created without PRL_BUF_NEXT_ACTION");
+    return PRL_OK;
+}
+
 static int check_push_args(const prl_buf *b, int64_t n, const void *state, const void *action,
                            const void *reward, const void *terminated, const void *truncated,
-                           const void *ids, const void *cnt) {
+                           const void *ids, const void *cnt, const void *next_action) {
     PRL_REQUIRE(b, "null buffer");
     PRL_REQUIRE(n >= 0, "negative count");
+    int rc = check_next_action(b, next_action);
+    if (rc) return rc;
     if (n == 0) return PRL_OK;
     PRL_REQUIRE(state && action && reward && terminated && truncated, "null field array");
     PRL_REQUIRE((ids == nullptr) == (cnt == nullptr), "next_avail_ids and next_avail_cnt go together");
@@ -186,7 +200,7 @@ static int check_push_args(const prl_buf *b, int64_t n, const void *state, const
 // pack transitions [i0, i0 + m) of struct-of-arrays host sources into m consecutive records at `st` (pure CPU)
 static void pack_records_host(const prl_buf *b, uint32_t *st, int64_t i0, int64_t m, const float *state, const void *action,
                               const float *reward, const float *next_state, const uint8_t *terminated, const uint8_t *truncated,
-                              const uint8_t *next_avail_ids, const int32_t *next_avail_cnt) {
+                              const uint8_t *next_avail_ids, const int32_t *next_avail_cnt, const int32_t *next_action) {
     const prl_buf_layout &L = b->lay;
     const int obs = b->desc.obs_dim, A = b->desc.n_actions, W = L.record_words;
     for (int64_t i = 0; i < m; i++) {
@@ -206,7 +220,8 @@ static void pack_records_host(const prl_buf *b, uint32_t *st, int64_t i0, int64_
         r[L.off_reward] = f2u(reward[s]);
         uint32_t cnt = (b->desc.flags & PRL_BUF_DISCRETE) ? (uint32_t)A : 0u;
         if (next_avail_cnt) cnt = (uint32_t)next_avail_cnt[s];
-        r[L.off_flags] = (terminated[s] ? 1u : 0u) | (truncated[s] ? 2u : 0u) | (cnt << 8);
+        r[L.off_flags] = (terminated[s] ? 1u : 0u) | (truncated[s] ? 2u : 0u) | (cnt << 8) |
+                         (next_action ? (uint32_t)next_action[s] << 24 : 0u);
         for (int p = L.off_avail; p < W; p++) r[p] = 0;
         if (b->desc.flags & PRL_BUF_DYNAMIC_ACTIONS) {
             uint8_t *ids = (uint8_t *)(r + L.off_avail);
@@ -218,14 +233,23 @@ static void pack_records_host(const prl_buf *b, uint32_t *st, int64_t i0, int64_
     }
 }
 
-extern "C" int prl_buf_push_host(prl_buf *b, int64_t n, const float *state, const void *action,
-                                 const float *reward, const float *next_state,
-                                 const uint8_t *terminated, const uint8_t *truncated,
-                                 const uint8_t *next_avail_ids, const int32_t *next_avail_cnt,
-                                 void *stream_) {
+// ids outside [0, n_actions) would alias other ids in the 8-bit field
+static int check_next_ids_host(const prl_buf *b, int64_t n, const int32_t *next_action) {
+    if (!next_action) return PRL_OK;
+    for (int64_t i = 0; i < n; i++)
+        PRL_REQUIRE(next_action[i] >= 0 && next_action[i] < b->desc.n_actions, "next action %d of transition %lld outside [0, %d)",
+                    next_action[i], (long long)i, b->desc.n_actions);
+    return PRL_OK;
+}
+
+static int push_host(prl_buf *b, int64_t n, const float *state, const void *action, const float *reward, const float *next_state,
+                     const uint8_t *terminated, const uint8_t *truncated, const uint8_t *next_avail_ids,
+                     const int32_t *next_avail_cnt, const int32_t *next_action, void *stream_) {
     int rc = check_push_args(b, n, state, action, reward, terminated, truncated, next_avail_ids,
-                             next_avail_cnt);
+                             next_avail_cnt, next_action);
     if (rc || n == 0) return rc;
+    rc = check_next_ids_host(b, n, next_action);
+    if (rc) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     rc = ensure_staging(b);
     if (rc) return rc;
@@ -245,7 +269,8 @@ extern "C" int prl_buf_push_host(prl_buf *b, int64_t n, const float *state, cons
         b->stage_next ^= 1;
         PRL_CUDA(cudaEventSynchronize(b->stage_done[sb]));
         uint32_t *st = b->stage[sb];
-        pack_records_host(b, st, i0, m, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt);
+        pack_records_host(b, st, i0, m, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt,
+                          next_action);
         PRL_CUDA(cudaMemcpyAsync(b->records + b->write_pos * W, st, m * (int64_t)W * 4,
                                  cudaMemcpyHostToDevice, stream));
         PRL_CUDA(cudaEventRecord(b->stage_done[sb], stream));
@@ -256,17 +281,44 @@ extern "C" int prl_buf_push_host(prl_buf *b, int64_t n, const float *state, cons
     return PRL_OK;
 }
 
+extern "C" int prl_buf_push_host(prl_buf *b, int64_t n, const float *state, const void *action,
+                                 const float *reward, const float *next_state,
+                                 const uint8_t *terminated, const uint8_t *truncated,
+                                 const uint8_t *next_avail_ids, const int32_t *next_avail_cnt,
+                                 void *stream_) {
+    return push_host(b, n, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, nullptr,
+                     stream_);
+}
+
+extern "C" int prl_buf_push_host_sarsa(prl_buf *b, int64_t n, const float *state, const void *action, const float *reward,
+                                       const float *next_state, const uint8_t *terminated, const uint8_t *truncated,
+                                       const uint8_t *next_avail_ids, const int32_t *next_avail_cnt, const int32_t *next_action,
+                                       void *stream_) {
+    PRL_REQUIRE(next_action || n == 0, "null next_action");
+    return push_host(b, n, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, next_action,
+                     stream_);
+}
+
 // The same push for `count` buffers of one layout at once (a vectorised environment feeding a learner group):
 // sources are [count][n][...] host arrays.  Records are packed by a few worker threads (pure CPU work), the copies are
 // enqueued by the calling thread.  Buffers whose push would wrap the ring or exceed the staging area take the
 // single-buffer path.
-extern "C" int prl_buf_push_host_multi(prl_buf *const *bufs, int count, int64_t n, const float *state, const void *action,
-                                       const float *reward, const float *next_state, const uint8_t *terminated,
-                                       const uint8_t *truncated, void *stream_) {
+static int push_host_multi(prl_buf *const *bufs, int count, int64_t n, const float *state, const void *action, const float *reward,
+                           const float *next_state, const uint8_t *terminated, const uint8_t *truncated, const int32_t *next_action,
+                           void *stream_) {
     PRL_REQUIRE(bufs && count > 0, "null / empty buffer list");
     PRL_REQUIRE(n >= 0, "negative count");
+    for (int i = 0; i < count; i++) {
+        int rc = check_next_action(bufs[i], next_action);
+        if (rc) return rc;
+    }
     if (n == 0) return PRL_OK;
     PRL_REQUIRE(state && action && reward && terminated && truncated, "null field array");
+    if (next_action)
+        for (int i = 0; i < count; i++) {
+            int rc = check_next_ids_host(bufs[i], n, next_action + (size_t)i * n);
+            if (rc) return rc;
+        }
     cudaStream_t stream = (cudaStream_t)stream_;
     struct Job { prl_buf *b; uint32_t *st; int sb; int idx; };
     std::vector<Job> fast;
@@ -289,7 +341,8 @@ extern "C" int prl_buf_push_host_multi(prl_buf *const *bufs, int count, int64_t 
         }
     }
     const int obs = bufs[0]->desc.obs_dim, aw = bufs[0]->lay.act_words;
-    auto src = [&](int i, const float *&s, const void *&a, const float *&r, const float *&ns, const uint8_t *&te, const uint8_t *&tr) {
+    auto src = [&](int i, const float *&s, const void *&a, const float *&r, const float *&ns, const uint8_t *&te, const uint8_t *&tr,
+                   const int32_t *&na) {
         s = state + (size_t)i * n * obs;
         a = (bufs[0]->desc.flags & PRL_BUF_DISCRETE) ? (const void *)((const int32_t *)action + (size_t)i * n)
                                                      : (const void *)((const float *)action + (size_t)i * n * aw);
@@ -297,13 +350,14 @@ extern "C" int prl_buf_push_host_multi(prl_buf *const *bufs, int count, int64_t 
         ns = next_state ? next_state + (size_t)i * n * obs : nullptr;
         te = terminated + (size_t)i * n;
         tr = truncated + (size_t)i * n;
+        na = next_action ? next_action + (size_t)i * n : nullptr;
     };
     const int T = (int)std::min<size_t>(8, fast.size());
     auto work = [&](int t) {
         for (size_t j = t; j < fast.size(); j += T) {
-            const float *s, *r, *ns; const void *a; const uint8_t *te, *tr;
-            src(fast[j].idx, s, a, r, ns, te, tr);
-            pack_records_host(fast[j].b, fast[j].st, 0, n, s, a, r, ns, te, tr, nullptr, nullptr);
+            const float *s, *r, *ns; const void *a; const uint8_t *te, *tr; const int32_t *na;
+            src(fast[j].idx, s, a, r, ns, te, tr, na);
+            pack_records_host(fast[j].b, fast[j].st, 0, n, s, a, r, ns, te, tr, nullptr, nullptr, na);
         }
     };
     std::vector<std::thread> pool;
@@ -320,12 +374,25 @@ extern "C" int prl_buf_push_host_multi(prl_buf *const *bufs, int count, int64_t 
         b->len = b->len + n > C ? C : b->len + n;
     }
     for (int i : slow) {
-        const float *s, *r, *ns; const void *a; const uint8_t *te, *tr;
-        src(i, s, a, r, ns, te, tr);
-        int rc = prl_buf_push_host(bufs[i], n, s, a, r, ns, te, tr, nullptr, nullptr, stream_);
+        const float *s, *r, *ns; const void *a; const uint8_t *te, *tr; const int32_t *na;
+        src(i, s, a, r, ns, te, tr, na);
+        int rc = push_host(bufs[i], n, s, a, r, ns, te, tr, nullptr, nullptr, na, stream_);
         if (rc) return rc;
     }
     return PRL_OK;
+}
+
+extern "C" int prl_buf_push_host_multi(prl_buf *const *bufs, int count, int64_t n, const float *state, const void *action,
+                                       const float *reward, const float *next_state, const uint8_t *terminated,
+                                       const uint8_t *truncated, void *stream_) {
+    return push_host_multi(bufs, count, n, state, action, reward, next_state, terminated, truncated, nullptr, stream_);
+}
+
+extern "C" int prl_buf_push_host_multi_sarsa(prl_buf *const *bufs, int count, int64_t n, const float *state, const void *action,
+                                             const float *reward, const float *next_state, const uint8_t *terminated,
+                                             const uint8_t *truncated, const int32_t *next_action, void *stream_) {
+    PRL_REQUIRE(next_action || n == 0, "null next_action");
+    return push_host_multi(bufs, count, n, state, action, reward, next_state, terminated, truncated, next_action, stream_);
 }
 
 // K1: pack struct-of-arrays device sources into ring records; one warp per
@@ -337,7 +404,8 @@ __global__ void k_pack_records(uint32_t *__restrict__ records, prl_buf_layout L,
                                const float *__restrict__ next_state,
                                const uint8_t *__restrict__ terminated,
                                const uint8_t *__restrict__ truncated,
-                               const uint8_t *__restrict__ ids, const int32_t *__restrict__ cnts) {
+                               const uint8_t *__restrict__ ids, const int32_t *__restrict__ cnts,
+                               const int32_t *__restrict__ next_action) {
     const int lane = threadIdx.x & 31;
     const int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     if (w >= n) return;
@@ -359,7 +427,8 @@ __global__ void k_pack_records(uint32_t *__restrict__ records, prl_buf_layout L,
         } else if (p == L.off_flags) {
             uint32_t c = (flags & PRL_BUF_DISCRETE) ? (uint32_t)A : 0u;
             if (cnts) c = (uint32_t)cnts[s];
-            v = (terminated[s] ? 1u : 0u) | (truncated[s] ? 2u : 0u) | (c << 8);
+            v = (terminated[s] ? 1u : 0u) | (truncated[s] ? 2u : 0u) | (c << 8) |
+                (next_action ? ((uint32_t)next_action[s] & 0xffu) << 24 : 0u);
         } else if (flags & PRL_BUF_DYNAMIC_ACTIONS) {
             int a0 = (p - L.off_avail) * 4;
             uint32_t c = cnts ? (uint32_t)cnts[s] : (uint32_t)A;
@@ -374,13 +443,11 @@ __global__ void k_pack_records(uint32_t *__restrict__ records, prl_buf_layout L,
     }
 }
 
-extern "C" int prl_buf_push_device(prl_buf *b, int64_t n, const float *state, const void *action,
-                                   const float *reward, const float *next_state,
-                                   const uint8_t *terminated, const uint8_t *truncated,
-                                   const uint8_t *next_avail_ids, const int32_t *next_avail_cnt,
-                                   void *stream_) {
+static int push_device(prl_buf *b, int64_t n, const float *state, const void *action, const float *reward, const float *next_state,
+                       const uint8_t *terminated, const uint8_t *truncated, const uint8_t *next_avail_ids,
+                       const int32_t *next_avail_cnt, const int32_t *next_action, void *stream_) {
     int rc = check_push_args(b, n, state, action, reward, terminated, truncated, next_avail_ids,
-                             next_avail_cnt);
+                             next_avail_cnt, next_action);
     if (rc || n == 0) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     const int64_t C = b->desc.capacity;
@@ -394,11 +461,29 @@ extern "C" int prl_buf_push_device(prl_buf *b, int64_t n, const float *state, co
     int64_t blocks = (m * 32 + threads - 1) / threads;
     k_pack_records<<<(unsigned)blocks, threads, 0, stream>>>(
         b->records, b->lay, b->desc.obs_dim, b->desc.n_actions, b->desc.flags, C, b->write_pos, first,
-        m, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt);
+        m, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, next_action);
     PRL_CUDA(cudaGetLastError());
     b->write_pos = (b->write_pos + m) % C;
     b->len = b->len + m > C ? C : b->len + m;
     return PRL_OK;
+}
+
+extern "C" int prl_buf_push_device(prl_buf *b, int64_t n, const float *state, const void *action,
+                                   const float *reward, const float *next_state,
+                                   const uint8_t *terminated, const uint8_t *truncated,
+                                   const uint8_t *next_avail_ids, const int32_t *next_avail_cnt,
+                                   void *stream_) {
+    return push_device(b, n, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, nullptr,
+                       stream_);
+}
+
+extern "C" int prl_buf_push_device_sarsa(prl_buf *b, int64_t n, const float *state, const void *action, const float *reward,
+                                         const float *next_state, const uint8_t *terminated, const uint8_t *truncated,
+                                         const uint8_t *next_avail_ids, const int32_t *next_avail_cnt, const int32_t *next_action,
+                                         void *stream_) {
+    PRL_REQUIRE(next_action || n == 0, "null next_action");
+    return push_device(b, n, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, next_action,
+                       stream_);
 }
 
 // Shard of a logical replay buffer of `world * capacity` transitions (SURVEY.md 8e): the transition with global
@@ -585,6 +670,23 @@ extern "C" int prl_buf_gather(const prl_buf *b, const int32_t *slot_dev, int k, 
                                                             b->desc.n_actions, b->desc.flags, slot_dev, k,
                                                             state, action, reward, next_state, terminated,
                                                             truncated, next_avail, next_unavail_mask);
+    PRL_CUDA(cudaGetLastError());
+    return PRL_OK;
+}
+
+// the committed next action of k records (PRL_BUF_NEXT_ACTION): bits 24..31 of the flags word, as int64 ids
+__global__ void k_gather_next_action(const uint32_t *__restrict__ records, prl_buf_layout L, const int32_t *__restrict__ slots, int k,
+                                     long long *__restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= k) return;
+    out[i] = (long long)(records[(size_t)slots[i] * L.record_words + L.off_flags] >> 24);
+}
+
+extern "C" int prl_buf_gather_next_action(const prl_buf *b, const int32_t *slot_dev, int k, int64_t *out_dev, void *stream_) {
+    PRL_REQUIRE(b && slot_dev && out_dev, "null argument");
+    PRL_REQUIRE(b->desc.flags & PRL_BUF_NEXT_ACTION, "the buffer was created without PRL_BUF_NEXT_ACTION: it stores no next action");
+    if (k <= 0) return PRL_OK;
+    k_gather_next_action<<<(k + 255) / 256, 256, 0, (cudaStream_t)stream_>>>(b->records, b->lay, slot_dev, k, (long long *)out_dev);
     PRL_CUDA(cudaGetLastError());
     return PRL_OK;
 }

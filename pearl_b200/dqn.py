@@ -27,8 +27,9 @@ import torch
 from . import _lib
 from . import cql as _cql
 from . import dueling as _duel
+from . import sarsa as _sarsa_mod
 from ._batch import action_ids
-from ._compat import _RefDeepQLearning, _RefDoubleDQN, TransitionBatch
+from ._compat import _RefDeepQLearning, _RefDeepSARSA, _RefDoubleDQN, TransitionBatch
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
 
 
@@ -45,6 +46,7 @@ def _linears(qnet) -> list:
 
 class _B200DQNMixin:
     _double = False
+    _sarsa = False          # DeepSARSA: prl_sarsa_* (sarsa.py)
 
     def __init__(self, *args: Any, max_rounds_per_call: int = 4096, rows_per_cta: int = 0,
                  engine: str = "auto", **kwargs: Any) -> None:
@@ -60,6 +62,8 @@ class _B200DQNMixin:
             raise NotImplementedError("the fused Q network assumes a one-hot action representation")
         self._n_actions = int(arm.max_number_actions)
         self._dueling = _duel.is_dueling(self._Q)       # DuelingQValueNetwork: prl_duel_* (dueling.py)
+        if self._sarsa and (self._dueling or self._conservative):
+            _sarsa_mod.check_config(self, engine)
         if self._dueling:
             self._obs_dim, self._duel_dims = _duel.shape_of(self._Q, self._n_actions)
         else:
@@ -70,11 +74,13 @@ class _B200DQNMixin:
                 raise NotImplementedError("unexpected Q-network shape")
         self._max_rounds = int(max_rounds_per_call)
         self._rows_per_cta = int(rows_per_cta)
-        if self._dueling:
+        if self._sarsa:
+            _sarsa_mod.check_config(self, engine)
+        elif self._dueling:
             _duel.check_config(self, engine)
         elif self._conservative:
             _cql.check_config(self, engine)
-        if self._dueling or self._conservative:
+        if self._dueling or self._conservative or self._sarsa:
             self.use_cuda_graph = True          # False: plain stream launches (profilers)
         self._handle = C.c_void_p(0)
         self._bound_ptr = None
@@ -91,9 +97,9 @@ class _B200DQNMixin:
             pass
 
     def _c(self, name: str):
-        """C entry point `name` of the learner this instance binds: prl_duel_* for a dueling Q network, prl_cql_* when
-        conservative, prl_dqn_* otherwise."""
-        prefix = "prl_duel_" if self._dueling else "prl_cql_" if self._conservative else "prl_dqn_"
+        """C entry point `name` of the learner this instance binds: prl_sarsa_* for DeepSARSA, prl_duel_* for a dueling Q
+        network, prl_cql_* when conservative, prl_dqn_* otherwise."""
+        prefix = "prl_sarsa_" if self._sarsa else "prl_duel_" if self._dueling else "prl_cql_" if self._conservative else "prl_dqn_"
         return getattr(self._libh, prefix + name)
 
     def _adam_hparams(self) -> dict:
@@ -135,7 +141,7 @@ class _B200DQNMixin:
         self._libh = _lib.init(device.index if device.index is not None else torch.cuda.current_device())
         hp = self._adam_hparams()
         bound_batch = max(int(need_batch), int(self._batch_size) if self._batch_size > 0 else 0, 1)
-        cfg = _duel.make_cfg(self, hp, bound_batch) if self._dueling else \
+        cfg = _sarsa_mod.make_cfg(self, hp, bound_batch) if self._sarsa else _duel.make_cfg(self, hp, bound_batch) if self._dueling else \
             _cql.make_cfg(self, hp, bound_batch) if self._conservative else _lib.DqnCfg(
             obs_dim=self._obs_dim, n_actions=self._n_actions, hidden1=self._hidden[0], hidden2=self._hidden[1],
             double_dqn=int(self._double), target_update_freq=int(self._target_update_freq),
@@ -257,6 +263,9 @@ class _B200DQNMixin:
                     step=int(self._c("adam_step")(self._handle)))
 
     def launch_info(self) -> dict:
+        if self._sarsa:
+            return dict(launches=int(self._c("last_launches")(self._handle)),
+                        graph_captures=int(self._c("graph_captures")(self._handle)))
         if self._dueling or self._conservative:
             return dict(launches=int(self._c("last_launches")(self._handle)))
         a, b, c = C.c_int32(0), C.c_int32(0), C.c_int32(0)
@@ -268,16 +277,17 @@ class _B200DQNMixin:
         `learn(B200ReplayBuffer)` then applies the mean gradient of all ranks' batches, exchanged
         inside the kernel.  All ranks must call learn() with the same number of rounds and start
         from identical parameters."""
-        if self._dueling or self._conservative:
-            raise NotImplementedError("dueling and conservative (CQL) updates run on one GPU: set_communicator is not supported")
+        if self._dueling or self._conservative or self._sarsa:
+            raise NotImplementedError("dueling, conservative (CQL) and DeepSARSA updates run on one GPU: set_communicator is not "
+                                      "supported")
         self._bind(1)
         self._comm = comm
         _lib.check(self._libh.prl_dqn_set_comm(self._handle, comm.handle if comm is not None else None))
 
     def set_kernel_timing(self, enable: bool = True) -> None:
-        if self._dueling or self._conservative:
-            raise NotImplementedError("kernel timing belongs to the fused DQN kernel; time dueling and conservative rounds with "
-                                      "CUDA events")
+        if self._dueling or self._conservative or self._sarsa:
+            raise NotImplementedError("kernel timing belongs to the fused DQN kernel; time dueling, conservative and DeepSARSA "
+                                      "rounds with CUDA events")
         self._bind(1)
         _lib.check(self._libh.prl_dqn_set_timing(self._handle, int(enable)))
 
@@ -305,7 +315,7 @@ class _B200DQNMixin:
                     for k, v in self.learn_batch(self.preprocess_batch(batch)).items():
                         report.setdefault(k, []).append(v)
             return report
-        if self._dueling or self._conservative:
+        if self._dueling or self._conservative or self._sarsa:
             return self._learn_rounds(replay_buffer, bs, rounds, trace)
         self._bind(bs)
         dev = self._device
@@ -349,18 +359,20 @@ class _B200DQNMixin:
         return report
 
     def _learn_rounds(self, replay_buffer, bs: int, rounds: int, trace: bool) -> dict:
-        """learn() of the dueling and conservative (CQL) learners over a B200ReplayBuffer: `rounds` x (sample -> round)
-        through prl_duel_learn / prl_cql_learn (which also takes alpha).  The ring holds no current action sets, so every
-        round uses the full set, as B200ReplayBuffer.sample reports it."""
+        """learn() of the dueling, conservative (CQL) and DeepSARSA learners over a B200ReplayBuffer: `rounds` x (sample ->
+        round) through prl_duel_learn / prl_cql_learn (which also takes alpha) / prl_sarsa_learn (which needs the committed
+        next actions of a B200SARSAReplayBuffer).  The ring holds no current action sets, so every round uses the full set,
+        as B200ReplayBuffer.sample reports it."""
         from .per import B200PrioritizedReplayBuffer
         if isinstance(replay_buffer, B200PrioritizedReplayBuffer):
-            raise NotImplementedError(("dueling DQN samples uniformly" if self._dueling else "conservative (CQL) updates sample "
-                                       "uniformly") + ": a B200PrioritizedReplayBuffer is not supported")
+            raise NotImplementedError(("DeepSARSA samples uniformly" if self._sarsa else "dueling DQN samples uniformly"
+                                       if self._dueling else "conservative (CQL) updates sample uniformly")
+                                      + ": a B200PrioritizedReplayBuffer is not supported")
         self._bind(bs)
         dev = self._device
         if replay_buffer.device != dev:
             raise RuntimeError(f"replay buffer is on {replay_buffer.device}, learner on {dev}")
-        alpha = () if self._dueling else (_cql.alpha(self),)
+        alpha = (_cql.alpha(self),) if self._conservative and not self._sarsa and not self._dueling else ()
         h = self._handle
         mae = torch.empty(rounds, dtype=torch.float32, device=dev)
         idx = torch.empty((rounds, bs), dtype=torch.int32, device=dev) if trace else None
@@ -381,6 +393,8 @@ class _B200DQNMixin:
         report = {"loss": mae.cpu().tolist()}
         if trace:
             report.update(idx=idx, launches=int(self._c("last_launches")(h)))
+            if self._sarsa:
+                report["graph_captures"] = int(self._c("graph_captures")(h))
         return report
 
     def _learn_prioritized(self, rb, bs: int, rounds: int, trace: bool) -> dict:
@@ -421,6 +435,8 @@ class _B200DQNMixin:
     def learn_batch(self, batch) -> dict:
         """`DeepTDLearning.learn_batch` on a caller-supplied batch (raw ids, or the one-hot
         tensors the reference's preprocess_batch produces)."""
+        if self._sarsa:
+            return _sarsa_mod.learn_batch(self, batch)
         if self._dueling:
             return _duel.learn_batch(self, batch)
         if self._conservative:
@@ -492,6 +508,8 @@ class B200LearnerGroup:
             raise ValueError("need one replay buffer per learner")
         if any(getattr(l, "_conservative", False) for l in learners):
             raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no conservative (CQL) update")
+        if any(getattr(l, "_sarsa", False) for l in learners):
+            raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no DeepSARSA update")
         if any(getattr(l, "_dueling", False) for l in learners):
             raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no dueling network")
         self.learners, self.buffers = list(learners), list(buffers)
@@ -588,3 +606,9 @@ class B200DeepQLearning(_B200DQNMixin, _RefDeepQLearning):
 class B200DoubleDQN(_B200DQNMixin, _RefDoubleDQN):
     """Drop-in for `pearl...double_dqn.DoubleDQN`."""
     _double = True
+
+
+class B200DeepSARSA(_B200DQNMixin, _RefDeepSARSA):
+    """Drop-in for `pearl...deep_sarsa.DeepSARSA`: learn() over a B200SARSAReplayBuffer, learn_batch on a batch with
+    `next_action` (sarsa.py, csrc/sarsa.cu)."""
+    _sarsa = True

@@ -32,6 +32,8 @@ def _stream_ptr(device) -> C.c_void_p:
 
 
 class B200ReplayBuffer(ReplayBuffer):
+    _record_flags = 0               # PRL_BUF_* bits a subclass adds to every record layout it allocates
+
     def __init__(self, capacity: int, device: Optional[torch.device | str | int] = None,
                  dynamic_action_space: bool = False, rng: str = "python") -> None:
         """
@@ -111,6 +113,7 @@ class B200ReplayBuffer(ReplayBuffer):
         flags = _lib.PRL_BUF_CONTINUOUS if self._is_action_continuous else _lib.PRL_BUF_DISCRETE
         if dynamic:
             flags |= _lib.PRL_BUF_DYNAMIC_ACTIONS
+        flags |= self._record_flags
         desc = _lib.BufDesc(self.capacity, obs_dim, act_dim, n_actions, flags)
         lay = _lib.BufLayout()
         _lib.check(self._lib.prl_buf_layout_of(C.byref(desc), C.byref(lay)))
@@ -253,13 +256,16 @@ class B200ReplayBuffer(ReplayBuffer):
             raise ValueError(f"state has {state.shape[1]} features, buffer stores {self.obs_dim}")
         if ids is not None and not (self._desc.flags & _lib.PRL_BUF_DYNAMIC_ACTIONS):
             self._upgrade_to_dynamic()
-        fn = self._lib.prl_buf_push_device if on_dev else self._lib.prl_buf_push_host
         with torch.cuda.device(self._device):
-            _lib.check(fn(self._handle, n, _lib.ptr(state), _lib.ptr(action), _lib.ptr(reward),
-                          _lib.ptr(next_state), _lib.ptr(terminated), _lib.ptr(truncated), _lib.ptr(ids),
-                          _lib.ptr(cnt), _stream_ptr(self._device)))
+            self._push_records(on_dev, n, [_lib.ptr(state), _lib.ptr(action), _lib.ptr(reward), _lib.ptr(next_state),
+                                           _lib.ptr(terminated), _lib.ptr(truncated), _lib.ptr(ids), _lib.ptr(cnt)])
         if on_dev:  # keep the sources alive until the pack kernel has run
             torch.cuda.current_stream(self._device).synchronize()
+
+    def _push_records(self, on_dev: bool, n: int, fields: list) -> None:
+        """The library push of n prepared transitions (`fields`: the pointer arguments of prl_buf_push_host / _device)."""
+        fn = self._lib.prl_buf_push_device if on_dev else self._lib.prl_buf_push_host
+        _lib.check(fn(self._handle, n, *fields, _stream_ptr(self._device)))
 
     # ------------------------------------------------------------------ multi-GPU sharding (SURVEY.md 8e)
     def set_shard(self, rank: int, world: int, global_pushed: int) -> None:
@@ -443,7 +449,12 @@ class B200ReplayBuffer(ReplayBuffer):
     def sample(self, batch_size: int) -> TransitionBatch:
         """`TensorBasedReplayBuffer.sample` (tensor_based_replay_buffer.py:253-282)."""
         _, slot = self.sample_indices(batch_size, 1)
-        g = self._gather_slots(slot[0])
+        return self._batch_of_slots(slot[0]).to(self._device_for_batches)
+
+    def _batch_of_slots(self, slot: torch.Tensor) -> TransitionBatch:
+        """The TransitionBatch of the records at ring slots `slot`, on the buffer's device."""
+        batch_size = slot.numel()
+        g = self._gather_slots(slot)
         if self._is_action_continuous:
             tb = TransitionBatch(state=g["state"], action=g["action"], reward=g["reward"],
                                  next_state=g["next_state"], terminated=g["terminated"],
@@ -460,4 +471,4 @@ class B200ReplayBuffer(ReplayBuffer):
                 next_available_actions=g["avail"].unsqueeze(-1),
                 next_unavailable_actions_mask=g["mask"],
                 terminated=g["terminated"], truncated=g["truncated"])
-        return tb.to(self._device_for_batches)
+        return tb
