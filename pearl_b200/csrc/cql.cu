@@ -27,7 +27,7 @@
 #include <new>
 
 #include "common.cuh"
-#include "dqn_family.cuh"
+#include "rounds.cuh"
 #include "gemm.cuh"
 
 using namespace prl;
@@ -154,8 +154,11 @@ __global__ void __launch_bounds__(128) k_cql_target(int B, int A, int dbl, const
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_cql : DqnRounds<prl_cql, CqlCall> {
+struct prl_cql : Rounds<prl_cql, CqlCall> {
     static constexpr const char *kFn = "prl_cql", *kName = "CQL";
+    static constexpr bool kTargetOn = true;
+    static constexpr int kGraphs = 3;
+    void fill_call(CqlCall &k) const { k.decay = (float)(1.0 - cfg.lr * cfg.weight_decay); }
     prl_cql_cfg cfg;
     int P;
     int W1, b1, W2, b2, W3, b3;
@@ -296,9 +299,10 @@ int prl_cql::round(prl_cql *s, prl_buf *buf, int B, cudaStream_t st) {
 
 extern "C" int prl_cql_learn(prl_cql *s, prl_buf *buf, int rounds, int batch, int64_t training_steps, double alpha, float *out_loss,
                              int32_t *out_logical, void *stream_) {
-    CqlCall dense{};
-    dense.alpha = (float)alpha;
-    return prl_cql::learn(s, buf, rounds, batch, training_steps, out_loss, out_logical, dense, stream_);
+    PRL_REQUIRE(s && buf && out_loss, "null argument");
+    CqlCall call{};
+    call.alpha = (float)alpha; call.out_loss = out_loss;
+    return prl_cql::learn(s, buf, rounds, batch, training_steps, out_logical, call, stream_);
 }
 
 extern "C" int prl_cql_learn_batch(prl_cql *s, int batch, const float *state, const int32_t *action_id, const float *reward,
@@ -310,7 +314,8 @@ extern "C" int prl_cql_learn_batch(prl_cql *s, int batch, const float *state, co
     dense.d_state = state; dense.d_next_state = next_state; dense.d_reward = reward; dense.d_action_id = action_id;
     dense.d_curr_ids = curr_ids; dense.d_next_ids = next_ids; dense.d_next_cnt = next_count; dense.d_term = terminated;
     dense.alpha = (float)alpha;
-    return prl_cql::learn_batch(s, batch, training_steps, out_loss, dense, stream_);
+    dense.out_loss = out_loss;
+    return prl_cql::learn_batch(s, batch, training_steps, dense, stream_);
 }
 
 // Q(s, a) for every action: the online forward of the round on n rows (chunks of max_batch rows through the workspace)

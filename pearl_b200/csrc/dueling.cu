@@ -32,7 +32,7 @@
 #include <new>
 
 #include "common.cuh"
-#include "dqn_family.cuh"
+#include "rounds.cuh"
 #include "gemm.cuh"
 
 using namespace prl;
@@ -190,8 +190,11 @@ struct DuelMlp { int W1, b1, W2, b2, W3, b3, in, h1, h2, out; };
 // activations of one forward pass on m rows with K advantage slots per row
 struct DuelAct { float *t1, *t2, *f, *v1, *v2, *V, *Pa, *a1, *a2, *adv; };
 
-struct prl_duel : DqnRounds<prl_duel, DuelCall> {
+struct prl_duel : Rounds<prl_duel, DuelCall> {
     static constexpr const char *kFn = "prl_duel", *kName = "dueling DQN";
+    static constexpr bool kTargetOn = true;
+    static constexpr int kGraphs = 3;
+    void fill_call(DuelCall &k) const { k.decay = (float)(1.0 - cfg.lr * cfg.weight_decay); }
     prl_duel_cfg cfg;
     int P;
     DuelMlp st, va, ad;
@@ -377,7 +380,10 @@ int prl_duel::round(prl_duel *s, prl_buf *buf, int B, cudaStream_t st) {
 
 extern "C" int prl_duel_learn(prl_duel *s, prl_buf *buf, int rounds, int batch, int64_t training_steps, float *out_loss,
                               int32_t *out_logical, void *stream_) {
-    return prl_duel::learn(s, buf, rounds, batch, training_steps, out_loss, out_logical, DuelCall{}, stream_);
+    PRL_REQUIRE(s && buf && out_loss, "null argument");
+    DuelCall call{};
+    call.out_loss = out_loss;
+    return prl_duel::learn(s, buf, rounds, batch, training_steps, out_logical, call, stream_);
 }
 
 extern "C" int prl_duel_learn_batch(prl_duel *s, int batch, const float *state, const int32_t *action_id, const float *reward,
@@ -389,7 +395,8 @@ extern "C" int prl_duel_learn_batch(prl_duel *s, int batch, const float *state, 
     dense.d_state = state; dense.d_next_state = next_state; dense.d_reward = reward; dense.d_action_id = action_id;
     dense.d_curr_ids = curr_ids; dense.d_next_ids = next_ids; dense.d_next_unavail = next_unavailable; dense.d_term = terminated;
     dense.query_alone = curr_ids ? 0 : 1;
-    return prl_duel::learn_batch(s, batch, training_steps, out_loss, dense, stream_);
+    dense.out_loss = out_loss;
+    return prl_duel::learn_batch(s, batch, training_steps, dense, stream_);
 }
 
 // Q(s, .) over an id set of K slots per row, the mean over that set: the forward of the round on n rows (chunks of

@@ -20,7 +20,7 @@
 
 #include "common.cuh"
 #include "gemm.cuh"
-#include "host_runtime.cuh"
+#include "rounds.cuh"
 
 using namespace prl;
 
@@ -145,7 +145,9 @@ __global__ void k_iql_bump(int *round_idx) { *round_idx += 1; }
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_iql {
+struct prl_iql : Rounds<prl_iql, IqlCall> {
+    static constexpr const char *kFn = "prl_iql";
+    static constexpr int kScal = 3, kGraphs = 3;   // actor, critic, value; buffer rounds and learn_batch
     prl_iql_cfg cfg;
     int Pa, Pc, Pv;
     int aW1, ab1, aW2, ab2, aW3, ab3;
@@ -155,25 +157,34 @@ struct prl_iql {
     float *critic, *critic_m, *critic_v, *critic_x, *critic_t;
     float *value, *value_m, *value_v, *value_x;
     const float *low, *high;
-    int64_t adam_step;
     // workspace
     float *S, *Act, *R, *T, *v1, *v2, *V, *P, *c1t, *c2t, *qt, *c1, *c2, *q, *h1, *h2, *out, *dout, *dV, *dv2, *dv1, *dq, *dc2, *dc1,
         *dh2, *dh1, *g_actor, *g_critic, *g_value;
     int *act;
-    int32_t *slots, *logical;
-    float2 *scal_a, *scal_c, *scal_v;
-    IqlCall *call;
-    int *round_idx;
-    bool use_graph;
-    cudaGraphExec_t graph_exec[2];            // [0] rounds from a replay buffer, [1] learn_batch on a dense batch
-    int graph_batch[2];
-    const uint32_t *graph_buf;
-    int launches_per_round;
-    Stage stage;
-    int64_t last_launches;
+    double &lr(int k) { return k == 0 ? cfg.actor_lr : k == 1 ? cfg.critic_lr : cfg.value_lr; }
+    void fill_call(IqlCall &k) const {
+        k.decay_a = (float)(1.0 - cfg.actor_lr * cfg.weight_decay);
+        k.decay_c = (float)(1.0 - cfg.critic_lr * cfg.weight_decay);
+        k.decay_v = (float)(1.0 - cfg.value_lr * cfg.weight_decay);
+    }
+    int buffer_ok(const prl_buf *buf) const;
+    static int round(prl_iql *s, prl_buf *buf, int B, cudaStream_t st);
 };
 
 static bool iql_discrete(const prl_iql_cfg &c) { return c.n_actions > 0; }
+
+int prl_iql::buffer_ok(const prl_buf *buf) const {
+    const prl_iql_cfg &c = cfg;
+    PRL_REQUIRE(buf->desc.obs_dim == c.obs_dim, "IQL: the buffer's obs_dim (%d) is not the configured %d", buf->desc.obs_dim, c.obs_dim);
+    if (iql_discrete(c))
+        PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.n_actions == c.n_actions,
+                    "IQL with discrete actions needs a discrete-action buffer with n_actions = %d", c.n_actions);
+    else
+        PRL_REQUIRE((buf->desc.flags & PRL_BUF_CONTINUOUS) && buf->desc.act_dim == c.act_dim,
+                    "IQL with continuous actions needs a continuous-action buffer with act_dim = %d", c.act_dim);
+    PRL_REQUIRE(buf->shard_world <= 1, "the buffer is one shard of a multi-GPU buffer: IQL samples local buffers only");
+    return PRL_OK;
+}
 
 static void iql_layout(prl_iql *s) {
     const prl_iql_cfg &c = s->cfg;
@@ -238,8 +249,7 @@ static int64_t iql_carve(prl_iql *s, void *base) {
     w(s->dh2, B * c.actor_h2); w(s->dh1, B * c.actor_h1);
     w(s->g_actor, s->Pa); w(s->g_critic, 2 * (int64_t)s->Pc); w(s->g_value, s->Pv);
     w(s->act, B);
-    w(s->slots, c.max_rounds * B); w(s->logical, c.max_rounds * B);
-    w(s->scal_a, 3 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | scal_v | call | round_idx
+    s->carve_tail(w, c.max_rounds, B);
     return w.bytes;
 }
 extern "C" int64_t prl_iql_workspace_bytes(const prl_iql_cfg *c) {
@@ -267,37 +277,20 @@ extern "C" int prl_iql_create(prl_iql **out, const prl_iql_cfg *cfg, float *acto
     s->low = low_dev; s->high = high_dev;
     s->adam_step = adam_step;
     iql_carve(s, workspace);
-    s->scal_c = s->scal_a + cfg->max_rounds; s->scal_v = s->scal_c + cfg->max_rounds;
-    s->call = (IqlCall *)(s->scal_v + cfg->max_rounds); s->round_idx = (int *)(s->call + 1);
-    static_assert(sizeof(IqlCall) + 4 <= 64 * 4, "call block fits the reserved tail");
-    s->use_graph = true; s->graph_exec[0] = s->graph_exec[1] = nullptr; s->graph_batch[0] = s->graph_batch[1] = 0;
-    s->graph_buf = nullptr; s->last_launches = 0; s->launches_per_round = 0;
-    cudaError_t e = s->stage.open((size_t)cfg->max_rounds * 24 + 256);
-    if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_iql_create: %s", cudaGetErrorString(e)); }
-    *out = s;
-    return PRL_OK;
+    return prl_iql::open(s, out);
 }
-extern "C" int prl_iql_destroy(prl_iql *s) {
-    if (!s) return PRL_OK;
-    s->stage.close();
-    for (int i = 0; i < 2; i++) if (s->graph_exec[i]) cudaGraphExecDestroy(s->graph_exec[i]);
-    delete s;
-    return PRL_OK;
-}
-extern "C" int64_t prl_iql_adam_step(const prl_iql *s) { return s ? s->adam_step : -1; }
-
+extern "C" int prl_iql_destroy(prl_iql *s) { return prl_iql::destroy(s); }
+extern "C" int64_t prl_iql_adam_step(const prl_iql *s) { return prl_iql::adam_step_of(s); }
 extern "C" int prl_iql_set_lr(prl_iql *s, double actor_lr, double critic_lr, double value_lr) {
-    PRL_REQUIRE(s, "null handle");
-    PRL_REQUIRE(actor_lr >= 0.0 && critic_lr >= 0.0 && value_lr >= 0.0, "learning rates must be non-negative");
-    s->cfg.actor_lr = actor_lr;
-    s->cfg.critic_lr = critic_lr;
-    s->cfg.value_lr = value_lr;
-    return PRL_OK;
+    return prl_iql::set_lr(s, actor_lr, critic_lr, value_lr);
 }
+extern "C" int prl_iql_set_graph(prl_iql *s, int enable) { return prl_iql::set_graph(s, enable); }
+extern "C" int64_t prl_iql_last_launches(const prl_iql *s) { return prl_iql::last_launches_of(s); }
 
 // one learner round, launched (or captured) on `st`; buf == null: the dense batch of the call block (learn_batch)
-static int iql_round(prl_iql *s, prl_buf *buf, int B, cudaStream_t st) {
+int prl_iql::round(prl_iql *s, prl_buf *buf, int B, cudaStream_t st) {
     const prl_iql_cfg &c = s->cfg;
+    const float2 *scal_a = s->scal, *scal_c = scal_a + c.max_rounds, *scal_v = scal_c + c.max_rounds;
     const bool disc = iql_discrete(c);
     const int O = c.obs_dim, N = disc ? c.n_actions : c.act_dim, D = O + N;
     const int H1 = c.actor_h1, H2 = c.actor_h2, C1 = c.critic_h1, C2 = c.critic_h2, V1 = c.value_h1, V2 = c.value_h2;
@@ -346,7 +339,7 @@ static int iql_round(prl_iql *s, prl_buf *buf, int B, cudaStream_t st) {
         L.bwd_w(s->dv2, V2, 0, B, V2, mat(s->v1, V1), V1, gv + s->vW2, V1, 0, gv + s->vb2, 0);
         L.bwd_x(s->dv2, V2, 0, B, V2, vw + s->vW2, V1, 0, 0, V1, s->dv1, V1, 0, s->v1, V1, 0, false);
         L.bwd_w(s->dv1, V1, 0, B, V1, mat(S, O), O, gv + s->vW1, O, 0, gv + s->vb1, 0);
-        k_adamw<<<(s->Pv + eb - 1) / eb, eb, 0, st>>>(s->Pv, s->value, s->value_m, s->value_v, s->value_x, gv, h, s->scal_v, s->round_idx,
+        k_adamw<<<(s->Pv + eb - 1) / eb, eb, 0, st>>>(s->Pv, s->value, s->value_m, s->value_v, s->value_x, gv, h, scal_v, s->round_idx,
                                                     nullptr, 0.f, 0.f, &s->call->decay_v);
         small += 2;
     }
@@ -365,7 +358,7 @@ static int iql_round(prl_iql *s, prl_buf *buf, int B, cudaStream_t st) {
             L.bwd_w(s->dc1, C1, sC1, B, C1, mat2(S, O, O, s->Act, N), D, gc + s->cW1, D, Pc, gc + s->cb1, Pc, 2);
         }
         const int n2p = 2 * s->Pc;
-        k_adamw<<<(n2p + eb - 1) / eb, eb, 0, st>>>(n2p, s->critic, s->critic_m, s->critic_v, s->critic_x, gc, h, s->scal_c, s->round_idx,
+        k_adamw<<<(n2p + eb - 1) / eb, eb, 0, st>>>(n2p, s->critic, s->critic_m, s->critic_v, s->critic_x, gc, h, scal_c, s->round_idx,
                                                   s->critic_t, (float)c.tau, (float)(1.0 - c.tau), &s->call->decay_c);
         small += 2;
     }
@@ -377,7 +370,7 @@ static int iql_round(prl_iql *s, prl_buf *buf, int B, cudaStream_t st) {
         L.bwd_w(s->dh2, H2, 0, B, H2, mat(s->h1, H1), H1, ga + s->aW2, H1, 0, ga + s->ab2, 0);
         L.bwd_x(s->dh2, H2, 0, B, H2, aw + s->aW2, H1, 0, 0, H1, s->dh1, H1, 0, s->h1, H1, 0, false);
         L.bwd_w(s->dh1, H1, 0, B, H1, mat(S, O), O, ga + s->aW1, O, 0, ga + s->ab1, 0);
-        k_adamw<<<(s->Pa + eb - 1) / eb, eb, 0, st>>>(s->Pa, s->actor, s->actor_m, s->actor_v, s->actor_x, ga, h, s->scal_a, s->round_idx,
+        k_adamw<<<(s->Pa + eb - 1) / eb, eb, 0, st>>>(s->Pa, s->actor, s->actor_m, s->actor_v, s->actor_x, ga, h, scal_a, s->round_idx,
                                                     nullptr, 0.f, 0.f, &s->call->decay_a);
         small++;
     }
@@ -387,73 +380,12 @@ static int iql_round(prl_iql *s, prl_buf *buf, int B, cudaStream_t st) {
     return PRL_OK;
 }
 
-// per-call block (Adam scalars of every round as torch evaluates them in double, decay factors, pointers), uploaded on `st`
-static int iql_upload(prl_iql *s, int rounds, const int32_t *bits, float *out_value, float *out_critic, float *out_actor, const IqlCall &dense,
-                      cudaStream_t st) {
-    const prl_iql_cfg &c = s->cfg;
-    float2 *hs;
-    int rc = s->stage.wait(&hs);
-    if (rc) return rc;
-    const int MR = c.max_rounds;
-    for (int r = 0; r < rounds; r++) {
-        hs[r] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-        hs[MR + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-        hs[2 * MR + r] = adam_scal(c.value_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-    }
-    IqlCall *hc = reinterpret_cast<IqlCall *>(hs + 3 * (size_t)MR);
-    *hc = dense;
-    hc->slots = s->slots; hc->bits = bits; hc->out_value = out_value; hc->out_critic = out_critic; hc->out_actor = out_actor;
-    hc->decay_a = (float)(1.0 - c.actor_lr * c.weight_decay);
-    hc->decay_c = (float)(1.0 - c.critic_lr * c.weight_decay);
-    hc->decay_v = (float)(1.0 - c.value_lr * c.weight_decay);
-    *reinterpret_cast<int *>(hc + 1) = 0;
-    // scal_a | scal_c | scal_v | call | round_idx are contiguous on the device in the same order
-    return s->stage.send(s->scal_a, 3 * (size_t)MR * 8 + sizeof(IqlCall) + 4, st);
-}
-
-static int iql_run(prl_iql *s, prl_buf *buf, int rounds, int batch, cudaStream_t st) {
-    const int g = buf ? 0 : 1;
-    if (s->use_graph) {
-        if (!s->graph_exec[g] || s->graph_batch[g] != batch || (buf && s->graph_buf != buf->records)) {
-            int rc = capture_graph(&s->graph_exec[g], "prl_iql", [&](cudaStream_t cs) { return iql_round(s, buf, batch, cs); });
-            if (rc) return rc;
-            s->graph_batch[g] = batch;
-            if (buf) s->graph_buf = buf->records;
-        }
-        for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec[g], st));
-    } else {
-        for (int r = 0; r < rounds; r++) {
-            int rc = iql_round(s, buf, batch, st);
-            if (rc) return rc;
-        }
-    }
-    PRL_CUDA(cudaGetLastError());
-    s->adam_step += rounds;
-    s->last_launches = (int64_t)s->launches_per_round * rounds;
-    return PRL_OK;
-}
-
 extern "C" int prl_iql_learn(prl_iql *s, prl_buf *buf, int rounds, int batch, const int32_t *bits_dev, float *out_value_loss,
                              float *out_critic_loss, float *out_actor_loss, int32_t *out_logical, void *stream_) {
     PRL_REQUIRE(s && buf && bits_dev && out_value_loss && out_critic_loss && out_actor_loss, "null argument");
-    const prl_iql_cfg &c = s->cfg;
-    PRL_REQUIRE(rounds > 0 && rounds <= c.max_rounds && batch > 0 && batch <= c.max_batch, "rounds / batch outside the configured maxima");
-    PRL_REQUIRE(buf->desc.obs_dim == c.obs_dim, "IQL: the buffer's obs_dim (%d) is not the configured %d", buf->desc.obs_dim, c.obs_dim);
-    if (iql_discrete(c))
-        PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.n_actions == c.n_actions,
-                    "IQL with discrete actions needs a discrete-action buffer with n_actions = %d", c.n_actions);
-    else
-        PRL_REQUIRE((buf->desc.flags & PRL_BUF_CONTINUOUS) && buf->desc.act_dim == c.act_dim,
-                    "IQL with continuous actions needs a continuous-action buffer with act_dim = %d", c.act_dim);
-    PRL_REQUIRE(buf->shard_world <= 1, "the buffer is one shard of a multi-GPU buffer: IQL samples local buffers only");
-    cudaStream_t st = (cudaStream_t)stream_;
-    int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
-    if (rc) return rc;
-    IqlCall dense;
-    memset(&dense, 0, sizeof(dense));
-    rc = iql_upload(s, rounds, bits_dev, out_value_loss, out_critic_loss, out_actor_loss, dense, st);
-    if (rc) return rc;
-    return iql_run(s, buf, rounds, batch, st);
+    IqlCall call{};
+    call.bits = bits_dev; call.out_value = out_value_loss; call.out_critic = out_critic_loss; call.out_actor = out_actor_loss;
+    return prl_iql::learn(s, buf, rounds, batch, 0, out_logical, call, stream_);
 }
 
 extern "C" int prl_iql_learn_batch(prl_iql *s, int batch, const float *state, const float *action, const int32_t *action_id,
@@ -461,23 +393,12 @@ extern "C" int prl_iql_learn_batch(prl_iql *s, int batch, const float *state, co
                                    float *out_value_loss, float *out_critic_loss, float *out_actor_loss, void *stream_) {
     PRL_REQUIRE(s && state && reward && next_state && terminated && bits_dev && out_value_loss && out_critic_loss && out_actor_loss,
                 "null argument");
-    const prl_iql_cfg &c = s->cfg;
-    PRL_REQUIRE(batch > 0 && batch <= c.max_batch, "batch outside the configured maximum");
-    PRL_REQUIRE(iql_discrete(c) ? action_id != nullptr : action != nullptr,
+    PRL_REQUIRE(batch > 0 && batch <= s->cfg.max_batch, "batch outside the configured maximum");
+    PRL_REQUIRE(iql_discrete(s->cfg) ? action_id != nullptr : action != nullptr,
                 "discrete IQL takes action ids, continuous IQL takes continuous actions");
-    cudaStream_t st = (cudaStream_t)stream_;
-    IqlCall dense;
-    memset(&dense, 0, sizeof(dense));
-    dense.d_state = state; dense.d_next_state = next_state; dense.d_reward = reward; dense.d_action = action;
-    dense.d_action_id = action_id; dense.d_term = terminated;
-    int rc = iql_upload(s, 1, bits_dev, out_value_loss, out_critic_loss, out_actor_loss, dense, st);
-    if (rc) return rc;
-    return iql_run(s, nullptr, 1, batch, st);
+    IqlCall call{};
+    call.d_state = state; call.d_next_state = next_state; call.d_reward = reward; call.d_action = action;
+    call.d_action_id = action_id; call.d_term = terminated;
+    call.bits = bits_dev; call.out_value = out_value_loss; call.out_critic = out_critic_loss; call.out_actor = out_actor_loss;
+    return prl_iql::learn_batch(s, batch, 0, call, stream_);
 }
-
-extern "C" int prl_iql_set_graph(prl_iql *s, int enable) {
-    PRL_REQUIRE(s, "null handle");
-    s->use_graph = enable != 0;
-    return PRL_OK;
-}
-extern "C" int64_t prl_iql_last_launches(const prl_iql *s) { return s ? s->last_launches : -1; }

@@ -236,7 +236,7 @@ extern "C" int prl_ppo_gae(int n, const float *values_dev, float last_next_value
 #include <new>
 
 #include "ac_nets.cuh"
-#include "host_runtime.cuh"
+#include "rounds.cuh"
 
 namespace {
 
@@ -350,27 +350,25 @@ __global__ void k_ppo_cuts(int n, const uint8_t *__restrict__ term, const uint8_
 
 }  // namespace
 
-struct prl_ppo {
+struct prl_ppo : Rounds<prl_ppo, PpoCall> {
+    static constexpr const char *kFn = "prl_ppo";
+    static constexpr int kScal = 2;   // actor, critic
     prl_ppo_cfg cfg;
     Mlp2 an, cn;          // actor (softmax head) and critic (scalar head) layouts
     float *actor, *actor_m, *actor_v, *actor_x, *critic, *critic_m, *critic_v, *critic_x;
-    int64_t adam_step;
     // workspace
     float *S, *h1, *h2, *logits, *v, *gae, *lam, *old, *ap, *dlogits, *dh2, *dh1, *dv, *g_actor, *g_critic, *reward, *last_value;
-    int32_t *act, *slots, *logical;
+    int32_t *act;
     uint8_t *term, *trunc;
     int *gae_heads;           // [1 + max_rollout]: count, then the chain-head positions of the GAE pass
-    float2 *scal_a, *scal_c;
-    PpoCall *call;
-    int *round_idx;
-    Stage stage;
-    bool use_graph;
-    cudaGraphExec_t graph_exec;
-    int graph_batch;
-    const uint32_t *graph_buf;
-    int launches_per_round;
-    int64_t last_launches;
     int64_t pre_n;      // rollout length of the last prl_ppo_preprocess
+    double &lr(int k) { return k == 0 ? cfg.actor_lr : cfg.critic_lr; }
+    int buffer_ok(const prl_buf *buf) const {
+        PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.obs_dim == cfg.obs_dim && buf->desc.n_actions == cfg.n_actions,
+                    "PPO needs a discrete-action buffer with matching dimensions");
+        return PRL_OK;
+    }
+    static int round(prl_ppo *s, prl_buf *buf, int B, cudaStream_t st);
 };
 
 // rollout rows evaluated per pass of the preprocessing: the whole rollout when it fits 65536 rows (a pass is 8 launches,
@@ -407,15 +405,15 @@ static int64_t ppo_carve(prl_ppo *s, void *base) {
     const prl_ppo_cfg &c = s->cfg;
     const int64_t R = c.max_batch > ppo_chunk(&c) ? c.max_batch : ppo_chunk(&c);   // rows of the widest pass
     const int64_t hmax1 = c.actor_h1 > c.critic_h1 ? c.actor_h1 : c.critic_h1, hmax2 = c.actor_h2 > c.critic_h2 ? c.actor_h2 : c.critic_h2;
-    const int64_t A = c.n_actions, MRB = (int64_t)c.max_rounds * c.max_batch;
+    const int64_t A = c.n_actions;
     Carve w{(char *)base};
     w(s->S, R * c.obs_dim); w(s->h1, R * hmax1); w(s->h2, R * hmax2); w(s->logits, R * A); w(s->v, R);
     w(s->gae, R); w(s->lam, R); w(s->old, R); w(s->ap, R); w(s->dlogits, R * A);
     w(s->dh2, R * hmax2); w(s->dh1, R * hmax1); w(s->dv, R); w(s->g_actor, s->an.P); w(s->g_critic, s->cn.P);
     w(s->reward, c.max_rollout); w(s->last_value, 64);
-    w(s->act, R); w(s->slots, MRB); w(s->logical, MRB);
+    w(s->act, R);
     w(s->term, c.max_rollout); w(s->trunc, c.max_rollout);
-    w(s->scal_a, 2 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | call | round_idx
+    s->carve_tail(w, c.max_rounds, c.max_batch);
     w(s->gae_heads, c.max_rollout + 1);                                                  // count, then the GAE chain heads
     return w.bytes;
 }
@@ -438,30 +436,12 @@ extern "C" int prl_ppo_create(prl_ppo **out, const prl_ppo_cfg *cfg, float *acto
     s->critic = critic_w; s->critic_m = critic_m; s->critic_v = critic_v; s->critic_x = critic_vmax;
     s->adam_step = adam_step;
     ppo_carve(s, workspace);
-    s->scal_c = s->scal_a + cfg->max_rounds;
-    s->call = (PpoCall *)(s->scal_c + cfg->max_rounds); s->round_idx = (int *)(s->call + 1);
-    static_assert(sizeof(PpoCall) + 4 <= 256, "call block fits the reserved tail");
-    s->use_graph = true; s->graph_exec = nullptr; s->graph_batch = 0; s->graph_buf = nullptr; s->last_launches = 0;
-    s->pre_n = 0;
-    cudaError_t e = s->stage.open((size_t)cfg->max_rounds * 16 + 256);
-    if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_ppo_create: %s", cudaGetErrorString(e)); }
-    *out = s;
-    return PRL_OK;
+    return prl_ppo::open(s, out);
 }
-extern "C" int prl_ppo_destroy(prl_ppo *s) {
-    if (!s) return PRL_OK;
-    s->stage.close();
-    if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
-    delete s;
-    return PRL_OK;
-}
-extern "C" int64_t prl_ppo_adam_step(const prl_ppo *s) { return s ? s->adam_step : -1; }
-extern "C" int prl_ppo_set_graph(prl_ppo *s, int enable) {
-    PRL_REQUIRE(s, "null handle");
-    s->use_graph = enable != 0;
-    return PRL_OK;
-}
-extern "C" int64_t prl_ppo_last_launches(const prl_ppo *s) { return s ? s->last_launches : -1; }
+extern "C" int prl_ppo_destroy(prl_ppo *s) { return prl_ppo::destroy(s); }
+extern "C" int64_t prl_ppo_adam_step(const prl_ppo *s) { return prl_ppo::adam_step_of(s); }
+extern "C" int prl_ppo_set_graph(prl_ppo *s, int enable) { return prl_ppo::set_graph(s, enable); }
+extern "C" int64_t prl_ppo_last_launches(const prl_ppo *s) { return prl_ppo::last_launches_of(s); }
 
 static void ppo_actor_forward(prl_ppo *s, GemmLauncher &L, int rows) {
     mlp2_forward(L, s->an, s->actor, s->S, rows, s->h1, s->h2, s->logits);
@@ -524,8 +504,9 @@ extern "C" int prl_ppo_gae_redo(prl_ppo *s, const float *values_dev, float next_
                       (float)(c.gamma * c.lam), out_gae, out_lam_return, s->gae_heads + 1, s->gae_heads, (cudaStream_t)stream_);
 }
 
-static int ppo_round(prl_ppo *s, prl_buf *buf, int B, cudaStream_t st) {
+int prl_ppo::round(prl_ppo *s, prl_buf *buf, int B, cudaStream_t st) {
     const prl_ppo_cfg &c = s->cfg;
+    const float2 *scal_a = s->scal, *scal_c = s->scal + c.max_rounds;
     const int O = c.obs_dim;
     GemmLauncher L; L.st = st;
     const AdamHp ha = adam_hp(c.actor_lr, c.beta1, c.beta2, c.eps, c.weight_decay), hc = adam_hp(c.critic_lr, c.beta1, c.beta2, c.eps, c.weight_decay);
@@ -536,13 +517,13 @@ static int ppo_round(prl_ppo *s, prl_buf *buf, int B, cudaStream_t st) {
     k_ppo_actor_loss<<<1, 256, 0, st>>>(B, c.n_actions, s->logits, s->act, s->gae, s->old, (float)c.epsilon, (float)c.entropy_bonus, s->ap, s->dlogits,
                                         s->call, s->round_idx);
     mlp2_backward(L, s->an, s->actor, s->g_actor, s->dlogits, s->S, s->h1, s->h2, s->dh2, s->dh1, B);
-    k_adamw<<<(s->an.P + eb - 1) / eb, eb, 0, st>>>(s->an.P, s->actor, s->actor_m, s->actor_v, s->actor_x, s->g_actor, ha, s->scal_a, s->round_idx,
+    k_adamw<<<(s->an.P + eb - 1) / eb, eb, 0, st>>>(s->an.P, s->actor, s->actor_m, s->actor_v, s->actor_x, s->g_actor, ha, scal_a, s->round_idx,
                                                   nullptr, 0.f, 0.f);
     // ---------------- critic step (critic_utils.py:139-167)
     ppo_critic_forward(s, L, B, s->v);
     k_ppo_critic_loss<<<1, 256, 0, st>>>(B, s->v, s->lam, s->dv, s->call, s->round_idx);
     mlp2_backward(L, s->cn, s->critic, s->g_critic, s->dv, s->S, s->h1, s->h2, s->dh2, s->dh1, B);   // + one k_head_bwd
-    k_adamw<<<(s->cn.P + eb - 1) / eb, eb, 0, st>>>(s->cn.P, s->critic, s->critic_m, s->critic_v, s->critic_x, s->g_critic, hc, s->scal_c,
+    k_adamw<<<(s->cn.P + eb - 1) / eb, eb, 0, st>>>(s->cn.P, s->critic, s->critic_m, s->critic_v, s->critic_x, s->g_critic, hc, scal_c,
                                                   s->round_idx, nullptr, 0.f, 0.f);
     k_ppo_bump<<<1, 1, 0, st>>>(s->round_idx);
     s->launches_per_round = L.count + 7;
@@ -554,41 +535,8 @@ extern "C" int prl_ppo_learn(prl_ppo *s, prl_buf *buf, int rounds, int batch, co
                              const float *action_probs_dev, float *out_actor_loss, float *out_critic_loss, int32_t *out_logical,
                              void *stream_) {
     PRL_REQUIRE(s && buf && gae_dev && lam_return_dev && action_probs_dev && out_actor_loss && out_critic_loss, "null argument");
-    const prl_ppo_cfg &c = s->cfg;
-    PRL_REQUIRE(rounds > 0 && rounds <= c.max_rounds && batch > 0 && batch <= c.max_batch, "rounds / batch outside the configured maxima");
-    PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.obs_dim == c.obs_dim && buf->desc.n_actions == c.n_actions,
-                "PPO needs a discrete-action buffer with matching dimensions");
-    cudaStream_t st = (cudaStream_t)stream_;
-    int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
-    if (rc) return rc;
-    float2 *hs;
-    rc = s->stage.wait(&hs);
-    if (rc) return rc;
-    for (int r = 0; r < rounds; r++) {
-        hs[r] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-        hs[c.max_rounds + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-    }
-    PpoCall *hc = reinterpret_cast<PpoCall *>(hs + 2 * (size_t)c.max_rounds);
-    hc->logical = out_logical ? out_logical : s->logical; hc->slots = s->slots; hc->gae = gae_dev; hc->lam_return = lam_return_dev;
-    hc->old_probs = action_probs_dev; hc->out_actor = out_actor_loss; hc->out_critic = out_critic_loss;
-    *reinterpret_cast<int *>(hc + 1) = 0;
-    rc = s->stage.send(s->scal_a, 2 * (size_t)c.max_rounds * 8 + sizeof(PpoCall) + 4, st);
-    if (rc) return rc;
-    if (s->use_graph) {
-        if (!s->graph_exec || s->graph_batch != batch || s->graph_buf != buf->records) {
-            rc = capture_graph(&s->graph_exec, "prl_ppo_learn", [&](cudaStream_t cs) { return ppo_round(s, buf, batch, cs); });
-            if (rc) return rc;
-            s->graph_batch = batch; s->graph_buf = buf->records;
-        }
-        for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec, st));
-    } else {
-        for (int r = 0; r < rounds; r++) {
-            rc = ppo_round(s, buf, batch, st);
-            if (rc) return rc;
-        }
-    }
-    PRL_CUDA(cudaGetLastError());
-    s->adam_step += rounds;
-    s->last_launches = (int64_t)s->launches_per_round * rounds;
-    return PRL_OK;
+    PpoCall call{};
+    call.logical = out_logical ? out_logical : s->logical; call.gae = gae_dev; call.lam_return = lam_return_dev;
+    call.old_probs = action_probs_dev; call.out_actor = out_actor_loss; call.out_critic = out_critic_loss;
+    return prl_ppo::learn(s, buf, rounds, batch, 0, out_logical, call, stream_);
 }

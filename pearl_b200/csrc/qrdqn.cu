@@ -21,7 +21,7 @@
 #include <new>
 
 #include "common.cuh"
-#include "dqn_family.cuh"
+#include "rounds.cuh"
 #include "gemm.cuh"
 
 using namespace prl;
@@ -182,8 +182,11 @@ __global__ void __launch_bounds__(256) k_qr_report(int B, int N, const float *__
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_qrdqn : DqnRounds<prl_qrdqn, QrCall> {
+struct prl_qrdqn : Rounds<prl_qrdqn, QrCall> {
     static constexpr const char *kFn = "prl_qrdqn", *kName = "QR-DQN";
+    static constexpr bool kTargetOn = true;
+    static constexpr int kGraphs = 3;
+    void fill_call(QrCall &k) const { k.decay = (float)(1.0 - cfg.lr * cfg.weight_decay); }
     prl_qrdqn_cfg cfg;
     int P;
     int W1, b1, W2, b2, W3, b3;
@@ -310,9 +313,10 @@ int prl_qrdqn::round(prl_qrdqn *s, prl_buf *buf, int B, cudaStream_t st) {
 
 extern "C" int prl_qrdqn_learn(prl_qrdqn *s, prl_buf *buf, int rounds, int batch, int64_t training_steps, double beta, float *out_loss,
                                int32_t *out_logical, void *stream_) {
-    QrCall dense{};
-    dense.beta = (float)beta;
-    return prl_qrdqn::learn(s, buf, rounds, batch, training_steps, out_loss, out_logical, dense, stream_);
+    PRL_REQUIRE(s && buf && out_loss, "null argument");
+    QrCall call{};
+    call.beta = (float)beta; call.out_loss = out_loss;
+    return prl_qrdqn::learn(s, buf, rounds, batch, training_steps, out_logical, call, stream_);
 }
 
 extern "C" int prl_qrdqn_learn_batch(prl_qrdqn *s, int batch, const float *state, const int32_t *action_id, const float *reward,
@@ -323,5 +327,6 @@ extern "C" int prl_qrdqn_learn_batch(prl_qrdqn *s, int batch, const float *state
     dense.d_state = state; dense.d_next_state = next_state; dense.d_reward = reward; dense.d_action_id = action_id;
     dense.d_next_ids = next_ids; dense.d_next_cnt = next_count; dense.d_term = terminated;
     dense.beta = (float)beta;
-    return prl_qrdqn::learn_batch(s, batch, training_steps, out_loss, dense, stream_);
+    dense.out_loss = out_loss;
+    return prl_qrdqn::learn_batch(s, batch, training_steps, dense, stream_);
 }

@@ -24,7 +24,7 @@
 
 #include "ac_nets.cuh"
 #include "common.cuh"
-#include "host_runtime.cuh"
+#include "rounds.cuh"
 
 using namespace prl;
 
@@ -132,24 +132,27 @@ __global__ void k_rf_bump(int *round_idx) { *round_idx += 1; }
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_reinforce {
+struct prl_reinforce : Rounds<prl_reinforce, RfCall> {
+    static constexpr const char *kFn = "prl_reinforce";
+    static constexpr int kScal = 2;   // actor, critic
     prl_reinforce_cfg cfg;
     Mlp2 an, cn;          // actor (softmax head) and critic (scalar head) layouts
     float *actor, *actor_m, *actor_v, *actor_x, *critic, *critic_m, *critic_v, *critic_x;
-    int64_t adam_step;
     // workspace
     float *S, *ah1, *ah2, *logits, *ch1, *ch2, *v, *dlogits, *dv, *dh2, *dh1, *g_actor, *g_critic, *boot;
-    int32_t *act, *slots, *logical;
-    float2 *scal_a, *scal_c;
-    RfCall *call;
-    int *round_idx;
-    Stage stage;
-    bool use_graph;
-    cudaGraphExec_t graph_exec;
-    int graph_batch;
-    const uint32_t *graph_buf;
-    int launches_per_round;
-    int64_t last_launches;
+    int32_t *act;
+    double &lr(int k) { return k == 0 ? cfg.actor_lr : cfg.critic_lr; }
+    void fill_call(RfCall &k) const {
+        k.decay_a = (float)(1.0 - cfg.actor_lr * cfg.weight_decay);
+        k.decay_c = (float)(1.0 - cfg.critic_lr * cfg.weight_decay);
+    }
+    int buffer_ok(const prl_buf *buf) const {
+        PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.obs_dim == cfg.obs_dim && buf->desc.n_actions == cfg.n_actions,
+                    "REINFORCE needs a discrete-action buffer with matching obs_dim / n_actions");
+        PRL_REQUIRE(buf->shard_world <= 1, "the buffer is one shard of a multi-GPU buffer: REINFORCE reads local buffers only");
+        return PRL_OK;
+    }
+    static int round(prl_reinforce *s, prl_buf *buf, int B, cudaStream_t st);
 };
 
 static int rf_check(const prl_reinforce_cfg *c) {
@@ -177,15 +180,15 @@ extern "C" int64_t prl_reinforce_critic_param_count(const prl_reinforce_cfg *c) 
 // the workspace, in order; base == null: only its size
 static int64_t rf_carve(prl_reinforce *s, void *base) {
     const prl_reinforce_cfg &c = s->cfg;
-    const int64_t B = c.max_batch, A = c.n_actions, O = c.obs_dim, MRB = (int64_t)c.max_rounds * c.max_batch;
+    const int64_t B = c.max_batch, A = c.n_actions, O = c.obs_dim;
     const int64_t hmax1 = c.actor_h1 > c.critic_h1 ? c.actor_h1 : c.critic_h1, hmax2 = c.actor_h2 > c.critic_h2 ? c.actor_h2 : c.critic_h2;
     Carve w{(char *)base};
     w(s->S, B * O); w(s->ah1, B * c.actor_h1); w(s->ah2, B * c.actor_h2); w(s->logits, B * A);
     w(s->ch1, B * c.critic_h1); w(s->ch2, B * c.critic_h2); w(s->v, B); w(s->dlogits, B * A); w(s->dv, B);
     w(s->dh2, B * hmax2); w(s->dh1, B * hmax1); w(s->g_actor, s->an.P); w(s->g_critic, s->cn.P);
     w(s->boot, 64);
-    w(s->act, B); w(s->slots, MRB); w(s->logical, MRB);
-    w(s->scal_a, 2 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | call | round_idx
+    w(s->act, B);
+    s->carve_tail(w, c.max_rounds, B);
     return w.bytes;
 }
 extern "C" int64_t prl_reinforce_workspace_bytes(const prl_reinforce_cfg *c) {
@@ -208,50 +211,20 @@ extern "C" int prl_reinforce_create(prl_reinforce **out, const prl_reinforce_cfg
     s->critic = critic_w; s->critic_m = critic_m; s->critic_v = critic_v; s->critic_x = critic_vmax;
     s->adam_step = adam_step;
     rf_carve(s, workspace);
-    s->scal_c = s->scal_a + cfg->max_rounds;
-    s->call = (RfCall *)(s->scal_c + cfg->max_rounds); s->round_idx = (int *)(s->call + 1);
-    static_assert(sizeof(RfCall) + 4 <= 32 * 8, "call block fits the reserved tail");
-    s->use_graph = true; s->graph_exec = nullptr; s->graph_batch = 0; s->graph_buf = nullptr; s->last_launches = 0;
-    s->launches_per_round = 0;
-    cudaError_t e = s->stage.open((size_t)cfg->max_rounds * 16 + 256);
-    if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_reinforce_create: %s", cudaGetErrorString(e)); }
-    *out = s;
-    return PRL_OK;
+    return prl_reinforce::open(s, out);
 }
-extern "C" int prl_reinforce_destroy(prl_reinforce *s) {
-    if (!s) return PRL_OK;
-    s->stage.close();
-    if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
-    delete s;
-    return PRL_OK;
-}
-extern "C" int64_t prl_reinforce_adam_step(const prl_reinforce *s) { return s ? s->adam_step : -1; }
+extern "C" int prl_reinforce_destroy(prl_reinforce *s) { return prl_reinforce::destroy(s); }
+extern "C" int64_t prl_reinforce_adam_step(const prl_reinforce *s) { return prl_reinforce::adam_step_of(s); }
 extern "C" int prl_reinforce_set_lr(prl_reinforce *s, double actor_lr, double critic_lr) {
-    PRL_REQUIRE(s, "null handle");
-    PRL_REQUIRE(actor_lr >= 0.0 && critic_lr >= 0.0, "learning rates must be non-negative");
-    s->cfg.actor_lr = actor_lr;
-    s->cfg.critic_lr = critic_lr;
-    return PRL_OK;
+    return prl_reinforce::set_lr(s, actor_lr, critic_lr);
 }
-extern "C" int prl_reinforce_set_graph(prl_reinforce *s, int enable) {
-    PRL_REQUIRE(s, "null handle");
-    s->use_graph = enable != 0;
-    return PRL_OK;
-}
-extern "C" int64_t prl_reinforce_last_launches(const prl_reinforce *s) { return s ? s->last_launches : -1; }
-
-static int rf_buffer_ok(const prl_reinforce *s, const prl_buf *buf) {
-    const prl_reinforce_cfg &c = s->cfg;
-    PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.obs_dim == c.obs_dim && buf->desc.n_actions == c.n_actions,
-                "REINFORCE needs a discrete-action buffer with matching obs_dim / n_actions");
-    PRL_REQUIRE(buf->shard_world <= 1, "the buffer is one shard of a multi-GPU buffer: REINFORCE reads local buffers only");
-    return PRL_OK;
-}
+extern "C" int prl_reinforce_set_graph(prl_reinforce *s, int enable) { return prl_reinforce::set_graph(s, enable); }
+extern "C" int64_t prl_reinforce_last_launches(const prl_reinforce *s) { return prl_reinforce::last_launches_of(s); }
 
 // REINFORCE.learn's return pass (reinforce.py:179-201): out_return_dev f32[2] = {R, critic(s'_newest) * (1 - terminated)}
 extern "C" int prl_reinforce_returns(prl_reinforce *s, prl_buf *buf, float *out_return_dev, void *stream_) {
     PRL_REQUIRE(s && buf && out_return_dev, "null argument");
-    int rc = rf_buffer_ok(s, buf);
+    int rc = s->buffer_ok(buf);
     if (rc) return rc;
     const int64_t n = buf->len;
     PRL_REQUIRE(n > 0, "empty buffer (reference: assert len(replay_buffer.memory) > 0)");
@@ -266,7 +239,7 @@ extern "C" int prl_reinforce_returns(prl_reinforce *s, prl_buf *buf, float *out_
 }
 
 // one learner round, launched (or captured) on `st`; everything round- or call-dependent is read through s->call / s->round_idx
-static int rf_round(prl_reinforce *s, prl_buf *buf, int B, cudaStream_t st) {
+int prl_reinforce::round(prl_reinforce *s, prl_buf *buf, int B, cudaStream_t st) {
     const prl_reinforce_cfg &c = s->cfg;
     // the decay factors are overridden by call->decay_a / decay_c (k_adamw's decay pointer)
     const AdamHp h = adam_hp(0.0, c.beta1, c.beta2, c.eps, c.weight_decay);
@@ -278,11 +251,11 @@ static int rf_round(prl_reinforce *s, prl_buf *buf, int B, cudaStream_t st) {
     k_rf_loss<<<1, 256, 0, st>>>(B, c.n_actions, s->logits, s->act, s->v, s->dlogits, s->dv, s->call, s->round_idx);
     // ---------------- actor step (actor_critic_base.py:333-343)
     mlp2_backward(L, s->an, s->actor, s->g_actor, s->dlogits, s->S, s->ah1, s->ah2, s->dh2, s->dh1, B);
-    k_adamw<<<(s->an.P + eb - 1) / eb, eb, 0, st>>>(s->an.P, s->actor, s->actor_m, s->actor_v, s->actor_x, s->g_actor, h, s->scal_a,
+    k_adamw<<<(s->an.P + eb - 1) / eb, eb, 0, st>>>(s->an.P, s->actor, s->actor_m, s->actor_v, s->actor_x, s->g_actor, h, s->scal,
                                                   s->round_idx, nullptr, 0.f, 0.f, &s->call->decay_a);
     // ---------------- critic step (actor_critic_base.py:344-349), same v: the critic has not changed
     mlp2_backward(L, s->cn, s->critic, s->g_critic, s->dv, s->S, s->ch1, s->ch2, s->dh2, s->dh1, B);   // + one k_head_bwd
-    k_adamw<<<(s->cn.P + eb - 1) / eb, eb, 0, st>>>(s->cn.P, s->critic, s->critic_m, s->critic_v, s->critic_x, s->g_critic, h, s->scal_c,
+    k_adamw<<<(s->cn.P + eb - 1) / eb, eb, 0, st>>>(s->cn.P, s->critic, s->critic_m, s->critic_v, s->critic_x, s->g_critic, h, s->scal + c.max_rounds,
                                                   s->round_idx, nullptr, 0.f, 0.f, &s->call->decay_c);
     k_rf_bump<<<1, 1, 0, st>>>(s->round_idx);
     s->launches_per_round = L.count + 6;   // gather, loss, head backward, 2 x adamw, round counter
@@ -294,45 +267,7 @@ static int rf_round(prl_reinforce *s, prl_buf *buf, int B, cudaStream_t st) {
 extern "C" int prl_reinforce_learn(prl_reinforce *s, prl_buf *buf, int rounds, int batch, const float *return_dev, float *out_actor_loss,
                                    float *out_critic_loss, int32_t *out_logical, void *stream_) {
     PRL_REQUIRE(s && buf && return_dev && out_actor_loss && out_critic_loss, "null argument");
-    const prl_reinforce_cfg &c = s->cfg;
-    PRL_REQUIRE(rounds > 0 && rounds <= c.max_rounds && batch > 0 && batch <= c.max_batch, "rounds / batch outside the configured maxima");
-    int rc = rf_buffer_ok(s, buf);
-    if (rc) return rc;
-    cudaStream_t st = (cudaStream_t)stream_;
-    rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
-    if (rc) return rc;
-    // per-call block: Adam scalars of every round (as torch evaluates them in double), decay factors, pointers
-    float2 *hs;
-    rc = s->stage.wait(&hs);
-    if (rc) return rc;
-    const int MR = c.max_rounds;
-    for (int r = 0; r < rounds; r++) {
-        hs[r] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-        hs[MR + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-    }
-    RfCall *hc = reinterpret_cast<RfCall *>(hs + 2 * (size_t)MR);
-    hc->slots = s->slots; hc->ret = return_dev; hc->out_actor = out_actor_loss; hc->out_critic = out_critic_loss;
-    hc->decay_a = (float)(1.0 - c.actor_lr * c.weight_decay);
-    hc->decay_c = (float)(1.0 - c.critic_lr * c.weight_decay);
-    *reinterpret_cast<int *>(hc + 1) = 0;
-    // scal_a | scal_c | call | round_idx are contiguous on the device in the same order
-    rc = s->stage.send(s->scal_a, 2 * (size_t)MR * 8 + sizeof(RfCall) + 4, st);
-    if (rc) return rc;
-    if (s->use_graph) {
-        if (!s->graph_exec || s->graph_batch != batch || s->graph_buf != buf->records) {
-            rc = capture_graph(&s->graph_exec, "prl_reinforce_learn", [&](cudaStream_t cs) { return rf_round(s, buf, batch, cs); });
-            if (rc) return rc;
-            s->graph_batch = batch; s->graph_buf = buf->records;
-        }
-        for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec, st));
-    } else {
-        for (int r = 0; r < rounds; r++) {
-            rc = rf_round(s, buf, batch, st);
-            if (rc) return rc;
-        }
-    }
-    PRL_CUDA(cudaGetLastError());
-    s->adam_step += rounds;
-    s->last_launches = (int64_t)s->launches_per_round * rounds;
-    return PRL_OK;
+    RfCall call{};
+    call.ret = return_dev; call.out_actor = out_actor_loss; call.out_critic = out_critic_loss;
+    return prl_reinforce::learn(s, buf, rounds, batch, 0, out_logical, call, stream_);
 }

@@ -19,7 +19,7 @@
 
 #include "common.cuh"
 #include "gemm.cuh"
-#include "host_runtime.cuh"
+#include "rounds.cuh"
 
 using namespace prl;
 
@@ -171,7 +171,9 @@ __global__ void k_sac_alpha(int B, const float *__restrict__ logp, float target_
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_sac {
+struct prl_sac : Rounds<prl_sac, SacCall> {
+    static constexpr const char *kFn = "prl_sac";
+    static constexpr int kScal = 2;   // actor, critic
     prl_sac_cfg cfg;
     int Pa, Pc;                       // actor parameters; parameters of ONE critic
     // actor layout offsets
@@ -181,21 +183,16 @@ struct prl_sac {
     float *critic, *critic_m, *critic_v, *critic_x, *critic_t;
     float *log_alpha, *alpha;         // log_alpha[4] = value, m, v, vmax ; alpha scalar
     const float *low, *high;
-    int64_t adam_step;
     // workspace
     float *S, *A, *R, *S2, *T, *h1, *h2, *mean, *z, *act_s, *na, *sd, *logp, *logp2, *c1, *c2, *q, *qt, *dq, *dc2, *dc1, *da, *dmean, *dz,
         *dh2, *dh1, *y, *g_actor, *g_critic;
-    int32_t *slots, *logical;
-    float2 *scal_a, *scal_c;
-    SacCall *call;
-    int *round_idx;
-    bool use_graph;
-    cudaGraphExec_t graph_exec;
-    int graph_batch;
-    const uint32_t *graph_buf;
-    int launches_per_round;
-    Stage stage;
-    int64_t last_launches;
+    double &lr(int k) { return k == 0 ? cfg.actor_lr : cfg.critic_lr; }
+    int buffer_ok(const prl_buf *buf) const {
+        PRL_REQUIRE((buf->desc.flags & PRL_BUF_CONTINUOUS) && buf->desc.obs_dim == cfg.obs_dim && buf->desc.act_dim == cfg.act_dim,
+                    "SAC needs a continuous-action buffer with matching dimensions");
+        return PRL_OK;
+    }
+    static int round(prl_sac *s, prl_buf *buf, int B, cudaStream_t st);
 };
 
 static void sac_layout(prl_sac *s) {
@@ -245,8 +242,7 @@ static int64_t sac_carve(prl_sac *s, void *base) {
     w(s->dq, 2 * B); w(s->dc2, 2 * B * c.critic_h2); w(s->dc1, 2 * B * c.critic_h1); w(s->da, 2 * B * A);
     w(s->dmean, B * A); w(s->dz, B * A); w(s->dh2, B * c.actor_h2); w(s->dh1, B * c.actor_h1); w(s->y, B);
     w(s->g_actor, s->Pa); w(s->g_critic, 2 * (int64_t)s->Pc);
-    w(s->slots, c.max_rounds * B); w(s->logical, c.max_rounds * B);
-    w(s->scal_a, 2 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | call | round_idx
+    s->carve_tail(w, c.max_rounds, B);
     return w.bytes;
 }
 extern "C" int64_t prl_sac_workspace_bytes(const prl_sac_cfg *c) {
@@ -272,28 +268,18 @@ extern "C" int prl_sac_create(prl_sac **out, const prl_sac_cfg *cfg, float *acto
     s->log_alpha = log_alpha4; s->alpha = alpha1; s->low = low_dev; s->high = high_dev;
     s->adam_step = adam_step;
     sac_carve(s, workspace);
-    s->scal_c = s->scal_a + cfg->max_rounds;
-    s->call = (SacCall *)(s->scal_c + cfg->max_rounds); s->round_idx = (int *)(s->call + 1);
-    s->use_graph = true; s->graph_exec = nullptr; s->graph_batch = 0; s->graph_buf = nullptr; s->last_launches = 0;
-    static_assert(sizeof(SacCall) + 4 <= 64 * 4, "call block fits the reserved tail");
-    cudaError_t e = s->stage.open((size_t)cfg->max_rounds * 16 + 256);
-    if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_sac_create: %s", cudaGetErrorString(e)); }
-    *out = s;
-    return PRL_OK;
+    return prl_sac::open(s, out);
 }
-extern "C" int prl_sac_destroy(prl_sac *s) {
-    if (!s) return PRL_OK;
-    s->stage.close();
-    if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
-    delete s;
-    return PRL_OK;
-}
-extern "C" int64_t prl_sac_adam_step(const prl_sac *s) { return s ? s->adam_step : -1; }
+extern "C" int prl_sac_destroy(prl_sac *s) { return prl_sac::destroy(s); }
+extern "C" int64_t prl_sac_adam_step(const prl_sac *s) { return prl_sac::adam_step_of(s); }
+extern "C" int prl_sac_set_graph(prl_sac *s, int enable) { return prl_sac::set_graph(s, enable); }
+extern "C" int64_t prl_sac_last_launches(const prl_sac *s) { return prl_sac::last_launches_of(s); }
 
 // one learner round, launched (or captured) on `st`; everything round-dependent is read on the device through
 // s->call / s->round_idx
-static int sac_round(prl_sac *s, prl_buf *buf, int B, cudaStream_t st) {
+int prl_sac::round(prl_sac *s, prl_buf *buf, int B, cudaStream_t st) {
     const prl_sac_cfg &c = s->cfg;
+    const float2 *scal_a = s->scal, *scal_c = s->scal + c.max_rounds;
     const int O = c.obs_dim, A = c.act_dim, D = O + A;
     const int H1 = c.actor_h1, H2 = c.actor_h2, C1 = c.critic_h1, C2 = c.critic_h2;
     const long long Pc = s->Pc;
@@ -338,7 +324,7 @@ static int sac_round(prl_sac *s, prl_buf *buf, int B, cudaStream_t st) {
         L.bwd_w(s->dh2, H2, 0, B, H2, mat(s->h1, H1), H1, ga + s->aW2, H1, 0, ga + s->ab2, 0);
         L.bwd_x(s->dh2, H2, 0, B, H2, aw + s->aW2, H1, 0, 0, H1, s->dh1, H1, 0, s->h1, H1, 0, false);
         L.bwd_w(s->dh1, H1, 0, B, H1, mat(s->S, O), O, ga + s->aW1, O, 0, ga + s->ab1, 0);
-        k_adamw<<<(s->Pa + eb - 1) / eb, eb, 0, st>>>(s->Pa, s->actor, s->actor_m, s->actor_v, s->actor_x, ga, ha, s->scal_a, s->round_idx, nullptr, 0.f, 0.f);
+        k_adamw<<<(s->Pa + eb - 1) / eb, eb, 0, st>>>(s->Pa, s->actor, s->actor_m, s->actor_v, s->actor_x, ga, ha, scal_a, s->round_idx, nullptr, 0.f, 0.f);
     }
     // ---------------- critic step with the UPDATED actor (:345-349; soft_actor_critic_continuous.py:155-205)
     actor_forward(s->S2);
@@ -356,12 +342,12 @@ static int sac_round(prl_sac *s, prl_buf *buf, int B, cudaStream_t st) {
         L.bwd_x(s->dc2, C2, sC2, B, C2, cw + s->cW2, C1, Pc, 0, C1, s->dc1, C1, sC1, s->c1, C1, sC1, false, 2);
         L.bwd_w(s->dc1, C1, sC1, B, C1, mat2(s->S, O, O, s->A, A), D, gc + s->cW1, D, Pc, gc + s->cb1, Pc, 2);
         const int n2p = 2 * s->Pc;
-        k_adamw<<<(n2p + eb - 1) / eb, eb, 0, st>>>(n2p, s->critic, s->critic_m, s->critic_v, s->critic_x, gc, hc, s->scal_c, s->round_idx,
+        k_adamw<<<(n2p + eb - 1) / eb, eb, 0, st>>>(n2p, s->critic, s->critic_m, s->critic_v, s->critic_x, gc, hc, scal_c, s->round_idx,
                                                   s->critic_t, (float)c.tau, (float)(1.0 - c.tau));
     }
     small = 12;
     // ---------------- entropy coefficient (soft_actor_critic_continuous.py:134-147); also advances the round counter
-    k_sac_alpha<<<1, 256, 0, st>>>(B, s->logp, -(float)A, s->log_alpha, s->alpha, hc, s->scal_c, s->round_idx, s->call, c.autotune);
+    k_sac_alpha<<<1, 256, 0, st>>>(B, s->logp, -(float)A, s->log_alpha, s->alpha, hc, scal_c, s->round_idx, s->call, c.autotune);
     s->launches_per_round = L.count + small;
     return PRL_OK;
 }
@@ -369,50 +355,7 @@ static int sac_round(prl_sac *s, prl_buf *buf, int B, cudaStream_t st) {
 extern "C" int prl_sac_learn(prl_sac *s, prl_buf *buf, int rounds, int batch, const float *noise_dev, float *out_actor_loss,
                              float *out_critic_loss, float *out_entropy_loss, int32_t *out_logical, void *stream_) {
     PRL_REQUIRE(s && buf && noise_dev && out_actor_loss && out_critic_loss && out_entropy_loss, "null argument");
-    const prl_sac_cfg &c = s->cfg;
-    PRL_REQUIRE(rounds > 0 && rounds <= c.max_rounds && batch > 0 && batch <= c.max_batch, "rounds / batch outside the configured maxima");
-    PRL_REQUIRE((buf->desc.flags & PRL_BUF_CONTINUOUS) && buf->desc.obs_dim == c.obs_dim && buf->desc.act_dim == c.act_dim,
-                "SAC needs a continuous-action buffer with matching dimensions");
-    cudaStream_t st = (cudaStream_t)stream_;
-    int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
-    if (rc) return rc;
-    // per-call block: AdamW scalars of every round (actor lr / critic lr, as torch evaluates them in double) + pointers
-    float2 *hs;
-    rc = s->stage.wait(&hs);
-    if (rc) return rc;
-    for (int r = 0; r < rounds; r++) {
-        hs[r] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-        hs[c.max_rounds + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-    }
-    SacCall *hc = reinterpret_cast<SacCall *>(hs + 2 * (size_t)c.max_rounds);
-    hc->noise = noise_dev; hc->slots = s->slots; hc->out_actor = out_actor_loss; hc->out_critic = out_critic_loss; hc->out_entropy = out_entropy_loss;
-    int *hround = reinterpret_cast<int *>(hc + 1);
-    *hround = 0;
-    // scal_a | scal_c | call | round_idx are contiguous on the device in the same order
-    rc = s->stage.send(s->scal_a, 2 * (size_t)c.max_rounds * 8 + sizeof(SacCall) + 4, st);
-    if (rc) return rc;
-
-    if (s->use_graph) {
-        if (!s->graph_exec || s->graph_batch != batch || s->graph_buf != buf->records) {
-            rc = capture_graph(&s->graph_exec, "prl_sac_learn", [&](cudaStream_t cs) { return sac_round(s, buf, batch, cs); });
-            if (rc) return rc;
-            s->graph_batch = batch; s->graph_buf = buf->records;
-        }
-        for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec, st));
-    } else {
-        for (int r = 0; r < rounds; r++) {
-            rc = sac_round(s, buf, batch, st);
-            if (rc) return rc;
-        }
-    }
-    PRL_CUDA(cudaGetLastError());
-    s->adam_step += rounds;
-    s->last_launches = s->launches_per_round * rounds;
-    return PRL_OK;
+    SacCall call{};
+    call.noise = noise_dev; call.out_actor = out_actor_loss; call.out_critic = out_critic_loss; call.out_entropy = out_entropy_loss;
+    return prl_sac::learn(s, buf, rounds, batch, 0, out_logical, call, stream_);
 }
-extern "C" int prl_sac_set_graph(prl_sac *s, int enable) {
-    PRL_REQUIRE(s, "null handle");
-    s->use_graph = enable != 0;
-    return PRL_OK;
-}
-extern "C" int64_t prl_sac_last_launches(const prl_sac *s) { return s ? s->last_launches : -1; }

@@ -20,7 +20,7 @@
 
 #include "common.cuh"
 #include "gemm.cuh"
-#include "host_runtime.cuh"
+#include "rounds.cuh"
 
 using namespace prl;
 
@@ -183,7 +183,9 @@ __global__ void __launch_bounds__(256) k_sacd_alpha(int B, const float *__restri
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_sacd {
+struct prl_sacd : Rounds<prl_sacd, SacdCall> {
+    static constexpr const char *kFn = "prl_sacd";
+    static constexpr int kScal = 3;   // actor, critic, entropy coefficient
     prl_sacd_cfg cfg;
     int Pa, Pc;
     int aW1, ab1, aW2, ab2, aW3, ab3;
@@ -191,21 +193,21 @@ struct prl_sacd {
     float *actor, *actor_m, *actor_v, *actor_x;
     float *critic, *critic_m, *critic_v, *critic_x, *critic_t;
     float *log_alpha, *alpha;
-    int64_t adam_step;
     // workspace
     float *S, *S2, *R, *T, *h1, *h2, *logits, *dlogit, *ent, *dh2, *dh1, *P, *c1, *c2, *q, *c1a, *c2a, *dq, *dc2, *dc1, *y, *qa, *g_actor, *g_critic;
     int *act, *cnt, *ids;
-    int32_t *slots, *logical;
-    float2 *scal_a, *scal_c, *scal_e;
-    SacdCall *call;
-    int *round_idx;
-    bool use_graph;
-    cudaGraphExec_t graph_exec;
-    int graph_batch;
-    const uint32_t *graph_buf;
-    int launches_per_round;
-    Stage stage;
-    int64_t last_launches;
+    double &lr(int k) { return k == 0 ? cfg.actor_lr : k == 1 ? cfg.critic_lr : cfg.entropy_lr; }
+    void fill_call(SacdCall &k) const {
+        k.decay_a = (float)(1.0 - cfg.actor_lr * cfg.weight_decay);
+        k.decay_c = (float)(1.0 - cfg.critic_lr * cfg.weight_decay);
+    }
+    int buffer_ok(const prl_buf *buf) const {
+        PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.obs_dim == cfg.obs_dim && buf->desc.n_actions == cfg.n_actions,
+                    "discrete SAC needs a discrete-action buffer with matching obs_dim / n_actions");
+        PRL_REQUIRE(buf->shard_world <= 1, "the buffer is one shard of a multi-GPU buffer: discrete SAC samples local buffers only");
+        return PRL_OK;
+    }
+    static int round(prl_sacd *s, prl_buf *buf, int B, cudaStream_t st);
 };
 
 static void sacd_layout(prl_sacd *s) {
@@ -255,8 +257,7 @@ static int64_t sacd_carve(prl_sacd *s, void *base) {
     w(s->dc2, 2 * B * c.critic_h2); w(s->dc1, 2 * B * c.critic_h1); w(s->y, B); w(s->qa, 2 * B);
     w(s->g_actor, s->Pa); w(s->g_critic, 2 * (int64_t)s->Pc);
     w(s->act, B); w(s->cnt, B); w(s->ids, BA);
-    w(s->slots, c.max_rounds * B); w(s->logical, c.max_rounds * B);
-    w(s->scal_a, 3 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | scal_e | call | round_idx
+    s->carve_tail(w, c.max_rounds, B);
     return w.bytes;
 }
 extern "C" int64_t prl_sacd_workspace_bytes(const prl_sacd_cfg *c) {
@@ -281,36 +282,18 @@ extern "C" int prl_sacd_create(prl_sacd **out, const prl_sacd_cfg *cfg, float *a
     s->log_alpha = log_alpha3; s->alpha = alpha1;
     s->adam_step = adam_step;
     sacd_carve(s, workspace);
-    s->scal_c = s->scal_a + cfg->max_rounds; s->scal_e = s->scal_c + cfg->max_rounds;
-    s->call = (SacdCall *)(s->scal_e + cfg->max_rounds); s->round_idx = (int *)(s->call + 1);
-    s->use_graph = true; s->graph_exec = nullptr; s->graph_batch = 0; s->graph_buf = nullptr; s->last_launches = 0;
-    s->launches_per_round = 0;
-    static_assert(sizeof(SacdCall) + 4 <= 64 * 4, "call block fits the reserved tail");
-    cudaError_t e = s->stage.open((size_t)cfg->max_rounds * 24 + 256);
-    if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_sacd_create: %s", cudaGetErrorString(e)); }
-    *out = s;
-    return PRL_OK;
+    return prl_sacd::open(s, out);
 }
-extern "C" int prl_sacd_destroy(prl_sacd *s) {
-    if (!s) return PRL_OK;
-    s->stage.close();
-    if (s->graph_exec) cudaGraphExecDestroy(s->graph_exec);
-    delete s;
-    return PRL_OK;
-}
-extern "C" int64_t prl_sacd_adam_step(const prl_sacd *s) { return s ? s->adam_step : -1; }
-
-extern "C" int prl_sacd_set_lr(prl_sacd *s, double actor_lr, double critic_lr) {
-    PRL_REQUIRE(s, "null handle");
-    PRL_REQUIRE(actor_lr >= 0.0 && critic_lr >= 0.0, "learning rates must be non-negative");
-    s->cfg.actor_lr = actor_lr;
-    s->cfg.critic_lr = critic_lr;
-    return PRL_OK;
-}
+extern "C" int prl_sacd_destroy(prl_sacd *s) { return prl_sacd::destroy(s); }
+extern "C" int64_t prl_sacd_adam_step(const prl_sacd *s) { return prl_sacd::adam_step_of(s); }
+extern "C" int prl_sacd_set_lr(prl_sacd *s, double actor_lr, double critic_lr) { return prl_sacd::set_lr(s, actor_lr, critic_lr); }
+extern "C" int prl_sacd_set_graph(prl_sacd *s, int enable) { return prl_sacd::set_graph(s, enable); }
+extern "C" int64_t prl_sacd_last_launches(const prl_sacd *s) { return prl_sacd::last_launches_of(s); }
 
 // one learner round, launched (or captured) on `st`; everything round- or call-dependent is read through s->call / s->round_idx
-static int sacd_round(prl_sacd *s, prl_buf *buf, int B, cudaStream_t st) {
+int prl_sacd::round(prl_sacd *s, prl_buf *buf, int B, cudaStream_t st) {
     const prl_sacd_cfg &c = s->cfg;
+    const float2 *scal_a = s->scal, *scal_c = scal_a + c.max_rounds, *scal_e = scal_c + c.max_rounds;
     const int O = c.obs_dim, A = c.n_actions, D = O + A, BA = B * A;
     const int H1 = c.actor_h1, H2 = c.actor_h2, C1 = c.critic_h1, C2 = c.critic_h2;
     const long long Pc = s->Pc;
@@ -350,7 +333,7 @@ static int sacd_round(prl_sacd *s, prl_buf *buf, int B, cudaStream_t st) {
         L.bwd_w(s->dh2, H2, 0, B, H2, mat(s->h1, H1), H1, ga + s->aW2, H1, 0, ga + s->ab2, 0);
         L.bwd_x(s->dh2, H2, 0, B, H2, aw + s->aW2, H1, 0, 0, H1, s->dh1, H1, 0, s->h1, H1, 0, false);
         L.bwd_w(s->dh1, H1, 0, B, H1, mat(s->S, O), O, ga + s->aW1, O, 0, ga + s->ab1, 0);
-        k_adamw<<<(s->Pa + eb - 1) / eb, eb, 0, st>>>(s->Pa, s->actor, s->actor_m, s->actor_v, s->actor_x, ga, h, s->scal_a, s->round_idx,
+        k_adamw<<<(s->Pa + eb - 1) / eb, eb, 0, st>>>(s->Pa, s->actor, s->actor_m, s->actor_v, s->actor_x, ga, h, scal_a, s->round_idx,
                                                     nullptr, 0.f, 0.f, &s->call->decay_a);
     }
     // ---------------- critic step with the UPDATED actor and the critic target (:345-349)
@@ -368,12 +351,12 @@ static int sacd_round(prl_sacd *s, prl_buf *buf, int B, cudaStream_t st) {
         L.bwd_w(s->dc1, C1, sA1, B, C1, mat(s->S, O), O, gc + s->cW1, D, Pc, gc + s->cb1, Pc, 2);   // state columns + b1
         k_fold_w1a_grad<<<dim3((C1 * A + eb - 1) / eb, 1, 2), eb, 0, st>>>(B, A, C1, s->act, s->dc1, gc + s->cW1 + O, D, Pc);
         const int n2p = 2 * s->Pc;
-        k_adamw<<<(n2p + eb - 1) / eb, eb, 0, st>>>(n2p, s->critic, s->critic_m, s->critic_v, s->critic_x, gc, h, s->scal_c, s->round_idx,
+        k_adamw<<<(n2p + eb - 1) / eb, eb, 0, st>>>(n2p, s->critic, s->critic_m, s->critic_v, s->critic_x, gc, h, scal_c, s->round_idx,
                                                   s->critic_t, (float)c.tau, (float)(1.0 - c.tau), &s->call->decay_c);
     }
     // ---------------- entropy coefficient (soft_actor_critic.py learn_batch); also advances the round counter
     k_sacd_alpha<<<1, 256, 0, st>>>(B, s->ent, (float)c.target_entropy, s->log_alpha, s->alpha, (float)(1.0 - c.beta1), (float)c.beta2,
-                                    (float)(1.0 - c.beta2), (float)c.entropy_eps, s->scal_e, s->round_idx, s->call, c.autotune);
+                                    (float)(1.0 - c.beta2), (float)c.entropy_eps, scal_e, s->round_idx, s->call, c.autotune);
     small += 10;   // gather, pick, actor loss, 2 x adamw, target, critic loss, head bwd, w1a grad, alpha (+ the expands)
     s->launches_per_round = L.count + small;
     return PRL_OK;
@@ -382,55 +365,7 @@ static int sacd_round(prl_sacd *s, prl_buf *buf, int B, cudaStream_t st) {
 extern "C" int prl_sacd_learn(prl_sacd *s, prl_buf *buf, int rounds, int batch, float *out_actor_loss, float *out_critic_loss,
                               float *out_entropy_loss, int32_t *out_logical, void *stream_) {
     PRL_REQUIRE(s && buf && out_actor_loss && out_critic_loss && out_entropy_loss, "null argument");
-    const prl_sacd_cfg &c = s->cfg;
-    PRL_REQUIRE(rounds > 0 && rounds <= c.max_rounds && batch > 0 && batch <= c.max_batch, "rounds / batch outside the configured maxima");
-    PRL_REQUIRE((buf->desc.flags & PRL_BUF_DISCRETE) && buf->desc.obs_dim == c.obs_dim && buf->desc.n_actions == c.n_actions,
-                "discrete SAC needs a discrete-action buffer with matching obs_dim / n_actions");
-    PRL_REQUIRE(buf->shard_world <= 1, "the buffer is one shard of a multi-GPU buffer: discrete SAC samples local buffers only");
-    cudaStream_t st = (cudaStream_t)stream_;
-    int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
-    if (rc) return rc;
-    // per-call block: Adam scalars of every round (as torch evaluates them in double), decay factors, pointers
-    float2 *hs;
-    rc = s->stage.wait(&hs);
-    if (rc) return rc;
-    const int MR = c.max_rounds;
-    for (int r = 0; r < rounds; r++) {
-        hs[r] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-        hs[MR + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-        hs[2 * MR + r] = adam_scal(c.entropy_lr, c.beta1, c.beta2, s->adam_step + r + 1);
-    }
-    SacdCall *hc = reinterpret_cast<SacdCall *>(hs + 3 * (size_t)MR);
-    hc->slots = s->slots; hc->out_actor = out_actor_loss; hc->out_critic = out_critic_loss; hc->out_entropy = out_entropy_loss;
-    hc->decay_a = (float)(1.0 - c.actor_lr * c.weight_decay);
-    hc->decay_c = (float)(1.0 - c.critic_lr * c.weight_decay);
-    int *hround = reinterpret_cast<int *>(hc + 1);
-    *hround = 0;
-    // scal_a | scal_c | scal_e | call | round_idx are contiguous on the device in the same order
-    rc = s->stage.send(s->scal_a, 3 * (size_t)MR * 8 + sizeof(SacdCall) + 4, st);
-    if (rc) return rc;
-
-    if (s->use_graph) {
-        if (!s->graph_exec || s->graph_batch != batch || s->graph_buf != buf->records) {
-            rc = capture_graph(&s->graph_exec, "prl_sacd_learn", [&](cudaStream_t cs) { return sacd_round(s, buf, batch, cs); });
-            if (rc) return rc;
-            s->graph_batch = batch; s->graph_buf = buf->records;
-        }
-        for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec, st));
-    } else {
-        for (int r = 0; r < rounds; r++) {
-            rc = sacd_round(s, buf, batch, st);
-            if (rc) return rc;
-        }
-    }
-    PRL_CUDA(cudaGetLastError());
-    s->adam_step += rounds;
-    s->last_launches = (int64_t)s->launches_per_round * rounds;
-    return PRL_OK;
+    SacdCall call{};
+    call.out_actor = out_actor_loss; call.out_critic = out_critic_loss; call.out_entropy = out_entropy_loss;
+    return prl_sacd::learn(s, buf, rounds, batch, 0, out_logical, call, stream_);
 }
-extern "C" int prl_sacd_set_graph(prl_sacd *s, int enable) {
-    PRL_REQUIRE(s, "null handle");
-    s->use_graph = enable != 0;
-    return PRL_OK;
-}
-extern "C" int64_t prl_sacd_last_launches(const prl_sacd *s) { return s ? s->last_launches : -1; }

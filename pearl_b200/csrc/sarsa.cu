@@ -9,10 +9,9 @@
 // One round: the soft target update in flagged rounds (with the CURRENT online parameters, before anything else), the
 // online net over the B rows at the taken action, the target net over the B rows at (s', a') — B rows, no max over next
 // actions, the available sets take no part — the Bellman target, the backward pass over B rows and AdamW(amsgrad).  The
-// one-hot action is folded into layer 1 (k_fold).  Fixed launch sequence captured into a CUDA graph and replayed; unlike
-// the other DQN-family handles, which keep one graph and re-capture when the batch changes, this one keeps a small cache
-// of graphs keyed by (batch, buffer): an on-policy learner clears its buffer after every learn(), so its batch follows the
-// episode length and repeats.  The AdamW step sizes, the decay factor and the per-round target-update flags are read
+// one-hot action is folded into layer 1 (k_fold).  Fixed launch sequence captured into a CUDA graph and replayed; this
+// handle keeps more captured rounds than the other DQN-family handles (kGraphs): an on-policy learner clears its buffer
+// after every learn(), so its batch follows the episode length and repeats.  The AdamW step sizes, the decay factor and the per-round target-update flags are read
 // through the per-call block, so prl_sarsa_set_lr needs no new capture.  fp32, fixed summation order, no float atomics:
 // bit-reproducible run to run.
 #include <math.h>
@@ -20,7 +19,7 @@
 #include <new>
 
 #include "common.cuh"
-#include "dqn_family.cuh"
+#include "rounds.cuh"
 #include "gemm.cuh"
 
 using namespace prl;
@@ -28,8 +27,6 @@ using namespace prl;
 namespace {
 
 constexpr int kMaxA = 255;   // next-action ids are stored as bytes
-constexpr int kGraphs = 64;  // graphs kept per handle: an on-policy loop whose batch follows the episode length below
-                             // batch_size (SARSA_method: 32) meets that many sizes; a graph of a round is a few KB
 
 // per-call block the captured round reads through
 struct SarsaCall {
@@ -92,8 +89,13 @@ __global__ void k_sarsa_target(int B, const float *__restrict__ q, const float *
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_sarsa : DqnRounds<prl_sarsa, SarsaCall> {
+struct prl_sarsa : Rounds<prl_sarsa, SarsaCall> {
     static constexpr const char *kFn = "prl_sarsa", *kName = "DeepSARSA";
+    static constexpr bool kTargetOn = true;
+    // an on-policy loop whose batch follows the episode length below batch_size (SARSA_method: 32) meets that many
+    // sizes; a graph of a round is a few KB
+    static constexpr int kGraphs = 64;
+    void fill_call(SarsaCall &k) const { k.decay = (float)(1.0 - cfg.lr * cfg.weight_decay); }
     prl_sarsa_cfg cfg;
     int P;
     int W1, b1, W2, b2, W3, b3;
@@ -101,22 +103,7 @@ struct prl_sarsa : DqnRounds<prl_sarsa, SarsaCall> {
     // workspace
     float *S, *S2, *R, *T, *P1, *c1, *c2, *qa, *P1t, *c1t, *c2t, *qt, *dq, *rowabs, *dc2, *dc1, *grad;
     int *act, *nact;
-    // graph cache, keyed by (dense batch, or the buffer's records and record stride, batch); the least recently used entry
-    // makes room.  The stride is part of the key because a captured round bakes in the layout, and a new buffer may reuse
-    // the storage address of an old one.
-    struct Graph {
-        cudaGraphExec_t exec = nullptr;
-        const uint32_t *records = nullptr;
-        int dense = 0, words = 0, batch = 0;
-        int64_t used = 0;
-    };
-    Graph graphs[kGraphs];
-    int64_t captures = 0, uses = 0;
-    ~prl_sarsa() {
-        for (Graph &g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    }
     static int round(prl_sarsa *s, prl_buf *buf, int B, cudaStream_t st);
-    int run(prl_buf *buf, int rounds, int batch, cudaStream_t st);   // hides DqnRounds::run: the cached-graph variant
 };
 
 static void sarsa_layout(prl_sarsa *s) {
@@ -191,7 +178,7 @@ extern "C" int prl_sarsa_set_adam_step(prl_sarsa *s, int64_t step) { return prl_
 extern "C" int prl_sarsa_set_lr(prl_sarsa *s, double lr) { return prl_sarsa::set_lr(s, lr); }
 extern "C" int prl_sarsa_set_graph(prl_sarsa *s, int enable) { return prl_sarsa::set_graph(s, enable); }
 extern "C" int64_t prl_sarsa_last_launches(const prl_sarsa *s) { return prl_sarsa::last_launches_of(s); }
-extern "C" int64_t prl_sarsa_graph_captures(const prl_sarsa *s) { return s ? s->captures : -1; }
+extern "C" int64_t prl_sarsa_graph_captures(const prl_sarsa *s) { return s ? s->graphs.captures : -1; }
 
 // the Q network at one action per row: layer 1 folded (state product + the action's W1 column), then two contractions
 static void sarsa_fwd(const prl_sarsa *s, GemmLauncher &L, const float *net, const float *X, int m, const int *ids, float *P1, float *c1,
@@ -245,48 +232,15 @@ int prl_sarsa::round(prl_sarsa *s, prl_buf *buf, int B, cudaStream_t st) {
     return PRL_OK;
 }
 
-// `rounds` rounds: replays of the cached graph of this (batch, buffer), captured on a miss, or eager launches
-int prl_sarsa::run(prl_buf *buf, int rounds, int batch, cudaStream_t st) {
-    if (use_graph) {
-        const int dense = buf ? 0 : 1;
-        const uint32_t *rec = buf ? buf->records : nullptr;
-        const int words = buf ? buf->lay.record_words : 0;
-        Graph *hit = nullptr;
-        for (Graph &e : graphs)
-            if (e.exec && e.dense == dense && e.batch == batch && e.records == rec && e.words == words) { hit = &e; break; }
-        if (!hit) {
-            for (Graph &e : graphs) if (!e.exec) { hit = &e; break; }
-            if (!hit) {
-                hit = &graphs[0];
-                for (Graph &e : graphs) if (e.used < hit->used) hit = &e;
-            }
-            // capture_graph releases the evicted graph (freed once its launches in flight complete)
-            int rc = capture_graph(&hit->exec, kFn, [&](cudaStream_t cs) { return round(this, buf, batch, cs); });
-            if (rc) return rc;
-            hit->dense = dense; hit->records = rec; hit->words = words; hit->batch = batch;
-            captures++;
-        }
-        hit->used = ++uses;
-        for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(hit->exec, st));
-    } else {
-        for (int r = 0; r < rounds; r++) {
-            int rc = round(this, buf, batch, st);
-            if (rc) return rc;
-        }
-    }
-    PRL_CUDA(cudaGetLastError());
-    adam_step += rounds;
-    last_launches = (int64_t)launches_per_round * rounds;
-    return PRL_OK;
-}
-
 extern "C" int prl_sarsa_learn(prl_sarsa *s, prl_buf *buf, int rounds, int batch, int64_t training_steps, float *out_loss,
                                int32_t *out_logical, void *stream_) {
-    PRL_REQUIRE(s && buf, "null argument");
+    PRL_REQUIRE(s && buf && out_loss, "null argument");
     PRL_REQUIRE(buf->desc.flags & PRL_BUF_NEXT_ACTION,
                 "DeepSARSA needs the committed next action of every transition: learn over a B200SARSAReplayBuffer "
                 "(a buffer created with PRL_BUF_NEXT_ACTION)");
-    return prl_sarsa::learn(s, buf, rounds, batch, training_steps, out_loss, out_logical, SarsaCall{}, stream_);
+    SarsaCall call{};
+    call.out_loss = out_loss;
+    return prl_sarsa::learn(s, buf, rounds, batch, training_steps, out_logical, call, stream_);
 }
 
 extern "C" int prl_sarsa_learn_batch(prl_sarsa *s, int batch, const float *state, const int32_t *action_id, const float *reward,
@@ -296,7 +250,8 @@ extern "C" int prl_sarsa_learn_batch(prl_sarsa *s, int batch, const float *state
     SarsaCall dense{};
     dense.d_state = state; dense.d_next_state = next_state; dense.d_reward = reward; dense.d_action_id = action_id;
     dense.d_next_action_id = next_action_id; dense.d_term = terminated;
-    return prl_sarsa::learn_batch(s, batch, training_steps, out_loss, dense, stream_);
+    dense.out_loss = out_loss;
+    return prl_sarsa::learn_batch(s, batch, training_steps, dense, stream_);
 }
 
 // Q(s, a) for every action: the online forward of the round on n rows (chunks of max_batch rows through the workspace)

@@ -8,7 +8,7 @@
 // DDPG is the same step with actor_update_freq = 1 and no target noise (this reference trains a twin critic for DDPG too).
 // Same launch structure as the SAC learner (sac.cu): one round = a fixed sequence of launches of the tiled contraction
 // kernel (gemm.cuh) plus small elementwise kernels, everything round-dependent read on the device through a per-call
-// block; two CUDA graphs (round with / without the actor update) are captured once and replayed.
+// block; the rounds with and without the actor update are captured as two CUDA graphs (rounds.cuh) and replayed.
 #include <math.h>
 #include <stdarg.h>
 
@@ -16,7 +16,7 @@
 
 #include "common.cuh"
 #include "gemm.cuh"
-#include "host_runtime.cuh"
+#include "rounds.cuh"
 
 using namespace prl;
 
@@ -122,7 +122,9 @@ __global__ void k_td3_bump(int *round_idx, int *actor_round_idx, int actor_updat
 
 }  // namespace
 
-struct prl_td3 {
+struct prl_td3 : Rounds<prl_td3, Td3Call> {
+    static constexpr const char *kFn = "prl_td3";
+    static constexpr int kScal = 2, kCounters = 2, kGraphs = 2;   // actor, critic; round_idx, actor_round_idx; variants
     prl_td3_cfg cfg;
     int Pa, Pc;                        // actor parameters; parameters of ONE critic
     int aW1, ab1, aW2, ab2, aW3, ab3;
@@ -130,20 +132,30 @@ struct prl_td3 {
     float *actor, *actor_m, *actor_v, *actor_x, *actor_t;
     float *critic, *critic_m, *critic_v, *critic_x, *critic_t;
     const float *low, *high;
-    int64_t actor_step, critic_step;
+    int64_t actor_step;                // the actor optimizer's step count; adam_step counts the critic's
     float *S, *A, *R, *S2, *T, *h1, *h2, *pre, *act_s, *na, *c1, *c2, *q, *qt, *dq, *dc2, *dc1, *da, *dpre, *dh2, *dh1, *y, *g_actor,
         *g_critic, *last_actor_loss;
-    int32_t *slots, *logical;
-    float2 *scal_a, *scal_c;
-    Td3Call *call;
-    int *round_idx, *actor_round_idx;
-    bool use_graph;
-    cudaGraphExec_t graph_exec[2];     // [0] round without, [1] with the actor update
-    int graph_batch;
-    const uint32_t *graph_buf;
-    int launches_per_round[2];
-    Stage stage;
-    int64_t last_launches;
+    int buffer_ok(const prl_buf *buf) const {
+        PRL_REQUIRE((buf->desc.flags & PRL_BUF_CONTINUOUS) && buf->desc.obs_dim == cfg.obs_dim && buf->desc.act_dim == cfg.act_dim,
+                    "TD3 / DDPG need a continuous-action buffer with matching dimensions");
+        return PRL_OK;
+    }
+    // 1: round r updates the actor.  PolicyLearner.learn increments _training_steps before learn_batch
+    // (policy_learner.py:183), TD3 tests `_training_steps % actor_update_freq == 0` (td3.py:121)
+    int variant(int r) const { return cfg.actor_update_freq <= 1 || (steps0 + r) % cfg.actor_update_freq == 0 ? 1 : 0; }
+    // the actor optimizer's own step count only advances on update rounds
+    void fill_scal(float2 *hs, int rounds) {
+        const prl_td3_cfg &c = cfg;
+        int n_actor = 0;
+        for (int r = 0; r < rounds; r++) {
+            hs[c.max_rounds + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, adam_step + r + 1);
+            if (variant(r)) {
+                hs[n_actor] = adam_scal(c.actor_lr, c.beta1, c.beta2, actor_step + n_actor + 1);
+                n_actor++;
+            }
+        }
+    }
+    int round_variant(prl_buf *buf, int B, int variant, cudaStream_t st);
 };
 
 static void td3_layout(prl_td3 *s) {
@@ -188,8 +200,7 @@ static int64_t td3_carve(prl_td3 *s, void *base) {
     w(s->dq, 2 * B); w(s->dc2, 2 * B * c.critic_h2); w(s->dc1, 2 * B * c.critic_h1); w(s->da, 2 * B * A);
     w(s->dpre, B * A); w(s->dh2, B * c.actor_h2); w(s->dh1, B * c.actor_h1); w(s->y, B);
     w(s->g_actor, s->Pa); w(s->g_critic, 2 * (int64_t)s->Pc); w(s->last_actor_loss, 4);
-    w(s->slots, c.max_rounds * B); w(s->logical, c.max_rounds * B);
-    w(s->scal_a, 2 * (int64_t)c.max_rounds + 32);                                        // scal_a | scal_c | call | round_idx | actor_round_idx
+    s->carve_tail(w, c.max_rounds, B);
     return w.bytes;
 }
 extern "C" int64_t prl_td3_workspace_bytes(const prl_td3_cfg *c) {
@@ -213,32 +224,25 @@ extern "C" int prl_td3_create(prl_td3 **out, const prl_td3_cfg *cfg, float *acto
     s->actor = actor_w; s->actor_m = actor_m; s->actor_v = actor_v; s->actor_x = actor_vmax; s->actor_t = actor_target_w;
     s->critic = critic_w; s->critic_m = critic_m; s->critic_v = critic_v; s->critic_x = critic_vmax; s->critic_t = critic_target_w;
     s->low = low_dev; s->high = high_dev;
-    s->actor_step = actor_adam_step; s->critic_step = critic_adam_step;
+    s->actor_step = actor_adam_step; s->adam_step = critic_adam_step;
     td3_carve(s, workspace);
-    s->scal_c = s->scal_a + cfg->max_rounds;
-    s->call = (Td3Call *)(s->scal_c + cfg->max_rounds); s->round_idx = (int *)(s->call + 1); s->actor_round_idx = s->round_idx + 1;
-    static_assert(sizeof(Td3Call) + 8 <= 64 * 4, "call block fits the reserved tail");
-    s->use_graph = true; s->graph_exec[0] = s->graph_exec[1] = nullptr; s->graph_batch = 0; s->graph_buf = nullptr;
-    s->last_launches = 0;
-    cudaError_t e = cudaMemset(s->last_actor_loss, 0, 16);
-    if (e == cudaSuccess) e = s->stage.open((size_t)cfg->max_rounds * 16 + 256);
+    const cudaError_t e = cudaMemset(s->last_actor_loss, 0, 16);
     if (e != cudaSuccess) { delete s; return fail(PRL_ECUDA, "prl_td3_create: %s", cudaGetErrorString(e)); }
-    *out = s;
-    return PRL_OK;
+    return prl_td3::open(s, out);
 }
-extern "C" int prl_td3_destroy(prl_td3 *s) {
-    if (!s) return PRL_OK;
-    s->stage.close();
-    for (int i = 0; i < 2; i++) if (s->graph_exec[i]) cudaGraphExecDestroy(s->graph_exec[i]);
-    delete s;
-    return PRL_OK;
-}
+extern "C" int prl_td3_destroy(prl_td3 *s) { return prl_td3::destroy(s); }
 extern "C" int64_t prl_td3_actor_adam_step(const prl_td3 *s) { return s ? s->actor_step : -1; }
-extern "C" int64_t prl_td3_critic_adam_step(const prl_td3 *s) { return s ? s->critic_step : -1; }
+extern "C" int64_t prl_td3_critic_adam_step(const prl_td3 *s) { return prl_td3::adam_step_of(s); }
+extern "C" int prl_td3_set_graph(prl_td3 *s, int enable) { return prl_td3::set_graph(s, enable); }
+extern "C" int64_t prl_td3_last_launches(const prl_td3 *s) { return prl_td3::last_launches_of(s); }
 
-// one learner round, launched (or captured) on `st`
-static int td3_round(prl_td3 *s, prl_buf *buf, int B, bool update_actor, cudaStream_t st) {
+// one learner round, launched (or captured) on `st`; variant 1: with the actor update
+int prl_td3::round_variant(prl_buf *buf, int B, int variant, cudaStream_t st) {
+    prl_td3 *s = this;
+    const bool update_actor = variant == 1;
     const prl_td3_cfg &c = s->cfg;
+    const float2 *scal_a = s->scal, *scal_c = s->scal + c.max_rounds;
+    int *actor_round_idx = s->round_idx + 1;
     const int O = c.obs_dim, A = c.act_dim, D = O + A;
     const int H1 = c.actor_h1, H2 = c.actor_h2, C1 = c.critic_h1, C2 = c.critic_h2;
     const long long Pc = s->Pc;
@@ -278,7 +282,7 @@ static int td3_round(prl_td3 *s, prl_buf *buf, int B, bool update_actor, cudaStr
         L.bwd_w(s->dh2, H2, 0, B, H2, mat(s->h1, H1), H1, ga + s->aW2, H1, 0, ga + s->ab2, 0);
         L.bwd_x(s->dh2, H2, 0, B, H2, aw + s->aW2, H1, 0, 0, H1, s->dh1, H1, 0, s->h1, H1, 0, false);
         L.bwd_w(s->dh1, H1, 0, B, H1, mat(s->S, O), O, ga + s->aW1, O, 0, ga + s->ab1, 0);
-        k_adamw<<<(s->Pa + eb - 1) / eb, eb, 0, st>>>(s->Pa, s->actor, s->actor_m, s->actor_v, s->actor_x, ga, ha, s->scal_a, s->actor_round_idx,
+        k_adamw<<<(s->Pa + eb - 1) / eb, eb, 0, st>>>(s->Pa, s->actor, s->actor_m, s->actor_v, s->actor_x, ga, ha, scal_a, actor_round_idx,
                                                      nullptr, 0.f, 0.f);
         small += 5;
     } else {
@@ -302,7 +306,7 @@ static int td3_round(prl_td3 *s, prl_buf *buf, int B, bool update_actor, cudaStr
         L.bwd_w(s->dc1, C1, sC1, B, C1, mat2(s->S, O, O, s->A, A), D, gc + s->cW1, D, Pc, gc + s->cb1, Pc, 2);
         const int n2p = 2 * s->Pc;
         // the critic targets follow only on rounds with an actor update (td3.py:136-147); DDPG: every round
-        k_adamw<<<(n2p + eb - 1) / eb, eb, 0, st>>>(n2p, s->critic, s->critic_m, s->critic_v, s->critic_x, gc, hc, s->scal_c, s->round_idx,
+        k_adamw<<<(n2p + eb - 1) / eb, eb, 0, st>>>(n2p, s->critic, s->critic_m, s->critic_v, s->critic_x, gc, hc, scal_c, s->round_idx,
                                                   update_actor ? s->critic_t : nullptr, (float)c.critic_tau, (float)(1.0 - c.critic_tau));
     }
     small += 6;
@@ -310,68 +314,19 @@ static int td3_round(prl_td3 *s, prl_buf *buf, int B, bool update_actor, cudaStr
         k_td3_soft_update<<<(s->Pa + eb - 1) / eb, eb, 0, st>>>(s->Pa, s->actor_t, s->actor, (float)c.actor_tau, (float)(1.0 - c.actor_tau));
         small++;
     }
-    k_td3_bump<<<1, 1, 0, st>>>(s->round_idx, s->actor_round_idx, update_actor ? 1 : 0);
+    k_td3_bump<<<1, 1, 0, st>>>(s->round_idx, actor_round_idx, update_actor ? 1 : 0);
     small++;
-    s->launches_per_round[update_actor ? 1 : 0] = L.count + small;
+    s->launches_per_round = L.count + small;
     return PRL_OK;
 }
 
 extern "C" int prl_td3_learn(prl_td3 *s, prl_buf *buf, int rounds, int batch, int64_t training_steps0, const float *noise_dev,
                              float *out_actor_loss, float *out_critic_loss, int32_t *out_logical, void *stream_) {
     PRL_REQUIRE(s && buf && out_actor_loss && out_critic_loss, "null argument");
-    const prl_td3_cfg &c = s->cfg;
-    PRL_REQUIRE(rounds > 0 && rounds <= c.max_rounds && batch > 0 && batch <= c.max_batch, "rounds / batch outside the configured maxima");
-    PRL_REQUIRE((buf->desc.flags & PRL_BUF_CONTINUOUS) && buf->desc.obs_dim == c.obs_dim && buf->desc.act_dim == c.act_dim,
-                "TD3 / DDPG need a continuous-action buffer with matching dimensions");
-    cudaStream_t st = (cudaStream_t)stream_;
-    int rc = prl_buf_sample_indices(buf, rounds, batch, out_logical ? out_logical : s->logical, s->slots, stream_);
+    Td3Call call{};
+    call.noise = noise_dev; call.out_actor = out_actor_loss; call.out_critic = out_critic_loss;
+    const int rc = prl_td3::learn(s, buf, rounds, batch, training_steps0, out_logical, call, stream_);
     if (rc) return rc;
-    // which rounds update the actor: PolicyLearner.learn increments _training_steps before learn_batch (policy_learner.py:183),
-    // TD3 tests `_training_steps % actor_update_freq == 0` (td3.py:121)
-    auto updates = [&](int r) { return c.actor_update_freq <= 1 || (training_steps0 + r + 1) % c.actor_update_freq == 0; };
-    float2 *hs;
-    rc = s->stage.wait(&hs);
-    if (rc) return rc;
-    int n_actor = 0;
-    for (int r = 0; r < rounds; r++) {
-        hs[c.max_rounds + r] = adam_scal(c.critic_lr, c.beta1, c.beta2, s->critic_step + r + 1);
-        if (updates(r)) {     // the actor optimizer's own step count: it only advances on update rounds
-            hs[n_actor] = adam_scal(c.actor_lr, c.beta1, c.beta2, s->actor_step + n_actor + 1);
-            n_actor++;
-        }
-    }
-    Td3Call *hc = reinterpret_cast<Td3Call *>(hs + 2 * (size_t)c.max_rounds);
-    hc->noise = noise_dev; hc->slots = s->slots; hc->out_actor = out_actor_loss; hc->out_critic = out_critic_loss;
-    int *hround = reinterpret_cast<int *>(hc + 1);
-    hround[0] = 0; hround[1] = 0;
-    rc = s->stage.send(s->scal_a, 2 * (size_t)c.max_rounds * 8 + sizeof(Td3Call) + 8, st);
-    if (rc) return rc;
-
-    if (s->use_graph) {
-        if (!s->graph_exec[0] || s->graph_batch != batch || s->graph_buf != buf->records) {
-            for (int u = 0; u < 2; u++) {
-                rc = capture_graph(&s->graph_exec[u], "prl_td3_learn", [&](cudaStream_t cs) { return td3_round(s, buf, batch, u == 1, cs); });
-                if (rc) return rc;
-            }
-            s->graph_batch = batch; s->graph_buf = buf->records;
-        }
-        for (int r = 0; r < rounds; r++) PRL_CUDA(cudaGraphLaunch(s->graph_exec[updates(r) ? 1 : 0], st));
-    } else {
-        for (int r = 0; r < rounds; r++) {
-            rc = td3_round(s, buf, batch, updates(r), st);
-            if (rc) return rc;
-        }
-    }
-    PRL_CUDA(cudaGetLastError());
-    s->critic_step += rounds;
-    s->actor_step += n_actor;
-    s->last_launches = 0;
-    for (int r = 0; r < rounds; r++) s->last_launches += s->launches_per_round[updates(r) ? 1 : 0];
+    for (int r = 0; r < rounds; r++) s->actor_step += s->variant(r);
     return PRL_OK;
 }
-extern "C" int prl_td3_set_graph(prl_td3 *s, int enable) {
-    PRL_REQUIRE(s, "null handle");
-    s->use_graph = enable != 0;
-    return PRL_OK;
-}
-extern "C" int64_t prl_td3_last_launches(const prl_td3 *s) { return s ? s->last_launches : -1; }
