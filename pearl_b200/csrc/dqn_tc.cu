@@ -20,16 +20,18 @@
 //            their operands are explicitly transposed tiles written with a 144-byte chunk pitch
 //            (bank-conflict-free column scatter), 64 batch rows per pass, the two warpgroups issuing the same
 //            products on equal shares of the output columns.  Their accumulators stay in registers for the whole step.
-//   AdamW    gradients registers -> shared staging, then one coalesced 16-byte sweep over the flat parameter
-//            vector (parameters / moments in L2) that also writes the operand-layout weight tiles.
+//   AdamW    gradients registers -> shared staging, then one sweep over the flat W1 | b1 | W2 range whose parameters and
+//            moments stream in by TMA bulk copies, in 16 KB chunks through an 8-slot ring in regions 3 and 1 (free once
+//            the last weight-gradient products have been waited for); 16-byte stores write the results and the
+//            operand-layout weight tiles.  b1 | b2 | W3 | b3 are updated one parameter per thread.  Shapes with
+//            D % 4 != 0 (1 or 2 actions) or parameters that are not 16-byte aligned take a scalar sweep instead.
 //
 // The weights are kept in global memory a second time IN THE OPERAND LAYOUT (hi tile = the fp32 values — the tensor
 // core truncates them to TF32 — and lo tile = x - trunc_tf32(x)), written by AdamW / the soft target update next to the
 // flat torch-order vectors, so staging a network's B operands is three TMA bulk copies (cp.async.bulk + mbarrier
 // complete_tx) issued by one thread.  The W2 tiles store their K axis in the order umma::kperm, which is the order in
 // which an accumulator's columns feed the next product's register A operand.  The target network's small vectors are
-// cached in shared memory between soft updates, AdamW walks one flat list with two groups of loads in flight, the soft
-// target update is applied to the tiles in tile order.
+// cached in shared memory between soft updates, the soft target update is applied to the tiles in tile order.
 //
 // Each 3xTF32 product is one chain of wgmma with a single wait at its end, and that only holds while ptxas can pipeline
 // the kernel's wgmma: ONE obstacle anywhere in the kernel makes it wait after every wgmma of the kernel.  What must
@@ -65,6 +67,9 @@ constexpr int SBUF = 16384;          // layer-1 row staging of one warpgroup: [6
 // transposed-tile arena (regions 1+2) for the weight-gradient products, 64 batch rows per pass
 constexpr int TL = 144;              // chunk pitch of transposed tiles
 constexpr int AR_A_HI = 0, AR_A_LO = 18432, AR_B_HI = 36864, AR_B_LO = 73728, AR_E = 110592;
+// AdamW ring: chunks of ACH flat parameters, one slot = the chunk's w | m | v | vmax (16 KB); slots 0-3 in region 3,
+// 4-7 in region 1
+constexpr int ACH = 1024, ARING = 8, ASLOT = 4 * ACH * 4;
 
 struct TcLearner {            // one per CTA, in global memory
     const uint32_t *records;
@@ -87,6 +92,7 @@ struct TcArgs {
     float decay, omb1, beta2, omb2, eps, gamma, tau, omtau, inv_b2;
     long long *prof;   // optional [rounds][16] SM-clock stamps of one CTA
     int prof_cta;      // which CTA writes them (PRL_TC_PROF_CTA, default 0: the learners do not all run at the same speed)
+    int adam_tma;      // D % 4 == 0 and every learner's w / m / v / vmax 16-byte aligned: AdamW streams them by TMA
 };
 
 #define TC_STAMP(idx)                                                                          \
@@ -103,7 +109,7 @@ struct Misc {
     float rew[MAX_B], term[MAX_B];
     float redw[8][HID];
     float redmae[8], reddb3[8];
-    unsigned long long bar[3];   // 0: target tiles; 1: online W1 tiles; 2: online W2 tiles
+    unsigned long long bar[3 + ARING];   // 0: target tiles; 1: online W1 tiles; 2: online W2 tiles; 3 + s: AdamW ring slot s
     // kept here rather than in registers: the wgmma chains need the registers (section 3.1 of DESIGN.md)
     TcLearner L;                 // this CTA's learner, per-round arrays shifted to the launch's first round
     float dw3[16][NTH];          // per-thread dW3 partial sums, carried across the row tiles
@@ -308,7 +314,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     }
     uint64_t *bar = reinterpret_cast<uint64_t *>(mi.bar);
     if (tid == 0)
-        for (int i = 0; i < 3; i++) umma::mbar_init(bar + i, 1);
+        for (int i = 0; i < 3 + ARING; i++) umma::mbar_init(bar + i, 1);
     // the operand-layout tiles follow the flat parameters (which the host may have changed between calls)
     auto To = [&] { return net_tiles(L.tiles, d.obs); };
     auto Tt = [&] { return net_tiles(L.tiles + net_tile_floats(d.obs), d.obs); };
@@ -327,6 +333,20 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     auto tma_w2 = [&](const NetTiles &t, uint64_t *b) {
         mbar_expect_tx(b, w2_bytes);
         bulk_g2s(smem + REG3, t.w2, w2_bytes, b);
+    };
+    // AdamW streams W1 | b1 | W2 (one flat range; D % 4 == 0 keeps every 16-byte group inside one of the three) through the
+    // ring: chunk k goes to slot k % ARING, whose barrier completes once per use
+    const int an = d.ob2, nch = (an + ACH - 1) / ACH;
+    auto aslot = [&](int s) { return smem + (s < 4 ? REG3 : REG1) + (s & 3) * ASLOT; };
+    auto adam_issue = [&](int k) {
+        const int off = k * ACH, s = k % ARING;
+        const uint32_t bytes = 4u * (an - off < ACH ? an - off : ACH);
+        char *dst = aslot(s);
+        mbar_expect_tx(bar + 3 + s, 4 * bytes);
+        bulk_g2s(dst, L.w + off, bytes, bar + 3 + s);
+        bulk_g2s(dst + ACH * 4, L.m + off, bytes, bar + 3 + s);
+        bulk_g2s(dst + ACH * 8, L.v + off, bytes, bar + 3 + s);
+        bulk_g2s(dst + ACH * 12, L.vmax + off, bytes, bar + 3 + s);
     };
     uint32_t par_w1 = 0;   // phase parity of bar[1] (one completion per row tile)
     const umma::Tile W2_hi = umma::make_tile(smem + REG3, 64, 128), W2_lo = umma::make_tile(smem + REG3 + 16384, 64, 128);
@@ -633,6 +653,11 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             umma::fence_async_smem();   // the arena was written through the generic proxy, the next W1 copy is a TMA write
             __syncthreads();            // the arena is free: the next tile's W1 copy / the gradient staging may overwrite it
         }
+        // regions 3 (W2 / W2^T, whose generic writes were fenced when W2^T was built) and 1 (the arena's first half) are
+        // free: AdamW's first chunks load during the gradient staging.
+        // Issuing them under the last tile's weight-gradient products instead made the kernel slower.
+        if (a.adam_tma && tid == 0)
+            for (int k = 0; k < ARING && k < nch; k++) adam_issue(k);
 
         TC_STAMP(8);
         // ================= AdamW ==========
@@ -681,10 +706,11 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 if (h == 0 && t4 == 0) gs_b2[j] = gb2[2 * p];
             }
             __syncthreads();
-            // 2) AdamW over the flat parameter vector, all 256 threads, fully coalesced 16-byte accesses.  The sweep is bound by
-            //    L2 round trips, not bytes: W1 | W2 are walked as ONE flat list of 16-byte groups (no 4-lane tail passes per W1
-            //    row) in batches of two groups per thread whose 8 loads are issued before the first use, and the loads of the
-            //    small vectors (b1 | b2 | W3 | b3, one parameter per thread) are in flight across the whole sweep.
+            TC_STAMP(7);
+            // 2) AdamW over the flat parameter vector, all 256 threads.  The sweep is bound by L2 round trips, not bytes: W1 | b1 |
+            //    W2 arrive by TMA in chunks of ACH parameters through an ARING-slot ring in regions 3 and 1, up to 128 KB of
+            //    loads in flight and no thread holding load registers.  The loads of the small vectors (b1 | b2 | W3 | b3,
+            //    one parameter per thread) are in flight across the whole sweep.
             const float2 sc = L.scal[round];
             AdamScalarsTc hs;
             hs.decay = a.decay; hs.omb1 = a.omb1; hs.beta2 = a.beta2; hs.omb2 = a.omb2; hs.eps = a.eps;
@@ -707,58 +733,50 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 L.out_mae[round] = e / (float)a.B;   // reported "loss": mean |q - y|
             }
             if (si >= 0) { sw = __ldcg(L.w + si); sm = __ldcg(L.m + si); sv2 = __ldcg(L.v + si); sx = __ldcg(L.vmax + si); }
-            const bool vecD = ((d.D & 3) == 0) && ((d.oW2 & 3) == 0);
-            if (vecD) {
-                constexpr int U = 2;
-                const int D4 = d.D >> 2, n1 = HID * D4, ntot = n1 + HID * HID / 4;
-                for (int q0 = tid; q0 < ntot; q0 += U * NTH) {
-                    float4 w4[U], m4[U], v4[U], x4[U];
-#pragma unroll
-                    for (int u = 0; u < U; u++) {
-                        const int q = q0 + u * NTH;
-                        if (q < ntot) {
-                            const int i = q < n1 ? d.oW1 + q * 4 : d.oW2 + (q - n1) * 4;   // W1 rows are contiguous: row * D + c4 * 4 == q * 4
-                            w4[u] = __ldcg(reinterpret_cast<const float4 *>(L.w + i)); m4[u] = __ldcg(reinterpret_cast<const float4 *>(L.m + i));
-                            v4[u] = __ldcg(reinterpret_cast<const float4 *>(L.v + i)); x4[u] = __ldcg(reinterpret_cast<const float4 *>(L.vmax + i));
+            if (a.adam_tma) {
+                // one 16-byte group of chunk k per thread: w | m | v | vmax from the chunk's ring slot (TMA), the gradient from
+                // the staging, the results to global memory with 16-byte stores; b1's groups ride along and are left to the tail
+                const int n1 = HID * d.D;
+                for (int k = 0; k < nch; k++) {
+                    const int s = k % ARING, uses = (nch - 1 - s) / ARING + 1;
+                    umma::mbar_wait(bar + 3 + s, (uint32_t)(round * uses + k / ARING) & 1u);
+                    const int i = k * ACH + 4 * tid;
+                    if (i < an && (i < n1 || i >= d.oW2)) {
+                        const float4 *sl = reinterpret_cast<const float4 *>(aslot(s)) + tid;
+                        float4 w = sl[0], mm = sl[ACH / 4], vv = sl[ACH / 2], xx = sl[3 * ACH / 4];
+                        const bool is_w1 = i < n1;
+                        int row, c;
+                        const float *gp;
+                        if (is_w1) {
+                            row = i / d.D; c = i - row * d.D;
+                            gp = gs_w1 + row * pitch1 + c;
+                        } else {
+                            const int e = i - d.oW2;
+                            row = e >> 6; c = e & 63;
+                            gp = gs_w2 + row * 65 + c;
+                        }
+                        w.x = adam_math(w.x, mm.x, vv.x, xx.x, gp[0], hs); w.y = adam_math(w.y, mm.y, vv.y, xx.y, gp[1], hs);
+                        w.z = adam_math(w.z, mm.z, vv.z, xx.z, gp[2], hs); w.w = adam_math(w.w, mm.w, vv.w, xx.w, gp[3], hs);
+                        *reinterpret_cast<float4 *>(L.w + i) = w; *reinterpret_cast<float4 *>(L.m + i) = mm;
+                        *reinterpret_cast<float4 *>(L.v + i) = vv; *reinterpret_cast<float4 *>(L.vmax + i) = xx;
+                        // the same values in the operand-layout tiles (hi = the value, lo = residual)
+                        if (is_w1) {
+                            if (c < d.obs) {
+                                const int ti = umma::tile_index(row, c, k1);
+                                *reinterpret_cast<float4 *>(To().w1hi + ti) = w;
+                                *reinterpret_cast<float4 *>(To().w1lo + ti) = make_float4(tf32_lo(w.x), tf32_lo(w.y), tf32_lo(w.z), tf32_lo(w.w));
+                            }
+                        } else {   // kperm order: columns c, c + 2 and c + 1, c + 3 are neighbours
+                            const int te = umma::tile_index(row, umma::kperm(c), HID), to = umma::tile_index(row, umma::kperm(c + 1), HID);
+                            *reinterpret_cast<float2 *>(To().w2 + te) = make_float2(w.x, w.z);
+                            *reinterpret_cast<float2 *>(To().w2 + to) = make_float2(w.y, w.w);
+                            *reinterpret_cast<float2 *>(To().w2 + 4096 + te) = make_float2(tf32_lo(w.x), tf32_lo(w.z));
+                            *reinterpret_cast<float2 *>(To().w2 + 4096 + to) = make_float2(tf32_lo(w.y), tf32_lo(w.w));
                         }
                     }
-#pragma unroll
-                    for (int u = 0; u < U; u++) {
-                        const int q = q0 + u * NTH;
-                        if (q < ntot) {
-                            const bool is_w1 = q < n1;
-                            int i, row, c;
-                            const float *gp;
-                            if (is_w1) {
-                                row = q / D4; c = (q - row * D4) * 4;
-                                i = d.oW1 + q * 4;
-                                gp = gs_w1 + row * pitch1 + c;
-                            } else {
-                                const int q4 = q - n1;
-                                row = q4 >> 4; c = (q4 & 15) * 4;
-                                i = d.oW2 + q4 * 4;
-                                gp = gs_w2 + row * 65 + c;
-                            }
-                            float4 w = w4[u], mm = m4[u], vv = v4[u], xx = x4[u];
-                            w.x = adam_math(w.x, mm.x, vv.x, xx.x, gp[0], hs); w.y = adam_math(w.y, mm.y, vv.y, xx.y, gp[1], hs);
-                            w.z = adam_math(w.z, mm.z, vv.z, xx.z, gp[2], hs); w.w = adam_math(w.w, mm.w, vv.w, xx.w, gp[3], hs);
-                            *reinterpret_cast<float4 *>(L.w + i) = w; *reinterpret_cast<float4 *>(L.m + i) = mm;
-                            *reinterpret_cast<float4 *>(L.v + i) = vv; *reinterpret_cast<float4 *>(L.vmax + i) = xx;
-                            // the same values in the operand-layout tiles (hi = the value, lo = residual)
-                            if (is_w1) {
-                                if (c < d.obs) {
-                                    const int ti = umma::tile_index(row, c, k1);
-                                    *reinterpret_cast<float4 *>(To().w1hi + ti) = w;
-                                    *reinterpret_cast<float4 *>(To().w1lo + ti) = make_float4(tf32_lo(w.x), tf32_lo(w.y), tf32_lo(w.z), tf32_lo(w.w));
-                                }
-                            } else {   // kperm order: columns c, c + 2 and c + 1, c + 3 are neighbours
-                                const int te = umma::tile_index(row, umma::kperm(c), HID), to = umma::tile_index(row, umma::kperm(c + 1), HID);
-                                *reinterpret_cast<float2 *>(To().w2 + te) = make_float2(w.x, w.z);
-                                *reinterpret_cast<float2 *>(To().w2 + to) = make_float2(w.y, w.w);
-                                *reinterpret_cast<float2 *>(To().w2 + 4096 + te) = make_float2(tf32_lo(w.x), tf32_lo(w.z));
-                                *reinterpret_cast<float2 *>(To().w2 + 4096 + to) = make_float2(tf32_lo(w.y), tf32_lo(w.w));
-                            }
-                        }
+                    if (k + ARING < nch) {   // every thread is done with slot s: refill it with chunk k + ARING
+                        __syncthreads();
+                        if (tid == 0) adam_issue(k + ARING);
                     }
                 }
             } else {
@@ -776,9 +794,10 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                     L.m[i] = mm; L.v[i] = vv; L.vmax[i] = xx;
                 }
                 __syncthreads();
-                rebuild_tiles(L.w, d, To(), tid);         // unaligned shapes (D % 4 != 0): tiles from the flat vector
+                rebuild_tiles(L.w, d, To(), tid);         // D % 4 != 0 or unaligned parameters: tiles from the flat vector
             }
-            fence_proxy_async_all();                    // the tile writes are read by TMA in the next round
+            TC_STAMP(10);
+            fence_proxy_async_all();                    // the tile writes and W1 | W2 are read by TMA in the next round
             if (si >= 0) {
                 L.w[si] = adam_math(sw, sm, sv2, sx, sg, hs);
                 L.m[si] = sm; L.v[si] = sv2; L.vmax[si] = sx;
@@ -847,6 +866,9 @@ extern "C" int prl_dqn_learn_multi(prl_dqn *const *dqns, prl_buf *const *bufs, i
     }
     PRL_CUDA(cudaEventSynchronize(h_done));
     size_t samp_smem = 0;
+    // AdamW streams the flat parameters and moments by TMA bulk copies (16-byte granules): every group of 4 parameters
+    // must stay inside one of W1 / b1 / W2 and every pointer must be 16-byte aligned, else the scalar sweep runs
+    bool adam_tma = ((c.obs_dim + c.n_actions) & 3) == 0;
     for (int i = 0; i < count; i++) {
         prl_dqn *q = dqns[i];
         prl_buf *b = bufs[i];
@@ -881,6 +903,7 @@ extern "C" int prl_dqn_learn_multi(prl_dqn *const *dqns, prl_buf *const *bufs, i
         L.records = b->records; L.slots = q->slots;
         L.tiles = q->tc_tiles;
         L.w = q->w; L.wt = q->wt; L.m = q->m; L.v = q->v; L.vmax = q->vmax;
+        adam_tma = adam_tma && (((uintptr_t)q->w | (uintptr_t)q->m | (uintptr_t)q->v | (uintptr_t)q->vmax) & 15) == 0;
         L.scal = shared_scal ? q0->scal_dev : q->scal_dev;
         L.out_mae = out_mae[i]; L.out_q = out_q ? out_q[i] : nullptr; L.out_y = out_y ? out_y[i] : nullptr;
         L.steps0 = training_steps0[i];
@@ -909,6 +932,7 @@ extern "C" int prl_dqn_learn_multi(prl_dqn *const *dqns, prl_buf *const *bufs, i
     a.tau = (float)c.tau;
     a.omtau = (float)(1.0 - c.tau);
     a.inv_b2 = 2.0f / (float)batch;
+    a.adam_tma = adam_tma ? 1 : 0;
     a.prof = q0->prof;
     { static const int c = [] { const char *e = getenv("PRL_TC_PROF_CTA"); return e ? atoi(e) : 0; }(); a.prof_cta = c; }
     const size_t smem = MISC_OFF + sizeof(Misc);

@@ -39,13 +39,14 @@ grp.learn()
 torch.cuda.synchronize()
 s = st.cpu()[4:].double()
 # stamps written by k_dqn_tc: 0 round start, 1 row scalars + soft update done, 2 target tiles loaded, 3 phase T done,
-# 4 online tiles + W2^T ready, 5 tile 0 layer 1 done, 6 tile 0 forward / dZ2 / dH1 done, 8 weight gradients done, 9 AdamW done
-names = ["row scalars + soft upd", "load target weights", "phase T (layer 1 + all actions)", "load online weights + W2^T",
-         "tile 0: online layer 1", "tile 0: fwd L2 + dZ2 + dH1", None, "rest (weight grads, other tiles)", "AdamW"]
+# 4 online tiles + W2^T ready, 5 tile 0 layer 1 done, 6 tile 0 forward / dZ2 / dH1 done, 8 weight gradients done,
+# 7 gradients staged in shared memory, 10 AdamW sweep over W1 | b1 | W2 done, 9 small-parameter tail done (round end)
+phases = [("row scalars + soft upd", 0, 1), ("load target weights", 1, 2), ("phase T (layer 1 + all actions)", 2, 3),
+          ("load online weights + W2^T", 3, 4), ("tile 0: online layer 1", 4, 5), ("tile 0: fwd L2 + dZ2 + dH1", 5, 6),
+          ("rest (weight grads, other tiles)", 6, 8), ("AdamW: gradient staging", 8, 7), ("AdamW: sweep", 7, 10),
+          ("AdamW: small-parameter tail", 10, 9)]
 tot = (s[1:, 0] - s[:-1, 0]).mean()
 print(f"{tot:.0f} clk/round (CTA {os.environ.get('PRL_TC_PROF_CTA', '0')} with {R} learners resident)")
-for i, n in enumerate(names):
-    if n is not None:
-        j = 8 if i == 7 else i + 1      # stamp 7 is not written: "rest" runs from stamp 6 to stamp 8
-        k = 6 if i == 7 else i
-        print(f"  {n:36s} {(s[:, j]-s[:, k]).mean():10.0f} clk")
+for n, k, j in phases:
+    print(f"  {n:36s} {(s[:, j]-s[:, k]).mean():10.0f} clk")
+print(f"  {'AdamW (total)':36s} {(s[:, 9]-s[:, 8]).mean():10.0f} clk")

@@ -24,12 +24,13 @@ L.set_kernel_timing(True)
 L.learn(b)
 ms = L.last_kernel_ms()
 s = st.cpu()[4:].double()
-names = ["row scalars + soft upd", "load target weights", "target layer 1 (2 tiles)", "all-actions (32 tiles)", "load online weights",
-         "online layer 1", "tile0: fwd L2 + dZ2 + dH1", "rest (weight grads t0, tile1 all)", "AdamW"]
+# stamps written by k_dqn_tc (see tools/tc_bench.py): AdamW is split into gradient staging (8 -> 7), the sweep over
+# W1 | b1 | W2 (7 -> 10) and the small-parameter tail (10 -> 9)
+phases = [("row scalars + soft upd", 0, 1), ("load target weights", 1, 2), ("phase T (layer 1 + all actions)", 2, 3),
+          ("load online weights + W2^T", 3, 4), ("tile 0: online layer 1", 4, 5), ("tile 0: fwd L2 + dZ2 + dH1", 5, 6),
+          ("rest (weight grads, other tiles)", 6, 8), ("AdamW: gradient staging", 8, 7), ("AdamW: sweep", 7, 10),
+          ("AdamW: small-parameter tail", 10, 9)]
 tot = (s[1:, 0] - s[:-1, 0]).mean()
 print(f"kernel {ms*1e3/rounds:.1f} us/round; {tot:.0f} clk/round")
-for i, n in enumerate(names):
-    print(f"  {n:36s} {(s[:, i+1]-s[:, i]).mean():10.0f} clk")
-
-print("online layer 1, group 0, chunk 1: loads+split+tmem st %.0f | fence+sync %.0f | issue %.0f | wait %.0f | (chunk0 total %.0f) | tail-to-barrier %.0f" % (
-    (s[:, 11]-s[:, 10]).mean(), (s[:, 12]-s[:, 11]).mean(), (s[:, 13]-s[:, 12]).mean(), (s[:, 14]-s[:, 13]).mean(), (s[:, 10]-s[:, 5]).mean(), (s[:, 6]-s[:, 15]).mean()))
+for n, k, j in phases:
+    print(f"  {n:36s} {(s[:, j]-s[:, k]).mean():10.0f} clk")
