@@ -474,6 +474,40 @@ int prl_td3_learn(prl_td3 *td3, prl_buf *buf, int rounds, int batch, int64_t tra
                   float *out_actor_loss_dev, float *out_critic_loss_dev, int32_t *out_logical_dev, void *stream);
 int prl_td3_set_graph(prl_td3 *td3, int enable);
 int64_t prl_td3_last_launches(const prl_td3 *td3);
+/* Rounds captured as CUDA graphs so far.  Ring and dense-batch rounds, with and without the actor update, are kept
+ * side by side: alternating learn and learn_batch captures nothing after the first of each. */
+int64_t prl_td3_graph_captures(const prl_td3 *td3);
+/* One round on the caller's dense batch: TD3.learn_batch (td3.py:106-147) / ActorCriticBase.learn_batch
+ * (actor_critic_base.py:309-366), as PearlAgent.learn_batch and offline_learning() call it
+ * (offline_learning_and_evaluation.py:217-224).  training_steps = learner._training_steps as it is (learn_batch does not
+ * advance it): the actor and target updates run when training_steps % actor_update_freq == 0.
+ * state / next_state: device f32[batch][obs]; action: f32[batch][A]; reward: f32[batch]; terminated: u8[batch];
+ * noise_dev: f32[1][batch][A] (null: DDPG); out_*_loss: device f32[1]. */
+int prl_td3_learn_batch(prl_td3 *td3, int batch, const float *state, const float *action, const float *reward,
+                        const float *next_state, const uint8_t *terminated, int64_t training_steps, const float *noise_dev,
+                        float *out_actor_loss_dev, float *out_critic_loss_dev, void *stream);
+/* The loss a round without an actor update reports: TD3's _last_actor_loss (td3.py:104,122).  A handle starts at 0; a
+ * handle re-created mid-training (a learning-rate change, a larger batch) is seeded with the learner's value. */
+int prl_td3_set_last_actor_loss(prl_td3 *td3, float value);
+
+/* ---- TD3BC (offline TD3 with a behaviour-cloning actor term) -------------------------------------
+ * Replaces TD3BC._actor_loss (policy_learners/sequential_decision_making/td3.py:298-318) inside the TD3 round above:
+ *   a = sample_action(s) (tanh, scaled to the box), q = Q1(s, a), b = behavior_policy(s) under no_grad,
+ *   lambda = alpha_bc / mean|q| (detached), loss = mean((a - b)^2) - lambda mean(q).
+ * behavior_policy is a VanillaContinuousActorNetwork called through forward(): b is the raw tanh output in [-1, 1], not
+ * scaled to the box (actor_networks.py:472-473).  Behaviour weights: device f32, flat W1[h1][obs] b1 W2[h2][h1] b2
+ * W3[A][h2] b3, read by every round (not copied).  The handle is a prl_td3: destroy, step counts, set_graph, learn,
+ * learn_batch and the setters above apply to it. */
+typedef struct prl_td3bc_cfg {
+    int32_t behavior_h1, behavior_h2;
+} prl_td3bc_cfg;
+int64_t prl_td3bc_workspace_bytes(const prl_td3_cfg *cfg, const prl_td3bc_cfg *bc);
+int prl_td3bc_create(prl_td3 **out, const prl_td3_cfg *cfg, const prl_td3bc_cfg *bc, const float *behavior_w, float *actor_w,
+                     float *actor_m, float *actor_v, float *actor_vmax, float *actor_target_w, float *critic_w,
+                     float *critic_m, float *critic_v, float *critic_vmax, float *critic_target_w, const float *low_dev,
+                     const float *high_dev, int64_t actor_adam_step, int64_t critic_adam_step, void *workspace);
+/* TD3BC.alpha_bc (td3.py:295), read by the next call; TD3BC handles only */
+int prl_td3_set_alpha_bc(prl_td3 *td3, double alpha_bc);
 
 /* ---- Implicit Q-Learning (offline actor-critic) ----------------------------------------------------
  * Replaces ImplicitQLearning.learn_batch (policy_learners/sequential_decision_making/implicit_q_learning.py:159-302),

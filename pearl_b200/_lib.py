@@ -58,6 +58,10 @@ class Td3Cfg(C.Structure):
                 ("actor_tau", C.c_double), ("critic_tau", C.c_double), ("noise_clip", C.c_double)]
 
 
+class Td3bcCfg(C.Structure):
+    _fields_ = [("behavior_h1", C.c_int32), ("behavior_h2", C.c_int32)]
+
+
 class IqlCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("act_dim", C.c_int32), ("actor_h1", C.c_int32),
                 ("actor_h2", C.c_int32), ("critic_h1", C.c_int32), ("critic_h2", C.c_int32), ("value_h1", C.c_int32),
@@ -203,6 +207,12 @@ _SIGNATURES = {
     "prl_td3_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, _P, _P, _P, _P, _P]),
     "prl_td3_set_graph": (C.c_int, [_P, C.c_int]),
     "prl_td3_last_launches": (C.c_int64, [_P]),
+    "prl_td3_graph_captures": (C.c_int64, [_P]),
+    "prl_td3_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 5 + [C.c_int64] + [_P] * 4),
+    "prl_td3_set_last_actor_loss": (C.c_int, [_P, C.c_float]),
+    "prl_td3bc_workspace_bytes": (C.c_int64, [C.POINTER(Td3Cfg), C.POINTER(Td3bcCfg)]),
+    "prl_td3bc_create": (C.c_int, [C.POINTER(_P), C.POINTER(Td3Cfg), C.POINTER(Td3bcCfg)] + [_P] * 13 + [C.c_int64, C.c_int64, _P]),
+    "prl_td3_set_alpha_bc": (C.c_int, [_P, C.c_double]),
     "prl_iql_actor_param_count": (C.c_int64, [C.POINTER(IqlCfg)]),
     "prl_iql_critic_param_count": (C.c_int64, [C.POINTER(IqlCfg)]),
     "prl_iql_value_param_count": (C.c_int64, [C.POINTER(IqlCfg)]),

@@ -4,7 +4,8 @@
     B200SoftActorCritic             (SoftActorCritic, soft_actor_critic.py: discrete actions)
     B200ProximalPolicyOptimization  (ProximalPolicyOptimization, ppo.py:96-293)
     B200REINFORCE                   (REINFORCE, reinforce.py: use_critic=True)
-    B200TD3 / B200DeepDeterministicPolicyGradient  (td3.py:43-202, ddpg.py:41-157)
+    B200TD3 / B200DeepDeterministicPolicyGradient  (td3.py:43-202, ddpg.py:41-157; learn_batch runs on the GPU too)
+    B200TD3BC                       (TD3BC, td3.py:241-343: offline TD3 with a behaviour-cloning actor term; learn_batch too)
     B200ImplicitQLearning           (ImplicitQLearning, implicit_q_learning.py: offline RL; learn_batch runs on the GPU too)
     B200QuantileRegressionDeepQLearning  (QuantileRegressionDeepQLearning, QR-DQN; not an actor-critic, but bound the same
                                     way: `_Q`, `_Q_target` and the optimizer state are views; learn_batch runs on the GPU too)
@@ -35,6 +36,7 @@ from .sac import B200ContinuousSoftActorCritic as SacCore
 from .sac_discrete import B200SoftActorCritic as SacdCore
 from .td3 import B200DeepDeterministicPolicyGradient as DdpgCore
 from .td3 import B200TD3 as Td3Core
+from .td3 import B200TD3BC as Td3bcCore
 
 try:  # pragma: no cover - depends on the environment
     from pearl.policy_learners.sequential_decision_making.ddpg import DeepDeterministicPolicyGradient as _RefDDPG
@@ -55,6 +57,13 @@ try:  # pragma: no cover - depends on the environment; kept apart so the classes
     HAVE_REFERENCE_IQL = True
 except Exception:
     HAVE_REFERENCE_IQL = False
+
+try:  # pragma: no cover - depends on the environment; kept apart so the classes above do not depend on it
+    from pearl.policy_learners.sequential_decision_making.td3 import TD3BC as _RefTD3BC
+
+    HAVE_REFERENCE_TD3BC = True
+except Exception:
+    HAVE_REFERENCE_TD3BC = False
 
 try:  # pragma: no cover - depends on the environment; kept apart so the classes above do not depend on it
     from pearl.policy_learners.sequential_decision_making.reinforce import REINFORCE as _RefREINFORCE
@@ -473,6 +482,27 @@ if HAVE_REFERENCE:
                 core._handle = C.c_void_p(0)
             core._adam_steps = (int(steps[0]), int(steps[1]))
 
+        def _bind_extras(self, core):
+            """The reference's `_last_actor_loss` (TD3) is what the core's rounds without an actor update report."""
+            if hasattr(self, "_last_actor_loss") and float(self._last_actor_loss) != core._last_actor_loss:
+                core.set_last_actor_loss(float(self._last_actor_loss))
+
+        def _after_learn(self, core):
+            if hasattr(self, "_last_actor_loss"):
+                self._last_actor_loss = core._last_actor_loss
+
+        def learn_batch(self, batch) -> dict:
+            """TD3.learn_batch / ActorCriticBase.learn_batch on the GPU: one round on a caller-supplied batch (continuous
+            actions), as PearlAgent.learn_batch and offline_learning() call it.  Like the reference it does not advance the
+            training-step count, so the actor and target updates follow `_training_steps % actor_update_freq`."""
+            core = self._ensure_core()
+            core._training_steps = int(self._training_steps)
+            report = core.learn_batch(batch)
+            for (opt, _, _), step in zip(self._optimizer_triples(core), self._core_steps(core)):
+                _set_steps(opt, step)
+            self._after_learn(core)
+            return report
+
     class B200TD3(_DeterministicMixin, _RefTD3):
         """Drop-in for `pearl...td3.TD3`."""
 
@@ -490,6 +520,40 @@ else:
     B200ProximalPolicyOptimization = PpoCore
     B200TD3 = Td3Core
     B200DeepDeterministicPolicyGradient = DdpgCore
+
+if HAVE_REFERENCE and HAVE_REFERENCE_TD3BC:
+
+    class B200TD3BC(_DeterministicMixin, _RefTD3BC):
+        """Drop-in for `pearl...td3.TD3BC`.  `behavior_policy` must be a VanillaContinuousActorNetwork with two hidden layers
+        over the learner's state and action dimensions.  Its parameters are copied into the CUDA learner on every call (not
+        re-pointed: the behaviour network is often another agent's actor), and `alpha_bc` is read on every call."""
+        _core_cls = Td3bcCore
+
+        def _core_kwargs(self):
+            bp = self._behavior_policy
+            if type(bp).__name__ != "VanillaContinuousActorNetwork" or len(_shapes(bp)) != 6:
+                raise NotImplementedError("the CUDA TD3BC learner is built for a behavior_policy that is a VanillaContinuousActorNetwork "
+                                          f"with two hidden layers (got {type(bp).__name__} with {len(_shapes(bp))} parameter tensors)")
+            obs, b1, b2, act = _mlp3(_shapes(bp), "behavior_policy")
+            a_obs, _, _, a_act = _mlp3(_shapes(self._actor), "actor")
+            if (obs, act) != (a_obs, a_act):
+                raise NotImplementedError(f"behavior_policy maps {obs} state features to {act} actions; the learner has "
+                                          f"{a_obs} and {a_act}")
+            return dict(actor_update_freq=int(self._actor_update_freq), actor_update_noise=float(self._actor_update_noise),
+                        actor_update_noise_clip=float(self._actor_update_noise_clip), behavior_hidden_dims=[b1, b2],
+                        alpha_bc=float(self.alpha_bc))
+
+        def _bind_extras(self, core):
+            super()._bind_extras(core)
+            core.alpha_bc = float(self.alpha_bc)
+            flat, off = core.behavior_params, 0
+            for p in self._behavior_policy.parameters():
+                n = p.numel()
+                flat[off:off + n].copy_(p.detach().reshape(-1))
+                off += n
+
+else:
+    B200TD3BC = Td3bcCore
 
 
 def _iql_core_kwargs(pl) -> dict:

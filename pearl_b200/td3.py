@@ -3,7 +3,10 @@
 actor_critic_base.py:309-366) on a B200: `learn(replay_buffer)` runs `training_rounds` x (sample -> [delayed] actor step ->
 twin-critic step -> [delayed] soft target updates) on the GPU through `prl_td3_learn` (include/pearl_b200.h).  Same constructor
 argument names and the same report keys (`actor_loss`, `critic_loss`) as the reference.  PyTorch holds the flat parameter
-vectors and draws the target-policy noise (the reference's `torch.normal`); no math happens in Python.  No CPU fallback."""
+vectors and draws the target-policy noise (the reference's `torch.normal`); no math happens in Python.  No CPU fallback.
+`learn_batch(batch)` runs one round on a caller-supplied batch (`prl_td3_learn_batch`), as PearlAgent.learn_batch and
+offline_learning() call it.  B200TD3BC is Pearl's TD3BC (td3.py:241-318): the same round with a behaviour-cloning term in
+the actor loss."""
 from __future__ import annotations
 
 import ctypes as C
@@ -46,6 +49,7 @@ class B200TD3:
         self._actor_update_noise_clip = float(self._default_clip if actor_update_noise_clip is None else actor_update_noise_clip)
         self._max_rounds = max(int(max_rounds_per_call), 1)
         self._training_steps = 0
+        self._last_actor_loss = 0.0    # what rounds without an actor update report (td3.py:104,122)
         self.use_cuda_graph = True
         self._handle = C.c_void_p(0)
         self._bound_batch = 0
@@ -127,16 +131,54 @@ class B200TD3:
             self._lib.prl_td3_destroy(self._handle)
             self._handle = C.c_void_p(0)
         cfg = self._cfg(max(need_batch, self._batch_size if self._batch_size > 0 else need_batch))
-        self._workspace = torch.empty(int(self._lib.prl_td3_workspace_bytes(C.byref(cfg))), dtype=torch.uint8, device=self._device)
+        self._workspace = torch.empty(self._workspace_bytes(cfg), dtype=torch.uint8, device=self._device)
         h = C.c_void_p(0)
         p = _lib.ptr
+        args = (p(self.actor_params), p(self._actor_state[0]), p(self._actor_state[1]), p(self._actor_state[2]), p(self.actor_target_params),
+                p(self.critic_params), p(self._critic_state[0]), p(self._critic_state[1]), p(self._critic_state[2]),
+                p(self.critic_target_params), p(self._low), p(self._high), self._adam_steps[0], self._adam_steps[1], p(self._workspace))
         with torch.cuda.device(self._device):
-            _lib.check(self._lib.prl_td3_create(
-                C.byref(h), C.byref(cfg), p(self.actor_params), p(self._actor_state[0]), p(self._actor_state[1]), p(self._actor_state[2]),
-                p(self.actor_target_params), p(self.critic_params), p(self._critic_state[0]), p(self._critic_state[1]),
-                p(self._critic_state[2]), p(self.critic_target_params), p(self._low), p(self._high), self._adam_steps[0],
-                self._adam_steps[1], p(self._workspace)))
+            _lib.check(self._create(h, cfg, args))
+            # a handle re-created mid-training reports the learner's last actor loss, not 0, until its next actor update
+            _lib.check(self._lib.prl_td3_set_last_actor_loss(h, float(self._last_actor_loss)))
         self._handle, self._bound_batch = h, cfg.max_batch
+
+    def _workspace_bytes(self, cfg) -> int:
+        return int(self._lib.prl_td3_workspace_bytes(C.byref(cfg)))
+
+    def _create(self, h, cfg, args) -> int:
+        return self._lib.prl_td3_create(C.byref(h), C.byref(cfg), *args)
+
+    def set_learning_rates(self, actor_lr: float, critic_lr: float) -> None:
+        """New AdamW learning rates: the handle is re-created with them at the current step counts (parameters, moments and
+        the last actor loss live outside it)."""
+        if self._handle.value:
+            self._adam_steps = (int(self._lib.prl_td3_actor_adam_step(self._handle)), int(self._lib.prl_td3_critic_adam_step(self._handle)))
+            self._lib.prl_td3_destroy(self._handle)
+            self._handle = C.c_void_p(0)
+        self._actor_learning_rate, self._critic_learning_rate = float(actor_lr), float(critic_lr)
+
+    def set_last_actor_loss(self, value: float) -> None:
+        """The actor loss that rounds without an actor update report (the reference's `_last_actor_loss`)."""
+        self._last_actor_loss = float(value)
+        if self._handle.value:
+            with torch.cuda.device(self._device):
+                _lib.check(self._lib.prl_td3_set_last_actor_loss(self._handle, self._last_actor_loss))
+
+    def _before_call(self) -> None:
+        pass
+
+    def _noise(self, noise: Optional[torch.Tensor], r: int, B: int, start: int = 0) -> Optional[torch.Tensor]:
+        """[r, B, A] target-policy noise: rows start.. of `noise`, or torch.normal(0, actor_update_noise) draws (td3.py:155-160)."""
+        if self._actor_update_noise <= 0.0:
+            return None
+        A, dev = self._action_dim, self._device
+        if noise is not None:
+            nz = noise[start:start + r].to(device=dev, dtype=torch.float32).contiguous()
+            if tuple(nz.shape) != (r, B, A):
+                raise ValueError(f"noise must be [rounds, {B}, {A}]")
+            return nz
+        return torch.randn((r, B, A), dtype=torch.float32, device=dev, generator=self._gen) * self._actor_update_noise
 
     # ------------------------------------------------------------------ PolicyLearner.learn (policy_learner.py:162-204)
     def learn(self, replay_buffer: B200ReplayBuffer, noise: Optional[torch.Tensor] = None, trace: Optional[dict] = None) -> dict:
@@ -148,20 +190,14 @@ class B200TD3:
             raise ValueError("TD3 / DDPG need a replay buffer with is_action_continuous=True")
         B = len(replay_buffer) if (self._batch_size == -1 or len(replay_buffer) < self._batch_size) else self._batch_size
         self._bind(B)
-        R, A, dev = self._training_rounds, self._action_dim, self._device
+        self._before_call()
+        R, dev = self._training_rounds, self._device
         report = {"actor_loss": [], "critic_loss": []}
         idx_all = []
         done = 0
         while done < R:
             r = min(self._max_rounds, R - done)
-            nz = None
-            if self._actor_update_noise > 0.0:
-                if noise is not None:
-                    nz = noise[done:done + r].to(device=dev, dtype=torch.float32).contiguous()
-                    if tuple(nz.shape) != (r, B, A):
-                        raise ValueError(f"noise must be [rounds, {B}, {A}]")
-                else:       # torch.normal(mean=0, std=actor_update_noise, size=next_action.size())   (td3.py:155-160)
-                    nz = torch.randn((r, B, A), dtype=torch.float32, device=dev, generator=self._gen) * self._actor_update_noise
+            nz = self._noise(noise, r, B, done)
             out = torch.empty((2, r), dtype=torch.float32, device=dev)
             idx = torch.empty((r, B), dtype=torch.int32, device=dev) if trace is not None else None
             replay_buffer._rng_push()
@@ -180,7 +216,42 @@ class B200TD3:
             done += r
         if trace is not None:
             trace["idx"] = torch.cat(idx_all)
+        self._last_actor_loss = float(report["actor_loss"][-1])
         return report
+
+    # ------------------------------------------------------------------ TD3.learn_batch (td3.py:106-147)
+    def learn_batch(self, batch, noise: Optional[torch.Tensor] = None) -> dict:
+        """One round on a caller-supplied batch (state, action, reward, next_state, terminated; CPU or GPU tensors,
+        `terminated` bool or uint8).  Like the reference it does not advance the training-step count: the actor and the
+        targets are updated when `_training_steps % actor_update_freq == 0`.  `noise`: [B, A] or [1, B, A] target-policy
+        noise draws, else drawn from the learner's generator."""
+        B, dev = int(batch.state.shape[0]), self._device
+        if batch.state.dim() != 2 or int(batch.state.shape[1]) != self._state_dim:
+            raise ValueError(f"batch.state must be [B, {self._state_dim}], got {tuple(batch.state.shape)}")
+        f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
+        act = f32(batch.action)
+        if act.dim() != 2 or tuple(act.shape) != (B, self._action_dim):
+            raise ValueError(f"batch.action must be [{B}, {self._action_dim}] continuous actions, got {tuple(batch.action.shape)}")
+        if tuple(batch.next_state.shape) != tuple(batch.state.shape):
+            raise ValueError(f"batch.next_state must be [B, {self._state_dim}], got {tuple(batch.next_state.shape)}")
+        state, next_state, reward = f32(batch.state), f32(batch.next_state), f32(batch.reward.reshape(B))
+        term = batch.terminated.reshape(B).to(device=dev, dtype=torch.uint8).contiguous()
+        self._bind(B)
+        self._before_call()
+        nz = self._noise(None if noise is None else noise.reshape(1, *noise.shape[-2:]), 1, B)
+        out = torch.empty((2, 1), dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(self._lib.prl_td3_set_graph(self._handle, int(self.use_cuda_graph)))
+            _lib.check(self._lib.prl_td3_learn_batch(self._handle, B, _lib.ptr(state), _lib.ptr(act), _lib.ptr(reward), _lib.ptr(next_state),
+                                                     _lib.ptr(term), int(self._training_steps), _lib.ptr(nz), _lib.ptr(out[0]),
+                                                     _lib.ptr(out[1]), _stream_ptr(dev)))
+        host = out.cpu()
+        self._last_actor_loss = float(host[0, 0])
+        return {"actor_loss": float(host[0, 0]), "critic_loss": float(host[1, 0])}
+
+    @property
+    def graph_captures(self) -> int:
+        return int(self._lib.prl_td3_graph_captures(self._handle)) if self._handle.value else 0
 
 
 class B200DeepDeterministicPolicyGradient(B200TD3):
@@ -192,3 +263,42 @@ class B200DeepDeterministicPolicyGradient(B200TD3):
             if kwargs.get(k) is not None:
                 raise TypeError(f"DeepDeterministicPolicyGradient has no `{k}` (use B200TD3)")
         super().__init__(*args, **kwargs)
+
+
+class B200TD3BC(B200TD3):
+    """TD3BC (td3.py:241-318): TD3 whose actor loss is mean((a - b)^2) - alpha_bc / mean|Q1(s, a)| * mean(Q1(s, a)), with
+    b = behavior_policy(s), a VanillaContinuousActorNetwork called through forward(): its raw tanh output, not scaled to
+    the box.  `behavior_params` holds the behaviour network's flat W1 b1 W2 b2 W3 b3; `behavior_hidden_dims` are its two
+    hidden widths (they may differ from the actor's).  `alpha_bc` is read on every call."""
+
+    def __init__(self, *args, behavior_hidden_dims: Optional[Iterable[int]] = None, alpha_bc: float = 2.5, **kwargs) -> None:
+        super().__init__(*args, **kwargs)
+        dims = list(behavior_hidden_dims if behavior_hidden_dims is not None else self._actor_hidden_dims)
+        if len(dims) != 2 or min(dims) <= 0:
+            raise NotImplementedError("the CUDA TD3BC learner is built for a behaviour network with two hidden layers")
+        self._behavior_hidden_dims = [int(d) for d in dims]
+        self.alpha_bc = float(alpha_bc)
+        O, A, (h1, h2) = self._state_dim, self._action_dim, self._behavior_hidden_dims
+        self.behavior_params = torch.zeros(h1 * O + h1 + h2 * h1 + h2 + A * h2 + A, dtype=torch.float32, device=self._device)
+
+    def _bc_cfg(self) -> _lib.Td3bcCfg:
+        return _lib.Td3bcCfg(*self._behavior_hidden_dims)
+
+    def _workspace_bytes(self, cfg) -> int:
+        return int(self._lib.prl_td3bc_workspace_bytes(C.byref(cfg), C.byref(self._bc_cfg())))
+
+    def _create(self, h, cfg, args) -> int:
+        return self._lib.prl_td3bc_create(C.byref(h), C.byref(cfg), C.byref(self._bc_cfg()), _lib.ptr(self.behavior_params), *args)
+
+    def _before_call(self) -> None:
+        with torch.cuda.device(self._device):
+            _lib.check(self._lib.prl_td3_set_alpha_bc(self._handle, float(self.alpha_bc)))
+
+    def load_parameters(self, actor, q1, q2, actor_target=None, q1_target=None, q2_target=None, behavior=None) -> None:
+        """As B200TD3.load_parameters; `behavior`: the behaviour network's flat parameters (parameters() order)."""
+        super().load_parameters(actor, q1, q2, actor_target, q1_target, q2_target)
+        if behavior is not None:
+            b = torch.as_tensor(behavior, dtype=torch.float32).reshape(-1)
+            if b.numel() != self.behavior_params.numel():
+                raise ValueError(f"behavior has {b.numel()} parameters, the behaviour network {self.behavior_params.numel()}")
+            self.behavior_params.copy_(b.to(self._device))
