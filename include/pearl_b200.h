@@ -721,6 +721,67 @@ int prl_duel_q_values(prl_duel *duel, int n, const float *state, const int32_t *
 int prl_duel_set_graph(prl_duel *duel, int enable);
 int64_t prl_duel_last_launches(const prl_duel *duel);
 
+/* ---- multi-head DQN / DoubleDQN (plain or conservative) ------------------------------------------
+ * Replaces VanillaQValueMultiHeadNetwork.get_q_values (neural_networks/sequential_decision_making/q_value_networks.py:
+ * 185-241), DeepTDLearning.forward / loss / learn_batch (policy_learners/sequential_decision_making/deep_td_learning.py:
+ * 269-360), DeepQLearning / DoubleDQN.get_next_state_values (deep_q_learning.py:130-167, double_dqn.py:29-57) and, when
+ * conservative, compute_cql_loss (utils/functional_utils/learning/loss_fn_utils.py:17-71), driven by PolicyLearner.learn
+ * (prl_mhq_learn: sample -> round, `rounds` times) or called on a caller's batch (prl_mhq_learn_batch: one round,
+ * PearlAgent.learn_batch / offline_learning).  The network maps a state to one Q value per action, Q(s) = W3 relu(W2
+ * relu(W1 s + b1) + b2) + b3; a query slot holding id k reads Q(s)[k] exactly (the reference's bmm with a one-hot slot).
+ * Per round:
+ *   when (training_steps + 1) % target_update_freq == 0, FIRST target = tau * online + (1 - tau) * target;
+ *   q_b = Q(s_b)[a_b]; y_b = V_b gamma (1 - terminated_b) + r_b with V_b = max over available next slots k of
+ *   Q'(s'_b)[id_k] (DQN) or Q'(s'_b)[id_k*], k* = first argmax over available next slots of Q(s'_b)[id_k] (DoubleDQN);
+ *   L = mean_b (q_b - y_b)^2, plus, when conservative, alpha cql with cql = mean_b logsumexp_k Q(s_b)[c_b[k]]
+ *   - (1 / (B A)) sum_b [(A - 1) Q(s_b)[c_b[0]] + Q(s_b)[c_b[1]]] (the reference gathers the current-slot values with the
+ *   ONE-HOT action, as prl_cql documents; c_b[k] are the current slots including padding, id 0, so padded slots add on
+ *   one head column); one AdamW(amsgrad) step.  Reported loss: mean_b |q_b - y_b| (the Bellman error only).
+ * 1 <= n_actions <= 255 (2 <= n_actions when conservative: A = 1 makes the reference's gather index out of range);
+ * 2 max_batch max(obs_dim, hidden1, hidden2, n_actions) < 2^31 and param_count < 2^31 (32-bit element offsets);
+ * param_count / workspace_bytes return -1 and create returns EINVAL beyond these.  Flat layout (fp32, row-major
+ * [out][in], torch's parameter order): W1[h1][obs] b1 W2[h2][h1] b2 W3[A][h2] b3[A].  Sharded buffers, continuous-action
+ * buffers, buffers of other obs_dim / n_actions, and batch / rounds above the configured maxima are rejected (EINVAL)
+ * before any launch. */
+typedef struct prl_mhq_cfg {
+    int32_t obs_dim, n_actions, hidden1, hidden2;
+    int32_t double_dqn;            /* 0: DeepQLearning, 1: DoubleDQN */
+    int32_t conservative;          /* 1: is_conservative=True (CQL term with the per-call alpha) */
+    int32_t target_update_freq, max_batch, max_rounds;
+    double lr, beta1, beta2, eps, weight_decay, gamma, tau;
+} prl_mhq_cfg;
+typedef struct prl_mhq prl_mhq;
+int64_t prl_mhq_param_count(const prl_mhq_cfg *cfg);
+int64_t prl_mhq_workspace_bytes(const prl_mhq_cfg *cfg);
+/* w, w_target, exp_avg, exp_avg_sq, max_exp_avg_sq: device f32[param_count] owned by the caller (the argument order of
+ * prl_dqn_create); adam_step: optimizer steps already taken (torch's `step`). */
+int prl_mhq_create(prl_mhq **out, const prl_mhq_cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq,
+                   float *max_exp_avg_sq, int64_t adam_step, void *workspace_dev);
+int prl_mhq_destroy(prl_mhq *mhq);
+int64_t prl_mhq_adam_step(const prl_mhq *mhq);
+int prl_mhq_set_adam_step(prl_mhq *mhq, int64_t step);
+/* New AdamW learning rate from the next call on; every lr-dependent scalar travels in the per-call block: no re-capture. */
+int prl_mhq_set_lr(prl_mhq *mhq, double lr);
+/* training_steps = the learner's count before the call (PolicyLearner.learn increments it before each round); alpha =
+ * conservative_alpha (ignored unless conservative); out_loss_dev: device f32[rounds]; out_logical_dev (optional)
+ * i32[rounds][batch] = sampled indices.  The ring stores no current action sets: every round uses the full set, as
+ * B200ReplayBuffer.sample reports it. */
+int prl_mhq_learn(prl_mhq *mhq, prl_buf *buf, int rounds, int batch, int64_t training_steps, double alpha,
+                  float *out_loss_dev, int32_t *out_logical_dev, void *stream);
+/* One round on a dense device batch: state / next_state f32[batch][obs], action_id i32[batch], reward f32[batch],
+ * terminated u8[batch]; curr_ids i32[batch][n_actions] (slot k of the current set, padding included; read only when
+ * conservative), null = every action; next_ids i32[batch][n_actions] and next_count i32[batch] (slots at and beyond it
+ * are unavailable), both null when every action is available next; training_steps = the count learn_batch sees
+ * (agent.learn_batch does not advance it); out_loss_dev: device f32[1]. */
+int prl_mhq_learn_batch(prl_mhq *mhq, int batch, const float *state, const int32_t *action_id, const float *reward,
+                        const float *next_state, const uint8_t *terminated, const int32_t *curr_ids, const int32_t *next_ids,
+                        const int32_t *next_count, int64_t training_steps, double alpha, float *out_loss_dev, void *stream);
+/* Q(s)[a] for every action (DeepTDLearning.act, deep_td_learning.py:200-254): device state f32[n][obs_dim] ->
+ * out_q f32[n][n_actions], online (target = 0) or target network. */
+int prl_mhq_q_values(prl_mhq *mhq, int n, const float *state, int target, float *out_q_dev, void *stream);
+int prl_mhq_set_graph(prl_mhq *mhq, int enable);
+int64_t prl_mhq_last_launches(const prl_mhq *mhq);
+
 /* ---- DeepSARSA ------------------------------------------------------------------------------------
  * Replaces DeepSARSA.get_next_state_values (policy_learners/sequential_decision_making/deep_sarsa.py:58-75) on
  * DeepTDLearning.forward / loss / learn_batch (deep_td_learning.py:269-360) with VanillaQValueNetwork.get_q_values

@@ -6,7 +6,8 @@
 Hand-written CUDA in libpearlb200.so (C ABI: include/pearl_b200.h), called through
 ctypes; PyTorch only allocates memory and provides streams.  No CPU fallback.
 """
-from ._compat import HAVE_PEARL, DuelingQValueNetwork, OneHotActionTensorRepresentationModule, TransitionBatch  # noqa: F401
+from ._compat import (HAVE_PEARL, DuelingQValueNetwork, OneHotActionTensorRepresentationModule, TransitionBatch,  # noqa: F401
+                      VanillaQValueMultiHeadNetwork)
 from .dqn import B200DeepQLearning, B200DeepSARSA, B200DoubleDQN, B200LearnerGroup  # noqa: F401
 from .replay_buffer import B200ReplayBuffer  # noqa: F401
 from .sarsa_buffer import B200SARSAReplayBuffer  # noqa: F401
@@ -23,5 +24,5 @@ from .dist import B200Communicator, all_gather_bytes, shard_owner  # noqa: F401
 __all__ = ["B200ReplayBuffer", "B200DeepQLearning", "B200DoubleDQN", "TransitionBatch",
            "OneHotActionTensorRepresentationModule", "HAVE_PEARL", "B200Communicator", "B200LearnerGroup", "B200PrioritizedReplayBuffer", "gae_and_lambda_returns", "B200ContinuousSoftActorCritic", "B200SoftActorCritic", "B200ProximalPolicyOptimization",
            "B200TD3", "B200DeepDeterministicPolicyGradient", "B200HindsightExperienceReplayBuffer", "B200ImplicitQLearning",
-           "B200QuantileRegressionDeepQLearning", "B200REINFORCE", "DuelingQValueNetwork",
+           "B200QuantileRegressionDeepQLearning", "B200REINFORCE", "DuelingQValueNetwork", "VanillaQValueMultiHeadNetwork",
            "B200DeepSARSA", "B200SARSAReplayBuffer", "B200TD3BC"]

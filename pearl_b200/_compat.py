@@ -24,6 +24,7 @@ try:  # pragma: no cover - depends on the environment
         DeepQLearning as _RefDeepQLearning,
     )
     from pearl.neural_networks.sequential_decision_making.q_value_networks import DuelingQValueNetwork
+    from pearl.neural_networks.sequential_decision_making.q_value_networks import VanillaQValueMultiHeadNetwork
     from pearl.policy_learners.sequential_decision_making.double_dqn import DoubleDQN as _RefDoubleDQN
     from pearl.policy_learners.sequential_decision_making.deep_sarsa import DeepSARSA as _RefDeepSARSA
     from pearl.policy_learners.exploration_modules.common.epsilon_greedy_exploration import EGreedyExploration
@@ -163,6 +164,32 @@ except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
         def action_dim(self) -> int:
             return self._action_dim
 
+    class VanillaQValueMultiHeadNetwork(nn.Module):
+        """Same constructor, module tree and state_dict keys as VanillaQValueMultiHeadNetwork
+        (pearl/neural_networks/sequential_decision_making/q_value_networks.py:185-241): `_model` = mlp_block(state_dim,
+        hidden_dims, output_dim), one Q value per action; `use_layer_norm` puts a LayerNorm after each hidden Linear, as
+        mlp_block does."""
+
+        def __init__(self, state_dim: int, action_dim: int, hidden_dims, output_dim: int, use_layer_norm: bool = False) -> None:
+            super().__init__()
+            self._state_dim, self._action_dim, self._output_dim = state_dim, action_dim, output_dim
+            dims = [state_dim] + list(hidden_dims) + [output_dim]
+            blocks = [nn.Sequential(*([nn.Linear(dims[i], dims[i + 1])] + ([nn.LayerNorm(dims[i + 1])] if use_layer_norm else [])
+                                      + [nn.ReLU()])) for i in range(len(dims) - 2)]
+            blocks.append(nn.Sequential(nn.Linear(dims[-2], dims[-1])))
+            self._model = nn.Sequential(*blocks)
+
+        def forward(self, x: torch.Tensor) -> torch.Tensor:
+            return self._model(x)
+
+        @property
+        def state_dim(self) -> int:
+            return self._state_dim
+
+        @property
+        def action_dim(self) -> int:
+            return self._action_dim
+
     class _RefDeepQLearning(nn.Module):
         """Attribute-compatible stand-in for DeepQLearning's constructor
         (deep_q_learning.py:40-59, deep_td_learning.py:60-185)."""
@@ -193,6 +220,9 @@ except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
                 self._Q = network_instance
             elif network_type is DuelingQValueNetwork:   # deep_td_learning.py make_specified_network
                 self._Q = DuelingQValueNetwork(state_dim=state_dim, action_dim=A, hidden_dims=hidden_dims, output_dim=1)
+            elif network_type is VanillaQValueMultiHeadNetwork:
+                self._Q = VanillaQValueMultiHeadNetwork(state_dim=state_dim, action_dim=A, hidden_dims=hidden_dims,
+                                                        output_dim=action_representation_module.max_number_actions)
             else:
                 self._Q = _QNet(state_dim, A, hidden_dims)
             self._Q_target = copy.deepcopy(self._Q)

@@ -93,6 +93,14 @@ class DuelCfg(C.Structure):
                 ("eps", C.c_double), ("weight_decay", C.c_double), ("gamma", C.c_double), ("tau", C.c_double)]
 
 
+class MhqCfg(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden1", C.c_int32), ("hidden2", C.c_int32),
+                ("double_dqn", C.c_int32), ("conservative", C.c_int32), ("target_update_freq", C.c_int32),
+                ("max_batch", C.c_int32), ("max_rounds", C.c_int32), ("lr", C.c_double), ("beta1", C.c_double),
+                ("beta2", C.c_double), ("eps", C.c_double), ("weight_decay", C.c_double), ("gamma", C.c_double),
+                ("tau", C.c_double)]
+
+
 class SarsaCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden1", C.c_int32), ("hidden2", C.c_int32),
                 ("target_update_freq", C.c_int32), ("max_batch", C.c_int32), ("max_rounds", C.c_int32), ("lr", C.c_double),
@@ -259,6 +267,18 @@ _SIGNATURES = {
     "prl_duel_q_values": (C.c_int, [_P, C.c_int, _P, _P, C.c_int, C.c_int, _P, _P]),
     "prl_duel_set_graph": (C.c_int, [_P, C.c_int]),
     "prl_duel_last_launches": (C.c_int64, [_P]),
+    "prl_mhq_param_count": (C.c_int64, [C.POINTER(MhqCfg)]),
+    "prl_mhq_workspace_bytes": (C.c_int64, [C.POINTER(MhqCfg)]),
+    "prl_mhq_create": (C.c_int, [C.POINTER(_P), C.POINTER(MhqCfg), _P, _P, _P, _P, _P, C.c_int64, _P]),
+    "prl_mhq_destroy": (C.c_int, [_P]),
+    "prl_mhq_adam_step": (C.c_int64, [_P]),
+    "prl_mhq_set_adam_step": (C.c_int, [_P, C.c_int64]),
+    "prl_mhq_set_lr": (C.c_int, [_P, C.c_double]),
+    "prl_mhq_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, C.c_double, _P, _P, _P]),
+    "prl_mhq_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 8 + [C.c_int64, C.c_double, _P, _P]),
+    "prl_mhq_q_values": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
+    "prl_mhq_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_mhq_last_launches": (C.c_int64, [_P]),
     "prl_sarsa_param_count": (C.c_int64, [C.POINTER(SarsaCfg)]),
     "prl_sarsa_workspace_bytes": (C.c_int64, [C.POINTER(SarsaCfg)]),
     "prl_sarsa_create": (C.c_int, [C.POINTER(_P), C.POINTER(SarsaCfg), _P, _P, _P, _P, _P, C.c_int64, _P]),

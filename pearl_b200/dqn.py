@@ -5,6 +5,7 @@ in one persistent CUDA kernel (libpearlb200.so), replacing
     DeepTDLearning.learn_batch     .../sequential_decision_making/deep_td_learning.py:269-360
     DeepQLearning / DoubleDQN.get_next_state_values   deep_q_learning.py:130-167, double_dqn.py:29-57
     VanillaQValueNetwork.get_q_values                 q_value_networks.py:152-174
+        (VanillaQValueMultiHeadNetwork, q_value_networks.py:185-241: multihead.py)
     torch.optim.AdamW(amsgrad=True).step, update_target_network (common/utils.py:214-226)
 
 Constructor arguments, attributes (`_Q`, `_Q_target`, `optimizer`, `_training_steps`,
@@ -27,6 +28,7 @@ import torch
 from . import _lib
 from . import cql as _cql
 from . import dueling as _duel
+from . import multihead as _mh
 from . import sarsa as _sarsa_mod
 from ._batch import action_ids
 from ._compat import _RefDeepQLearning, _RefDeepSARSA, _RefDoubleDQN, TransitionBatch
@@ -62,10 +64,13 @@ class _B200DQNMixin:
             raise NotImplementedError("the fused Q network assumes a one-hot action representation")
         self._n_actions = int(arm.max_number_actions)
         self._dueling = _duel.is_dueling(self._Q)       # DuelingQValueNetwork: prl_duel_* (dueling.py)
-        if self._sarsa and (self._dueling or self._conservative):
+        self._multihead = _mh.is_multihead(self._Q)     # VanillaQValueMultiHeadNetwork: prl_mhq_* (multihead.py)
+        if self._sarsa and (self._dueling or self._conservative or self._multihead):
             _sarsa_mod.check_config(self, engine)
         if self._dueling:
             self._obs_dim, self._duel_dims = _duel.shape_of(self._Q, self._n_actions)
+        elif self._multihead:
+            self._obs_dim, self._hidden = _mh.shape_of(self._Q, self._n_actions)
         else:
             lin = _linears(self._Q)
             self._obs_dim = lin[0].in_features - self._n_actions
@@ -78,9 +83,11 @@ class _B200DQNMixin:
             _sarsa_mod.check_config(self, engine)
         elif self._dueling:
             _duel.check_config(self, engine)
+        elif self._multihead:
+            _mh.check_config(self, engine)
         elif self._conservative:
             _cql.check_config(self, engine)
-        if self._dueling or self._conservative or self._sarsa:
+        if self._dueling or self._multihead or self._conservative or self._sarsa:
             self.use_cuda_graph = True          # False: plain stream launches (profilers)
         self._handle = C.c_void_p(0)
         self._bound_ptr = None
@@ -98,8 +105,10 @@ class _B200DQNMixin:
 
     def _c(self, name: str):
         """C entry point `name` of the learner this instance binds: prl_sarsa_* for DeepSARSA, prl_duel_* for a dueling Q
-        network, prl_cql_* when conservative, prl_dqn_* otherwise."""
-        prefix = "prl_sarsa_" if self._sarsa else "prl_duel_" if self._dueling else "prl_cql_" if self._conservative else "prl_dqn_"
+        network, prl_mhq_* for a multi-head Q network (plain or conservative), prl_cql_* when conservative, prl_dqn_*
+        otherwise."""
+        prefix = "prl_sarsa_" if self._sarsa else "prl_duel_" if self._dueling else "prl_mhq_" if self._multihead else \
+            "prl_cql_" if self._conservative else "prl_dqn_"
         return getattr(self._libh, prefix + name)
 
     def _adam_hparams(self) -> dict:
@@ -142,7 +151,7 @@ class _B200DQNMixin:
         hp = self._adam_hparams()
         bound_batch = max(int(need_batch), int(self._batch_size) if self._batch_size > 0 else 0, 1)
         cfg = _sarsa_mod.make_cfg(self, hp, bound_batch) if self._sarsa else _duel.make_cfg(self, hp, bound_batch) if self._dueling else \
-            _cql.make_cfg(self, hp, bound_batch) if self._conservative else _lib.DqnCfg(
+            _mh.make_cfg(self, hp, bound_batch) if self._multihead else _cql.make_cfg(self, hp, bound_batch) if self._conservative else _lib.DqnCfg(
             obs_dim=self._obs_dim, n_actions=self._n_actions, hidden1=self._hidden[0], hidden2=self._hidden[1],
             double_dqn=int(self._double), target_update_freq=int(self._target_update_freq),
             max_batch=bound_batch, max_rounds=self._max_rounds, rows_per_cta=self._rows_per_cta,
@@ -266,7 +275,7 @@ class _B200DQNMixin:
         if self._sarsa:
             return dict(launches=int(self._c("last_launches")(self._handle)),
                         graph_captures=int(self._c("graph_captures")(self._handle)))
-        if self._dueling or self._conservative:
+        if self._dueling or self._multihead or self._conservative:
             return dict(launches=int(self._c("last_launches")(self._handle)))
         a, b, c = C.c_int32(0), C.c_int32(0), C.c_int32(0)
         self._libh.prl_dqn_last_launch_info(self._handle, C.byref(a), C.byref(b), C.byref(c))
@@ -277,17 +286,17 @@ class _B200DQNMixin:
         `learn(B200ReplayBuffer)` then applies the mean gradient of all ranks' batches, exchanged
         inside the kernel.  All ranks must call learn() with the same number of rounds and start
         from identical parameters."""
-        if self._dueling or self._conservative or self._sarsa:
-            raise NotImplementedError("dueling, conservative (CQL) and DeepSARSA updates run on one GPU: set_communicator is not "
-                                      "supported")
+        if self._dueling or self._multihead or self._conservative or self._sarsa:
+            raise NotImplementedError("dueling, multi-head, conservative (CQL) and DeepSARSA updates run on one GPU: "
+                                      "set_communicator is not supported")
         self._bind(1)
         self._comm = comm
         _lib.check(self._libh.prl_dqn_set_comm(self._handle, comm.handle if comm is not None else None))
 
     def set_kernel_timing(self, enable: bool = True) -> None:
-        if self._dueling or self._conservative or self._sarsa:
-            raise NotImplementedError("kernel timing belongs to the fused DQN kernel; time dueling, conservative and DeepSARSA "
-                                      "rounds with CUDA events")
+        if self._dueling or self._multihead or self._conservative or self._sarsa:
+            raise NotImplementedError("kernel timing belongs to the fused DQN kernel; time dueling, multi-head, conservative and "
+                                      "DeepSARSA rounds with CUDA events")
         self._bind(1)
         _lib.check(self._libh.prl_dqn_set_timing(self._handle, int(enable)))
 
@@ -315,7 +324,7 @@ class _B200DQNMixin:
                     for k, v in self.learn_batch(self.preprocess_batch(batch)).items():
                         report.setdefault(k, []).append(v)
             return report
-        if self._dueling or self._conservative or self._sarsa:
+        if self._dueling or self._multihead or self._conservative or self._sarsa:
             return self._learn_rounds(replay_buffer, bs, rounds, trace)
         self._bind(bs)
         dev = self._device
@@ -359,20 +368,22 @@ class _B200DQNMixin:
         return report
 
     def _learn_rounds(self, replay_buffer, bs: int, rounds: int, trace: bool) -> dict:
-        """learn() of the dueling, conservative (CQL) and DeepSARSA learners over a B200ReplayBuffer: `rounds` x (sample ->
-        round) through prl_duel_learn / prl_cql_learn (which also takes alpha) / prl_sarsa_learn (which needs the committed
-        next actions of a B200SARSAReplayBuffer).  The ring holds no current action sets, so every round uses the full set,
+        """learn() of the dueling, multi-head, conservative (CQL) and DeepSARSA learners over a B200ReplayBuffer: `rounds` x
+        (sample -> round) through prl_duel_learn / prl_mhq_learn and prl_cql_learn (which also take alpha) / prl_sarsa_learn
+        (which needs the committed next actions of a B200SARSAReplayBuffer).  The ring holds no current action sets, so every round uses the full set,
         as B200ReplayBuffer.sample reports it."""
         from .per import B200PrioritizedReplayBuffer
         if isinstance(replay_buffer, B200PrioritizedReplayBuffer):
             raise NotImplementedError(("DeepSARSA samples uniformly" if self._sarsa else "dueling DQN samples uniformly"
-                                       if self._dueling else "conservative (CQL) updates sample uniformly")
+                                       if self._dueling else "multi-head DQN samples uniformly" if self._multihead else
+                                       "conservative (CQL) updates sample uniformly")
                                       + ": a B200PrioritizedReplayBuffer is not supported")
         self._bind(bs)
         dev = self._device
         if replay_buffer.device != dev:
             raise RuntimeError(f"replay buffer is on {replay_buffer.device}, learner on {dev}")
-        alpha = (_cql.alpha(self),) if self._conservative and not self._sarsa and not self._dueling else ()
+        alpha = (_mh.alpha(self),) if self._multihead else \
+            (_cql.alpha(self),) if self._conservative and not self._sarsa and not self._dueling else ()
         h = self._handle
         mae = torch.empty(rounds, dtype=torch.float32, device=dev)
         idx = torch.empty((rounds, bs), dtype=torch.int32, device=dev) if trace else None
@@ -439,6 +450,8 @@ class _B200DQNMixin:
             return _sarsa_mod.learn_batch(self, batch)
         if self._dueling:
             return _duel.learn_batch(self, batch)
+        if self._multihead:
+            return _mh.learn_batch(self, batch)
         if self._conservative:
             return _cql.learn_batch(self, batch)
         B = len(batch)
@@ -471,6 +484,8 @@ class _B200DQNMixin:
         """Q(s, a) for every action id: [n, obs] -> [n, n_actions]."""
         if self._dueling:
             return _duel.q_values(self, states, target)
+        if self._multihead:
+            return _mh.q_values(self, states, target)
         self._bind(1)
         dev = self._device
         s = states.to(device=dev, dtype=torch.float32).reshape(-1, self._obs_dim).contiguous()
@@ -512,6 +527,8 @@ class B200LearnerGroup:
             raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no DeepSARSA update")
         if any(getattr(l, "_dueling", False) for l in learners):
             raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no dueling network")
+        if any(getattr(l, "_multihead", False) for l in learners):
+            raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no multi-head network")
         self.learners, self.buffers = list(learners), list(buffers)
 
     def learn(self) -> list:

@@ -23,6 +23,8 @@ def check_config(pl, engine: str) -> None:
         raise NotImplementedError("DeepSARSA with is_conservative=True (CQL) is not supported")
     if pl._dueling:
         raise NotImplementedError("DeepSARSA with a DuelingQValueNetwork is not supported")
+    if getattr(pl, "_multihead", False):
+        raise NotImplementedError("DeepSARSA with a VanillaQValueMultiHeadNetwork is not supported")
 
 
 def make_cfg(pl, hp: dict, max_batch: int) -> _lib.SarsaCfg:
