@@ -950,6 +950,53 @@ int prl_test_contraction(int op, int engine, int M, int N, int K, const float *a
                          const float *bias, const float *mask, int relu, int accumulate, float *c, float *c_tail, int nets,
                          void *stream);
 
+/* ---- contextual bandit: LinearBandit (LinUCB) ------------------------------------------------------------------
+ * Replaces LinearRegression.learn_batch / calculate_coefs / apply_discounting / forward / calculate_sigma
+ * (neural_networks/contextual_bandit/linear_regression.py:192-270), LinearBandit.learn_batch / _maybe_apply_discounting
+ * (policy_learners/contextual_bandits/linear_bandit.py:123-164), driven by PolicyLearner.learn (prl_cb_learn: sample ->
+ * round, `rounds` times) or called on a caller's batch (prl_cb_learn_batch: one round, PearlAgent.learn_batch /
+ * offline_learning), and the UCB scores of LinearBandit.act / get_scores (ucb_exploration.py:40-93, action_utils.py:150-158).
+ * With x = state || action features (k = obs_dim + action_dim) and x1 = [1, x] (d = k + 1), per round:
+ *   A += x1^T (x1 w), b += x1^T (y w), sum_weight += sum w   (fp32, the partial sums added in a fixed order);
+ *   when discount_interval > 0 and (double)sum_weight - last_discount >= discount_interval: A, b *= gamma (when gamma < 1)
+ *   and last_discount = sum_weight;  inv_A = inv(A + lambda I), coefs = inv_A b  (Gauss-Jordan with partial pivoting in
+ *   fp64, rounded to fp32);  prediction = x1 . coefs with the new coefs.
+ * d <= 128; l2_reg_lambda > 0 (the reference's pinv fallback is not implemented); workspace_bytes returns -1 and create
+ * returns EINVAL beyond these.  Weights must be non-negative (not checked here): with a negative weight A + lambda I can
+ * be singular, where the reference falls back to pinv and this solve returns non-finite values.  In learn, action_rep folds the stored id into the row: 1 = one-hot over action_dim =
+ * n_actions columns, 2 = binary code, bit p of the id at column p (BinaryActionTensorRepresentationModule);
+ * learn refuses action_rep 0.  Sharded buffers, continuous-action buffers, buffers of other obs_dim / n_actions, and
+ * batch / rounds above the configured maxima are rejected (EINVAL) before any launch. */
+typedef struct prl_cb_cfg {
+    int32_t obs_dim, n_actions, action_dim;
+    int32_t action_rep;            /* 0: none (learn_batch / scores only), 1: one-hot, 2: binary */
+    int32_t max_batch, max_rounds;
+    double l2_reg_lambda, gamma, discount_interval;
+} prl_cb_cfg;
+typedef struct prl_cb prl_cb;
+int64_t prl_cb_workspace_bytes(const prl_cb_cfg *cfg);
+/* A f32[d][d], b f32[d], sum_weight f32[1], inv_A f32[d][d], coefs f32[d], last_discount f64[1]: device memory owned by the
+ * caller (the reference's buffers _A, _b, _sum_weight, _inv_A, _coefs and last_sum_weight_when_discounted). */
+int prl_cb_create(prl_cb **out, const prl_cb_cfg *cfg, float *A, float *b, float *sum_weight, float *inv_A, float *coefs,
+                  double *last_discount, void *workspace_dev);
+int prl_cb_destroy(prl_cb *cb);
+int prl_cb_set_graph(prl_cb *cb, int enable);
+int64_t prl_cb_last_launches(const prl_cb *cb);
+/* out_pred_dev / out_label_dev / out_weight_dev: device f32[rounds][batch] (label and weight may be null);
+ * out_logical_dev (optional) i32[rounds][batch] = sampled indices.  Every stored transition has weight 1. */
+int prl_cb_learn(prl_cb *cb, prl_buf *buf, int rounds, int batch, float *out_pred_dev, float *out_label_dev, float *out_weight_dev,
+                 int32_t *out_logical_dev, void *stream);
+/* One round on a dense device batch: state f32[batch][obs_dim], action f32[batch][action_dim] (the represented action, used
+ * as given), reward f32[batch], weight f32[batch] (null: every weight 1); out_pred_dev f32[batch]. */
+int prl_cb_learn_batch(prl_cb *cb, int batch, const float *state, const float *action, const float *reward, const float *weight,
+                       float *out_pred_dev, void *stream);
+/* Scores of n states x n_space actions: state f32[n][obs_dim], act_feat f32[n_space][action_dim] (the represented actions of
+ * the space); out_scores f32[n][n_space] = x1 . coefs (+ alpha sigma when with_sigma, sigma = sqrt(x1^T inv_A x1), NaN ->
+ * 0); out_index (optional) i32[n] = first maximum over the positions where mask u8[n][n_space] is non-zero (mask null:
+ * every position; 0 when none is). */
+int prl_cb_scores(prl_cb *cb, int n, const float *state, int n_space, const float *act_feat, double alpha, int with_sigma,
+                  const uint8_t *mask, float *out_scores, int32_t *out_index, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

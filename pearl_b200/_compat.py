@@ -281,3 +281,129 @@ except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
                              exploration_module=exploration_module if exploration_module is not None else EGreedyExploration(0.05),
                              action_representation_module=action_representation_module, optimizer=optimizer, **kwargs)
             self.on_policy = True
+
+
+try:  # pragma: no cover - depends on the environment; kept apart so the names above do not depend on it
+    from pearl.action_representation_modules.binary_action_representation_module import (
+        BinaryActionTensorRepresentationModule,
+    )
+    from pearl.action_representation_modules.identity_action_representation_module import (
+        IdentityActionRepresentationModule,
+    )
+    from pearl.policy_learners.contextual_bandits.linear_bandit import LinearBandit as _RefLinearBandit
+    from pearl.policy_learners.exploration_modules.common.tiebreaking_strategy import TiebreakingStrategy
+    from pearl.policy_learners.exploration_modules.contextual_bandits.ucb_exploration import UCBExploration
+
+    HAVE_PEARL_BANDITS = True
+except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
+    HAVE_PEARL_BANDITS = False
+
+
+if not HAVE_PEARL_BANDITS:
+    from enum import Enum
+
+    class TiebreakingStrategy(Enum):  # exploration_modules/common/tiebreaking_strategy.py
+        NO_TIEBREAKING = 0
+        PER_ROW_TIEBREAKING = 1
+        BATCH_TIEBREAKING = 2
+
+    class UCBExploration:
+        """Attribute-compatible stand-in for UCBExploration (exploration_modules/contextual_bandits/ucb_exploration.py):
+        scores = values + alpha * sigma."""
+
+        def __init__(self, alpha: float, randomized_tiebreaking: TiebreakingStrategy = TiebreakingStrategy.NO_TIEBREAKING) -> None:
+            self._alpha = alpha
+            self.randomized_tiebreaking = randomized_tiebreaking
+
+    class IdentityActionRepresentationModule(nn.Module):
+        def __init__(self, max_number_actions: int = -1, representation_dim: int = -1) -> None:
+            super().__init__()
+            self._max_number_actions, self._representation_dim = max_number_actions, representation_dim
+
+        def forward(self, x: torch.Tensor) -> torch.Tensor:
+            return x
+
+        @property
+        def max_number_actions(self) -> int:
+            return self._max_number_actions
+
+        @property
+        def representation_dim(self) -> int:
+            return self._representation_dim
+
+    class BinaryActionTensorRepresentationModule(nn.Module):
+        """Same as binary_action_representation_module.py: bit p of the action id at column p."""
+
+        def __init__(self, bits_num: int) -> None:
+            super().__init__()
+            self._bits_num = bits_num
+            self._max_number_actions = 2 ** bits_num
+
+        def forward(self, x: torch.Tensor) -> torch.Tensor:
+            if x.dim() == 1:
+                x = x.unsqueeze(-1)
+            mask = 2 ** torch.arange(self._bits_num, device=x.device)
+            return x.bitwise_and(mask).ne(0).to(torch.float32)
+
+        @property
+        def max_number_actions(self) -> int:
+            return self._max_number_actions
+
+        @property
+        def representation_dim(self) -> int:
+            return self._bits_num
+
+    class _LinearRegression(nn.Module):
+        """Same constructor, buffers and state_dict keys as LinearRegression
+        (neural_networks/contextual_bandit/linear_regression.py:20-87)."""
+
+        def __init__(self, feature_dim: int, l2_reg_lambda: float = 1.0, gamma: float = 1.0, force_pinv: bool = False,
+                     initial_coefs: Optional[torch.Tensor] = None) -> None:
+            super().__init__()
+            assert 0 < gamma <= 1, f"gamma should be in (0, 1]. Got gamma={gamma} instead"
+            self._feature_dim = feature_dim
+            self.gamma, self.l2_reg_lambda, self.force_pinv = gamma, l2_reg_lambda, force_pinv
+            d = feature_dim + 1
+            self.register_buffer("_A", torch.zeros(d, d))
+            self.register_buffer("_b", torch.zeros(d))
+            self.register_buffer("_sum_weight", torch.zeros(1))
+            self.register_buffer("_inv_A", torch.zeros(d, d))
+            if initial_coefs is not None:
+                assert initial_coefs.shape == (d,), f"initial_coefs shape {initial_coefs.shape} != {(d,)}"
+                self.register_buffer("_coefs", initial_coefs.clone())
+            else:
+                self.register_buffer("_coefs", torch.zeros(d))
+
+    class _RefLinearBandit(nn.Module):
+        """Attribute-compatible stand-in for LinearBandit's constructor (policy_learners/contextual_bandits/linear_bandit.py:
+        93-121 on top of ContextualBanditBase / PolicyLearner): same arguments, defaults and state_dict keys."""
+
+        def __init__(self, feature_dim: int, exploration_module=None, l2_reg_lambda: float = 1.0, gamma: float = 1.0,
+                     apply_discounting_interval: float = 0.0, force_pinv: bool = False, training_rounds: int = 100,
+                     batch_size: int = 128, action_representation_module=None, initial_coefs=None) -> None:
+            super().__init__()
+            self.exploration_module = exploration_module
+            self.action_representation_module = (action_representation_module if action_representation_module is not None
+                                                 else IdentityActionRepresentationModule())
+            self._history_summarization_module = None
+            self._training_rounds, self._batch_size, self._training_steps = training_rounds, batch_size, 0
+            self.on_policy, self._is_action_continuous = False, False
+            self._feature_dim = feature_dim
+            self.model = _LinearRegression(feature_dim=feature_dim, l2_reg_lambda=l2_reg_lambda, gamma=gamma, force_pinv=force_pinv,
+                                           initial_coefs=initial_coefs)
+            self.apply_discounting_interval = apply_discounting_interval
+            self.last_sum_weight_when_discounted = 0.0
+
+        @property
+        def feature_dim(self) -> int:
+            return self._feature_dim
+
+        @property
+        def batch_size(self) -> int:
+            return self._batch_size
+
+        def set_history_summarization_module(self, value) -> None:
+            self._history_summarization_module = value
+
+        def reset(self, action_space) -> None:
+            pass

@@ -123,6 +123,12 @@ class ReinforceCfg(C.Structure):
                 ("eps", C.c_double), ("weight_decay", C.c_double)]
 
 
+class CbCfg(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("action_dim", C.c_int32), ("action_rep", C.c_int32),
+                ("max_batch", C.c_int32), ("max_rounds", C.c_int32), ("l2_reg_lambda", C.c_double), ("gamma", C.c_double),
+                ("discount_interval", C.c_double)]
+
+
 class DqnCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden1", C.c_int32),
                 ("hidden2", C.c_int32), ("double_dqn", C.c_int32), ("target_update_freq", C.c_int32),
@@ -292,6 +298,14 @@ _SIGNATURES = {
     "prl_sarsa_set_graph": (C.c_int, [_P, C.c_int]),
     "prl_sarsa_last_launches": (C.c_int64, [_P]),
     "prl_sarsa_graph_captures": (C.c_int64, [_P]),
+    "prl_cb_workspace_bytes": (C.c_int64, [C.POINTER(CbCfg)]),
+    "prl_cb_create": (C.c_int, [C.POINTER(_P), C.POINTER(CbCfg)] + [_P] * 7),
+    "prl_cb_destroy": (C.c_int, [_P]),
+    "prl_cb_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_cb_last_launches": (C.c_int64, [_P]),
+    "prl_cb_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
+    "prl_cb_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 6),
+    "prl_cb_scores": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_double, C.c_int, _P, _P, _P, _P]),
     "prl_ppo_actor_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_critic_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_workspace_bytes": (C.c_int64, [C.POINTER(PpoCfg)]),

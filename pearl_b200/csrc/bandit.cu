@@ -1,0 +1,432 @@
+// bandit.cu — LinearBandit (LinUCB) driven by PolicyLearner.learn or called directly on a caller's batch
+// (PearlAgent.learn_batch / offline_learning), and its UCB scoring, replacing
+//   neural_networks/contextual_bandit/linear_regression.py   LinearRegression.learn_batch (A += x^T (x w), symmetrized;
+//       b += x^T (y w); sum_weight += sum w), calculate_coefs (inv_A = inv(A + lambda I), coefs = inv_A b),
+//       apply_discounting (A, b *= gamma), forward ([1, x] . coefs) and calculate_sigma (sqrt([1, x]^T inv_A [1, x]))
+//   policy_learners/contextual_bandits/linear_bandit.py       learn_batch (x = state || represented action, the model's
+//       learn_batch, _maybe_apply_discounting, prediction = model(x) after the update), act / get_scores
+//   policy_learners/exploration_modules/contextual_bandits/ucb_exploration.py   values + alpha sigma, NaN sigma -> 0
+//   utils/functional_utils/learning/action_utils.py          get_model_action_index_batch (NO_TIEBREAKING: first max
+//       over the available positions)
+//
+// Round (5 launches, captured once per (batch, buffer) into a CUDA graph and replayed, DESIGN.md §3.4):
+//   k_cb_load     the B feature rows x = state || action representation (one-hot or binary code of the stored id, or the
+//                 caller's dense action matrix), the label y and the weight w (1, or the caller's vector)
+//   k_cb_stats    partial sums of x^T (x w), x^T (y w) and sum w over chunks of kChunk rows, one chunk per CTA column
+//   k_cb_reduce   the chunks added in ascending order and added into A, b and sum_weight (fp32, as the reference's buffers)
+//   k_cb_solve    one CTA: the discounting decision (in double, as the reference's Python compares .item() floats), then
+//                 inv(A + lambda I) by Gauss-Jordan elimination with partial pivoting in fp64 shared memory, rounded to fp32
+//                 on the way out, and coefs = inv_A b (fp64, rounded)
+//   k_cb_predict  prediction = [1, x] . coefs with the new coefs; label and weight copied out
+// No float atomics and a fixed summation order everywhere: bit-reproducible run to run, graph or eager, and independent of
+// how the rounds are split into calls.
+//
+// Why Gauss-Jordan with pivoting rather than Cholesky: like torch.linalg.inv (LU with partial pivoting) it needs no
+// positive definiteness, which the fp32 accumulation of A cannot guarantee once A + lambda I is ill-conditioned.
+// fp64 keeps the kernel's own rounding far below the fp32 reference's (DESIGN.md, the ridge solve).  With lambda > 0 and
+// non-negative weights (the plugin refuses the rest) A + lambda I is nonsingular; non-finite rows (NaN or inf states,
+// rewards or weights) propagate into inv_A and coefs as they do through the reference's inverse.
+#include <math.h>
+
+#include <new>
+
+#include "common.cuh"
+#include "rounds.cuh"
+
+using namespace prl;
+
+namespace {
+
+constexpr int kMaxD = 128;     // ridge width + 1 (the intercept): d^2 doubles fill 128 KB of shared memory
+constexpr int kChunk = 256;    // rows per partial sum of k_cb_stats
+constexpr int kStage = 32;     // rows staged in shared memory at a time
+constexpr int kSolveThreads = 512;
+
+// per-call block the captured round reads through
+struct CbCall {
+    const int32_t *slots;                     // [rounds][B] (learn)
+    float *out_pred, *out_label, *out_weight; // [rounds][B]
+    // learn_batch: the caller's dense batch
+    const float *d_state, *d_action, *d_reward, *d_weight;   // d_weight may be null: every weight is 1
+    int d_action_ld;                                          // row pitch of d_action (its width)
+};
+
+// entries of one partial: the packed lower triangle of x^T (x w) (row i, column j <= i at i (i + 1) / 2 + j), then the d
+// entries of x^T (y w), then sum w
+__host__ __device__ inline int cb_entries(int d) { return d * (d + 1) / 2 + d + 1; }
+
+// rows of one round: X[b] = state || action features, Y[b], W[b].  records == null: the caller's dense batch.
+// rep 1: one-hot of the stored id over act_dim columns; rep 2: its act_dim low bits (bit p at column p)
+__global__ void k_cb_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int act_dim, int rep,
+                          const CbCall *__restrict__ call, const int *__restrict__ round_idx, int B, float *__restrict__ X,
+                          float *__restrict__ Y, float *__restrict__ W) {
+    const int lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (w >= B) return;
+    const int k = obs + act_dim;
+    float *x = X + (size_t)w * k;
+    if (!records) {
+        for (int p = lane; p < obs; p += 32) x[p] = call->d_state[(size_t)w * obs + p];
+        for (int p = lane; p < act_dim; p += 32) x[obs + p] = call->d_action[(size_t)w * call->d_action_ld + p];
+        if (lane == 0) {
+            Y[w] = call->d_reward[w];
+            W[w] = call->d_weight ? call->d_weight[w] : 1.f;
+        }
+        return;
+    }
+    const int32_t *slots = call->slots + (size_t)(*round_idx) * B;
+    const uint32_t *r = records + (size_t)slots[w] * L.record_words;
+    for (int p = lane; p < obs; p += 32) x[p] = __uint_as_float(r[L.off_state + p]);
+    const int id = (int)r[L.off_action];
+    for (int p = lane; p < act_dim; p += 32) x[obs + p] = rep == 1 ? (p == id ? 1.f : 0.f) : (((id >> p) & 1) ? 1.f : 0.f);
+    if (lane == 0) {
+        Y[w] = __uint_as_float(r[L.off_reward]);
+        W[w] = 1.f;
+    }
+}
+
+// partial sums of the rows of chunk blockIdx.x into P[chunk][e], one entry per thread (blockIdx.y selects the entries),
+// rows in ascending order.  The rows [1, x] are staged kStage at a time with x w and y w beside them.
+__global__ void __launch_bounds__(256) k_cb_stats(int B, int k, const float *__restrict__ X, const float *__restrict__ Y,
+                                                  const float *__restrict__ W, float *__restrict__ P) {
+    __shared__ float xs[kStage][kMaxD], xws[kStage][kMaxD], yw[kStage], ws[kStage];
+    const int d = k + 1, T = d * (d + 1) / 2, E = T + d + 1;
+    const int e = blockIdx.y * blockDim.x + threadIdx.x;
+    // the entry's operands: kind 0 = A[i][j], 1 = b[i], 2 = sum w
+    int kind = 2, i = 0, j = 0;
+    if (e < T) {
+        kind = 0;
+        i = (int)((sqrtf(8.f * (float)e + 1.f) - 1.f) * 0.5f);
+        while (i * (i + 1) / 2 > e) i--;
+        while ((i + 1) * (i + 2) / 2 <= e) i++;
+        j = e - i * (i + 1) / 2;
+    } else if (e < T + d) {
+        kind = 1;
+        i = e - T;
+    }
+    const int r0 = blockIdx.x * kChunk, r1 = min(B, r0 + kChunk);
+    float acc = 0.f;
+    for (int s0 = r0; s0 < r1; s0 += kStage) {
+        const int n = min(kStage, r1 - s0);
+        __syncthreads();
+        for (int t = threadIdx.x; t < n * d; t += blockDim.x) {
+            const int rr = t / d, c = t - rr * d;
+            const float v = c == 0 ? 1.f : X[(size_t)(s0 + rr) * k + c - 1];
+            xs[rr][c] = v;
+            xws[rr][c] = __fmul_rn(v, W[s0 + rr]);
+        }
+        for (int t = threadIdx.x; t < n; t += blockDim.x) {
+            yw[t] = __fmul_rn(Y[s0 + t], W[s0 + t]);
+            ws[t] = W[s0 + t];
+        }
+        __syncthreads();
+        if (e < E) {
+            if (kind == 0)
+                for (int rr = 0; rr < n; rr++) acc = fmaf(xs[rr][i], xws[rr][j], acc);
+            else if (kind == 1)
+                for (int rr = 0; rr < n; rr++) acc = fmaf(xs[rr][i], yw[rr], acc);
+            else
+                for (int rr = 0; rr < n; rr++) acc = __fadd_rn(acc, ws[rr]);
+        }
+    }
+    if (e < E) P[(size_t)blockIdx.x * E + e] = acc;
+}
+
+// the chunks' partials added in ascending chunk order, then added into A (both triangles), b and sum_weight
+__global__ void k_cb_reduce(int d, int chunks, const float *__restrict__ P, float *__restrict__ A, float *__restrict__ b,
+                            float *__restrict__ sum_weight) {
+    const int T = d * (d + 1) / 2, E = T + d + 1;
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= E) return;
+    float s = 0.f;
+    for (int c = 0; c < chunks; c++) s = __fadd_rn(s, P[(size_t)c * E + e]);
+    if (e < T) {
+        int i = (int)((sqrtf(8.f * (float)e + 1.f) - 1.f) * 0.5f);
+        while (i * (i + 1) / 2 > e) i--;
+        while ((i + 1) * (i + 2) / 2 <= e) i++;
+        const int j = e - i * (i + 1) / 2;
+        A[(size_t)i * d + j] = __fadd_rn(A[(size_t)i * d + j], s);
+        if (i != j) A[(size_t)j * d + i] = __fadd_rn(A[(size_t)j * d + i], s);
+    } else if (e < T + d) {
+        b[e - T] = __fadd_rn(b[e - T], s);
+    } else {
+        *sum_weight = __fadd_rn(*sum_weight, s);
+    }
+}
+
+// _maybe_apply_discounting, then calculate_coefs.  One CTA; M = A + lambda I in fp64 shared memory [d][d], inverted in place
+// by Gauss-Jordan elimination with partial pivoting (first largest |pivot|, as LAPACK's idamax picks), the row exchanges
+// undone as column exchanges at the end.  Then round_idx advances (k_cb_predict reads the round it finished).
+__global__ void __launch_bounds__(kSolveThreads) k_cb_solve(int d, float lam, float gamma, double interval, float *__restrict__ A,
+                                                            float *__restrict__ b, const float *__restrict__ sum_weight,
+                                                            double *__restrict__ last_discount, float *__restrict__ inv_A,
+                                                            float *__restrict__ coefs, int *__restrict__ round_idx) {
+    extern __shared__ double sm[];
+    double *M = sm, *bb = sm + (size_t)d * d;
+    __shared__ double f[kMaxD];
+    __shared__ int piv[kMaxD];
+    __shared__ int disc;
+    const int tid = threadIdx.x, nt = blockDim.x, dd = d * d;
+    if (tid == 0) {
+        const double sw = (double)*sum_weight;
+        disc = interval > 0.0 && sw - *last_discount >= interval;
+        if (disc) *last_discount = sw;
+    }
+    __syncthreads();
+    if (disc && gamma < 1.f) {                 // apply_discounting: sum_weight is not discounted
+        for (int t = tid; t < dd; t += nt) A[t] = __fmul_rn(A[t], gamma);
+        for (int t = tid; t < d; t += nt) b[t] = __fmul_rn(b[t], gamma);
+        __syncthreads();
+    }
+    for (int t = tid; t < dd; t += nt) {
+        const int i = t / d, j = t - i * d;
+        M[t] = (double)(i == j ? __fadd_rn(A[t], lam) : A[t]);
+    }
+    for (int t = tid; t < d; t += nt) bb[t] = (double)b[t];
+    __syncthreads();
+    for (int k = 0; k < d; k++) {
+        if (tid < 32) {
+            double best = -1.0;
+            int bi = d;
+            for (int i = k + tid; i < d; i += 32) {
+                const double v = fabs(M[(size_t)i * d + k]);
+                if (v > best) { best = v; bi = i; }
+            }
+#pragma unroll
+            for (int o = 16; o; o >>= 1) {
+                const double ov = __shfl_xor_sync(0xffffffffu, best, o);
+                const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+                if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+            }
+            if (tid == 0) piv[k] = bi < d ? bi : k;     // a column of NaNs has no pivot row: keep row k
+        }
+        __syncthreads();
+        const int p = piv[k];
+        if (p != k)
+            for (int j = tid; j < d; j += nt) {
+                const double t = M[(size_t)k * d + j];
+                M[(size_t)k * d + j] = M[(size_t)p * d + j];
+                M[(size_t)p * d + j] = t;
+            }
+        __syncthreads();
+        const double pv = M[(size_t)k * d + k];
+        __syncthreads();
+        for (int t = tid; t < 2 * d; t += nt) {
+            if (t < d) M[(size_t)k * d + t] = (t == k ? 1.0 : M[(size_t)k * d + t]) / pv;
+            else f[t - d] = t - d == k ? 0.0 : M[(size_t)(t - d) * d + k];
+        }
+        __syncthreads();
+        for (int t = tid; t < dd; t += nt) {
+            const int i = t / d, j = t - i * d;
+            if (i == k) continue;
+            M[t] = fma(-f[i], M[(size_t)k * d + j], j == k ? 0.0 : M[t]);
+        }
+        __syncthreads();
+    }
+    for (int k = d - 1; k >= 0; k--) {
+        const int p = piv[k];
+        if (p != k)
+            for (int i = tid; i < d; i += nt) {
+                const double t = M[(size_t)i * d + k];
+                M[(size_t)i * d + k] = M[(size_t)i * d + p];
+                M[(size_t)i * d + p] = t;
+            }
+        __syncthreads();
+    }
+    for (int t = tid; t < dd; t += nt) inv_A[t] = (float)M[t];
+    for (int i = tid; i < d; i += nt) {
+        double c = 0.0;
+        for (int j = 0; j < d; j++) c = fma(M[(size_t)i * d + j], bb[j], c);
+        coefs[i] = (float)c;
+    }
+    if (tid == 0) *round_idx += 1;
+}
+
+// LinearBandit.learn_batch's report of the round k_cb_solve finished: prediction = model(x) with the new coefs
+__global__ void k_cb_predict(int B, int k, const float *__restrict__ X, const float *__restrict__ Y, const float *__restrict__ W,
+                             const float *__restrict__ coefs, const CbCall *__restrict__ call, const int *__restrict__ round_idx) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= B) return;
+    const size_t o = (size_t)(*round_idx - 1) * B + r;
+    const float *x = X + (size_t)r * k;
+    float s = coefs[0];
+    for (int j = 0; j < k; j++) s = fmaf(x[j], coefs[j + 1], s);
+    call->out_pred[o] = s;
+    if (call->out_label) call->out_label[o] = Y[r];
+    if (call->out_weight) call->out_weight[o] = W[r];
+}
+
+// scores of n states x S actions, one warp per (state, action) row x = [1, state, action features a]:
+//   mu = x . coefs;  with_sigma: mu + alpha sigma, sigma = sqrt(x^T inv_A x), NaN (a negative form) -> 0
+__global__ void __launch_bounds__(256) k_cb_scores(int n, int S, int obs, int act_dim, const float *__restrict__ state,
+                                                   const float *__restrict__ act_feat, const float *__restrict__ inv_A,
+                                                   const float *__restrict__ coefs, int with_sigma, float alpha,
+                                                   float *__restrict__ out) {
+    __shared__ float xs[8][kMaxD];
+    const int lane = threadIdx.x & 31, wb = threadIdx.x >> 5;
+    const long long row = (long long)blockIdx.x * 8 + wb;
+    if (row >= (long long)n * S) return;
+    const int s = (int)(row / S), a = (int)(row - (long long)s * S), d = obs + act_dim + 1;
+    float *x = xs[wb];
+    for (int c = lane; c < d; c += 32)
+        x[c] = c == 0 ? 1.f : (c <= obs ? state[(size_t)s * obs + c - 1] : act_feat[(size_t)a * act_dim + c - 1 - obs]);
+    __syncwarp();
+    float mu = 0.f, q = 0.f;
+    for (int j = lane; j < d; j += 32) {
+        mu = fmaf(x[j], coefs[j], mu);
+        if (with_sigma) {
+            float t = 0.f;
+            for (int i = 0; i < d; i++) t = fmaf(x[i], inv_A[(size_t)i * d + j], t);
+            q = fmaf(t, x[j], q);
+        }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        mu += __shfl_xor_sync(0xffffffffu, mu, o);
+        q += __shfl_xor_sync(0xffffffffu, q, o);
+    }
+    if (lane == 0) {
+        float v = mu;
+        if (with_sigma) {
+            float sg = sqrtf(q);
+            if (isnan(sg)) sg = 0.f;
+            v = __fadd_rn(mu, __fmul_rn(alpha, sg));
+        }
+        out[row] = v;
+    }
+}
+
+// first maximum of each state's scores over the positions whose mask is non-zero (every position when mask is null);
+// 0 when no position is available
+__global__ void k_cb_argmax(int n, int S, const float *__restrict__ scores, const uint8_t *__restrict__ mask, int32_t *__restrict__ idx) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    int bi = -1;
+    float best = 0.f;
+    for (int a = 0; a < S; a++) {
+        if (mask && !mask[(size_t)s * S + a]) continue;
+        const float v = scores[(size_t)s * S + a];
+        if (bi < 0 || v > best) { best = v; bi = a; }
+    }
+    idx[s] = bi < 0 ? 0 : bi;
+}
+
+}  // namespace
+
+// ------------------------------------------------------------------ host side
+struct prl_cb : Rounds<prl_cb, CbCall> {
+    static constexpr const char *kFn = "prl_cb", *kName = "LinearBandit";
+    prl_cb_cfg cfg;
+    int k, d;
+    float *A, *b, *sum_weight, *inv_A, *coefs;
+    double *last_discount;
+    float *X, *Y, *W, *P;
+    void fill_scal(float2 *, int) {}          // no optimizer
+    static int round(prl_cb *s, prl_buf *buf, int B, cudaStream_t st);
+};
+
+static size_t cb_solve_smem(int d) { return ((size_t)d * d + d) * sizeof(double); }
+
+static int cb_check(const prl_cb_cfg *c) {
+    PRL_REQUIRE(c, "null cfg");
+    PRL_REQUIRE(c->obs_dim >= 0 && c->action_dim >= 0 && c->obs_dim + c->action_dim >= 1, "obs_dim + action_dim must be positive");
+    PRL_REQUIRE(c->obs_dim + c->action_dim + 1 <= kMaxD,
+                "obs_dim + action_dim = %d: the ridge solve supports at most %d features (%d with the intercept)",
+                c->obs_dim + c->action_dim, kMaxD - 1, kMaxD);
+    PRL_REQUIRE(c->action_rep >= 0 && c->action_rep <= 2, "action_rep must be 0 (none), 1 (one-hot) or 2 (binary)");
+    PRL_REQUIRE(c->action_rep != 1 || c->action_dim == c->n_actions, "a one-hot representation has action_dim = n_actions");
+    PRL_REQUIRE(c->action_rep != 2 || (c->action_dim >= 1 && c->action_dim <= 30 && c->n_actions <= (1 << c->action_dim)),
+                "a binary representation needs 1 <= action_dim <= 30 bits and n_actions <= 2^action_dim");
+    PRL_REQUIRE(c->l2_reg_lambda > 0.0, "l2_reg_lambda must be positive (A + lambda I must be invertible)");
+    PRL_REQUIRE(c->gamma > 0.0 && c->gamma <= 1.0, "gamma must be in (0, 1]");
+    PRL_REQUIRE(c->max_batch > 0 && c->max_rounds > 0, "max_batch / max_rounds must be positive");
+    PRL_REQUIRE((int64_t)c->max_batch * (c->obs_dim + c->action_dim) < ((int64_t)1 << 31),
+                "max_batch * (obs_dim + action_dim) must stay below 2^31 (32-bit element offsets)");
+    return PRL_OK;
+}
+
+// the workspace, in order; base == null: only its size
+static int64_t cb_carve(prl_cb *s, void *base) {
+    const prl_cb_cfg &c = s->cfg;
+    const int64_t B = c.max_batch, K = c.obs_dim + c.action_dim, chunks = (B + kChunk - 1) / kChunk;
+    Carve w{(char *)base};
+    w(s->X, B * K); w(s->Y, B); w(s->W, B);
+    w(s->P, chunks * cb_entries((int)K + 1));
+    s->carve_tail(w, c.max_rounds, B);
+    return w.bytes;
+}
+
+extern "C" int64_t prl_cb_workspace_bytes(const prl_cb_cfg *c) {
+    if (cb_check(c)) return -1;
+    prl_cb t; t.cfg = *c;
+    return cb_carve(&t, nullptr);
+}
+
+extern "C" int prl_cb_create(prl_cb **out, const prl_cb_cfg *cfg, float *A, float *b, float *sum_weight, float *inv_A, float *coefs,
+                             double *last_discount, void *workspace) {
+    PRL_REQUIRE(out && A && b && sum_weight && inv_A && coefs && last_discount && workspace, "null argument");
+    int rc = cb_check(cfg);
+    if (rc) return rc;
+    const int d = cfg->obs_dim + cfg->action_dim + 1;
+    // the attribute belongs to the kernel, not to this handle: raise it to what the widest supported d needs, so that a
+    // later handle of a smaller d cannot lower it under the launches of a live wider one
+    PRL_CUDA(cudaFuncSetAttribute(k_cb_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cb_solve_smem(kMaxD)));
+    prl_cb *s = new (std::nothrow) prl_cb();
+    if (!s) return fail(PRL_ENOMEM, "out of host memory");
+    s->cfg = *cfg;
+    s->k = d - 1; s->d = d;
+    s->A = A; s->b = b; s->sum_weight = sum_weight; s->inv_A = inv_A; s->coefs = coefs; s->last_discount = last_discount;
+    cb_carve(s, workspace);
+    return prl_cb::open(s, out);
+}
+extern "C" int prl_cb_destroy(prl_cb *s) { return prl_cb::destroy(s); }
+extern "C" int prl_cb_set_graph(prl_cb *s, int enable) { return prl_cb::set_graph(s, enable); }
+extern "C" int64_t prl_cb_last_launches(const prl_cb *s) { return prl_cb::last_launches_of(s); }
+
+// one learner round, launched (or captured) on `st`; buf == null: the dense batch of the call block (learn_batch)
+int prl_cb::round(prl_cb *s, prl_buf *buf, int B, cudaStream_t st) {
+    const prl_cb_cfg &c = s->cfg;
+    const int k = s->k, d = s->d, E = cb_entries(d), chunks = (B + kChunk - 1) / kChunk, eb = 256;
+    k_cb_load<<<(B * 32 + eb - 1) / eb, eb, 0, st>>>(buf ? buf->records : nullptr, buf ? buf->lay : prl_buf_layout{}, c.obs_dim,
+                                                    c.action_dim, c.action_rep, s->call, s->round_idx, B, s->X, s->Y, s->W);
+    k_cb_stats<<<dim3(chunks, (E + 255) / 256), 256, 0, st>>>(B, k, s->X, s->Y, s->W, s->P);
+    k_cb_reduce<<<(E + eb - 1) / eb, eb, 0, st>>>(d, chunks, s->P, s->A, s->b, s->sum_weight);
+    k_cb_solve<<<1, kSolveThreads, cb_solve_smem(d), st>>>(d, (float)c.l2_reg_lambda, (float)c.gamma, c.discount_interval, s->A, s->b,
+                                                           s->sum_weight, s->last_discount, s->inv_A, s->coefs, s->round_idx);
+    k_cb_predict<<<(B + eb - 1) / eb, eb, 0, st>>>(B, k, s->X, s->Y, s->W, s->coefs, s->call, s->round_idx);
+    s->launches_per_round = 5;
+    return PRL_OK;
+}
+
+extern "C" int prl_cb_learn(prl_cb *s, prl_buf *buf, int rounds, int batch, float *out_pred, float *out_label, float *out_weight,
+                            int32_t *out_logical, void *stream_) {
+    PRL_REQUIRE(s && buf && out_pred, "null argument");
+    PRL_REQUIRE(s->cfg.action_rep != 0, "learn over a buffer needs a one-hot or binary action representation (action_rep 1 or 2)");
+    CbCall call{};
+    call.out_pred = out_pred; call.out_label = out_label; call.out_weight = out_weight;
+    return prl_cb::learn(s, buf, rounds, batch, 0, out_logical, call, stream_);
+}
+
+extern "C" int prl_cb_learn_batch(prl_cb *s, int batch, const float *state, const float *action, const float *reward,
+                                  const float *weight, float *out_pred, void *stream_) {
+    PRL_REQUIRE(s && (state || s->cfg.obs_dim == 0) && (action || s->cfg.action_dim == 0) && reward && out_pred, "null argument");
+    CbCall dense{};
+    dense.d_state = state; dense.d_action = action; dense.d_reward = reward; dense.d_weight = weight;
+    dense.d_action_ld = s->cfg.action_dim;
+    dense.out_pred = out_pred;
+    return prl_cb::learn_batch(s, batch, 0, dense, stream_);
+}
+
+extern "C" int prl_cb_scores(prl_cb *s, int n, const float *state, int n_space, const float *act_feat, double alpha, int with_sigma,
+                             const uint8_t *mask, float *out_scores, int32_t *out_index, void *stream_) {
+    PRL_REQUIRE(s && out_scores && (state || s->cfg.obs_dim == 0) && (act_feat || s->cfg.action_dim == 0), "null argument");
+    PRL_REQUIRE(n >= 0 && n_space >= 1 && (int64_t)n * n_space < ((int64_t)1 << 31), "n * n_space must be in [0, 2^31)");
+    if (n == 0) return PRL_OK;
+    const prl_cb_cfg &c = s->cfg;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const long long rows = (long long)n * n_space;
+    k_cb_scores<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(n, n_space, c.obs_dim, c.action_dim, state, act_feat, s->inv_A, s->coefs,
+                                                            with_sigma, (float)alpha, out_scores);
+    if (out_index) k_cb_argmax<<<(n + 255) / 256, 256, 0, st>>>(n, n_space, out_scores, mask, out_index);
+    PRL_CUDA(cudaGetLastError());
+    return PRL_OK;
+}
