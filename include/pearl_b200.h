@@ -997,6 +997,58 @@ int prl_cb_learn_batch(prl_cb *cb, int batch, const float *state, const float *a
 int prl_cb_scores(prl_cb *cb, int n, const float *state, int n_space, const float *act_feat, double alpha, int with_sigma,
                   const uint8_t *mask, float *out_scores, int32_t *out_index, void *stream);
 
+/* ---- contextual bandit: NeuralLinearBandit (neural LinUCB) -------------------------------------------------------
+ * Replaces NeuralLinearBandit.learn_batch / act / get_scores (policy_learners/contextual_bandits/neural_linear_bandit.py)
+ * over NeuralLinearRegression (neural_networks/contextual_bandit/neural_linear_regression.py) with two hidden layers.
+ * Network input x = state (action_dim 0: state_features_only) or state || action features; nn_output = mlp_block(x,
+ * [h1, h2], output_dim = h2) with ReLU, each layer of equal in / out width wrapped as x + layer(x) when skip.  Per round:
+ *   forward with the current parameters; mu = nn_output . e2e weight (e2e) or [1, nn_output] . coefs (the coefs before
+ *   this round's ridge update); p = sigmoid(mu) when sigmoid, else mu; loss = sum(w l(p, y)) / sum(w), l = mse (0),
+ *   l1 (1) or binary cross-entropy (2, needs sigmoid); backward and one AdamW(amsgrad) step over the network (and the e2e
+ *   weight when e2e); then the ridge of prl_cb (A, b, sum_weight, discounting, inv_A, coefs) on the pre-step nn_output.
+ * Flat parameters w f32[param_count] in torch's parameters() order: W1[h1][f] b1 W2[h2][h1] b2 W3[h2][h2] b3, then the
+ * e2e weight [h2]; m / v / vmax are the AdamW exp_avg / exp_avg_sq / max_exp_avg_sq of the same layout.  The ridge
+ * buffers are as prl_cb_create's, with d = h2 + 1.  1 <= h2 <= 127; l2_reg_lambda > 0.  score_rows: rows the workspace
+ * holds for prl_nlb_scores per chunk (0: max_batch). */
+typedef struct prl_nlb_cfg {
+    int32_t obs_dim, n_actions, action_dim;
+    int32_t action_rep;            /* 0: none (state alone, or learn_batch / scores), 1: one-hot, 2: binary */
+    int32_t h1, h2, skip, e2e;
+    int32_t loss;                  /* 0: mse, 1: mae, 2: binary cross-entropy */
+    int32_t sigmoid;               /* output activation: 0 linear, 1 sigmoid */
+    int32_t max_batch, max_rounds, score_rows;
+    double lr, beta1, beta2, eps, weight_decay;
+    double l2_reg_lambda, gamma, discount_interval;
+} prl_nlb_cfg;
+typedef struct prl_nlb prl_nlb;
+int64_t prl_nlb_param_count(const prl_nlb_cfg *cfg);
+int64_t prl_nlb_workspace_bytes(const prl_nlb_cfg *cfg);
+int prl_nlb_create(prl_nlb **out, const prl_nlb_cfg *cfg, float *w, float *m, float *v, float *vmax, int64_t adam_step, float *A,
+                   float *b, float *sum_weight, float *inv_A, float *coefs, double *last_discount, void *workspace_dev);
+int prl_nlb_destroy(prl_nlb *nlb);
+int prl_nlb_set_graph(prl_nlb *nlb, int enable);
+int prl_nlb_set_lr(prl_nlb *nlb, double lr);           /* from the next call on; no new capture */
+int64_t prl_nlb_adam_step(const prl_nlb *nlb);
+int prl_nlb_set_adam_step(prl_nlb *nlb, int64_t step);
+int64_t prl_nlb_last_launches(const prl_nlb *nlb);
+int64_t prl_nlb_graph_captures(const prl_nlb *nlb);   /* rounds captured into CUDA graphs so far */
+/* out_pred_dev (the pre-step, post-activation predictions) / out_label_dev / out_weight_dev: device f32[rounds][batch]
+ * (label and weight may be null); out_loss_dev / out_mu_dev f32[rounds]: the loss and the mean prediction of each round;
+ * out_logical_dev (optional) i32[rounds][batch] = sampled indices.  Every stored transition has weight 1. */
+int prl_nlb_learn(prl_nlb *nlb, prl_buf *buf, int rounds, int batch, float *out_pred_dev, float *out_label_dev,
+                  float *out_weight_dev, float *out_loss_dev, float *out_mu_dev, int32_t *out_logical_dev, void *stream);
+/* One round on a dense device batch (as prl_cb_learn_batch; action null when action_dim is 0).  zero_weight != 0: the
+ * weights sum to 0, so the round takes no optimizer step (the loss is 0 and the AdamW step count does not advance) and only
+ * the ridge is updated, as the reference's short circuit; the caller decides it (the reference reads the sum on the host). */
+int prl_nlb_learn_batch(prl_nlb *nlb, int batch, const float *state, const float *action, const float *reward, const float *weight,
+                        int zero_weight, float *out_pred_dev, float *out_loss_dev, float *out_mu_dev, void *stream);
+/* Scores of n states x n_space actions (state and act_feat as prl_cb_scores; act_feat may be null when action_dim is 0):
+ * mu from the network's output as in a round, sigma = sqrt([1, nn_output]^T inv_A [1, nn_output]) (NaN -> 0);
+ * mode 0 (act): mu + alpha sigma; 1: activation(mu + alpha sigma); 2: activation(mu) + alpha sigma (separate_uncertainty).
+ * out_index as prl_cb_scores. */
+int prl_nlb_scores(prl_nlb *nlb, int n, const float *state, int n_space, const float *act_feat, double alpha, int mode,
+                   const uint8_t *mask, float *out_scores, int32_t *out_index, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -20,6 +20,7 @@ from .actor_critic import (B200ContinuousSoftActorCritic, B200DeepDeterministicP
                            B200ImplicitQLearning, B200ProximalPolicyOptimization, B200QuantileRegressionDeepQLearning,
                            B200REINFORCE, B200SoftActorCritic, B200TD3, B200TD3BC)
 from .bandit import B200LinearBandit  # noqa: F401
+from .neural_linear import B200NeuralLinearBandit  # noqa: F401
 from ._compat import BinaryActionTensorRepresentationModule, UCBExploration  # noqa: F401
 from .dist import B200Communicator, all_gather_bytes, shard_owner  # noqa: F401
 
@@ -27,5 +28,5 @@ __all__ = ["B200ReplayBuffer", "B200DeepQLearning", "B200DoubleDQN", "Transition
            "OneHotActionTensorRepresentationModule", "HAVE_PEARL", "B200Communicator", "B200LearnerGroup", "B200PrioritizedReplayBuffer", "gae_and_lambda_returns", "B200ContinuousSoftActorCritic", "B200SoftActorCritic", "B200ProximalPolicyOptimization",
            "B200TD3", "B200DeepDeterministicPolicyGradient", "B200HindsightExperienceReplayBuffer", "B200ImplicitQLearning",
            "B200QuantileRegressionDeepQLearning", "B200REINFORCE", "DuelingQValueNetwork", "VanillaQValueMultiHeadNetwork",
-           "B200DeepSARSA", "B200SARSAReplayBuffer", "B200TD3BC", "B200LinearBandit", "UCBExploration",
+           "B200DeepSARSA", "B200SARSAReplayBuffer", "B200TD3BC", "B200LinearBandit", "B200NeuralLinearBandit", "UCBExploration",
            "BinaryActionTensorRepresentationModule"]

@@ -291,6 +291,8 @@ try:  # pragma: no cover - depends on the environment; kept apart so the names a
         IdentityActionRepresentationModule,
     )
     from pearl.policy_learners.contextual_bandits.linear_bandit import LinearBandit as _RefLinearBandit
+    from pearl.policy_learners.contextual_bandits.neural_linear_bandit import NeuralLinearBandit as _RefNeuralLinearBandit
+    from pearl.neural_networks.common.utils import LossType
     from pearl.policy_learners.exploration_modules.common.tiebreaking_strategy import TiebreakingStrategy
     from pearl.policy_learners.exploration_modules.contextual_bandits.ucb_exploration import UCBExploration
 
@@ -403,6 +405,103 @@ if not HAVE_PEARL_BANDITS:
             return self._batch_size
 
         def set_history_summarization_module(self, value) -> None:
+            self._history_summarization_module = value
+
+        def reset(self, action_space) -> None:
+            pass
+
+    class LossType(Enum):  # neural_networks/common/utils.py
+        MSE = "mse"
+        MAE = "mae"
+        CROSS_ENTROPY = "cross_entropy"
+
+    class ResidualWrapper(nn.Module):  # neural_networks/common/residual_wrapper.py: x + module(x)
+        def __init__(self, module: nn.Module) -> None:
+            super().__init__()
+            self.module = module
+
+        def forward(self, x: torch.Tensor) -> torch.Tensor:
+            return x + self.module(x)
+
+    class _ValueNetwork(nn.Module):
+        """Same module tree as VanillaValueNetwork over mlp_block with ReLU hidden layers and no normalization or dropout
+        (neural_networks/common/utils.py mlp_block): `_model.{i}.0` = Linear, or `_model.{i}.module.0` when a layer of
+        equal in / out width is wrapped in a ResidualWrapper."""
+
+        def __init__(self, input_dim: int, hidden_dims, output_dim: int, use_skip_connections: bool = False) -> None:
+            super().__init__()
+            dims = [input_dim] + list(hidden_dims) + [output_dim]
+            layers = []
+            for i in range(len(dims) - 1):
+                block = nn.Sequential(*([nn.Linear(dims[i], dims[i + 1])] + ([nn.ReLU()] if i < len(dims) - 2 else [])))
+                layers.append(ResidualWrapper(block) if use_skip_connections and dims[i] == dims[i + 1] else block)
+            self._model = nn.Sequential(*layers)
+
+        def forward(self, x: torch.Tensor) -> torch.Tensor:
+            return self._model(x)
+
+    class _NeuralLinearRegression(nn.Module):
+        """Same module tree and state_dict keys as NeuralLinearRegression (neural_networks/contextual_bandit/
+        neural_linear_regression.py): `_nn_layers`, `_linear_regression_layer`, `output_activation`, `linear_layer_e2e`."""
+
+        def __init__(self, feature_dim: int, hidden_dims, l2_reg_lambda_linear: float = 1.0, gamma: float = 1.0,
+                     force_pinv: bool = False, output_activation_name: str = "linear", use_skip_connections: bool = True,
+                     nn_e2e: bool = True) -> None:
+            super().__init__()
+            self._feature_dim = feature_dim
+            self._nn_layers = _ValueNetwork(feature_dim, hidden_dims, hidden_dims[-1], use_skip_connections)
+            self._linear_regression_layer = _LinearRegression(feature_dim=hidden_dims[-1], l2_reg_lambda=l2_reg_lambda_linear,
+                                                              gamma=gamma, force_pinv=force_pinv)
+            self.output_activation = {"linear": nn.Identity, "sigmoid": nn.Sigmoid}[output_activation_name]()
+            self.linear_layer_e2e = nn.Linear(in_features=hidden_dims[-1], out_features=1, bias=False)
+            self.nn_e2e = nn_e2e
+
+    class _RefNeuralLinearBandit(nn.Module):
+        """Attribute-compatible stand-in for NeuralLinearBandit's constructor (policy_learners/contextual_bandits/
+        neural_linear_bandit.py on top of ContextualBanditBase / PolicyLearner): same arguments, defaults and state_dict
+        keys, for the configurations the CUDA learner runs (ReLU hidden layers, no normalization or dropout)."""
+
+        def __init__(self, feature_dim: int, hidden_dims, exploration_module=None, action_representation_module=None,
+                     training_rounds: int = 100, batch_size: int = 128, learning_rate: float = 0.0003,
+                     l2_reg_lambda_linear: float = 1.0, gamma: float = 1.0, apply_discounting_interval: float = 0.0,
+                     force_pinv: bool = False, state_features_only: bool = True, loss_type=LossType.MSE,
+                     output_activation_name: str = "linear", use_batch_norm: bool = False, use_layer_norm: bool = False,
+                     hidden_activation: str = "relu", last_activation=None, dropout_ratio: float = 0.0,
+                     use_skip_connections: bool = False, nn_e2e: bool = True, separate_uncertainty: bool = False) -> None:
+            super().__init__()
+            assert len(hidden_dims) >= 1
+            self.exploration_module = exploration_module
+            self.action_representation_module = (action_representation_module if action_representation_module is not None
+                                                 else IdentityActionRepresentationModule())
+            self._history_summarization_module = None
+            self._training_rounds, self._batch_size, self._training_steps = training_rounds, batch_size, 0
+            self.on_policy, self._is_action_continuous = False, False
+            self._feature_dim = feature_dim
+            self.model = _NeuralLinearRegression(feature_dim=feature_dim, hidden_dims=hidden_dims,
+                                                 l2_reg_lambda_linear=l2_reg_lambda_linear, gamma=gamma, force_pinv=force_pinv,
+                                                 output_activation_name=output_activation_name,
+                                                 use_skip_connections=use_skip_connections, nn_e2e=nn_e2e)
+            self._optimizer = torch.optim.AdamW(self.model.parameters(), lr=learning_rate, amsgrad=True)
+            self._state_features_only = state_features_only
+            self.loss_type = LossType(loss_type) if isinstance(loss_type, str) else loss_type
+            self.apply_discounting_interval = apply_discounting_interval
+            self.last_sum_weight_when_discounted = 0.0
+            self.separate_uncertainty = separate_uncertainty
+
+        @property
+        def feature_dim(self) -> int:
+            return self._feature_dim
+
+        @property
+        def batch_size(self) -> int:
+            return self._batch_size
+
+        @property
+        def optimizer(self):
+            return self._optimizer
+
+        def set_history_summarization_module(self, value) -> None:
+            self._optimizer.add_param_group({"params": value.parameters()})
             self._history_summarization_module = value
 
         def reset(self, action_space) -> None:
