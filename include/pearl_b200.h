@@ -65,12 +65,15 @@ int prl_sm_count(void);
  *     [off_avail .. ) (PRL_BUF_DYNAMIC_ACTIONS only) n_actions u8 ids of the
  *                     next available actions (padded with 0), as the reference
  *                     pads `next_available_actions` (tensor_based_replay_buffer.py:179-251)
+ *     [cost]          (PRL_BUF_COST only) the transition's cost, f32, right after
+ *                     everything above (prl_buf_cost_offset): no other offset moves
  * FIFO eviction like deque(maxlen=capacity): logical index 0 = oldest.
  */
 #define PRL_BUF_DISCRETE 0x1          /* action is one int32 id in [0, n_actions) */
 #define PRL_BUF_CONTINUOUS 0x2        /* action is act_dim floats */
 #define PRL_BUF_DYNAMIC_ACTIONS 0x4   /* per-transition next-available-action sets */
 #define PRL_BUF_NEXT_ACTION 0x8       /* discrete only: the committed next action id of SARSA in the flags word */
+#define PRL_BUF_COST 0x10             /* one f32 cost per transition (TransitionBatch.cost, the reward-constrained safety module) */
 
 typedef struct prl_buf_desc {
     int64_t capacity;
@@ -193,6 +196,28 @@ int prl_buf_gather(const prl_buf *buf, const int32_t *slot_dev, int k, float *st
  * any other buffer. */
 int prl_buf_gather_next_action(const prl_buf *buf, const int32_t *slot_dev, int k, int64_t *out_dev,
                                void *stream);
+
+/* Costs (PRL_BUF_COST; the reference stores `cost` when the first pushed transition
+ * has one, tensor_based_replay_buffer.py:55-133, and collates it into
+ * TransitionBatch.cost).  The cost word follows every other field of the record, so
+ * every offset of prl_buf_layout is the one the same flags without PRL_BUF_COST give.
+ * prl_buf_cost_offset: *out = the cost word's offset in the record; PRL_EINVAL for a
+ * descriptor without PRL_BUF_COST.
+ * The pushes take the arguments of prl_buf_push_host / prl_buf_push_device plus
+ * cost f32[n].  A PRL_BUF_COST buffer refuses the plain pushes (and the SARSA and
+ * multi-buffer pushes), a plain buffer refuses these (PRL_EINVAL): no cost is ever
+ * stored as 0 by omission.  A sharded PRL_BUF_COST buffer is refused by
+ * prl_buf_set_shard.  prl_buf_gather_cost: out_dev f32[k]. */
+int prl_buf_cost_offset(const prl_buf_desc *desc, int32_t *out);
+int prl_buf_push_host_cost(prl_buf *buf, int64_t n, const float *state, const void *action,
+                           const float *reward, const float *next_state, const uint8_t *terminated,
+                           const uint8_t *truncated, const uint8_t *next_avail_ids,
+                           const int32_t *next_avail_cnt, const float *cost, void *stream);
+int prl_buf_push_device_cost(prl_buf *buf, int64_t n, const float *state, const void *action,
+                             const float *reward, const float *next_state, const uint8_t *terminated,
+                             const uint8_t *truncated, const uint8_t *next_avail_ids,
+                             const int32_t *next_avail_cnt, const float *cost, void *stream);
+int prl_buf_gather_cost(const prl_buf *buf, const int32_t *slot_dev, int k, float *out_dev, void *stream);
 
 /* ---- DQN / DoubleDQN learner ---------------------------------------------
  * Replaces DeepTDLearning.learn_batch + DeepQLearning / DoubleDQN
@@ -508,6 +533,53 @@ int prl_td3bc_create(prl_td3 **out, const prl_td3_cfg *cfg, const prl_td3bc_cfg 
                      const float *high_dev, int64_t actor_adam_step, int64_t critic_adam_step, void *workspace);
 /* TD3BC.alpha_bc (td3.py:295), read by the next call; TD3BC handles only */
 int prl_td3_set_alpha_bc(prl_td3 *td3, double alpha_bc);
+
+/* Cost-shaped rewards (ActorCriticBase.preprocess_batch, actor_critic_base.py:368-383, with a reward-constrained safety
+ * module): enable != 0 makes every round of the next prl_td3_learn calls train on reward - fp32(lambda) * cost, two
+ * rounded fp32 operations as torch evaluates them, with the cost read from the ring (a PRL_BUF_COST buffer: prl_td3_learn
+ * refuses any other while shaping is on).  lambda travels in the per-call block: changing it never re-captures a round.
+ * prl_td3_learn_batch never shapes (its batch is already preprocessed).  A handle starts with shaping off. */
+int prl_td3_set_cost_lambda(prl_td3 *td3, int enable, double lambda);
+
+/* ---- reward-constrained safety module (the cost critic and the Lagrange multiplier) ----------------
+ * Replaces RCSafetyModuleCostCriticContinuousAction.learn (safety_modules/reward_constrained_safety_module.py:115-216)
+ * for a TD3 / DDPG / TD3BC policy learner, called once per PearlAgent.learn after the policy learner's rounds
+ * (pearl_agent.py:213-220).  One call = one sample of `batch` indices (continuing the buffer's MT19937 stream) and one
+ * fixed launch sequence, captured as a CUDA graph:
+ *   a' = actor(s') (VanillaContinuousActorNetwork.sample_action: tanh scaled to the box, no noise),
+ *   y = min(Qc1', Qc2')(s', a') * cost_gamma * (1 - terminated) + cost,
+ *   twin MSE loss (mse1 + mse2) / 2 (critic_utils.py:170-203), AdamW(amsgrad) step with the soft update of the target
+ *   twin (every call), cq = mean(max(Qc1, Qc2)(s, actor(s))) with the UPDATED twin (one CTA, fixed order),
+ *   lambda = clip(lambda + lr_lambda * (cq * (1 - cost_gamma) - constraint_value), 0, lambda_ub) in float64 with the
+ *   reference's Python evaluation order.
+ * The twin cost critic, its target and the AdamW vectors are caller-owned (flat as prl_sac's critic: q1 then q2).  The
+ * policy's actor weights, its box and the multiplier travel in the per-call step block, so a re-created policy learner
+ * needs no new handle.  The host never waits inside prl_rcsafety_learn. */
+typedef struct prl_rcsafety_cfg {
+    int32_t obs_dim, act_dim, actor_h1, actor_h2, critic_h1, critic_h2;
+    int32_t max_batch;
+    double critic_lr, beta1, beta2, eps, weight_decay, cost_gamma, tau;
+} prl_rcsafety_cfg;
+typedef struct prl_rcsafety_step {
+    const float *actor_w;           /* device: the policy's actor, flat W1 b1 W2 b2 W3 b3 (prl_td3's layout) */
+    const float *low, *high;        /* device f32[act_dim]: the box the actor scales to */
+    double lambda_in, constraint_value, lr_lambda, lambda_ub;
+    double *out;                    /* device f64[3]: the new lambda, the cost-critic loss, cq */
+} prl_rcsafety_step;
+typedef struct prl_rcsafety prl_rcsafety;
+int64_t prl_rcsafety_param_count(const prl_rcsafety_cfg *cfg);   /* ONE cost critic; the twin vector holds two */
+int64_t prl_rcsafety_workspace_bytes(const prl_rcsafety_cfg *cfg);
+int prl_rcsafety_create(prl_rcsafety **out, const prl_rcsafety_cfg *cfg, float *critic_w, float *critic_m, float *critic_v,
+                        float *critic_vmax, float *critic_target_w, int64_t adam_step, void *workspace);
+int prl_rcsafety_destroy(prl_rcsafety *rc);
+int64_t prl_rcsafety_adam_step(const prl_rcsafety *rc);
+int prl_rcsafety_set_graph(prl_rcsafety *rc, int enable);
+int64_t prl_rcsafety_graph_captures(const prl_rcsafety *rc);
+int64_t prl_rcsafety_last_launches(const prl_rcsafety *rc);
+/* buf: a local continuous-action PRL_BUF_COST buffer of the configured dimensions.  out_logical_dev: optional device
+ * i32[batch], the sampled logical indices. */
+int prl_rcsafety_learn(prl_rcsafety *rc, prl_buf *buf, int batch, const prl_rcsafety_step *step, int32_t *out_logical_dev,
+                       void *stream);
 
 /* ---- Implicit Q-Learning (offline actor-critic) ----------------------------------------------------
  * Replaces ImplicitQLearning.learn_batch (policy_learners/sequential_decision_making/implicit_q_learning.py:159-302),

@@ -15,6 +15,7 @@ PRL_BUF_DISCRETE = 0x1
 PRL_BUF_CONTINUOUS = 0x2
 PRL_BUF_DYNAMIC_ACTIONS = 0x4
 PRL_BUF_NEXT_ACTION = 0x8
+PRL_BUF_COST = 0x10
 PRL_EINVAL = -1
 
 
@@ -60,6 +61,18 @@ class Td3Cfg(C.Structure):
 
 class Td3bcCfg(C.Structure):
     _fields_ = [("behavior_h1", C.c_int32), ("behavior_h2", C.c_int32)]
+
+
+class RcsafetyCfg(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("act_dim", C.c_int32), ("actor_h1", C.c_int32), ("actor_h2", C.c_int32),
+                ("critic_h1", C.c_int32), ("critic_h2", C.c_int32), ("max_batch", C.c_int32), ("critic_lr", C.c_double),
+                ("beta1", C.c_double), ("beta2", C.c_double), ("eps", C.c_double), ("weight_decay", C.c_double),
+                ("cost_gamma", C.c_double), ("tau", C.c_double)]
+
+
+class RcsafetyStep(C.Structure):
+    _fields_ = [("actor_w", C.c_void_p), ("low", C.c_void_p), ("high", C.c_void_p), ("lambda_in", C.c_double),
+                ("constraint_value", C.c_double), ("lr_lambda", C.c_double), ("lambda_ub", C.c_double), ("out", C.c_void_p)]
 
 
 class IqlCfg(C.Structure):
@@ -169,6 +182,10 @@ _SIGNATURES = {
     "prl_buf_push_device_sarsa": (C.c_int, [_P, C.c_int64] + [_P] * 10),
     "prl_buf_push_host_multi_sarsa": (C.c_int, [_P, C.c_int, C.c_int64] + [_P] * 8),
     "prl_buf_gather_next_action": (C.c_int, [_P, _P, C.c_int, _P, _P]),
+    "prl_buf_cost_offset": (C.c_int, [C.POINTER(BufDesc), C.POINTER(C.c_int32)]),
+    "prl_buf_push_host_cost": (C.c_int, [_P, C.c_int64] + [_P] * 10),
+    "prl_buf_push_device_cost": (C.c_int, [_P, C.c_int64] + [_P] * 10),
+    "prl_buf_gather_cost": (C.c_int, [_P, _P, C.c_int, _P, _P]),
     "prl_rng_set_state": (C.c_int, [_P, _P, _P]),
     "prl_rng_get_state": (C.c_int, [_P, _P, _P]),
     "prl_rng_seed": (C.c_int, [_P, _P, C.c_int, _P]),
@@ -236,6 +253,16 @@ _SIGNATURES = {
     "prl_td3bc_workspace_bytes": (C.c_int64, [C.POINTER(Td3Cfg), C.POINTER(Td3bcCfg)]),
     "prl_td3bc_create": (C.c_int, [C.POINTER(_P), C.POINTER(Td3Cfg), C.POINTER(Td3bcCfg)] + [_P] * 13 + [C.c_int64, C.c_int64, _P]),
     "prl_td3_set_alpha_bc": (C.c_int, [_P, C.c_double]),
+    "prl_td3_set_cost_lambda": (C.c_int, [_P, C.c_int, C.c_double]),
+    "prl_rcsafety_param_count": (C.c_int64, [C.POINTER(RcsafetyCfg)]),
+    "prl_rcsafety_workspace_bytes": (C.c_int64, [C.POINTER(RcsafetyCfg)]),
+    "prl_rcsafety_create": (C.c_int, [C.POINTER(_P), C.POINTER(RcsafetyCfg)] + [_P] * 5 + [C.c_int64, _P]),
+    "prl_rcsafety_destroy": (C.c_int, [_P]),
+    "prl_rcsafety_adam_step": (C.c_int64, [_P]),
+    "prl_rcsafety_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_rcsafety_graph_captures": (C.c_int64, [_P]),
+    "prl_rcsafety_last_launches": (C.c_int64, [_P]),
+    "prl_rcsafety_learn": (C.c_int, [_P, _P, C.c_int, C.POINTER(RcsafetyStep), _P, _P]),
     "prl_iql_actor_param_count": (C.c_int64, [C.POINTER(IqlCfg)]),
     "prl_iql_critic_param_count": (C.c_int64, [C.POINTER(IqlCfg)]),
     "prl_iql_value_param_count": (C.c_int64, [C.POINTER(IqlCfg)]),

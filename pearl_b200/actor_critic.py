@@ -225,11 +225,20 @@ class _B200ActorCriticMixin:
                 self._restart_core(core, steps)
         return core
 
+    # the CUDA learner trains on reward - lambda * cost when the safety module has a multiplier (TD3 / DDPG / TD3BC)
+    _cost_shaping = False
+
     # ---- PolicyLearner.learn (policy_learner.py:162-204)
     def learn(self, replay_buffer) -> dict:
         if len(replay_buffer) == 0:
             return {}
+        lam = getattr(getattr(self, "safety_module", None), "lambda_constraint", None)
+        if lam is not None and not self._cost_shaping:
+            raise NotImplementedError(f"{type(self).__name__}: the CUDA learner does not implement the reward-constrained "
+                                      "safety module (cost-shaped rewards); the CUDA TD3 / DDPG / TD3BC learners do")
         core = self._ensure_core()
+        if self._cost_shaping:
+            core.lambda_constraint = None if lam is None else float(lam)
         core._training_rounds, core._batch_size = int(self._training_rounds), int(self._batch_size)
         core._training_steps = int(self._training_steps)
         report = core.learn(replay_buffer)
@@ -445,6 +454,7 @@ if HAVE_REFERENCE:
 
     class _DeterministicMixin(_B200ActorCriticMixin):
         _core_cls = Td3Core
+        _cost_shaping = True
 
         def _core_kwargs(self) -> dict:
             return {}

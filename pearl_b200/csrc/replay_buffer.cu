@@ -73,9 +73,28 @@ extern "C" int prl_buf_layout_of(const prl_buf_desc *d, prl_buf_layout *out) {
     l.off_avail = l.off_flags + 1;
     int words = l.off_avail;
     if (d->flags & PRL_BUF_DYNAMIC_ACTIONS) words += (d->n_actions + 3) / 4;
+    if (d->flags & PRL_BUF_COST) words += 1;      // the cost word goes last: no offset above moves
     l.record_words = round_up(words, 4);
     l.storage_bytes = d->capacity * (int64_t)l.record_words * 4;
     *out = l;
+    return PRL_OK;
+}
+
+// the cost word of a PRL_BUF_COST record: right after the dynamic action ids (or after the flags word); -1 without costs
+static int cost_word(const prl_buf_desc *d) {
+    if (!(d->flags & PRL_BUF_COST)) return -1;
+    prl_buf_layout l;
+    prl_buf_layout_of(d, &l);
+    return l.off_avail + ((d->flags & PRL_BUF_DYNAMIC_ACTIONS) ? (d->n_actions + 3) / 4 : 0);
+}
+
+extern "C" int prl_buf_cost_offset(const prl_buf_desc *d, int32_t *out) {
+    PRL_REQUIRE(d && out, "null argument");
+    prl_buf_layout l;
+    const int rc = prl_buf_layout_of(d, &l);
+    if (rc) return rc;
+    PRL_REQUIRE(d->flags & PRL_BUF_COST, "the descriptor has no PRL_BUF_COST: its records store no cost");
+    *out = cost_word(d);
     return PRL_OK;
 }
 
@@ -181,12 +200,24 @@ static int check_next_action(const prl_buf *b, const void *next_action) {
     return PRL_OK;
 }
 
+// cost: the costs of a PRL_BUF_COST buffer (the *_cost entries), null for every other buffer
+static int check_cost(const prl_buf *b, const void *cost) {
+    PRL_REQUIRE(b, "null buffer");
+    if (b->desc.flags & PRL_BUF_COST)
+        PRL_REQUIRE(cost, "the buffer stores costs (PRL_BUF_COST): push with the *_cost entries");
+    else
+        PRL_REQUIRE(!cost, "costs given for a buffer created without PRL_BUF_COST");
+    return PRL_OK;
+}
+
 static int check_push_args(const prl_buf *b, int64_t n, const void *state, const void *action,
                            const void *reward, const void *terminated, const void *truncated,
-                           const void *ids, const void *cnt, const void *next_action) {
+                           const void *ids, const void *cnt, const void *next_action, const void *cost) {
     PRL_REQUIRE(b, "null buffer");
     PRL_REQUIRE(n >= 0, "negative count");
     int rc = check_next_action(b, next_action);
+    if (rc) return rc;
+    rc = check_cost(b, cost);
     if (rc) return rc;
     if (n == 0) return PRL_OK;
     PRL_REQUIRE(state && action && reward && terminated && truncated, "null field array");
@@ -200,9 +231,10 @@ static int check_push_args(const prl_buf *b, int64_t n, const void *state, const
 // pack transitions [i0, i0 + m) of struct-of-arrays host sources into m consecutive records at `st` (pure CPU)
 static void pack_records_host(const prl_buf *b, uint32_t *st, int64_t i0, int64_t m, const float *state, const void *action,
                               const float *reward, const float *next_state, const uint8_t *terminated, const uint8_t *truncated,
-                              const uint8_t *next_avail_ids, const int32_t *next_avail_cnt, const int32_t *next_action) {
+                              const uint8_t *next_avail_ids, const int32_t *next_avail_cnt, const int32_t *next_action,
+                              const float *cost) {
     const prl_buf_layout &L = b->lay;
-    const int obs = b->desc.obs_dim, A = b->desc.n_actions, W = L.record_words;
+    const int obs = b->desc.obs_dim, A = b->desc.n_actions, W = L.record_words, off_cost = cost_word(&b->desc);
     for (int64_t i = 0; i < m; i++) {
         const int64_t s = i0 + i;
         uint32_t *r = st + i * W;
@@ -230,6 +262,7 @@ static void pack_records_host(const prl_buf *b, uint32_t *st, int64_t i0, int64_
             else
                 for (int a = 0; a < A; a++) ids[a] = (uint8_t)a;
         }
+        if (cost) r[off_cost] = f2u(cost[s]);
     }
 }
 
@@ -244,9 +277,9 @@ static int check_next_ids_host(const prl_buf *b, int64_t n, const int32_t *next_
 
 static int push_host(prl_buf *b, int64_t n, const float *state, const void *action, const float *reward, const float *next_state,
                      const uint8_t *terminated, const uint8_t *truncated, const uint8_t *next_avail_ids,
-                     const int32_t *next_avail_cnt, const int32_t *next_action, void *stream_) {
+                     const int32_t *next_avail_cnt, const int32_t *next_action, const float *cost, void *stream_) {
     int rc = check_push_args(b, n, state, action, reward, terminated, truncated, next_avail_ids,
-                             next_avail_cnt, next_action);
+                             next_avail_cnt, next_action, cost);
     if (rc || n == 0) return rc;
     rc = check_next_ids_host(b, n, next_action);
     if (rc) return rc;
@@ -270,7 +303,7 @@ static int push_host(prl_buf *b, int64_t n, const float *state, const void *acti
         PRL_CUDA(cudaEventSynchronize(b->stage_done[sb]));
         uint32_t *st = b->stage[sb];
         pack_records_host(b, st, i0, m, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt,
-                          next_action);
+                          next_action, cost);
         PRL_CUDA(cudaMemcpyAsync(b->records + b->write_pos * W, st, m * (int64_t)W * 4,
                                  cudaMemcpyHostToDevice, stream));
         PRL_CUDA(cudaEventRecord(b->stage_done[sb], stream));
@@ -287,7 +320,15 @@ extern "C" int prl_buf_push_host(prl_buf *b, int64_t n, const float *state, cons
                                  const uint8_t *next_avail_ids, const int32_t *next_avail_cnt,
                                  void *stream_) {
     return push_host(b, n, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, nullptr,
-                     stream_);
+                     nullptr, stream_);
+}
+
+extern "C" int prl_buf_push_host_cost(prl_buf *b, int64_t n, const float *state, const void *action, const float *reward,
+                                      const float *next_state, const uint8_t *terminated, const uint8_t *truncated,
+                                      const uint8_t *next_avail_ids, const int32_t *next_avail_cnt, const float *cost, void *stream_) {
+    PRL_REQUIRE(cost || n == 0, "null cost");
+    return push_host(b, n, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, nullptr,
+                     cost, stream_);
 }
 
 extern "C" int prl_buf_push_host_sarsa(prl_buf *b, int64_t n, const float *state, const void *action, const float *reward,
@@ -296,7 +337,7 @@ extern "C" int prl_buf_push_host_sarsa(prl_buf *b, int64_t n, const float *state
                                        void *stream_) {
     PRL_REQUIRE(next_action || n == 0, "null next_action");
     return push_host(b, n, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, next_action,
-                     stream_);
+                     nullptr, stream_);
 }
 
 // The same push for `count` buffers of one layout at once (a vectorised environment feeding a learner group):
@@ -310,6 +351,9 @@ static int push_host_multi(prl_buf *const *bufs, int count, int64_t n, const flo
     PRL_REQUIRE(n >= 0, "negative count");
     for (int i = 0; i < count; i++) {
         int rc = check_next_action(bufs[i], next_action);
+        if (rc) return rc;
+        // no cost argument here: a cost buffer is refused rather than given cost 0
+        rc = check_cost(bufs[i], nullptr);
         if (rc) return rc;
     }
     if (n == 0) return PRL_OK;
@@ -357,7 +401,7 @@ static int push_host_multi(prl_buf *const *bufs, int count, int64_t n, const flo
         for (size_t j = t; j < fast.size(); j += T) {
             const float *s, *r, *ns; const void *a; const uint8_t *te, *tr; const int32_t *na;
             src(fast[j].idx, s, a, r, ns, te, tr, na);
-            pack_records_host(fast[j].b, fast[j].st, 0, n, s, a, r, ns, te, tr, nullptr, nullptr, na);
+            pack_records_host(fast[j].b, fast[j].st, 0, n, s, a, r, ns, te, tr, nullptr, nullptr, na, nullptr);
         }
     };
     std::vector<std::thread> pool;
@@ -376,7 +420,7 @@ static int push_host_multi(prl_buf *const *bufs, int count, int64_t n, const flo
     for (int i : slow) {
         const float *s, *r, *ns; const void *a; const uint8_t *te, *tr; const int32_t *na;
         src(i, s, a, r, ns, te, tr, na);
-        int rc = push_host(bufs[i], n, s, a, r, ns, te, tr, nullptr, nullptr, na, stream_);
+        int rc = push_host(bufs[i], n, s, a, r, ns, te, tr, nullptr, nullptr, na, nullptr, stream_);
         if (rc) return rc;
     }
     return PRL_OK;
@@ -405,7 +449,7 @@ __global__ void k_pack_records(uint32_t *__restrict__ records, prl_buf_layout L,
                                const uint8_t *__restrict__ terminated,
                                const uint8_t *__restrict__ truncated,
                                const uint8_t *__restrict__ ids, const int32_t *__restrict__ cnts,
-                               const int32_t *__restrict__ next_action) {
+                               const int32_t *__restrict__ next_action, int off_cost, const float *__restrict__ cost) {
     const int lane = threadIdx.x & 31;
     const int64_t w = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
     if (w >= n) return;
@@ -429,7 +473,9 @@ __global__ void k_pack_records(uint32_t *__restrict__ records, prl_buf_layout L,
             if (cnts) c = (uint32_t)cnts[s];
             v = (terminated[s] ? 1u : 0u) | (truncated[s] ? 2u : 0u) | (c << 8) |
                 (next_action ? ((uint32_t)next_action[s] & 0xffu) << 24 : 0u);
-        } else if (flags & PRL_BUF_DYNAMIC_ACTIONS) {
+        } else if (p == off_cost) {
+            v = __float_as_uint(cost[s]);
+        } else if ((flags & PRL_BUF_DYNAMIC_ACTIONS) && (off_cost < 0 || p < off_cost)) {
             int a0 = (p - L.off_avail) * 4;
             uint32_t c = cnts ? (uint32_t)cnts[s] : (uint32_t)A;
             for (int j = 0; j < 4; j++) {
@@ -445,9 +491,9 @@ __global__ void k_pack_records(uint32_t *__restrict__ records, prl_buf_layout L,
 
 static int push_device(prl_buf *b, int64_t n, const float *state, const void *action, const float *reward, const float *next_state,
                        const uint8_t *terminated, const uint8_t *truncated, const uint8_t *next_avail_ids,
-                       const int32_t *next_avail_cnt, const int32_t *next_action, void *stream_) {
+                       const int32_t *next_avail_cnt, const int32_t *next_action, const float *cost, void *stream_) {
     int rc = check_push_args(b, n, state, action, reward, terminated, truncated, next_avail_ids,
-                             next_avail_cnt, next_action);
+                             next_avail_cnt, next_action, cost);
     if (rc || n == 0) return rc;
     cudaStream_t stream = (cudaStream_t)stream_;
     const int64_t C = b->desc.capacity;
@@ -461,7 +507,8 @@ static int push_device(prl_buf *b, int64_t n, const float *state, const void *ac
     int64_t blocks = (m * 32 + threads - 1) / threads;
     k_pack_records<<<(unsigned)blocks, threads, 0, stream>>>(
         b->records, b->lay, b->desc.obs_dim, b->desc.n_actions, b->desc.flags, C, b->write_pos, first,
-        m, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, next_action);
+        m, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, next_action,
+        cost_word(&b->desc), cost);
     PRL_CUDA(cudaGetLastError());
     b->write_pos = (b->write_pos + m) % C;
     b->len = b->len + m > C ? C : b->len + m;
@@ -474,7 +521,16 @@ extern "C" int prl_buf_push_device(prl_buf *b, int64_t n, const float *state, co
                                    const uint8_t *next_avail_ids, const int32_t *next_avail_cnt,
                                    void *stream_) {
     return push_device(b, n, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, nullptr,
-                       stream_);
+                       nullptr, stream_);
+}
+
+extern "C" int prl_buf_push_device_cost(prl_buf *b, int64_t n, const float *state, const void *action, const float *reward,
+                                        const float *next_state, const uint8_t *terminated, const uint8_t *truncated,
+                                        const uint8_t *next_avail_ids, const int32_t *next_avail_cnt, const float *cost,
+                                        void *stream_) {
+    PRL_REQUIRE(cost || n == 0, "null cost");
+    return push_device(b, n, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, nullptr,
+                       cost, stream_);
 }
 
 extern "C" int prl_buf_push_device_sarsa(prl_buf *b, int64_t n, const float *state, const void *action, const float *reward,
@@ -483,7 +539,7 @@ extern "C" int prl_buf_push_device_sarsa(prl_buf *b, int64_t n, const float *sta
                                          void *stream_) {
     PRL_REQUIRE(next_action || n == 0, "null next_action");
     return push_device(b, n, state, action, reward, next_state, terminated, truncated, next_avail_ids, next_avail_cnt, next_action,
-                       stream_);
+                       nullptr, stream_);
 }
 
 // Shard of a logical replay buffer of `world * capacity` transitions (SURVEY.md 8e): the transition with global
@@ -492,6 +548,7 @@ extern "C" int prl_buf_push_device_sarsa(prl_buf *b, int64_t n, const float *sta
 extern "C" int prl_buf_set_shard(prl_buf *b, int rank, int world, int64_t global_pushed) {
     PRL_REQUIRE(b, "null buffer");
     PRL_REQUIRE(world >= 1 && world <= 16 && rank >= 0 && rank < world && global_pushed >= 0, "bad shard description");
+    PRL_REQUIRE(world == 1 || !(b->desc.flags & PRL_BUF_COST), "a buffer with costs (PRL_BUF_COST) cannot be sharded");
     const int64_t mine = global_pushed / world + ((global_pushed % world) > rank ? 1 : 0);   // g < global_pushed, g mod world == rank
     const int64_t expect = mine < b->desc.capacity ? mine : b->desc.capacity;
     PRL_REQUIRE(world == 1 || b->len == expect,
@@ -687,6 +744,24 @@ extern "C" int prl_buf_gather_next_action(const prl_buf *b, const int32_t *slot_
     PRL_REQUIRE(b->desc.flags & PRL_BUF_NEXT_ACTION, "the buffer was created without PRL_BUF_NEXT_ACTION: it stores no next action");
     if (k <= 0) return PRL_OK;
     k_gather_next_action<<<(k + 255) / 256, 256, 0, (cudaStream_t)stream_>>>(b->records, b->lay, slot_dev, k, (long long *)out_dev);
+    PRL_CUDA(cudaGetLastError());
+    return PRL_OK;
+}
+
+// the cost word of k records (PRL_BUF_COST)
+__global__ void k_gather_cost(const uint32_t *__restrict__ records, int W, int off_cost, const int32_t *__restrict__ slots, int k,
+                              float *__restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= k) return;
+    out[i] = __uint_as_float(records[(size_t)slots[i] * W + off_cost]);
+}
+
+extern "C" int prl_buf_gather_cost(const prl_buf *b, const int32_t *slot_dev, int k, float *out_dev, void *stream_) {
+    PRL_REQUIRE(b && slot_dev && out_dev, "null argument");
+    PRL_REQUIRE(b->desc.flags & PRL_BUF_COST, "the buffer was created without PRL_BUF_COST: it stores no cost");
+    if (k <= 0) return PRL_OK;
+    k_gather_cost<<<(k + 255) / 256, 256, 0, (cudaStream_t)stream_>>>(b->records, b->lay.record_words, cost_word(&b->desc), slot_dev, k,
+                                                                      out_dev);
     PRL_CUDA(cudaGetLastError());
     return PRL_OK;
 }

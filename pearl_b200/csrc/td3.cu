@@ -33,10 +33,14 @@ struct Td3Call {
     const float *d_state, *d_action, *d_reward, *d_next_state;
     const uint8_t *d_term;
     float alpha_bc;          // TD3BC: read every call, never baked into a captured round
+    int shape;               // 1: train on reward - fp32(lambda) * cost (prl_td3_set_cost_lambda); read every call
+    double lambda;
 };
 
 // records == null: copy the caller's dense batch from the call block instead of gathering from the ring
-__global__ void k_td3_gather(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int act, const Td3Call *__restrict__ call,
+// off_cost >= 0: the ring's cost word; with call->shape the reward is ActorCriticBase.preprocess_batch's
+// reward - lambda * cost, two fp32 roundings as torch does them (a Python float times an fp32 tensor is an fp32 product)
+__global__ void k_td3_gather(const uint32_t *__restrict__ records, prl_buf_layout L, int off_cost, int obs, int act, const Td3Call *__restrict__ call,
                              const int *__restrict__ round_idx, int B, float *__restrict__ S, float *__restrict__ A, float *__restrict__ R,
                              float *__restrict__ S2, float *__restrict__ T) {
     const int lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -57,7 +61,12 @@ __global__ void k_td3_gather(const uint32_t *__restrict__ records, prl_buf_layou
         S2[(size_t)w * obs + p] = __uint_as_float(r[L.off_next_state + p]);
     }
     for (int p = lane; p < act; p += 32) A[(size_t)w * act + p] = __uint_as_float(r[L.off_action + p]);
-    if (lane == 0) { R[w] = __uint_as_float(r[L.off_reward]); T[w] = (r[L.off_flags] & 1u) ? 1.f : 0.f; }
+    if (lane == 0) {
+        float rw = __uint_as_float(r[L.off_reward]);
+        if (off_cost >= 0 && call->shape) rw = __fsub_rn(rw, __fmul_rn((float)call->lambda, __uint_as_float(r[off_cost])));
+        R[w] = rw;
+        T[w] = (r[L.off_flags] & 1u) ? 1.f : 0.f;
+    }
 }
 
 // VanillaContinuousActorNetwork.sample_action: tanh head, action_scaling (actor_networks.py:29-51,475-485);
@@ -192,6 +201,8 @@ struct prl_td3 : Rounds<prl_td3, Td3Call> {
     const float *low, *high;
     int64_t actor_step;                // the actor optimizer's step count; adam_step counts the critic's
     float alpha_bc = 2.5f;             // TD3BC: copied into each call block
+    int shape = 0;                     // prl_td3_set_cost_lambda: copied into the call blocks of prl_td3_learn
+    double lambda = 0.0;
     float *S, *A, *R, *S2, *T, *h1, *h2, *pre, *act_s, *na, *c1, *c2, *q, *qt, *dq, *dc2, *dc1, *da, *dpre, *dh2, *dh1, *y, *g_actor,
         *g_critic, *last_actor_loss;
     float *bb1, *bb2, *bpre, *bact;    // TD3BC: the behaviour network's activations, pre-tanh output, tanh output
@@ -328,6 +339,13 @@ extern "C" int64_t prl_td3_critic_adam_step(const prl_td3 *s) { return prl_td3::
 extern "C" int prl_td3_set_graph(prl_td3 *s, int enable) { return prl_td3::set_graph(s, enable); }
 extern "C" int64_t prl_td3_last_launches(const prl_td3 *s) { return prl_td3::last_launches_of(s); }
 extern "C" int64_t prl_td3_graph_captures(const prl_td3 *s) { return s ? s->graphs.captures : -1; }
+extern "C" int prl_td3_set_cost_lambda(prl_td3 *s, int enable, double lambda) {
+    PRL_REQUIRE(s, "null handle");
+    PRL_REQUIRE(!enable || isfinite(lambda), "lambda must be finite");
+    s->shape = enable ? 1 : 0;
+    s->lambda = enable ? lambda : 0.0;
+    return PRL_OK;
+}
 extern "C" int prl_td3_set_alpha_bc(prl_td3 *s, double alpha_bc) {
     PRL_REQUIRE(s, "null handle");
     PRL_REQUIRE(s->is_bc(), "alpha_bc belongs to a TD3BC handle (prl_td3bc_create)");
@@ -368,8 +386,11 @@ int prl_td3::round_variant(prl_buf *buf, int B, int variant, cudaStream_t st) {
     };
     const int eb = 256;
     int small = 0;
-    k_td3_gather<<<(B * 32 + eb - 1) / eb, eb, 0, st>>>(buf ? buf->records : nullptr, buf ? buf->lay : prl_buf_layout{}, O, A, s->call,
-                                                        s->round_idx, B, s->S, s->A, s->R, s->S2, s->T);
+    // the cost word follows from the buffer's flags and layout, which the graph key compares
+    int32_t off_cost = -1;
+    if (buf && (buf->desc.flags & PRL_BUF_COST)) prl_buf_cost_offset(&buf->desc, &off_cost);
+    k_td3_gather<<<(B * 32 + eb - 1) / eb, eb, 0, st>>>(buf ? buf->records : nullptr, buf ? buf->lay : prl_buf_layout{}, off_cost, O, A,
+                                                        s->call, s->round_idx, B, s->S, s->A, s->R, s->S2, s->T);
     small++;
     if (update_actor) {
         // ---------------- actor step: maximise Q1(s, pi(s))   (ddpg.py:105-121)
@@ -442,8 +463,11 @@ int prl_td3::round_variant(prl_buf *buf, int B, int variant, cudaStream_t st) {
 extern "C" int prl_td3_learn(prl_td3 *s, prl_buf *buf, int rounds, int batch, int64_t training_steps0, const float *noise_dev,
                              float *out_actor_loss, float *out_critic_loss, int32_t *out_logical, void *stream_) {
     PRL_REQUIRE(s && buf && out_actor_loss && out_critic_loss, "null argument");
+    PRL_REQUIRE(!s->shape || (buf->desc.flags & PRL_BUF_COST),
+                "cost-shaped rewards need a buffer with costs (PRL_BUF_COST): the reference fails on batch.cost = None");
     Td3Call call{};
     call.noise = noise_dev; call.out_actor = out_actor_loss; call.out_critic = out_critic_loss;
+    call.shape = s->shape; call.lambda = s->lambda;
     const int rc = prl_td3::learn(s, buf, rounds, batch, training_steps0, out_logical, call, stream_);
     if (rc) return rc;
     for (int r = 0; r < rounds; r++) s->actor_step += s->variant(r);

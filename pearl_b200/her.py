@@ -14,6 +14,8 @@ from .replay_buffer import B200ReplayBuffer
 
 
 class B200HindsightExperienceReplayBuffer(B200ReplayBuffer):
+    _stores_costs = False           # its records carry no cost word: `cost` is refused
+
     def __init__(self, capacity: int, goal_dim: int, reward_fn: Callable, terminated_fn: Optional[Callable] = None, **kwargs) -> None:
         super().__init__(capacity, **kwargs)
         self._goal_dim = int(goal_dim)

@@ -14,6 +14,8 @@ from .replay_buffer import B200ReplayBuffer, _stream_ptr
 
 
 class B200PrioritizedReplayBuffer(B200ReplayBuffer):
+    _stores_costs = False           # its records carry no cost word: `cost` is refused
+
     def __init__(self, capacity: int, alpha: float = 0.6, beta: float = 0.4, eps: float = 1e-6, seed: int = 0,
                  **kwargs) -> None:
         super().__init__(capacity, **kwargs)

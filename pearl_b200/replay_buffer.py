@@ -33,6 +33,7 @@ def _stream_ptr(device) -> C.c_void_p:
 
 class B200ReplayBuffer(ReplayBuffer):
     _record_flags = 0               # PRL_BUF_* bits a subclass adds to every record layout it allocates
+    _stores_costs = True            # False: a subclass that refuses `cost` (its records have no cost word)
 
     def __init__(self, capacity: int, device: Optional[torch.device | str | int] = None,
                  dynamic_action_space: bool = False, rng: str = "python") -> None:
@@ -65,6 +66,7 @@ class B200ReplayBuffer(ReplayBuffer):
         self._lib = _lib.init(self._device.index)
         self._rng_mode = rng
         self._want_dynamic = bool(dynamic_action_space)
+        self._has_cost = False        # decided by the first push, as the reference decides from transitions[0].cost
         self._handle = C.c_void_p(0)
         self._storage = None
         self._mt = torch.zeros(625, dtype=torch.int32, device=self._device)
@@ -106,6 +108,11 @@ class B200ReplayBuffer(ReplayBuffer):
         return self._handle
 
     @property
+    def has_cost(self) -> bool:
+        """True when the records store a cost (the first push carried one); sample() then fills TransitionBatch.cost."""
+        return self._has_cost
+
+    @property
     def record_bytes(self) -> int:
         return 0 if self._layout is None else 4 * self._layout.record_words
 
@@ -113,6 +120,8 @@ class B200ReplayBuffer(ReplayBuffer):
         flags = _lib.PRL_BUF_CONTINUOUS if self._is_action_continuous else _lib.PRL_BUF_DISCRETE
         if dynamic:
             flags |= _lib.PRL_BUF_DYNAMIC_ACTIONS
+        if self._has_cost:
+            flags |= _lib.PRL_BUF_COST
         flags |= self._record_flags
         desc = _lib.BufDesc(self.capacity, obs_dim, act_dim, n_actions, flags)
         lay = _lib.BufLayout()
@@ -138,7 +147,7 @@ class B200ReplayBuffer(ReplayBuffer):
             cnt = (~old["mask"].bool()).sum(1).to(torch.int32)
             self.push_batch(old["state"], old["action"].to(torch.int32), old["reward"], old["next_state"],
                             old["terminated"], old["truncated"],
-                            next_available_ids=old["avail"].to(torch.uint8), next_available_count=cnt)
+                            next_available_ids=old["avail"].to(torch.uint8), next_available_count=cnt, cost=old.get("cost"))
 
     # ------------------------------------------------------------------ RNG
     def seed(self, seed: int) -> None:
@@ -183,8 +192,8 @@ class B200ReplayBuffer(ReplayBuffer):
     def push(self, state, action, reward, terminated, truncated, curr_available_actions=None,
              next_state=None, next_available_actions=None, max_number_actions=None, cost=None) -> None:
         """One transition, same signature as the reference (tensor_based_replay_buffer.py:55-69)."""
-        if cost is not None:
-            raise NotImplementedError("B200ReplayBuffer does not store costs")
+        if cost is not None and not self._stores_costs:
+            raise NotImplementedError(f"{type(self).__name__} does not store costs")
         st = torch.as_tensor(state, dtype=torch.float32).reshape(-1).cpu()
         nst = None if next_state is None else torch.as_tensor(next_state, dtype=torch.float32).reshape(-1).cpu()
         ids = cnt = None
@@ -209,18 +218,23 @@ class B200ReplayBuffer(ReplayBuffer):
                         None if nst is None else nst.unsqueeze(0),
                         torch.tensor([bool(terminated)]), torch.tensor([bool(truncated)]),
                         next_available_ids=ids, next_available_count=cnt,
-                        max_number_actions=max_number_actions)
+                        max_number_actions=max_number_actions,
+                        cost=None if cost is None else torch.tensor([float(cost)], dtype=torch.float32))
 
     def push_batch(self, state, action, reward, next_state, terminated, truncated,
-                   next_available_ids=None, next_available_count=None, max_number_actions=None) -> None:
+                   next_available_ids=None, next_available_count=None, max_number_actions=None, cost=None) -> None:
         """Vectorised push of n transitions (host or device tensors, struct-of-arrays).
 
         state/next_state [n, obs]; action [n] ints (discrete) or [n, act_dim] floats;
         reward [n]; terminated/truncated [n] bool; optional next_available_ids
         [n, A] uint8 + next_available_count [n] int32 (omit when every action is
-        available).  Host tensors are staged through pinned memory inside the
-        library; device tensors are packed by a kernel.
+        available); cost [n] floats (the first push decides whether the buffer
+        stores costs, and every later push must agree).  Host tensors are staged
+        through pinned memory inside the library; device tensors are packed by a
+        kernel.
         """
+        if cost is not None and not self._stores_costs:
+            raise NotImplementedError(f"{type(self).__name__} does not store costs")
         state = torch.as_tensor(state)
         n = state.shape[0]
         if n == 0:
@@ -250,15 +264,25 @@ class B200ReplayBuffer(ReplayBuffer):
                     raise ValueError("max_number_actions is required for the first discrete push")
         ids = prep(next_available_ids, torch.uint8)
         cnt = prep(next_available_count, torch.int32)
+        cost = prep(None if cost is None else torch.as_tensor(cost).reshape(n), torch.float32)
         if not self._handle.value:
+            self._has_cost = cost is not None
             self._allocate(state.shape[1], n_act, act_dim, self._want_dynamic or ids is not None)
+        elif (cost is not None) != self._has_cost:
+            raise ValueError("this buffer stores costs: every push needs one" if self._has_cost else
+                             "this buffer stores no costs (its first push had none): a push with costs is refused")
         if state.shape[1] != self.obs_dim:
             raise ValueError(f"state has {state.shape[1]} features, buffer stores {self.obs_dim}")
         if ids is not None and not (self._desc.flags & _lib.PRL_BUF_DYNAMIC_ACTIONS):
             self._upgrade_to_dynamic()
         with torch.cuda.device(self._device):
-            self._push_records(on_dev, n, [_lib.ptr(state), _lib.ptr(action), _lib.ptr(reward), _lib.ptr(next_state),
-                                           _lib.ptr(terminated), _lib.ptr(truncated), _lib.ptr(ids), _lib.ptr(cnt)])
+            fields = [_lib.ptr(state), _lib.ptr(action), _lib.ptr(reward), _lib.ptr(next_state), _lib.ptr(terminated),
+                      _lib.ptr(truncated), _lib.ptr(ids), _lib.ptr(cnt)]
+            if cost is not None:
+                fn = self._lib.prl_buf_push_device_cost if on_dev else self._lib.prl_buf_push_host_cost
+                _lib.check(fn(self._handle, n, *fields, _lib.ptr(cost), _stream_ptr(self._device)))
+            else:
+                self._push_records(on_dev, n, fields)
         if on_dev:  # keep the sources alive until the pack kernel has run
             torch.cuda.current_stream(self._device).synchronize()
 
@@ -306,7 +330,8 @@ class B200ReplayBuffer(ReplayBuffer):
             raise NotImplementedError("snapshot a sharded buffer shard by shard with set_shard cleared")
         n = self.local_len()
         out = dict(capacity=self.capacity, len=n, is_action_continuous=bool(self._is_action_continuous),
-                   obs_dim=self.obs_dim, n_actions=self.n_actions, act_dim=self.act_dim, rng_mode=self._rng_mode)
+                   obs_dim=self.obs_dim, n_actions=self.n_actions, act_dim=self.act_dim, rng_mode=self._rng_mode,
+                   cost=self._has_cost)
         if n:
             W = self._layout.record_words
             head = int(self._lib.prl_buf_head(self._handle))
@@ -326,10 +351,15 @@ class B200ReplayBuffer(ReplayBuffer):
             self.clear()
         if n == 0:
             return
-        if not self._handle.value or bool(self._desc.flags & _lib.PRL_BUF_DYNAMIC_ACTIONS) != bool(sd["dynamic"]):
+        has_cost = bool(sd.get("cost", False))      # a snapshot from before costs were stored is a plain buffer
+        if has_cost and not self._stores_costs:
+            raise NotImplementedError(f"{type(self).__name__} does not store costs")
+        if (not self._handle.value or bool(self._desc.flags & _lib.PRL_BUF_DYNAMIC_ACTIONS) != bool(sd["dynamic"])
+                or has_cost != self._has_cost):
             if self._handle.value:
                 self._lib.prl_buf_destroy(self._handle)
                 self._handle = C.c_void_p(0)
+            self._has_cost = has_cost
             self._allocate(int(sd["obs_dim"]), int(sd["n_actions"] or 0), int(sd["act_dim"]), bool(sd["dynamic"]))
         W = self._layout.record_words
         if int(sd["record_words"]) != W:
@@ -439,6 +469,10 @@ class B200ReplayBuffer(ReplayBuffer):
                 _lib.ptr(out["reward"]), _lib.ptr(out["next_state"]), _lib.ptr(out["terminated"]),
                 _lib.ptr(out["truncated"]), _lib.ptr(out["avail"]), _lib.ptr(out["mask"]),
                 _stream_ptr(dev)))
+            if self._has_cost:
+                out["cost"] = torch.empty((k,), dtype=torch.float32, device=dev)
+                _lib.check(self._lib.prl_buf_gather_cost(self.handle, _lib.ptr(slot.contiguous()), k, _lib.ptr(out["cost"]),
+                                                         _stream_ptr(dev)))
         return out
 
     def _gather_logical(self, logical: torch.Tensor) -> dict:
@@ -458,7 +492,7 @@ class B200ReplayBuffer(ReplayBuffer):
         if self._is_action_continuous:
             tb = TransitionBatch(state=g["state"], action=g["action"], reward=g["reward"],
                                  next_state=g["next_state"], terminated=g["terminated"],
-                                 truncated=g["truncated"])
+                                 truncated=g["truncated"], cost=g.get("cost"))
         else:
             A = self.n_actions
             curr = torch.arange(A, dtype=torch.float32, device=self._device).view(1, A, 1).expand(
@@ -470,5 +504,5 @@ class B200ReplayBuffer(ReplayBuffer):
                 curr_unavailable_actions_mask=torch.zeros((batch_size, A), dtype=torch.bool, device=self._device),
                 next_available_actions=g["avail"].unsqueeze(-1),
                 next_unavailable_actions_mask=g["mask"],
-                terminated=g["terminated"], truncated=g["truncated"])
+                terminated=g["terminated"], truncated=g["truncated"], cost=g.get("cost"))
         return tb

@@ -66,6 +66,7 @@ class B200SARSAReplayBuffer(B200ReplayBuffer):
     data, tests, benchmarks).  Discrete actions only."""
 
     _record_flags = _lib.PRL_BUF_NEXT_ACTION
+    _stores_costs = False           # its records carry no cost word: `cost` is refused
 
     def __init__(self, capacity: int, device=None, dynamic_action_space: bool = False, rng: str = "python") -> None:
         super().__init__(capacity, device=device, dynamic_action_space=dynamic_action_space, rng=rng)

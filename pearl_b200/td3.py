@@ -6,7 +6,8 @@ argument names and the same report keys (`actor_loss`, `critic_loss`) as the ref
 vectors and draws the target-policy noise (the reference's `torch.normal`); no math happens in Python.  No CPU fallback.
 `learn_batch(batch)` runs one round on a caller-supplied batch (`prl_td3_learn_batch`), as PearlAgent.learn_batch and
 offline_learning() call it.  B200TD3BC is Pearl's TD3BC (td3.py:241-318): the same round with a behaviour-cloning term in
-the actor loss."""
+the actor loss.  With a reward-constrained safety module's multiplier (`lambda_constraint`, or `safety_module.lambda_constraint`)
+`learn` trains on reward - lambda * cost, as ActorCriticBase.preprocess_batch does (actor_critic_base.py:368-383)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -28,7 +29,8 @@ class B200TD3:
                  discount_factor: float = 0.99, training_rounds: int = 1, batch_size: int = 256,
                  actor_update_freq: Optional[int] = None, actor_update_noise: Optional[float] = None,
                  actor_update_noise_clip: Optional[float] = None, *, low=None, high=None,
-                 device: Optional[torch.device | str | int] = None, max_rounds_per_call: int = 1024, seed: Optional[int] = None) -> None:
+                 device: Optional[torch.device | str | int] = None, max_rounds_per_call: int = 1024, seed: Optional[int] = None,
+                 lambda_constraint: Optional[float] = None, safety_module: Any = None) -> None:
         self._device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if self._device.index is None:
             self._device = torch.device("cuda", torch.cuda.current_device())
@@ -50,6 +52,9 @@ class B200TD3:
         self._max_rounds = max(int(max_rounds_per_call), 1)
         self._training_steps = 0
         self._last_actor_loss = 0.0    # what rounds without an actor update report (td3.py:104,122)
+        # the reward-constrained multiplier: `lambda_constraint` when set, else the safety module's, else no shaping
+        self.lambda_constraint = None if lambda_constraint is None else float(lambda_constraint)
+        self.safety_module = safety_module
         self.use_cuda_graph = True
         self._handle = C.c_void_p(0)
         self._bound_batch = 0
@@ -168,6 +173,13 @@ class B200TD3:
     def _before_call(self) -> None:
         pass
 
+    def _cost_lambda(self) -> Optional[float]:
+        """The multiplier learn() shapes rewards with (None: none), read on every call."""
+        if self.lambda_constraint is not None:
+            return float(self.lambda_constraint)
+        lam = getattr(self.safety_module, "lambda_constraint", None)
+        return None if lam is None else float(lam)
+
     def _noise(self, noise: Optional[torch.Tensor], r: int, B: int, start: int = 0) -> Optional[torch.Tensor]:
         """[r, B, A] target-policy noise: rows start.. of `noise`, or torch.normal(0, actor_update_noise) draws (td3.py:155-160)."""
         if self._actor_update_noise <= 0.0:
@@ -188,9 +200,15 @@ class B200TD3:
             return {}
         if not replay_buffer.is_action_continuous:
             raise ValueError("TD3 / DDPG need a replay buffer with is_action_continuous=True")
+        lam = self._cost_lambda()
+        if lam is not None and not replay_buffer.has_cost:
+            raise ValueError("a reward-constrained multiplier is set but the replay buffer stores no costs (the reference "
+                             "fails on batch.cost = None)")
         B = len(replay_buffer) if (self._batch_size == -1 or len(replay_buffer) < self._batch_size) else self._batch_size
         self._bind(B)
         self._before_call()
+        with torch.cuda.device(self._device):
+            _lib.check(self._lib.prl_td3_set_cost_lambda(self._handle, int(lam is not None), 0.0 if lam is None else lam))
         R, dev = self._training_rounds, self._device
         report = {"actor_loss": [], "critic_loss": []}
         idx_all = []
