@@ -19,7 +19,8 @@
 //            dW2 = dZ2^T H1, dW1s = dZ1^T S, and [db | dW1a] = dZ^T E with E = [1 | onehot(action)];
 //            their operands are explicitly transposed tiles written with a 144-byte chunk pitch
 //            (bank-conflict-free column scatter), 64 batch rows per pass, the two warpgroups issuing the same
-//            products on equal shares of the output columns.  Their accumulators stay in registers for the whole step.
+//            products on equal shares of the output columns.  The warpgroup that owns the pass's rows scatters their
+//            dZ2^T, H1^T and dZ1^T, the other one E^T, and both S^T.  The accumulators stay in registers for the whole step.
 //   AdamW    gradients registers -> shared staging, then one sweep over the flat W1 | b1 | W2 range whose parameters and
 //            moments stream in by TMA bulk copies, in 16 KB chunks through an 8-slot ring in regions 3 and 1 (free once
 //            the last weight-gradient products have been waited for); 16-byte stores write the results and the
@@ -40,6 +41,12 @@
 // C7520), and no conditional load feeding an A fragment; and each chain fits in the registers together with everything
 // live across it (C7511 / C7512), which is why H1 and dZ2 wait in shared memory while dH1 is formed and the learner
 // descriptor and the dW3 partial sums live in shared memory.  tests/test_dqn_tc_sass.py checks the SASS.
+// Spills cost more here than usual: the 225 KB of shared memory leave at most 28 KB of L1 for the spill frame of 256
+// threads, so spill traffic reaches L2.  Values that are the same in every round must not be hoisted out of the round
+// loop into registers: the wgmma descriptors are built next to each wgmma (umma::Tile::desc) and the shared-memory
+// offsets that follow from the thread index are recomputed where they are used (tid_here).  Hoisted, both stay live
+// across every chain and make up most of the spills.  tests/test_dqn_tc_spills.py bounds the spill bytes and keeps
+// spill reloads out of the chains.
 #include <math.h>
 #include <stdarg.h>
 #include <stdlib.h>
@@ -120,6 +127,18 @@ __device__ __forceinline__ void cp_async16_zfill_tc(void *smem_dst, const void *
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(sa), "l"(gmem_src), "r"(src_bytes) : "memory");
 }
 
+// threadIdx.x, opaque to the compiler at the point of use: the shared-memory offsets derived from it are recomputed where
+// they are needed instead of being hoisted out of the round loop and kept live (and spilled) across the wgmma chains
+__device__ __forceinline__ int tid_here() {
+    int t = threadIdx.x;
+    asm volatile("" : "+r"(t));
+    return t;
+}
+// this thread's row p (0, 1) of its warpgroup's 64-row block (umma::acc_row), from tid_here()
+__device__ __forceinline__ int acc_row_here(int p) {
+    const int t = tid_here();
+    return ((t >> 5) & 3) * 16 + ((t & 31) >> 2) + 8 * p;
+}
 __device__ __forceinline__ void group_sync(int g) { asm volatile("bar.sync %0, %1;" ::"r"(1 + g), "r"(128) : "memory"); }
 
 __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
@@ -164,7 +183,7 @@ __device__ void rebuild_tiles(const float *__restrict__ net, const Dims &d, cons
 }
 // the small fp32 vectors of a network (action columns + b1, b2, w3, b3); all loads of a thread issued before the first use
 __device__ void load_smalls(const float *__restrict__ net, const Dims &d, Misc::Smalls &mi) {
-    const int tid = threadIdx.x;
+    const int tid = tid_here();
     float wa[4], bb[4];                                           // A * 64 <= 1024 elements: <= 4 per thread
 #pragma unroll
     for (int u = 0; u < 4; u++) {
@@ -209,7 +228,7 @@ __device__ __forceinline__ float adam_math(float w, float &m, float &v, float &x
 // chunk kc + 1 is in flight while chunk kc is multiplied, and chunk 0 of a block is issued by the caller (l1_issue)
 // ahead of layer1_block, as early as its buffer is free.
 __device__ __forceinline__ void l1_issue(const TcArgs &a, const TcLearner &L, const Misc &mi, char *smem, int field_off, int row0, int kc) {
-    const int m = threadIdx.x & 127, g = threadIdx.x >> 7;
+    const int ft = tid_here(), m = ft & 127, g = ft >> 7;
     float *sbuf = reinterpret_cast<float *>(smem + REG2 + g * 2 * SBUF + (kc & 1) * SBUF);
 #pragma unroll 4
     for (int i = 0; i < 8; i++) {
@@ -222,7 +241,7 @@ __device__ __forceinline__ void l1_issue(const TcArgs &a, const TcLearner &L, co
 }
 __device__ __forceinline__ void layer1_block(const TcArgs &a, const TcLearner &L, const Misc &mi, char *smem, int field_off, int row0,
                                              float (&t1)[32]) {
-    const int g = threadIdx.x >> 7, t = threadIdx.x & 3;
+    const int g = threadIdx.x >> 7;
     const int k1 = k1_cols(a.d.obs);
     const umma::Tile B_hi = umma::make_tile(smem + REG1, k1, 128), B_lo = umma::make_tile(smem + REG1 + HALF, k1, 128);
     for (int kc = 0; kc * 64 < k1; kc++) {
@@ -231,6 +250,7 @@ __device__ __forceinline__ void layer1_block(const TcArgs &a, const TcLearner &L
         cp_async_wait<1>();
         group_sync(g);
         const float *sbuf = reinterpret_cast<const float *>(smem + REG2 + g * 2 * SBUF + (kc & 1) * SBUF);
+        const int t = tid_here() & 3, r0 = acc_row_here(0);
         float hi[32], lo[32];
 #pragma unroll
         for (int ks = 0; ks < 8; ks++)
@@ -238,7 +258,7 @@ __device__ __forceinline__ void layer1_block(const TcArgs &a, const TcLearner &L
             for (int q = 0; q < 2; q++)
 #pragma unroll
                 for (int p = 0; p < 2; p++) {
-                    const int r = umma::acc_row(p), k = 8 * ks + t + 4 * q;
+                    const int r = r0 + 8 * p, k = 8 * ks + t + 4 * q;
                     umma::split_tf32(sbuf[r * 64 + (((k >> 2) ^ (r & 7)) << 2) + (k & 3)], hi[4 * ks + 2 * q + p], lo[4 * ks + 2 * q + p]);
                 }
         group_sync(g);   // the buffer is free for chunk kc + 2 (or chunk 0 of the next block)
@@ -304,7 +324,6 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     const int h = tid >> 7, t4 = tid & 3;
     const int ntiles = a.B >> 7;
     const int W = a.lay.record_words;
-    const int rA = umma::acc_row(0), rB = umma::acc_row(1);   // this thread's two rows of its warpgroup's 64-row block
 
     // De-phase the learners: identical CTAs started together run in lock-step and hit L2 / HBM with their AdamW sweeps
     // (432 KB each) and row gathers all at once; a start offset of up to ~50 us spreads those bursts over the round.
@@ -412,7 +431,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             // chunk 0 of the next layer-1 block (the next row tile, or phase O's first) loads during the action loop
             if (i + 1 < ntiles) l1_issue(a, L, mi, smem, a.lay.off_next_state, row0 + 128, 0);
             else l1_issue(a, L, mi, smem, a.lay.off_state, h * 64, 0);
-            const int rows[2] = {row0 + rA, row0 + rB};
+            const int rows[2] = {row0 + acc_row_here(0), row0 + acc_row_here(1)};
             int cnt[2];
             const uint8_t *ids[2];
             float best[2] = {-INFINITY, -INFINITY};
@@ -423,6 +442,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                                                                 : kIota;
             }
             for (int act = 0; act < d.A; act++) {
+                const int t4 = tid_here() & 3;
                 float hi[32], lo[32], acc[32];
 #pragma unroll
                 for (int p = 0; p < 2; p++) {
@@ -496,7 +516,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             umma::mbar_wait(bar + 1, par_w1);
             par_w1 ^= 1;
             __syncthreads();   // also: the W2^T tiles are complete
-            const int rows[2] = {row0 + rA, row0 + rB};
+            const int rows[2] = {row0 + acc_row_here(0), row0 + acc_row_here(1)};
             float h1[32], z[32], hi[32], lo[32];
             layer1_block(a, L, mi, smem, a.lay.off_state, row0, h1);
             if (i == 0) TC_STAMP(5);
@@ -573,8 +593,10 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             }
             if (i == 0) TC_STAMP(6);
 
-            // ---- weight gradients: contractions over the batch rows, 64 rows (one warpgroup's block) per pass
+            // ---- weight gradients: contractions over the batch rows, 64 rows (one warpgroup's block) per pass; the owner of the
+            //      block scatters the transposes of its rows while the other warpgroup builds E^T
             for (int hf = 0; hf < 2; hf++) {
+                const int ft = tid_here(), h = ft >> 7, t4 = ft & 3, lane = ft & 31, warp = ft >> 5, rA = acc_row_here(0), rB = rA + 8;
                 const bool mine = h == hf;
                 const bool first = (i == 0 && hf == 0);
                 __syncthreads();   // previous products have been waited for: the arena is free
@@ -589,13 +611,16 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                                 arena[AR_A_HI / 4 + idx] = z[c]; arena[AR_A_LO / 4 + idx] = tf32_lo(z[c]);       // dZ2^T
                                 arena[AR_B_HI / 4 + idx] = h1[c]; arena[AR_B_LO / 4 + idx] = tf32_lo(h1[c]);     // H1^T
                             }
+                } else {
 #pragma unroll
-                    for (int p = 0; p < 2; p++)
+                    for (int p = 0; p < 2; p++) {                     // E^T: [1 | onehot(action)] of the owner's rows
+                        const int r = p ? rB : rA, act = mi.act[i * 128 + hf * 64 + r];
 #pragma unroll
-                        for (int x = 0; x < 8; x++) {                 // E^T: [1 | onehot(action)]
+                        for (int x = 0; x < 8; x++) {
                             const int er = t4 * 8 + x;
-                            arena[AR_E / 4 + umma::tile_index2(er, p ? rB : rA, 64, TL)] = (er == 0 || er == ai[p] + 1) ? 1.f : 0.f;
+                            arena[AR_E / 4 + umma::tile_index2(er, r, 64, TL)] = (er == 0 || er == act + 1) ? 1.f : 0.f;
                         }
+                    }
                 }
                 umma::fence_async_smem();
                 __syncthreads();
@@ -603,7 +628,8 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 umma::gemm3<8>(gb2, TA_hi, TA_lo, TE, TE, 64, !first, false, true);
                 umma::wg_commit();
                 // S^T: every warp reads whole state rows of this half coalesced (lane = k) and scatters them into column rq of
-                // the transposed tile; the first four rows are requested BEFORE waiting for the dW2 product
+                // the transposed tile.  The first four rows are prefetched into L1 under the dW2 product: held in registers
+                // across it they are spilled, and each spill store waits for its load.
                 float sv[4][4];
                 auto st_rows_load = [&](int r0) {
 #pragma unroll
@@ -626,9 +652,14 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                             }
                     }
                 };
-                st_rows_load(0);
+                if (lane < 16 && 32 * (lane & 3) < d.obs) {   // lane 4 ri + c: 128-byte line c of row warp + 8 ri
+                    const float *src = reinterpret_cast<const float *>(L.records + (size_t)mi.slot[i * 128 + hf * 64 + warp + 8 * (lane >> 2)] * W) +
+                                       a.lay.off_state + 32 * (lane & 3);
+                    asm volatile("prefetch.global.L1 [%0];" ::"l"(src));
+                }
                 umma::wg_wait<0>();
                 __syncthreads();
+                st_rows_load(0);
                 if (mine) {
 #pragma unroll
                     for (int j = 0; j < 8; j++)
@@ -682,7 +713,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             float *gs_b1 = gs_w1 + 64 * pitch1, *gs_b2 = gs_b1 + 64;
 #pragma unroll
             for (int p = 0; p < 2; p++) {
-                const int j = p ? rB : rA;                             // the gradient's row = hidden unit
+                const int j = acc_row_here(p);                         // the gradient's row = hidden unit
 #pragma unroll
                 for (int jb = 0; jb < 4; jb++)
 #pragma unroll

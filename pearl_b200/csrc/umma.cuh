@@ -68,7 +68,14 @@ __device__ __forceinline__ uint64_t make_desc2(uint32_t smem_addr, int lbo_bytes
 struct Tile {
     uint32_t addr;  // shared-memory byte address
     int lbo, sbo;   // bytes
-    __device__ __forceinline__ uint64_t desc(int kstep) const { return make_desc2(addr + (uint32_t)kstep * 2 * lbo, lbo, sbo); }
+    // The descriptor of K step `kstep`, built from the 32-bit address right where its wgmma is issued.  The address passes
+    // through an empty volatile asm, so the compiler cannot hoist the descriptors out of the loops around a product and
+    // keep every K step's 64-bit descriptor live (and spilled) across a whole kernel.
+    __device__ __forceinline__ uint64_t desc(int kstep) const {
+        uint32_t a = addr;
+        asm volatile("" : "+r"(a));
+        return make_desc2(a + (uint32_t)kstep * 2 * lbo, lbo, sbo);
+    }
     __device__ __forceinline__ Tile rows_from(int r) const { return Tile{addr + (uint32_t)(r >> 3) * sbo, lbo, sbo}; }  // r % 8 == 0
     __device__ __forceinline__ Tile shifted(uint32_t bytes) const { return Tile{addr + bytes, lbo, sbo}; }
 };
@@ -149,21 +156,18 @@ __device__ __forceinline__ void mma_rs<64>(float *d, const float *a, uint64_t b_
 
 // 3xTF32, SS form: d[64 x N] (+)= A[64 x K] * B[N x K]^T; executed by every thread of ONE warpgroup, which must have
 // fenced its shared-memory writes (fence_async_smem + barrier) before.  *_exact: the operand is exactly representable in
-// TF32 (0/1 indicators), its lo tile is not needed.  Descriptors are built once; a K step of 8 only adds (2*lbo)>>4 to the
-// 14-bit start-address field.  The caller commits and waits (wg_commit / wg_wait).
+// TF32 (0/1 indicators), its lo tile is not needed.  Each wgmma gets its descriptors from Tile::desc.  The caller commits
+// and waits (wg_commit / wg_wait).
 template <int N>
 __device__ __forceinline__ void gemm3(float *d, Tile a_hi, Tile a_lo, Tile b_hi, Tile b_lo, int K, bool accumulate_first,
                                       bool a_exact = false, bool b_exact = false) {
-    uint64_t ah = a_hi.desc(0), al = a_lo.desc(0), bh = b_hi.desc(0), bl = b_lo.desc(0);
-    const uint64_t da = (uint64_t)((2 * a_hi.lbo) >> 4), db = (uint64_t)((2 * b_hi.lbo) >> 4);
     bool acc = accumulate_first;
     wg_fence();
     for (int ks = 0; ks < (K >> 3); ks++) {
-        if (!a_exact) { Mma<N>::ss(d, al, bh, acc); acc = true; }   // small terms first
-        if (!b_exact) { Mma<N>::ss(d, ah, bl, acc); acc = true; }
-        Mma<N>::ss(d, ah, bh, acc);
+        if (!a_exact) { Mma<N>::ss(d, a_lo.desc(ks), b_hi.desc(ks), acc); acc = true; }   // small terms first
+        if (!b_exact) { Mma<N>::ss(d, a_hi.desc(ks), b_lo.desc(ks), acc); acc = true; }
+        Mma<N>::ss(d, a_hi.desc(ks), b_hi.desc(ks), acc);
         acc = true;
-        ah += da; al += da; bh += db; bl += db;
     }
 }
 
@@ -173,16 +177,13 @@ __device__ __forceinline__ void gemm3(float *d, Tile a_hi, Tile a_lo, Tile b_hi,
 template <int N, int KSTEPS>
 __device__ __forceinline__ void gemm3_rs(float *d, const float *a_hi, const float *a_lo, Tile b_hi, Tile b_lo, bool accumulate_first,
                                          int ksteps = KSTEPS) {
-    uint64_t bh = b_hi.desc(0), bl = b_lo.desc(0);
-    const uint64_t db = (uint64_t)((2 * b_hi.lbo) >> 4);
     wg_fence();
 #pragma unroll
     for (int ks = 0; ks < KSTEPS; ks++) {
         if (ks >= ksteps) break;
-        mma_rs<N>(d, a_lo + 4 * ks, bh, accumulate_first || ks > 0);
-        mma_rs<N>(d, a_hi + 4 * ks, bl, true);
-        mma_rs<N>(d, a_hi + 4 * ks, bh, true);
-        bh += db; bl += db;
+        mma_rs<N>(d, a_lo + 4 * ks, b_hi.desc(ks), accumulate_first || ks > 0);
+        mma_rs<N>(d, a_hi + 4 * ks, b_lo.desc(ks), true);
+        mma_rs<N>(d, a_hi + 4 * ks, b_hi.desc(ks), true);
     }
 }
 
