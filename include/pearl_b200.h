@@ -1121,6 +1121,63 @@ int prl_nlb_learn_batch(prl_nlb *nlb, int batch, const float *state, const float
 int prl_nlb_scores(prl_nlb *nlb, int n, const float *state, int n_space, const float *act_feat, double alpha, int mode,
                    const uint8_t *mask, float *out_scores, int32_t *out_index, void *stream);
 
+/* ---- contextual bandit: NeuralBandit (SquareCB / FastCB / greedy) -------------------------------------------------
+ * Replaces NeuralBandit.learn_batch / act / get_scores (policy_learners/contextual_bandits/neural_bandit.py) over
+ * VanillaValueNetwork with two hidden layers and one output.  Network input x = state (action_dim 0: state_features_only)
+ * or state || action features; p = mlp_block(x, [h1, h2], output_dim = 1) with ReLU.  Per round: forward with the current
+ * parameters; loss = sum(w l(p, y)) / sum(w), l = mse (0) or l1 (1), with no short circuit (a zero sum gives inf / NaN);
+ * backward and one AdamW(amsgrad) step over the network.  Flat parameters w f32[param_count] in torch's parameters()
+ * order: W1[h1][f] b1 W2[h2][h1] b2 W3[1][h2] b3; m / v / vmax are the AdamW exp_avg / exp_avg_sq / max_exp_avg_sq of
+ * the same layout.  score_rows: rows the workspace holds for scoring per chunk (0: max_batch). */
+typedef struct prl_nb_cfg {
+    int32_t obs_dim, n_actions, action_dim;
+    int32_t action_rep;            /* 0: none (state alone, or learn_batch / scores), 1: one-hot, 2: binary */
+    int32_t h1, h2;
+    int32_t loss;                  /* 0: mse, 1: mae (l1) */
+    int32_t max_batch, max_rounds, score_rows;
+    double lr, beta1, beta2, eps, weight_decay;
+} prl_nb_cfg;
+typedef struct prl_nb prl_nb;
+int64_t prl_nb_param_count(const prl_nb_cfg *cfg);
+int64_t prl_nb_workspace_bytes(const prl_nb_cfg *cfg);
+int prl_nb_create(prl_nb **out, const prl_nb_cfg *cfg, float *w, float *m, float *v, float *vmax, int64_t adam_step,
+                  void *workspace_dev);
+int prl_nb_destroy(prl_nb *nb);
+int prl_nb_set_graph(prl_nb *nb, int enable);
+int prl_nb_set_lr(prl_nb *nb, double lr);              /* from the next call on; no new capture */
+int64_t prl_nb_adam_step(const prl_nb *nb);
+int prl_nb_set_adam_step(prl_nb *nb, int64_t step);
+int64_t prl_nb_last_launches(const prl_nb *nb);
+int64_t prl_nb_graph_captures(const prl_nb *nb);     /* rounds captured into CUDA graphs so far */
+/* out_pred_dev (the pre-step network output) / out_label_dev / out_weight_dev: device f32[rounds][batch] (label and weight
+ * may be null); out_loss_dev f32[rounds]; out_logical_dev (optional) i32[rounds][batch] = sampled indices.  Every stored
+ * transition has weight 1. */
+int prl_nb_learn(prl_nb *nb, prl_buf *buf, int rounds, int batch, float *out_pred_dev, float *out_label_dev,
+                 float *out_weight_dev, float *out_loss_dev, int32_t *out_logical_dev, void *stream);
+/* One round on a dense device batch (as prl_nlb_learn_batch; action null when action_dim is 0, weight null: all 1;
+ * weights of either sign). */
+int prl_nb_learn_batch(prl_nb *nb, int batch, const float *state, const float *action, const float *reward, const float *weight,
+                       float *out_pred_dev, float *out_loss_dev, void *stream);
+/* The network's output over n states x n_space actions (state and act_feat as prl_nlb_scores) into out_scores_dev
+ * f32[n][n_space]. */
+int prl_nb_scores(prl_nb *nb, int n, const float *state, int n_space, const float *act_feat, float *out_scores_dev, void *stream);
+/* act: the scores as prl_nb_scores into out_values_dev, then
+ *   kind 0 (NoExploration): out_index_dev i32[n] = the first maximum of each state over the positions whose mask
+ *          (u8[n][n_space], may be null) is non-zero, 0 when none is;
+ *   kind 1 (SquareCB) / 2 (FastCB), n = 1: prl_nb_explore on the state's values; the mask is ignored, as the reference
+ *          ignores it.
+ * No host synchronisation. */
+int prl_nb_act(prl_nb *nb, int n, const float *state, int n_space, const float *act_feat, int kind, double gamma, double lb,
+               double ub, int clamp, const float *E_dev, const uint8_t *mask, float *out_values_dev, float *out_prob_dev,
+               int32_t *out_index_dev, void *stream);
+/* SquareCB / FastCB action choice of one state (squarecb_exploration.py act), in fp32 with gamma, lb and ub rounded to
+ * fp32: values clamped to [lb, ub] when clamp (always for FastCB); the first maximum; p = 1 / (A + gamma gap) (SquareCB) or
+ * (max - lb) / (A (max - lb) + gamma gap), 1 / A when max <= lb (FastCB); p[max] = 1 - the sum of the others; pn = p / sum p;
+ * out_index_dev i32[1] = the first maximum of pn / E over E_dev f32[n_space], the exponential draws of torch's one-sample
+ * multinomial.  out_prob_dev f32[n_space] (may be null) = pn.  Device pointers; no handle. */
+int prl_nb_explore(int n_space, const float *values_dev, int kind, double gamma, double lb, double ub, int clamp, const float *E_dev,
+                   float *out_prob_dev, int32_t *out_index_dev, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

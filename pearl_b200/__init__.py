@@ -21,9 +21,11 @@ from .actor_critic import (B200ContinuousSoftActorCritic, B200DeepDeterministicP
                            B200REINFORCE, B200SoftActorCritic, B200TD3, B200TD3BC)
 from .bandit import B200LinearBandit  # noqa: F401
 from .neural_linear import B200NeuralLinearBandit  # noqa: F401
+from .neural_bandit import B200NeuralBandit  # noqa: F401
 # a subclass of the reference's RCSafetyModuleCostCriticContinuousAction when Pearl is importable, stand-alone otherwise
 from .rc_safety import B200RCSafetyModuleCostCriticContinuousAction  # noqa: F401
 from ._compat import BinaryActionTensorRepresentationModule, UCBExploration  # noqa: F401
+from ._compat import FastCBExploration, LossType, NoExploration, SquareCBExploration  # noqa: F401
 from .dist import B200Communicator, all_gather_bytes, shard_owner  # noqa: F401
 
 __all__ = ["B200ReplayBuffer", "B200DeepQLearning", "B200DoubleDQN", "TransitionBatch",
@@ -31,4 +33,5 @@ __all__ = ["B200ReplayBuffer", "B200DeepQLearning", "B200DoubleDQN", "Transition
            "B200TD3", "B200DeepDeterministicPolicyGradient", "B200HindsightExperienceReplayBuffer", "B200ImplicitQLearning",
            "B200QuantileRegressionDeepQLearning", "B200REINFORCE", "DuelingQValueNetwork", "VanillaQValueMultiHeadNetwork",
            "B200DeepSARSA", "B200SARSAReplayBuffer", "B200TD3BC", "B200LinearBandit", "B200NeuralLinearBandit", "UCBExploration",
-           "BinaryActionTensorRepresentationModule", "B200RCSafetyModuleCostCriticContinuousAction"]
+           "BinaryActionTensorRepresentationModule", "B200RCSafetyModuleCostCriticContinuousAction", "B200NeuralBandit",
+           "SquareCBExploration", "FastCBExploration", "NoExploration", "LossType"]

@@ -292,6 +292,11 @@ try:  # pragma: no cover - depends on the environment; kept apart so the names a
     )
     from pearl.policy_learners.contextual_bandits.linear_bandit import LinearBandit as _RefLinearBandit
     from pearl.policy_learners.contextual_bandits.neural_linear_bandit import NeuralLinearBandit as _RefNeuralLinearBandit
+    from pearl.policy_learners.contextual_bandits.neural_bandit import NeuralBandit as _RefNeuralBandit
+    from pearl.policy_learners.exploration_modules.common.no_exploration import NoExploration
+    from pearl.policy_learners.exploration_modules.contextual_bandits.squarecb_exploration import (
+        FastCBExploration, SquareCBExploration,
+    )
     from pearl.neural_networks.common.utils import LossType
     from pearl.policy_learners.exploration_modules.common.tiebreaking_strategy import TiebreakingStrategy
     from pearl.policy_learners.exploration_modules.contextual_bandits.ucb_exploration import UCBExploration
@@ -487,6 +492,70 @@ if not HAVE_PEARL_BANDITS:
             self.apply_discounting_interval = apply_discounting_interval
             self.last_sum_weight_when_discounted = 0.0
             self.separate_uncertainty = separate_uncertainty
+
+        @property
+        def feature_dim(self) -> int:
+            return self._feature_dim
+
+        @property
+        def batch_size(self) -> int:
+            return self._batch_size
+
+        @property
+        def optimizer(self):
+            return self._optimizer
+
+        def set_history_summarization_module(self, value) -> None:
+            self._optimizer.add_param_group({"params": value.parameters()})
+            self._history_summarization_module = value
+
+        def reset(self, action_space) -> None:
+            pass
+
+    class SquareCBExploration:
+        """Attribute-compatible stand-in for SquareCBExploration (exploration_modules/contextual_bandits/
+        squarecb_exploration.py): the constructor and the attributes the CUDA learner reads."""
+
+        def __init__(self, gamma: float, reward_lb: float = 0.0, reward_ub: float = 1.0, clamp_values: bool = False,
+                     randomized_tiebreaking: bool = False) -> None:
+            self._gamma = gamma
+            self.reward_lb = reward_lb
+            self.reward_ub = reward_ub
+            self.clamp_values = clamp_values
+            self.randomized_tiebreaking = randomized_tiebreaking
+
+    class FastCBExploration(SquareCBExploration):
+        """Stand-in for FastCBExploration: SquareCB's attributes with clamping always on."""
+
+        def __init__(self, gamma: float, reward_lb: float = 0.0, reward_ub: float = 1.0) -> None:
+            super().__init__(gamma=gamma, reward_lb=reward_lb, reward_ub=reward_ub, clamp_values=True)
+
+    class NoExploration:
+        """Stand-in for NoExploration (exploration_modules/common/no_exploration.py): the first maximum of the values."""
+
+        def __init__(self, randomized_tiebreaking: bool = False) -> None:
+            self.randomized_tiebreaking = randomized_tiebreaking
+
+    class _RefNeuralBandit(nn.Module):
+        """Attribute-compatible stand-in for NeuralBandit's constructor (policy_learners/contextual_bandits/neural_bandit.py
+        on top of ContextualBanditBase / PolicyLearner): same arguments, defaults and state_dict keys
+        (`model._model.{0,1,2}.0.{weight,bias}`, VanillaValueNetwork's mlp_block)."""
+
+        def __init__(self, feature_dim: int, hidden_dims, exploration_module, output_dim: int = 1, training_rounds: int = 100,
+                     batch_size: int = 128, learning_rate: float = 0.001, state_features_only: bool = False,
+                     loss_type=LossType.MSE, action_representation_module=None) -> None:
+            super().__init__()
+            self.exploration_module = exploration_module
+            self.action_representation_module = (action_representation_module if action_representation_module is not None
+                                                 else IdentityActionRepresentationModule())
+            self._history_summarization_module = None
+            self._training_rounds, self._batch_size, self._training_steps = training_rounds, batch_size, 0
+            self.on_policy, self._is_action_continuous = False, False
+            self._feature_dim = feature_dim
+            self.model = _ValueNetwork(feature_dim, hidden_dims, output_dim)
+            self._optimizer = torch.optim.AdamW(self.model.parameters(), lr=learning_rate, amsgrad=True)
+            self._state_features_only = state_features_only
+            self.loss_type = LossType(loss_type) if isinstance(loss_type, str) else loss_type
 
         @property
         def feature_dim(self) -> int:

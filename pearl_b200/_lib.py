@@ -151,6 +151,13 @@ class NlbCfg(C.Structure):
                 ("discount_interval", C.c_double)]
 
 
+class NbCfg(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("action_dim", C.c_int32), ("action_rep", C.c_int32),
+                ("h1", C.c_int32), ("h2", C.c_int32), ("loss", C.c_int32), ("max_batch", C.c_int32), ("max_rounds", C.c_int32),
+                ("score_rows", C.c_int32), ("lr", C.c_double), ("beta1", C.c_double), ("beta2", C.c_double),
+                ("eps", C.c_double), ("weight_decay", C.c_double)]
+
+
 class DqnCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden1", C.c_int32),
                 ("hidden2", C.c_int32), ("double_dqn", C.c_int32), ("target_update_freq", C.c_int32),
@@ -355,6 +362,22 @@ _SIGNATURES = {
     "prl_nlb_learn": (C.c_int, [_P, _P, C.c_int, C.c_int] + [_P] * 7),
     "prl_nlb_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 4 + [C.c_int] + [_P] * 4),
     "prl_nlb_scores": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_double, C.c_int, _P, _P, _P, _P]),
+    "prl_nb_param_count": (C.c_int64, [C.POINTER(NbCfg)]),
+    "prl_nb_workspace_bytes": (C.c_int64, [C.POINTER(NbCfg)]),
+    "prl_nb_create": (C.c_int, [C.POINTER(_P), C.POINTER(NbCfg)] + [_P] * 4 + [C.c_int64, _P]),
+    "prl_nb_destroy": (C.c_int, [_P]),
+    "prl_nb_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_nb_set_lr": (C.c_int, [_P, C.c_double]),
+    "prl_nb_adam_step": (C.c_int64, [_P]),
+    "prl_nb_set_adam_step": (C.c_int, [_P, C.c_int64]),
+    "prl_nb_last_launches": (C.c_int64, [_P]),
+    "prl_nb_graph_captures": (C.c_int64, [_P]),
+    "prl_nb_learn": (C.c_int, [_P, _P, C.c_int, C.c_int] + [_P] * 6),
+    "prl_nb_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 7),
+    "prl_nb_scores": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P, _P]),
+    "prl_nb_act": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int]
+                   + [_P] * 6),
+    "prl_nb_explore": (C.c_int, [C.c_int, _P, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, _P, _P, _P, _P]),
     "prl_ppo_actor_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_critic_param_count": (C.c_int64, [C.POINTER(PpoCfg)]),
     "prl_ppo_workspace_bytes": (C.c_int64, [C.POINTER(PpoCfg)]),

@@ -174,18 +174,6 @@ __global__ void k_nl_grad(int B, NlHead h, const float *__restrict__ G, const fl
     dN[e] = __fmul_rn(gm, h.e2e ? we[j] : coefs[j + 1]);
 }
 
-// feature rows [r0, r0 + m) of the n x S scoring rows: X[i] = state[s] || act_feat[a] (row = s S + a), one warp per row
-__global__ void k_nl_feat(int m, long long r0, int S, int obs, int act_dim, const float *__restrict__ state,
-                          const float *__restrict__ act_feat, float *__restrict__ X) {
-    const int lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (w >= m) return;
-    const long long row = r0 + w;
-    const int s = (int)(row / S), a = (int)(row - (long long)s * S), k = obs + act_dim;
-    float *x = X + (size_t)w * k;
-    for (int p = lane; p < obs; p += 32) x[p] = state[(size_t)s * obs + p];
-    for (int p = lane; p < act_dim; p += 32) x[obs + p] = act_feat[(size_t)a * act_dim + p];
-}
-
 // scores of rows [r0, r0 + m), one warp per row x1 = [1, nn_output]: mu as k_nl_rows, sigma = sqrt(x1^T inv_A x1) (NaN -> 0)
 //   mode 0 (act):                            mu + alpha sigma
 //   mode 1 (get_scores, combined):           activation(mu + alpha sigma)
@@ -440,7 +428,7 @@ extern "C" int prl_nlb_scores(prl_nlb *s, int n, const float *state, int n_space
     GemmLauncher L; L.st = st;
     for (long long r0 = 0; r0 < total; r0 += s->rows) {
         const int m = (int)(total - r0 < s->rows ? total - r0 : s->rows);
-        k_nl_feat<<<(m * 32 + 255) / 256, 256, 0, st>>>(m, r0, n_space, c.obs_dim, c.action_dim, state, act_feat, s->X);
+        k_cb_feat<<<(m * 32 + 255) / 256, 256, 0, st>>>(m, r0, n_space, c.obs_dim, c.action_dim, state, act_feat, s->X);
         s->forward(L, m);
         k_nl_scores<<<(m + 7) / 8, 256, 0, st>>>(m, r0, h, s->N, s->w + s->net.P, s->inv_A, s->coefs, mode, (float)alpha, out_scores);
     }

@@ -2,7 +2,8 @@
 // shared by the learners that fit one on feature rows: LinearBandit (bandit.cu, rows = state || action features) and
 // NeuralLinearBandit (neural_linear.cu, rows = the network's output).  The row load, the fixed-order statistics and their
 // reduction into A, b and sum_weight, the discounting decision with the fp64 Gauss-Jordan solve, and the first-maximum
-// argmax of the UCB scores.  bandit.cu's header describes the numerics.
+// argmax of the UCB scores.  bandit.cu's header describes the numerics.  The row load, the scoring feature rows
+// (k_cb_feat) and the argmax also serve NeuralBandit (neural_bandit.cu), which has no ridge.
 //
 // Every kernel is `static`: each translation unit that includes this header has its own copy, so the solve's dynamic
 // shared-memory attribute is set per unit (cb_solve_prepare, called from each learner's create).
@@ -52,6 +53,18 @@ static __global__ void k_cb_load(const uint32_t *__restrict__ records, prl_buf_l
         Y[w] = __uint_as_float(r[L.off_reward]);
         W[w] = 1.f;
     }
+}
+
+// feature rows [r0, r0 + m) of the n x S scoring rows: X[i] = state[s] || act_feat[a] (row = s S + a), one warp per row
+static __global__ void k_cb_feat(int m, long long r0, int S, int obs, int act_dim, const float *__restrict__ state,
+                          const float *__restrict__ act_feat, float *__restrict__ X) {
+    const int lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (w >= m) return;
+    const long long row = r0 + w;
+    const int s = (int)(row / S), a = (int)(row - (long long)s * S), k = obs + act_dim;
+    float *x = X + (size_t)w * k;
+    for (int p = lane; p < obs; p += 32) x[p] = state[(size_t)s * obs + p];
+    for (int p = lane; p < act_dim; p += 32) x[obs + p] = act_feat[(size_t)a * act_dim + p];
 }
 
 // partial sums of the rows of chunk blockIdx.x into P[chunk][e], one entry per thread (blockIdx.y selects the entries),

@@ -8,7 +8,7 @@ reference's own.  Without Pearl it subclasses a stand-in (_compat.py) with the s
 state_dict keys.
 
 The network's parameters (and linear_layer_e2e's weight) are views of one flat device vector, and the optimizer's AdamW
-state (`exp_avg`, `exp_avg_sq`, `max_exp_avg_sq`, `step`) views of three more, as in the actor-critic plugins; the ridge
+state (`exp_avg`, `exp_avg_sq`, `max_exp_avg_sq`, `step`) views of three more (_flat_adamw.py); the ridge
 buffers of `model._linear_regression_layer` are the device memory the kernels update.  A state loaded with
 `load_state_dict` is what the next call reads, and the learning rate is read from `optimizer.param_groups` on every call.
 `last_sum_weight_when_discounted` lives on the device, as in bandit.py.  No CPU fallback.
@@ -25,8 +25,8 @@ from typing import Any, Optional
 import torch
 
 from . import _lib
-from ._compat import (BinaryActionTensorRepresentationModule, LossType, OneHotActionTensorRepresentationModule,
-                      TiebreakingStrategy, UCBExploration, _RefNeuralLinearBandit)
+from ._compat import LossType, TiebreakingStrategy, UCBExploration, _RefNeuralLinearBandit
+from ._flat_adamw import FlatAdamW
 from .bandit import MAX_RIDGE_WIDTH, _refuse_distributed
 from .per import B200PrioritizedReplayBuffer
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
@@ -35,7 +35,9 @@ SCORE_ROWS = 4096          # feature rows the workspace holds per scoring chunk
 _LOSS = {LossType.MSE: 0, LossType.MAE: 1, LossType.CROSS_ENTROPY: 2}
 
 
-class B200NeuralLinearBandit(_RefNeuralLinearBandit):
+class B200NeuralLinearBandit(FlatAdamW, _RefNeuralLinearBandit):
+    _RT, _ABI = "_nl", "prl_nlb"
+
     def __init__(self, feature_dim: int, hidden_dims: list, exploration_module=None, action_representation_module=None,
                  training_rounds: int = 100, batch_size: int = 128, learning_rate: float = 0.0003,
                  l2_reg_lambda_linear: float = 1.0, gamma: float = 1.0, apply_discounting_interval: float = 0.0,
@@ -112,66 +114,6 @@ class B200NeuralLinearBandit(_RefNeuralLinearBandit):
             self.model.to(dev)
         return dev
 
-    def _lr(self) -> float:
-        """lr of the AdamW(amsgrad=True) the reference constructs; other optimizers or settings are refused."""
-        opt = self._optimizer
-        groups = [g for g in opt.param_groups if len(g["params"])]
-        g = groups[0] if isinstance(opt, torch.optim.AdamW) and len(groups) == 1 else None
-        if (g is None or not g.get("amsgrad", False) or g.get("maximize", False) or tuple(g["betas"]) != (0.9, 0.999)
-                or float(g["eps"]) != 1e-8 or float(g["weight_decay"]) != 0.01):
-            raise NotImplementedError("the fused update implements torch.optim.AdamW(amsgrad=True) with default betas / eps / "
-                                      "weight_decay over the model's parameters")
-        return float(g["lr"])
-
-    def _adopt(self, dev: torch.device) -> torch.Tensor:
-        """The flat parameter vector, with the model's parameters re-pointed at views of it (copied in when they are not
-        views of it already: first use, `.to()`, or parameters replaced)."""
-        nl, params = self._nl, list(self.model.parameters())
-        flat = nl["flat"]
-        if flat is None or flat.device != dev or params[0].data_ptr() != flat.data_ptr():
-            n = sum(p.numel() for p in params)
-            flat = torch.empty(n, dtype=torch.float32, device=dev)
-            off = 0
-            for p in params:
-                k = p.numel()
-                flat[off:off + k].copy_(p.detach().reshape(-1).to(device=dev, dtype=torch.float32))
-                p.data = flat[off:off + k].view(p.shape)
-                off += k
-            nl["flat"] = flat
-        return flat
-
-    def _bind_optimizer(self, dev: torch.device, n_opt: int) -> None:
-        """`optimizer.state` as views of the flat AdamW vectors for the first n_opt parameters (all of them with e2e;
-        without it linear_layer_e2e never gets a gradient and torch keeps no state for it).  State that is there and is
-        not ours (built by torch, or loaded with optimizer.load_state_dict) is imported first."""
-        nl, params, st = self._nl, list(self.model.parameters()), self._optimizer.state
-        n = sum(p.numel() for p in params)
-        state = nl["state"]
-        if state is None or state[0].device != dev:
-            state = [torch.zeros(n, dtype=torch.float32, device=dev) for _ in range(3)]
-            nl["state"] = state
-        used = params[:n_opt]
-        if all(p in st and "exp_avg" in st[p] for p in used) and st[used[0]]["exp_avg"].data_ptr() == state[0].data_ptr():
-            return
-        if all(p in st and "exp_avg" in st[p] for p in used):
-            cat = lambda key: torch.cat([st[p][key].detach().reshape(-1).to(dev, torch.float32) for p in used])  # noqa: E731
-            m = sum(p.numel() for p in used)
-            state[0][:m].copy_(cat("exp_avg"))
-            state[1][:m].copy_(cat("exp_avg_sq"))
-            state[2][:m].copy_(cat("max_exp_avg_sq") if all("max_exp_avg_sq" in st[p] for p in used) else cat("exp_avg_sq"))
-            nl["step"] = int(float(st[used[0]]["step"]))
-            if nl["handle"].value:
-                _lib.check(nl["lib"].prl_nlb_set_adam_step(nl["handle"], nl["step"]))
-        off = 0
-        for i, p in enumerate(params):
-            k = p.numel()
-            if i < n_opt:
-                st[p] = dict(step=torch.tensor(float(nl["step"]), dtype=torch.float32), exp_avg=state[0][off:off + k].view(p.shape),
-                             exp_avg_sq=state[1][off:off + k].view(p.shape), max_exp_avg_sq=state[2][off:off + k].view(p.shape))
-            else:
-                st.pop(p, None)
-            off += k
-
     def _bind(self, dev: torch.device, obs: int, act_dim: int, rep: int, n_actions: int, batch: int, any_rep: bool = False) -> dict:
         """The prl_nlb handle over the current parameter, AdamW and ridge buffers for this row layout, re-created when a
         buffer moved, the layout or a setting changed or the batch outgrew it.  learn_batch and scoring read only the
@@ -226,32 +168,6 @@ class B200NeuralLinearBandit(_RefNeuralLinearBandit):
                                           *(p(t) for t in bufs), p(ws)))
         nl.update(handle=h, key=key, batch=B, ws=ws, lib=lib, lr=lr)
         return nl
-
-    def _after_step(self) -> None:
-        nl = self._nl
-        nl["step"] = int(nl["lib"].prl_nlb_adam_step(nl["handle"]))
-        for s in self._optimizer.state.values():
-            if "step" in s:
-                s["step"].fill_(float(nl["step"]))
-
-    def _representation(self) -> tuple[int, int]:
-        """(action_rep, action_dim) of the rows learn folds from the stored action ids."""
-        if self._state_features_only:
-            return 0, 0
-        mod = self.action_representation_module
-        if isinstance(mod, OneHotActionTensorRepresentationModule):
-            return 1, int(mod.max_number_actions)
-        if isinstance(mod, BinaryActionTensorRepresentationModule):
-            return 2, int(mod.representation_dim)
-        raise NotImplementedError(f"learn over a replay buffer folds the stored action id into the row as a one-hot or "
-                                  f"binary representation; {type(mod).__name__} is not supported")
-
-    def _check_learner(self) -> None:
-        _refuse_distributed()
-        h = getattr(self, "_history_summarization_module", None)
-        if h is not None and any(True for _ in h.parameters()):
-            raise NotImplementedError("a history summarization module with parameters: the CUDA bandit learner reads the "
-                                      "stored states as they are")
 
     # ------------------------------------------------------------------ PolicyLearner.learn (policy_learner.py:162-195)
     def learn(self, replay_buffer: B200ReplayBuffer, trace: Optional[dict] = None) -> dict[str, Any]:
