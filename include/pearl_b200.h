@@ -1068,6 +1068,25 @@ int prl_cb_learn_batch(prl_cb *cb, int batch, const float *state, const float *a
  * every position; 0 when none is). */
 int prl_cb_scores(prl_cb *cb, int n, const float *state, int n_space, const float *act_feat, double alpha, int with_sigma,
                   const uint8_t *mask, float *out_scores, int32_t *out_index, void *stream);
+/* Thompson sampling, replacing ThompsonSamplingExplorationLinear.get_scores's default branch
+ * (policy_learners/exploration_modules/contextual_bandits/thompson_sampling_exploration.py:63-72, MultivariateNormal(loc =
+ * coefs, precision_matrix = A + lambda I).sample()) for both ridge learners (LinearBandit: d = feature_dim + 1;
+ * NeuralLinearBandit: d = h2 + 1), on the device buffers A_dev f32[d][d] (symmetric) and coefs_dev f32[d]:
+ * out_theta_dev f32[d] = coefs + U^-T eps with M = A + (float)lambda I formed in fp32 and factored M = U U^T (U upper
+ * triangular) in fp64, for the caller's standard normal draws eps_dev f32[d].  1 <= d <= 128.  One CTA, no handle, no
+ * host synchronisation.  out_status_dev i32[1] = 0, or 1 when M is not positive definite (theta is then unwritten; the
+ * reference raises ValueError). */
+int prl_cb_ts_sample(int d, double lambda, const float *A_dev, const float *coefs_dev, const float *eps_dev, float *out_theta_dev,
+                     int32_t *out_status_dev, void *stream);
+/* Thompson scores of n states x n_space actions (state, act_feat, mask and out_index as prl_cb_scores), exactly one of:
+ *   theta_dev f32[d] (from prl_cb_ts_sample): out_scores = x1 . theta  (thompson_sampling_exploration.py:69-72);
+ *   z_dev f32[n][n_space] (enable_efficient_sampling, lines 53-61): out_scores = mu + z sigma, rounded after the product
+ *   and after the sum as torch.normal(mean = mu, std = sigma) computes it, mu = x1 . coefs, sigma = sqrt(x1^T inv_A x1);
+ *   out_status_dev i32[1] = 1 when a sigma is NaN (torch.normal raises there), else 0.
+ * out_status_dev may be null with theta. */
+int prl_cb_ts_scores(prl_cb *cb, int n, const float *state, int n_space, const float *act_feat, const float *theta_dev,
+                     const float *z_dev, const uint8_t *mask, float *out_scores, int32_t *out_index, int32_t *out_status_dev,
+                     void *stream);
 
 /* ---- contextual bandit: NeuralLinearBandit (neural LinUCB) -------------------------------------------------------
  * Replaces NeuralLinearBandit.learn_batch / act / get_scores (policy_learners/contextual_bandits/neural_linear_bandit.py)
@@ -1120,6 +1139,13 @@ int prl_nlb_learn_batch(prl_nlb *nlb, int batch, const float *state, const float
  * out_index as prl_cb_scores. */
 int prl_nlb_scores(prl_nlb *nlb, int n, const float *state, int n_space, const float *act_feat, double alpha, int mode,
                    const uint8_t *mask, float *out_scores, int32_t *out_index, void *stream);
+/* Thompson scores of n states x n_space actions (arguments as prl_nlb_scores), replacing the default branch of
+ * ThompsonSamplingExplorationLinear.get_scores (thompson_sampling_exploration.py:63-74) as NeuralLinearBandit.act /
+ * get_scores call it (neural_linear_bandit.py:252-258, 292-313): [1, nn_output] . theta_dev (f32[h2 + 1], from
+ * prl_cb_ts_sample on this handle's ridge buffers), through the output activation when activate (get_scores without
+ * separate_uncertainty); act and separate_uncertainty's get_scores pass activate = 0. */
+int prl_nlb_ts_scores(prl_nlb *nlb, int n, const float *state, int n_space, const float *act_feat, const float *theta_dev,
+                      int activate, const uint8_t *mask, float *out_scores, int32_t *out_index, void *stream);
 
 /* ---- contextual bandit: NeuralBandit (SquareCB / FastCB / greedy) -------------------------------------------------
  * Replaces NeuralBandit.learn_batch / act / get_scores (policy_learners/contextual_bandits/neural_bandit.py) over

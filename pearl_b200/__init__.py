@@ -26,6 +26,7 @@ from .neural_bandit import B200NeuralBandit  # noqa: F401
 from .rc_safety import B200RCSafetyModuleCostCriticContinuousAction  # noqa: F401
 from ._compat import BinaryActionTensorRepresentationModule, UCBExploration  # noqa: F401
 from ._compat import FastCBExploration, LossType, NoExploration, SquareCBExploration  # noqa: F401
+from ._compat import ThompsonSamplingExplorationLinear  # noqa: F401
 from .dist import B200Communicator, all_gather_bytes, shard_owner  # noqa: F401
 
 __all__ = ["B200ReplayBuffer", "B200DeepQLearning", "B200DoubleDQN", "TransitionBatch",
@@ -34,4 +35,4 @@ __all__ = ["B200ReplayBuffer", "B200DeepQLearning", "B200DoubleDQN", "Transition
            "B200QuantileRegressionDeepQLearning", "B200REINFORCE", "DuelingQValueNetwork", "VanillaQValueMultiHeadNetwork",
            "B200DeepSARSA", "B200SARSAReplayBuffer", "B200TD3BC", "B200LinearBandit", "B200NeuralLinearBandit", "UCBExploration",
            "BinaryActionTensorRepresentationModule", "B200RCSafetyModuleCostCriticContinuousAction", "B200NeuralBandit",
-           "SquareCBExploration", "FastCBExploration", "NoExploration", "LossType"]
+           "SquareCBExploration", "FastCBExploration", "NoExploration", "LossType", "ThompsonSamplingExplorationLinear"]

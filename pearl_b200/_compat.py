@@ -300,6 +300,9 @@ try:  # pragma: no cover - depends on the environment; kept apart so the names a
     from pearl.neural_networks.common.utils import LossType
     from pearl.policy_learners.exploration_modules.common.tiebreaking_strategy import TiebreakingStrategy
     from pearl.policy_learners.exploration_modules.contextual_bandits.ucb_exploration import UCBExploration
+    from pearl.policy_learners.exploration_modules.contextual_bandits.thompson_sampling_exploration import (
+        ThompsonSamplingExplorationLinear, ThompsonSamplingExplorationLinearDisjoint,
+    )
 
     HAVE_PEARL_BANDITS = True
 except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
@@ -321,6 +324,21 @@ if not HAVE_PEARL_BANDITS:
         def __init__(self, alpha: float, randomized_tiebreaking: TiebreakingStrategy = TiebreakingStrategy.NO_TIEBREAKING) -> None:
             self._alpha = alpha
             self.randomized_tiebreaking = randomized_tiebreaking
+
+    class ThompsonSamplingExplorationLinear:
+        """Attribute-compatible stand-in for ThompsonSamplingExplorationLinear (exploration_modules/contextual_bandits/
+        thompson_sampling_exploration.py): scores from coefficients sampled from N(coefs, (A + lambda I)^-1), or with
+        enable_efficient_sampling one normal draw per score around mu with sigma as its deviation."""
+
+        def __init__(self, enable_efficient_sampling: bool = False, randomized_tiebreaking: bool = False) -> None:
+            self._enable_efficient_sampling = enable_efficient_sampling
+            self.randomized_tiebreaking = randomized_tiebreaking
+
+    class ThompsonSamplingExplorationLinearDisjoint(ThompsonSamplingExplorationLinear):
+        """Stand-in for the disjoint explorer (one model per action), which the CUDA learners refuse."""
+
+        def __init__(self, enable_efficient_sampling: bool = False) -> None:
+            super().__init__(enable_efficient_sampling=enable_efficient_sampling)
 
     class IdentityActionRepresentationModule(nn.Module):
         def __init__(self, max_number_actions: int = -1, representation_dim: int = -1) -> None:

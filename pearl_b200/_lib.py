@@ -349,6 +349,8 @@ _SIGNATURES = {
     "prl_cb_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "prl_cb_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 6),
     "prl_cb_scores": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_double, C.c_int, _P, _P, _P, _P]),
+    "prl_cb_ts_sample": (C.c_int, [C.c_int, C.c_double] + [_P] * 6),
+    "prl_cb_ts_scores": (C.c_int, [_P, C.c_int, _P, C.c_int] + [_P] * 8),
     "prl_nlb_param_count": (C.c_int64, [C.POINTER(NlbCfg)]),
     "prl_nlb_workspace_bytes": (C.c_int64, [C.POINTER(NlbCfg)]),
     "prl_nlb_create": (C.c_int, [C.POINTER(_P), C.POINTER(NlbCfg)] + [_P] * 4 + [C.c_int64] + [_P] * 7),
@@ -362,6 +364,7 @@ _SIGNATURES = {
     "prl_nlb_learn": (C.c_int, [_P, _P, C.c_int, C.c_int] + [_P] * 7),
     "prl_nlb_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 4 + [C.c_int] + [_P] * 4),
     "prl_nlb_scores": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_double, C.c_int, _P, _P, _P, _P]),
+    "prl_nlb_ts_scores": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P, C.c_int, _P, _P, _P, _P]),
     "prl_nb_param_count": (C.c_int64, [C.POINTER(NbCfg)]),
     "prl_nb_workspace_bytes": (C.c_int64, [C.POINTER(NbCfg)]),
     "prl_nb_create": (C.c_int, [C.POINTER(_P), C.POINTER(NbCfg)] + [_P] * 4 + [C.c_int64, _P]),

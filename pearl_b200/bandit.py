@@ -14,7 +14,11 @@ when the attribute is accessed.  No CPU fallback.
     learn(B200ReplayBuffer)   PolicyLearner.learn: training_rounds x (sample, fold the stored action id into the row as the
                               one-hot or binary representation module would, learn_batch), one prl_cb_learn per chunk
     learn_batch(batch)        one round on a caller's batch; batch.action is the already represented action matrix
-    act / get_scores          UCB scores mu + alpha sigma (UCBExploration, NO_TIEBREAKING), prl_cb_scores
+    act / get_scores          UCB scores mu + alpha sigma (UCBExploration, NO_TIEBREAKING), prl_cb_scores; or Thompson
+                              sampling (ThompsonSamplingExplorationLinear): x . theta with theta ~ N(coefs, (A + lambda
+                              I)^-1) (prl_cb_ts_sample), or with efficient sampling mu + z sigma per score
+                              (prl_cb_ts_scores).  The standard normals come from torch's default CPU generator, the
+                              draws the reference makes; one status word is copied back per call.
 """
 from __future__ import annotations
 
@@ -24,12 +28,46 @@ from typing import Any, Optional
 import torch
 
 from . import _lib
-from ._compat import (BinaryActionTensorRepresentationModule, OneHotActionTensorRepresentationModule, TiebreakingStrategy,
-                      UCBExploration, _RefLinearBandit)
+from ._compat import (BinaryActionTensorRepresentationModule, OneHotActionTensorRepresentationModule,
+                      ThompsonSamplingExplorationLinear, TiebreakingStrategy, UCBExploration, _RefLinearBandit)
+from ._draws import PinnedDraws
 from .per import B200PrioritizedReplayBuffer
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
 
 MAX_RIDGE_WIDTH = 127      # d = width + 1 (the intercept) <= 128: the solve's fp64 matrix fills 128 KB of shared memory
+
+
+def _explorer(ex, learner: str, efficient_ok: bool = True) -> tuple[str, Any]:
+    """("ucb", alpha) for UCBExploration, ("ts", enable_efficient_sampling) for ThompsonSamplingExplorationLinear; the
+    rest is refused.  The disjoint Thompson explorer subclasses the joint one, so the class is matched exactly."""
+    if isinstance(ex, UCBExploration):
+        if ex.randomized_tiebreaking != TiebreakingStrategy.NO_TIEBREAKING:
+            raise NotImplementedError("randomized tie-breaking: the CUDA bandit learner picks the first maximum "
+                                      "(TiebreakingStrategy.NO_TIEBREAKING)")
+        return "ucb", float(ex._alpha)
+    if type(ex) is ThompsonSamplingExplorationLinear:
+        # the reference passes the explorer's flag on as a tie-breaking strategy: a bool selects the first maximum there
+        if ex.randomized_tiebreaking in (TiebreakingStrategy.PER_ROW_TIEBREAKING, TiebreakingStrategy.BATCH_TIEBREAKING):
+            raise NotImplementedError("randomized tie-breaking: the CUDA bandit learner picks the first maximum "
+                                      "(TiebreakingStrategy.NO_TIEBREAKING)")
+        efficient = bool(ex._enable_efficient_sampling)
+        if efficient and not efficient_ok:
+            raise NotImplementedError(f"ThompsonSamplingExplorationLinear(enable_efficient_sampling=True) on {learner}: the "
+                                      "reference fails its own shape assertion there (the network's output reaches the "
+                                      "explorer flattened), so there is nothing to reproduce; use the default sampling")
+        return "ts", efficient
+    raise NotImplementedError(f"act / get_scores with {type(ex).__name__}: the CUDA bandit learner scores with "
+                              "UCBExploration or ThompsonSamplingExplorationLinear")
+
+
+def _ts_failed(status: torch.Tensor, efficient: bool) -> None:
+    """Raise as the reference does when the sampler found A + lambda I not positive definite, or the efficient scores a
+    NaN sigma.  The status read is the Thompson path's one device-to-host copy."""
+    if int(status.item()) == 0:
+        return
+    if efficient:
+        raise RuntimeError("normal expects all elements of std >= 0.0")
+    raise ValueError("Thompson sampling: the precision matrix A + lambda I is not positive definite")
 
 
 def _refuse_distributed() -> None:
@@ -56,7 +94,7 @@ class B200LinearBandit(_RefLinearBandit):
                          gamma=gamma, apply_discounting_interval=apply_discounting_interval, force_pinv=force_pinv,
                          training_rounds=training_rounds, batch_size=batch_size,
                          action_representation_module=action_representation_module, initial_coefs=initial_coefs)
-        object.__setattr__(self, "_cb", dict(handle=C.c_void_p(0), key=None, batch=0, ws=None, lib=None))
+        object.__setattr__(self, "_cb", dict(handle=C.c_void_p(0), key=None, batch=0, ws=None, lib=None, draws=PinnedDraws()))
         self.max_rounds_per_call = max(int(max_rounds_per_call), 1)
         self.use_cuda_graph = True       # False: plain stream launches (profilers)
 
@@ -205,7 +243,10 @@ class B200LinearBandit(_RefLinearBandit):
                 "weight": batch.weight if batch.weight is not None else torch.ones_like(batch.reward)}
 
     # ------------------------------------------------------------------ act / get_scores (linear_bandit.py:168-223)
-    def _scores(self, subjective_state, action_space, alpha: float, with_sigma: bool, mask=None, want_index: bool = False):
+    def _scores(self, subjective_state, action_space, alpha: float, with_sigma: bool, mask=None, want_index: bool = False,
+                ts: Optional[bool] = None):
+        """UCB scores (ts None), or Thompson scores: from sampled coefficients (ts False) or, with efficient sampling (ts
+        True), one draw per score.  The draws come from torch's default CPU generator, as many as the reference makes."""
         _refuse_distributed()
         dev = self._device_of(subjective_state.device if torch.is_tensor(subjective_state) and subjective_state.is_cuda else None)
         feats = self.action_representation_module(torch.stack(list(action_space.actions)).to(dev))
@@ -218,29 +259,43 @@ class B200LinearBandit(_RefLinearBandit):
         scores = torch.empty((n, S), dtype=torch.float32, device=dev)
         index = torch.empty(n, dtype=torch.int32, device=dev) if want_index else None
         m = None if mask is None else torch.as_tensor(mask).to(dev).reshape(n, S).ne(0).to(torch.uint8).contiguous()
+        lib, h, p = cb["lib"], cb["handle"], _lib.ptr
         with torch.cuda.device(dev):
-            _lib.check(cb["lib"].prl_cb_scores(cb["handle"], n, _lib.ptr(states), S, _lib.ptr(feats), float(alpha), int(with_sigma),
-                                               _lib.ptr(m), _lib.ptr(scores), _lib.ptr(index), _stream_ptr(dev)))
+            if ts is None:
+                _lib.check(lib.prl_cb_scores(h, n, p(states), S, p(feats), float(alpha), int(with_sigma), p(m), p(scores),
+                                             p(index), _stream_ptr(dev)))
+                return scores, index
+            status = torch.empty(1, dtype=torch.int32, device=dev)
+            theta = z = None
+            if ts:      # torch.normal(mean, std): one standard normal per score, row-major
+                z = cb["draws"].put(torch.empty(n, S).normal_(), dev)
+            else:       # MultivariateNormal.sample(): d standard normals
+                d = self._feature_dim + 1
+                eps = cb["draws"].put(torch.empty(d).normal_(), dev)
+                theta = torch.empty(d, dtype=torch.float32, device=dev)
+                _lib.check(lib.prl_cb_ts_sample(d, float(self.model.l2_reg_lambda), p(self.model._A), p(self.model._coefs), p(eps),
+                                                p(theta), p(status), _stream_ptr(dev)))
+            _lib.check(lib.prl_cb_ts_scores(h, n, p(states), S, p(feats), p(theta), p(z), p(m), p(scores), p(index),
+                                            p(status) if ts else None, _stream_ptr(dev)))
+        _ts_failed(status, ts)
         return scores, index
-
-    def _ucb(self):
-        ex = self.exploration_module
-        if not isinstance(ex, UCBExploration):
-            raise NotImplementedError(f"act / get_scores with {type(ex).__name__}: the CUDA bandit learner scores with "
-                                      "UCBExploration")
-        if ex.randomized_tiebreaking != TiebreakingStrategy.NO_TIEBREAKING:
-            raise NotImplementedError("randomized tie-breaking: the CUDA bandit learner picks the first maximum "
-                                      "(TiebreakingStrategy.NO_TIEBREAKING)")
-        return float(ex._alpha)
 
     def act(self, subjective_state, available_action_space, action_availability_mask: Optional[torch.Tensor] = None,
             exploit: bool = False):
-        alpha = self._ucb()
-        _, index = self._scores(subjective_state, available_action_space, alpha, True, action_availability_mask, True)
+        kind, arg = _explorer(self.exploration_module, "LinearBandit")
+        ts = arg if kind == "ts" else None
+        _, index = self._scores(subjective_state, available_action_space, arg if ts is None else 0.0, True,
+                                action_availability_mask, True, ts=ts)
         actions_batch = torch.stack(list(available_action_space.actions)).to(index.device)
         return torch.nn.functional.embedding(index.long(), actions_batch.reshape(int(available_action_space.n), -1))
 
     def get_scores(self, subjective_state, action_space_to_score, exploit: bool = False) -> torch.Tensor:
-        alpha = 0.0 if exploit else self._ucb()
-        scores, _ = self._scores(subjective_state, action_space_to_score, alpha, not exploit)
+        if exploit:         # the model's mu, bypassing the explorer
+            scores, _ = self._scores(subjective_state, action_space_to_score, 0.0, False)
+            return scores.squeeze(-1)
+        kind, arg = _explorer(self.exploration_module, "LinearBandit")
+        if kind == "ts":
+            scores, _ = self._scores(subjective_state, action_space_to_score, 0.0, False, ts=arg)
+        else:
+            scores, _ = self._scores(subjective_state, action_space_to_score, arg, True)
         return scores.squeeze(-1)

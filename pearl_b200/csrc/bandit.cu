@@ -6,6 +6,8 @@
 //   policy_learners/contextual_bandits/linear_bandit.py       learn_batch (x = state || represented action, the model's
 //       learn_batch, _maybe_apply_discounting, prediction = model(x) after the update), act / get_scores
 //   policy_learners/exploration_modules/contextual_bandits/ucb_exploration.py   values + alpha sigma, NaN sigma -> 0
+//   policy_learners/exploration_modules/contextual_bandits/thompson_sampling_exploration.py   x . theta with theta from
+//       ridge.cuh's k_cb_ts_sample (prl_cb_ts_sample), or with efficient sampling mu + z sigma (k_cb_ts_scores)
 //   utils/functional_utils/learning/action_utils.py          get_model_action_index_batch (NO_TIEBREAKING: first max
 //       over the available positions)
 //
@@ -61,22 +63,17 @@ __global__ void k_cb_predict(int B, int k, const float *__restrict__ X, const fl
     if (call->out_weight) call->out_weight[o] = W[r];
 }
 
-// scores of n states x S actions, one warp per (state, action) row x = [1, state, action features a]:
-//   mu = x . coefs;  with_sigma: mu + alpha sigma, sigma = sqrt(x^T inv_A x), NaN (a negative form) -> 0
-__global__ void __launch_bounds__(256) k_cb_scores(int n, int S, int obs, int act_dim, const float *__restrict__ state,
-                                                   const float *__restrict__ act_feat, const float *__restrict__ inv_A,
-                                                   const float *__restrict__ coefs, int with_sigma, float alpha,
-                                                   float *__restrict__ out) {
-    __shared__ float xs[8][kMaxD];
-    const int lane = threadIdx.x & 31, wb = threadIdx.x >> 5;
-    const long long row = (long long)blockIdx.x * 8 + wb;
-    if (row >= (long long)n * S) return;
-    const int s = (int)(row / S), a = (int)(row - (long long)s * S), d = obs + act_dim + 1;
-    float *x = xs[wb];
+// one warp's row x = [1, state s, action features a] of the scores (the warp's slice xw of shared memory): mu = x . coefs
+// and, with_sigma, q = x^T inv_A x, both summed over the warp
+__device__ __forceinline__ void cb_row_form(int s, int a, int obs, int act_dim, const float *__restrict__ state,
+                                            const float *__restrict__ act_feat, const float *__restrict__ inv_A,
+                                            const float *__restrict__ coefs, int with_sigma, float *x, int lane, float &mu,
+                                            float &q) {
+    const int d = obs + act_dim + 1;
     for (int c = lane; c < d; c += 32)
         x[c] = c == 0 ? 1.f : (c <= obs ? state[(size_t)s * obs + c - 1] : act_feat[(size_t)a * act_dim + c - 1 - obs]);
     __syncwarp();
-    float mu = 0.f, q = 0.f;
+    mu = 0.f; q = 0.f;
     for (int j = lane; j < d; j += 32) {
         mu = fmaf(x[j], coefs[j], mu);
         if (with_sigma) {
@@ -90,6 +87,22 @@ __global__ void __launch_bounds__(256) k_cb_scores(int n, int S, int obs, int ac
         mu += __shfl_xor_sync(0xffffffffu, mu, o);
         q += __shfl_xor_sync(0xffffffffu, q, o);
     }
+}
+
+// scores of n states x S actions, one warp per (state, action) row x = [1, state, action features a]:
+//   mu = x . coefs;  with_sigma: mu + alpha sigma, sigma = sqrt(x^T inv_A x), NaN (a negative form) -> 0
+// Thompson sampling scores x . theta through this kernel with coefs = theta and no sigma.
+__global__ void __launch_bounds__(256) k_cb_scores(int n, int S, int obs, int act_dim, const float *__restrict__ state,
+                                                   const float *__restrict__ act_feat, const float *__restrict__ inv_A,
+                                                   const float *__restrict__ coefs, int with_sigma, float alpha,
+                                                   float *__restrict__ out) {
+    __shared__ float xs[8][kMaxD];
+    const int lane = threadIdx.x & 31, wb = threadIdx.x >> 5;
+    const long long row = (long long)blockIdx.x * 8 + wb;
+    if (row >= (long long)n * S) return;
+    const int s = (int)(row / S), a = (int)(row - (long long)s * S);
+    float mu, q;
+    cb_row_form(s, a, obs, act_dim, state, act_feat, inv_A, coefs, with_sigma, xs[wb], lane, mu, q);
     if (lane == 0) {
         float v = mu;
         if (with_sigma) {
@@ -98,6 +111,27 @@ __global__ void __launch_bounds__(256) k_cb_scores(int n, int S, int obs, int ac
             v = __fadd_rn(mu, __fmul_rn(alpha, sg));
         }
         out[row] = v;
+    }
+}
+
+// ThompsonSamplingExplorationLinear with enable_efficient_sampling: torch.normal(mean = mu, std = sigma) for the rows of
+// k_cb_scores, given the row's standard normal draw z[row]: z sigma, then + mu, each rounded (no FMA), as torch computes
+// it.  A NaN sigma (a negative form) sets *nan_sigma, where torch.normal raises; the UCB path's NaN -> 0 does not apply.
+__global__ void __launch_bounds__(256) k_cb_ts_scores(int n, int S, int obs, int act_dim, const float *__restrict__ state,
+                                                      const float *__restrict__ act_feat, const float *__restrict__ inv_A,
+                                                      const float *__restrict__ coefs, const float *__restrict__ z,
+                                                      float *__restrict__ out, int *__restrict__ nan_sigma) {
+    __shared__ float xs[8][kMaxD];
+    const int lane = threadIdx.x & 31, wb = threadIdx.x >> 5;
+    const long long row = (long long)blockIdx.x * 8 + wb;
+    if (row >= (long long)n * S) return;
+    const int s = (int)(row / S), a = (int)(row - (long long)s * S);
+    float mu, q;
+    cb_row_form(s, a, obs, act_dim, state, act_feat, inv_A, coefs, 1, xs[wb], lane, mu, q);
+    if (lane == 0) {
+        const float sg = sqrtf(q);
+        if (isnan(sg)) *nan_sigma = 1;
+        out[row] = __fadd_rn(mu, __fmul_rn(z[row], sg));
     }
 }
 
@@ -213,6 +247,39 @@ extern "C" int prl_cb_scores(prl_cb *s, int n, const float *state, int n_space, 
     const long long rows = (long long)n * n_space;
     k_cb_scores<<<(unsigned)((rows + 7) / 8), 256, 0, st>>>(n, n_space, c.obs_dim, c.action_dim, state, act_feat, s->inv_A, s->coefs,
                                                             with_sigma, (float)alpha, out_scores);
+    if (out_index) k_cb_argmax<<<(n + 255) / 256, 256, 0, st>>>(n, n_space, out_scores, mask, out_index);
+    PRL_CUDA(cudaGetLastError());
+    return PRL_OK;
+}
+
+// no handle: both ridge learners (and a caller holding only the buffers) sample through this one entry
+extern "C" int prl_cb_ts_sample(int d, double lam, const float *A, const float *coefs, const float *eps, float *out_theta,
+                                int32_t *out_status, void *stream_) {
+    PRL_REQUIRE(A && coefs && eps && out_theta && out_status, "null argument");
+    PRL_REQUIRE(d >= 1 && d <= kMaxD, "d = %d: the sampler supports 1 <= d <= %d", d, kMaxD);
+    PRL_CUDA(cb_solve_prepare());
+    PRL_CUDA(cb_ts_sample(d, (float)lam, A, coefs, eps, out_theta, out_status, (cudaStream_t)stream_));
+    return PRL_OK;
+}
+
+extern "C" int prl_cb_ts_scores(prl_cb *s, int n, const float *state, int n_space, const float *act_feat, const float *theta,
+                                const float *z, const uint8_t *mask, float *out_scores, int32_t *out_index, int32_t *out_status,
+                                void *stream_) {
+    PRL_REQUIRE(s && out_scores && (state || s->cfg.obs_dim == 0) && (act_feat || s->cfg.action_dim == 0), "null argument");
+    PRL_REQUIRE((theta != nullptr) != (z != nullptr), "exactly one of theta (sampled coefficients) and z (per-score draws)");
+    PRL_REQUIRE(!z || out_status, "the per-score draws need out_status for the NaN-sigma flag");
+    PRL_REQUIRE(n >= 0 && n_space >= 1 && (int64_t)n * n_space < ((int64_t)1 << 31), "n * n_space must be in [0, 2^31)");
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (z) PRL_CUDA(cudaMemsetAsync(out_status, 0, sizeof(int32_t), st));
+    if (n == 0) return PRL_OK;
+    const prl_cb_cfg &c = s->cfg;
+    const long long rows = (long long)n * n_space;
+    const unsigned grid = (unsigned)((rows + 7) / 8);
+    if (theta)
+        k_cb_scores<<<grid, 256, 0, st>>>(n, n_space, c.obs_dim, c.action_dim, state, act_feat, s->inv_A, theta, 0, 0.f, out_scores);
+    else
+        k_cb_ts_scores<<<grid, 256, 0, st>>>(n, n_space, c.obs_dim, c.action_dim, state, act_feat, s->inv_A, s->coefs, z, out_scores,
+                                             out_status);
     if (out_index) k_cb_argmax<<<(n + 255) / 256, 256, 0, st>>>(n, n_space, out_scores, mask, out_index);
     PRL_CUDA(cudaGetLastError());
     return PRL_OK;

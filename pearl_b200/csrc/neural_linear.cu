@@ -32,7 +32,8 @@
 //
 // Scoring (prl_nlb_scores) runs the network over the n x S feature rows in chunks of the workspace's rows, then per row
 // mu (as above) and sigma = sqrt([1, nn_output]^T inv_A [1, nn_output]) (NaN -> 0), combined as act or get_scores do;
-// the argmax of ridge.cuh follows.  No host synchronisation.
+// the argmax of ridge.cuh follows.  No host synchronisation.  Thompson sampling (prl_nlb_ts_scores) runs the same network
+// pass, then [1, nn_output] . theta with theta from ridge.cuh's k_cb_ts_sample.
 #include <math.h>
 
 #include <new>
@@ -208,6 +209,19 @@ __global__ void __launch_bounds__(256) k_nl_scores(int m, long long r0, NlHead h
     else if (mode == 1) { v = __fadd_rn(mu, u); if (h.sigmoid) v = 1.f / (1.f + expf(-v)); }
     else v = __fadd_rn(h.sigmoid ? 1.f / (1.f + expf(-mu)) : mu, u);
     out[r0 + w] = v;
+}
+
+// Thompson sampling scores of rows [r0, r0 + m), one warp per row: [1, nn_output] . theta (the sampled coefficients, in
+// place of the ridge's coefs whatever e2e is), then the output activation when `activate` (get_scores without
+// separate_uncertainty); act and separate_uncertainty's get_scores take the product as it is
+__global__ void __launch_bounds__(256) k_nl_ts_scores(int m, long long r0, NlHead h, const float *__restrict__ N,
+                                                      const float *__restrict__ theta, int activate, float *__restrict__ out) {
+    const int lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (w >= m) return;
+    h.e2e = 0;
+    const float mu = nl_mu(N + (size_t)w * h.h2, nullptr, theta, h, lane);
+    if (lane) return;
+    out[r0 + w] = activate && h.sigmoid ? 1.f / (1.f + expf(-mu)) : mu;
 }
 
 }  // namespace
@@ -431,6 +445,27 @@ extern "C" int prl_nlb_scores(prl_nlb *s, int n, const float *state, int n_space
         k_cb_feat<<<(m * 32 + 255) / 256, 256, 0, st>>>(m, r0, n_space, c.obs_dim, c.action_dim, state, act_feat, s->X);
         s->forward(L, m);
         k_nl_scores<<<(m + 7) / 8, 256, 0, st>>>(m, r0, h, s->N, s->w + s->net.P, s->inv_A, s->coefs, mode, (float)alpha, out_scores);
+    }
+    if (out_index) k_cb_argmax<<<(n + 255) / 256, 256, 0, st>>>(n, n_space, out_scores, mask, out_index);
+    PRL_CUDA(cudaGetLastError());
+    return PRL_OK;
+}
+
+extern "C" int prl_nlb_ts_scores(prl_nlb *s, int n, const float *state, int n_space, const float *act_feat, const float *theta,
+                                 int activate, const uint8_t *mask, float *out_scores, int32_t *out_index, void *stream_) {
+    PRL_REQUIRE(s && theta && out_scores && (state || s->cfg.obs_dim == 0) && (act_feat || s->cfg.action_dim == 0), "null argument");
+    PRL_REQUIRE(n >= 0 && n_space >= 1 && (int64_t)n * n_space < ((int64_t)1 << 31), "n * n_space must be in [0, 2^31)");
+    if (n == 0) return PRL_OK;
+    const prl_nlb_cfg &c = s->cfg;
+    cudaStream_t st = (cudaStream_t)stream_;
+    const long long total = (long long)n * n_space;
+    const NlHead h = s->head();
+    GemmLauncher L; L.st = st;
+    for (long long r0 = 0; r0 < total; r0 += s->rows) {
+        const int m = (int)(total - r0 < s->rows ? total - r0 : s->rows);
+        k_cb_feat<<<(m * 32 + 255) / 256, 256, 0, st>>>(m, r0, n_space, c.obs_dim, c.action_dim, state, act_feat, s->X);
+        s->forward(L, m);
+        k_nl_ts_scores<<<(m * 32 + 255) / 256, 256, 0, st>>>(m, r0, h, s->N, theta, activate, out_scores);
     }
     if (out_index) k_cb_argmax<<<(n + 255) / 256, 256, 0, st>>>(n, n_space, out_scores, mask, out_index);
     PRL_CUDA(cudaGetLastError());

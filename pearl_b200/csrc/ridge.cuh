@@ -239,12 +239,66 @@ static __global__ void k_cb_argmax(int n, int S, const float *__restrict__ score
     idx[s] = bi < 0 ? 0 : bi;
 }
 
+// ThompsonSamplingExplorationLinear's MultivariateNormal(loc = coefs, precision_matrix = A + lambda I).sample() for the
+// standard normal draws eps[d] the caller made.  One CTA.  M = A + lambda I is formed in fp32 as LinearRegression.A forms
+// it, then factored M = U U^T with U upper triangular in fp64 shared memory [d][d] (right-looking, from the last column
+// down; torch factors the index-reversed M, which is the same factorisation).  U overwrites M's upper triangle.  Then
+// U^T x = eps by forward substitution in one warp, and theta = coefs + x rounded to fp32: x has covariance
+// U^-T U^-1 = M^-1.  *status = 0, or 1 when a pivot is not positive (M is not positive definite, a NaN included), and
+// theta is then left unwritten: the reference's argument validation raises there.
+static __global__ void __launch_bounds__(kSolveThreads) k_cb_ts_sample(int d, float lam, const float *__restrict__ A,
+                                                                const float *__restrict__ coefs, const float *__restrict__ eps,
+                                                                float *__restrict__ theta, int *__restrict__ status) {
+    extern __shared__ double sm[];
+    double *M = sm, *r = sm + (size_t)d * d;
+    const int tid = threadIdx.x, nt = blockDim.x, dd = d * d;
+    for (int t = tid; t < dd; t += nt) {
+        const int i = t / d, j = t - i * d;
+        M[t] = (double)(i == j ? __fadd_rn(A[t], lam) : A[t]);
+    }
+    for (int t = tid; t < d; t += nt) r[t] = (double)eps[t];
+    __syncthreads();
+    for (int k = d - 1; k >= 0; k--) {
+        const double p = M[(size_t)k * d + k];
+        if (!(p > 0.0)) {                      // every thread read the same pivot: the whole CTA leaves
+            if (tid == 0) *status = 1;
+            return;
+        }
+        const double u = sqrt(p);
+        __syncthreads();
+        for (int i = tid; i <= k; i += nt) M[(size_t)i * d + k] = i == k ? u : M[(size_t)i * d + k] / u;
+        __syncthreads();
+        for (int t = tid; t < k * k; t += nt) {  // the leading block's upper triangle: M[i][j] -= U[i][k] U[j][k]
+            const int i = t / k, j = t - i * k;
+            if (i <= j) M[(size_t)i * d + j] = fma(-M[(size_t)i * d + k], M[(size_t)j * d + k], M[(size_t)i * d + j]);
+        }
+        __syncthreads();
+    }
+    if (tid >= 32) return;
+    for (int j = 0; j < d; j++) {              // x_j = r_j / U[j][j], then r_i -= U[j][i] x_j for i > j, in ascending j
+        const double x = r[j] / M[(size_t)j * d + j];
+        for (int i = j + 1 + tid; i < d; i += 32) r[i] = fma(-M[(size_t)j * d + i], x, r[i]);
+        if (tid == 0) theta[j] = (float)((double)coefs[j] + x);
+        __syncwarp();
+    }
+    if (tid == 0) *status = 0;
+}
+
 static size_t cb_solve_smem(int d) { return ((size_t)d * d + d) * sizeof(double); }
 
 // the attribute belongs to the kernel, not to a handle: raise it to what the widest supported d needs, so that a later
-// handle of a smaller d cannot lower it under the launches of a live wider one
+// handle of a smaller d cannot lower it under the launches of a live wider one.  The sampler has the same budget.
 static cudaError_t cb_solve_prepare() {
-    return cudaFuncSetAttribute(k_cb_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cb_solve_smem(kMaxD));
+    const cudaError_t e = cudaFuncSetAttribute(k_cb_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cb_solve_smem(kMaxD));
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(k_cb_ts_sample, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cb_solve_smem(kMaxD));
+}
+
+// the sampler on `st`, for the learners' ridge buffers
+static cudaError_t cb_ts_sample(int d, float lam, const float *A, const float *coefs, const float *eps, float *theta, int *status,
+                                cudaStream_t st) {
+    k_cb_ts_sample<<<1, kSolveThreads, cb_solve_smem(d), st>>>(d, lam, A, coefs, eps, theta, status);
+    return cudaGetLastError();
 }
 
 }  // namespace prl

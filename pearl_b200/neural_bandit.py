@@ -28,6 +28,7 @@ from typing import Any, Optional
 import torch
 
 from . import _lib
+from ._draws import PinnedDraws
 from ._compat import (FastCBExploration, LossType, NoExploration, SquareCBExploration, TiebreakingStrategy,
                       _RefNeuralBandit)
 from ._flat_adamw import FlatAdamW
@@ -60,7 +61,7 @@ class B200NeuralBandit(FlatAdamW, _RefNeuralBandit):
                          learning_rate=learning_rate, state_features_only=state_features_only, loss_type=loss_type,
                          action_representation_module=action_representation_module)
         object.__setattr__(self, "_nb", dict(handle=C.c_void_p(0), key=None, batch=0, ws=None, lib=None, lr=None, flat=None,
-                                             state=None, step=0, pin=None, E=None, prob=None))
+                                             state=None, step=0, draws=PinnedDraws(), prob=None))
         self._hidden = (int(hidden_dims[0]), int(hidden_dims[1]))
         self.max_rounds_per_call = max(int(max_rounds_per_call), 1)
         self.use_cuda_graph = True       # False: plain stream launches (profilers)
@@ -220,15 +221,6 @@ class B200NeuralBandit(FlatAdamW, _RefNeuralBandit):
             raise NotImplementedError("randomized tie-breaking: the CUDA NeuralBandit picks the first maximum")
         return kind
 
-    def _staging(self, dev: torch.device, A: int) -> dict:
-        """Pinned host staging for the exponential draws, and device buffers for them and the probabilities, of at least A."""
-        nb = self._nb
-        if nb["pin"] is None or nb["pin"].numel() < A or nb["E"].device != dev:
-            n = max(A, 64)
-            nb.update(pin=torch.empty(n, dtype=torch.float32, pin_memory=True), E=torch.empty(n, dtype=torch.float32, device=dev),
-                      prob=torch.empty(n, dtype=torch.float32, device=dev))
-        return nb
-
     def act(self, subjective_state, available_action_space, action_availability_mask: Optional[torch.Tensor] = None,
             exploit: bool = False):
         kind = self._explorer()
@@ -243,11 +235,8 @@ class B200NeuralBandit(FlatAdamW, _RefNeuralBandit):
         ex, E, prob = self.exploration_module, None, None
         if kind:
             # the draws torch's one-sample multinomial makes inside Categorical(p).sample(), from the same generator
-            draws = torch.empty(S).exponential_()
-            st = self._staging(dev, S)
-            st["pin"][:S].copy_(draws)
-            E, prob = st["E"][:S], st["prob"][:S]
-            E.copy_(st["pin"][:S], non_blocking=True)
+            E = nb["draws"].put(torch.empty(S).exponential_(), dev)
+            nb["prob"] = prob = torch.empty(S, dtype=torch.float32, device=dev)
         m = None
         if kind == 0 and action_availability_mask is not None:
             m = torch.as_tensor(action_availability_mask).to(dev).reshape(n, S).ne(0).to(torch.uint8).contiguous()

@@ -15,7 +15,9 @@ buffers of `model._linear_regression_layer` are the device memory the kernels up
 
     learn(B200ReplayBuffer)   PolicyLearner.learn: training_rounds x (sample, the row as learn_batch builds it, one round)
     learn_batch(batch)        one round on a caller's batch; batch.action is the already represented action matrix
-    act / get_scores          UCB on the network's output (UCBExploration, NO_TIEBREAKING)
+    act / get_scores          UCB on the network's output (UCBExploration, NO_TIEBREAKING), or Thompson sampling
+                              (ThompsonSamplingExplorationLinear's default mode): [1, nn_output] . theta with theta ~
+                              N(coefs, (A + lambda I)^-1), prl_cb_ts_sample / prl_nlb_ts_scores
 """
 from __future__ import annotations
 
@@ -25,9 +27,10 @@ from typing import Any, Optional
 import torch
 
 from . import _lib
-from ._compat import LossType, TiebreakingStrategy, UCBExploration, _RefNeuralLinearBandit
+from ._compat import LossType, _RefNeuralLinearBandit
+from ._draws import PinnedDraws
 from ._flat_adamw import FlatAdamW
-from .bandit import MAX_RIDGE_WIDTH, _refuse_distributed
+from .bandit import MAX_RIDGE_WIDTH, _explorer, _refuse_distributed, _ts_failed
 from .per import B200PrioritizedReplayBuffer
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
 
@@ -79,7 +82,7 @@ class B200NeuralLinearBandit(FlatAdamW, _RefNeuralLinearBandit):
                          dropout_ratio=dropout_ratio, use_skip_connections=use_skip_connections, nn_e2e=nn_e2e,
                          separate_uncertainty=separate_uncertainty)
         object.__setattr__(self, "_nl", dict(handle=C.c_void_p(0), key=None, batch=0, ws=None, lib=None, lr=None, flat=None,
-                                             state=None, step=0))
+                                             state=None, step=0, draws=PinnedDraws()))
         self._hidden = (int(hidden_dims[0]), int(hidden_dims[1]))
         self._skip = bool(use_skip_connections)
         self._sigmoid = output_activation_name == "sigmoid"
@@ -247,7 +250,11 @@ class B200NeuralLinearBandit(FlatAdamW, _RefNeuralLinearBandit):
                 "loss": stats[0], "mu_scores": stats[1]}
 
     # ------------------------------------------------------------------ act / get_scores
-    def _scores(self, subjective_state, action_space, alpha: float, mode: int, mask=None, want_index: bool = False):
+    def _scores(self, subjective_state, action_space, alpha: float, mode: int, mask=None, want_index: bool = False,
+                ts: bool = False):
+        """UCB scores in `mode` (prl_nlb_scores), or with ts Thompson scores [1, nn_output] . theta, theta sampled from
+        N(coefs, (A + lambda I)^-1) with d standard normals from torch's default CPU generator (mode 1: through the
+        output activation)."""
         _refuse_distributed()
         dev = self._device_of(subjective_state.device if torch.is_tensor(subjective_state) and subjective_state.is_cuda else None)
         S = int(action_space.n)
@@ -265,31 +272,36 @@ class B200NeuralLinearBandit(FlatAdamW, _RefNeuralLinearBandit):
         scores = torch.empty((n, S), dtype=torch.float32, device=dev)
         index = torch.empty(n, dtype=torch.int32, device=dev) if want_index else None
         m = None if mask is None else torch.as_tensor(mask).to(dev).reshape(n, S).ne(0).to(torch.uint8).contiguous()
+        lib, h, p = nl["lib"], nl["handle"], _lib.ptr
         with torch.cuda.device(dev):
-            _lib.check(nl["lib"].prl_nlb_scores(nl["handle"], n, _lib.ptr(states), S, _lib.ptr(feats), float(alpha), mode,
-                                                _lib.ptr(m), _lib.ptr(scores), _lib.ptr(index), _stream_ptr(dev)))
+            if not ts:
+                _lib.check(lib.prl_nlb_scores(h, n, p(states), S, p(feats), float(alpha), mode, p(m), p(scores), p(index),
+                                              _stream_ptr(dev)))
+                return scores, index
+            d = self._hidden[1] + 1
+            eps = nl["draws"].put(torch.empty(d).normal_(), dev)       # MultivariateNormal.sample(): d standard normals
+            theta = torch.empty(d, dtype=torch.float32, device=dev)
+            status = torch.empty(1, dtype=torch.int32, device=dev)
+            lin = self.model._linear_regression_layer
+            _lib.check(lib.prl_cb_ts_sample(d, float(lin.l2_reg_lambda), p(lin._A), p(lin._coefs), p(eps), p(theta), p(status),
+                                            _stream_ptr(dev)))
+            _lib.check(lib.prl_nlb_ts_scores(h, n, p(states), S, p(feats), p(theta), int(mode == 1), p(m), p(scores), p(index),
+                                             _stream_ptr(dev)))
+        _ts_failed(status, False)
         return scores, index
-
-    def _ucb(self) -> float:
-        ex = self.exploration_module
-        if not isinstance(ex, UCBExploration):
-            raise NotImplementedError(f"act / get_scores with {type(ex).__name__}: the CUDA bandit learner scores with "
-                                      "UCBExploration")
-        if ex.randomized_tiebreaking != TiebreakingStrategy.NO_TIEBREAKING:
-            raise NotImplementedError("randomized tie-breaking: the CUDA bandit learner picks the first maximum "
-                                      "(TiebreakingStrategy.NO_TIEBREAKING)")
-        return float(ex._alpha)
 
     def act(self, subjective_state, available_action_space, action_availability_mask: Optional[torch.Tensor] = None,
             exploit: bool = False):
-        alpha = self._ucb()
-        _, index = self._scores(subjective_state, available_action_space, alpha, 0, action_availability_mask, True)
+        kind, arg = _explorer(self.exploration_module, "NeuralLinearBandit", efficient_ok=False)
+        _, index = self._scores(subjective_state, available_action_space, arg if kind == "ucb" else 0.0, 0,
+                                action_availability_mask, True, ts=kind == "ts")
         actions_batch = torch.stack(list(available_action_space.actions)).to(index.device)
         return torch.nn.functional.embedding(index.long(), actions_batch.reshape(int(available_action_space.n), -1))
 
     @torch.no_grad()
     def get_scores(self, subjective_state, action_space_to_score, exploit: bool = False) -> torch.Tensor:
         assert not exploit, "exploit=True is not yet implemented for NeuralLinearBandit.get_scores"
-        alpha = self._ucb()
-        scores, _ = self._scores(subjective_state, action_space_to_score, alpha, 2 if self.separate_uncertainty else 1)
+        kind, arg = _explorer(self.exploration_module, "NeuralLinearBandit", efficient_ok=False)
+        scores, _ = self._scores(subjective_state, action_space_to_score, arg if kind == "ucb" else 0.0,
+                                 2 if self.separate_uncertainty else 1, ts=kind == "ts")
         return scores.squeeze(-1)
