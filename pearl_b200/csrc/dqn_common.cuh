@@ -78,8 +78,9 @@ struct prl_dqn {
 int prl_dqn_stage_scalars(prl_dqn *q, int rounds, cudaStream_t stream);
 
 // floats of the tensor-core learner's operand-layout weight tiles: per network W1 hi | W1 lo (64 x k1 each, k1 = obs
-// rounded up to a multiple of 64) and W2 hi | W2 lo (64 x 64 each), online then target; 0 for shapes outside its class
+// rounded up to a multiple of 64) and W2 hi | W2 lo (64 x 64 each), online then target, and the online network's
+// W2^T hi | W2^T lo (64 x 64 each); 0 for shapes outside its class
 inline int64_t prl_tc_tile_floats(const prl_dqn_cfg *c) {
     if (c->hidden1 != 64 || c->hidden2 != 64 || c->obs_dim > 128 || c->obs_dim % 8) return 0;
-    return 2ll * (128 * ((c->obs_dim + 63) & ~63) + 2 * 64 * 64);
+    return 2ll * (128 * ((c->obs_dim + 63) & ~63) + 2 * 64 * 64) + 2 * 64 * 64;
 }

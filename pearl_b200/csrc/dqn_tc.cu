@@ -20,7 +20,11 @@
 //            their operands are explicitly transposed tiles written with a 144-byte chunk pitch
 //            (bank-conflict-free column scatter), 64 batch rows per pass, the two warpgroups issuing the same
 //            products on equal shares of the output columns.  The warpgroup that owns the pass's rows scatters their
-//            dZ2^T, H1^T and dZ1^T, the other one E^T, and both S^T.  The accumulators stay in registers for the whole step.
+//            dZ2^T, H1^T and dZ1^T, the other one E^T.  For obs > 64 dW1s is computed as its transpose S^T dZ1, whose A
+//            operand S^T is read as register fragments straight out of layer 1's staging buffers (warpgroup h takes
+//            obs rows [64 h, 64 h + 64), its K chunk h) and whose B operand is the dZ1^T tile; for obs <= 64 both
+//            warpgroups scatter S^T from state rows re-read from global memory.  The accumulators stay in registers
+//            for the whole step.
 //   AdamW    gradients registers -> shared staging, then one sweep over the flat W1 | b1 | W2 range whose parameters and
 //            moments stream in by TMA bulk copies, in 16 KB chunks through an 8-slot ring in regions 3 and 1 (free once
 //            the last weight-gradient products have been waited for); 16-byte stores write the results and the
@@ -30,8 +34,10 @@
 // The weights are kept in global memory a second time IN THE OPERAND LAYOUT (hi tile = the fp32 values — the tensor
 // core truncates them to TF32 — and lo tile = x - trunc_tf32(x)), written by AdamW / the soft target update next to the
 // flat torch-order vectors, so staging a network's B operands is three TMA bulk copies (cp.async.bulk + mbarrier
-// complete_tx) issued by one thread.  The W2 tiles store their K axis in the order umma::kperm, which is the order in
-// which an accumulator's columns feed the next product's register A operand.  The target network's small vectors are
+// complete_tx) issued by one thread.  The W2 and W2^T tiles store their K axis in the order umma::kperm, which is the
+// order in which an accumulator's columns feed the next product's register A operand.  The online network's tiles are
+// fetched once per row tile: the weight-gradient passes use regions 1 and 3 for their transposed tiles and for dZ1,
+// which waits there for its pass.  The target network's small vectors are
 // cached in shared memory between soft updates, the soft target update is applied to the tiles in tile order.
 //
 // Each 3xTF32 product is one chain of wgmma with a single wait at its end, and that only holds while ptxas can pipeline
@@ -39,8 +45,9 @@
 // stay true: no function call in the kernel (not even printf, C7510); no wgmma under
 // a branch, including a runtime step count or a branch on the warpgroup index (both warpgroups issue the same products,
 // C7520), and no conditional load feeding an A fragment; and each chain fits in the registers together with everything
-// live across it (C7511 / C7512), which is why H1 and dZ2 wait in shared memory while dH1 is formed and the learner
-// descriptor and the dW3 partial sums live in shared memory.  tests/test_dqn_tc_sass.py checks the SASS.
+// live across it (C7511 / C7512), which is why H1 and dZ2 wait in shared memory while dH1 is formed, dZ1 until its
+// weight-gradient pass, and the learner descriptor and the dW3 partial sums live in shared memory.  For the same reason
+// the phase stamps (TC_STAMP) are predicated stores rather than branches.  tests/test_dqn_tc_sass.py checks the SASS.
 // Spills cost more here than usual: the 225 KB of shared memory leave at most 28 KB of L1 for the spill frame of 256
 // threads, so spill traffic reaches L2.  Values that are the same in every round must not be hoisted out of the round
 // loop into registers: the wgmma descriptors are built next to each wgmma (umma::Tile::desc) and the shared-memory
@@ -71,9 +78,11 @@ constexpr int MAX_B = 256;
 constexpr int REG1 = 0, REG2 = 65536, REG3 = 131072, MISC_OFF = 196608;
 constexpr int HALF = 32768;          // hi tile at region base, lo tile at base + HALF
 constexpr int SBUF = 16384;          // layer-1 row staging of one warpgroup: [64 rows][64 floats]
-// transposed-tile arena (regions 1+2) for the weight-gradient products, 64 batch rows per pass
+// transposed-tile arena for the weight-gradient products, 64 batch rows per pass: TA hi | lo, TE and TB lo in region 1,
+// TB hi in the W2^T half of region 3 (both re-fetched for the next row tile).  Region 2 is left alone: the state rows
+// that layer 1 staged there are the S^T operand of dW1s.
 constexpr int TL = 144;              // chunk pitch of transposed tiles
-constexpr int AR_A_HI = 0, AR_A_LO = 18432, AR_B_HI = 36864, AR_B_LO = 73728, AR_E = 110592;
+constexpr int AR_A_HI = 0, AR_A_LO = 18432, AR_E = 36864, AR_B_LO = 46080, AR_B_HI = REG3 + HALF;
 // AdamW ring: chunks of ACH flat parameters, one slot = the chunk's w | m | v | vmax (16 KB); slots 0-3 in region 3,
 // 4-7 in region 1
 constexpr int ACH = 1024, ARING = 8, ASLOT = 4 * ACH * 4;
@@ -102,10 +111,14 @@ struct TcArgs {
     int adam_tma;      // D % 4 == 0 and every learner's w / m / v / vmax 16-byte aligned: AdamW streams them by TMA
 };
 
-#define TC_STAMP(idx)                                                                          \
-    do {                                                                                       \
-        if (a.prof && blockIdx.x == a.prof_cta && threadIdx.x == 0) a.prof[(size_t)round * 16 + (idx)] = clock64(); \
-    } while (0)
+// A predicated store, not a branch: a stamp under `if` between two products costs the registers the chains need
+__device__ __forceinline__ void tc_stamp(const TcArgs &a, int round, int idx) {
+    long long *p = a.prof + (size_t)round * 16 + idx;
+    const unsigned on = (a.prof != nullptr) & (blockIdx.x == (unsigned)a.prof_cta) & (threadIdx.x == 0);
+    asm volatile("{\n\t.reg .pred q;\n\t.reg .u64 c;\n\tsetp.ne.u32 q, %1, 0;\n\tmov.u64 c, %%clock64;\n\t@q st.global.u64 [%0], c;\n\t}"
+                 ::"l"(p), "r"(on) : "memory");
+}
+#define TC_STAMP(idx) tc_stamp(a, round, (idx))
 
 struct Misc {
     // small fp32 vectors of a network: W1[:, obs + a] + b1, b2, w3, b3.  [0] online, [1] target (the target's only change at
@@ -116,7 +129,7 @@ struct Misc {
     float rew[MAX_B], term[MAX_B];
     float redw[8][HID];
     float redmae[8], reddb3[8];
-    unsigned long long bar[3 + ARING];   // 0: target tiles; 1: online W1 tiles; 2: online W2 tiles; 3 + s: AdamW ring slot s
+    unsigned long long bar[2 + ARING];   // 0: target tiles; 1: online tiles; 2 + s: AdamW ring slot s
     // kept here rather than in registers: the wgmma chains need the registers (section 3.1 of DESIGN.md)
     TcLearner L;                 // this CTA's learner, per-round arrays shifted to the launch's first round
     float dw3[16][NTH];          // per-thread dW3 partial sums, carried across the row tiles
@@ -155,17 +168,19 @@ using umma::tf32_lo;
 
 // Operand-layout copies of one network's matrices in global memory (floats):
 //   [W1 hi: 64 x k1][W1 lo][W2 hi: 64 x 64][W2 lo]      (the shared-memory images, tile by tile; the W2 tiles with their
-//   K axis in umma::kperm order; the W2^T tiles of the online network are transposed out of the W2 tiles in shared memory)
+//   K axis in umma::kperm order)
+// and for the online network then [W2^T hi: 64 x 64][W2^T lo], the B operand of dH1 = dZ2 W2 (contraction over W2's rows),
+// with its K axis in kperm order too.  The target network needs no W2^T.
 // The W1 tiles have K = k1 = obs rounded up to a multiple of 64, the columns from obs on are zero: every layer-1 K chunk is
 // a full 8-step product (no runtime step count inside a wgmma chain), and the padding adds exact zeros to the sums.
-struct NetTiles { float *w1hi, *w1lo, *w2; };   // w2: the 2 x 4096-float block W2 hi | W2 lo
+struct NetTiles { float *w1hi, *w1lo, *w2, *w2t; };   // w2 / w2t: 2 x 4096-float blocks hi | lo; w2t null for the target
 __host__ __device__ inline int k1_cols(int obs) { return (obs + 63) & ~63; }
-__host__ __device__ inline int net_tile_floats(int obs) { return 128 * k1_cols(obs) + 2 * HID * HID; }
-__device__ __forceinline__ NetTiles net_tiles(float *base, int obs) {
-    const int k1 = k1_cols(obs);
-    return NetTiles{base, base + 64 * k1, base + 128 * k1};
+__host__ __device__ inline int net_tile_floats(int obs) { return 128 * k1_cols(obs) + 2 * HID * HID; }   // without W2^T
+__device__ __forceinline__ NetTiles net_tiles(float *base, int obs, bool with_w2t) {
+    const int k1 = k1_cols(obs), n = net_tile_floats(obs);
+    return NetTiles{base, base + 64 * k1, base + 128 * k1, with_w2t ? base + n : nullptr};
 }
-// all tiles of one network from its flat parameter vector (kernel prologue, soft target update)
+// all tiles of one network from its flat parameter vector (kernel prologue, scalar AdamW sweep)
 __device__ void rebuild_tiles(const float *__restrict__ net, const Dims &d, const NetTiles &t, int tid) {
     const int k1 = k1_cols(d.obs);
     for (int e = tid; e < HID * k1; e += NTH) {
@@ -179,6 +194,10 @@ __device__ void rebuild_tiles(const float *__restrict__ net, const Dims &d, cons
         const float x = __ldcg(net + d.oW2 + e);
         const int i1 = umma::tile_index(j, umma::kperm(k), HID);
         t.w2[i1] = x; t.w2[4096 + i1] = tf32_lo(x);
+        if (t.w2t) {
+            const int i2 = umma::tile_index(k, umma::kperm(j), HID);
+            t.w2t[i2] = x; t.w2t[4096 + i2] = tf32_lo(x);
+        }
     }
 }
 // the small fp32 vectors of a network (action columns + b1, b2, w3, b3); all loads of a thread issued before the first use
@@ -333,25 +352,23 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     }
     uint64_t *bar = reinterpret_cast<uint64_t *>(mi.bar);
     if (tid == 0)
-        for (int i = 0; i < 3 + ARING; i++) umma::mbar_init(bar + i, 1);
+        for (int i = 0; i < 2 + ARING; i++) umma::mbar_init(bar + i, 1);
     // the operand-layout tiles follow the flat parameters (which the host may have changed between calls)
-    auto To = [&] { return net_tiles(L.tiles, d.obs); };
-    auto Tt = [&] { return net_tiles(L.tiles + net_tile_floats(d.obs), d.obs); };
+    auto To = [&] { return net_tiles(L.tiles, d.obs, true); };
+    auto Tt = [&] { return net_tiles(L.tiles + net_tile_floats(d.obs) + 2 * HID * HID, d.obs, false); };
     rebuild_tiles(L.w, d, To(), tid);
     rebuild_tiles(L.wt, d, Tt(), tid);
     fence_proxy_async_all();
     __syncthreads();
     const int k1 = k1_cols(d.obs);
     const uint32_t w1_bytes = 64u * k1 * 4, w2_bytes = 2u * HID * HID * 4;
-    // B-operand tiles of one network by TMA: W1 hi / lo into region 1, the W2 block into region 3
-    auto tma_w1 = [&](const NetTiles &t, uint64_t *b) {
-        mbar_expect_tx(b, 2 * w1_bytes);
+    // B-operand tiles of the online network by TMA, once per row tile (the weight-gradient passes overwrite them): W1 hi / lo
+    // into region 1, the W2 and W2^T blocks (adjacent in global memory) into region 3
+    auto tma_online = [&](const NetTiles &t, uint64_t *b) {
+        mbar_expect_tx(b, 2 * w1_bytes + 2 * w2_bytes);
         bulk_g2s(smem + REG1, t.w1hi, w1_bytes, b);
         bulk_g2s(smem + REG1 + HALF, t.w1lo, w1_bytes, b);
-    };
-    auto tma_w2 = [&](const NetTiles &t, uint64_t *b) {
-        mbar_expect_tx(b, w2_bytes);
-        bulk_g2s(smem + REG3, t.w2, w2_bytes, b);
+        bulk_g2s(smem + REG3, t.w2, 2 * w2_bytes, b);
     };
     // AdamW streams W1 | b1 | W2 (one flat range; D % 4 == 0 keeps every 16-byte group inside one of the three) through the
     // ring: chunk k goes to slot k % ARING, whose barrier completes once per use
@@ -361,11 +378,11 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
         const int off = k * ACH, s = k % ARING;
         const uint32_t bytes = 4u * (an - off < ACH ? an - off : ACH);
         char *dst = aslot(s);
-        mbar_expect_tx(bar + 3 + s, 4 * bytes);
-        bulk_g2s(dst, L.w + off, bytes, bar + 3 + s);
-        bulk_g2s(dst + ACH * 4, L.m + off, bytes, bar + 3 + s);
-        bulk_g2s(dst + ACH * 8, L.v + off, bytes, bar + 3 + s);
-        bulk_g2s(dst + ACH * 12, L.vmax + off, bytes, bar + 3 + s);
+        mbar_expect_tx(bar + 2 + s, 4 * bytes);
+        bulk_g2s(dst, L.w + off, bytes, bar + 2 + s);
+        bulk_g2s(dst + ACH * 4, L.m + off, bytes, bar + 2 + s);
+        bulk_g2s(dst + ACH * 8, L.v + off, bytes, bar + 2 + s);
+        bulk_g2s(dst + ACH * 12, L.vmax + off, bytes, bar + 2 + s);
     };
     uint32_t par_w1 = 0;   // phase parity of bar[1] (one completion per row tile)
     const umma::Tile W2_hi = umma::make_tile(smem + REG3, 64, 128), W2_lo = umma::make_tile(smem + REG3 + 16384, 64, 128);
@@ -485,40 +502,44 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
 
         // ================= phase O: online forward, loss, backward =================
         TC_STAMP(3);
-        if (tid == 0) { tma_w1(To(), bar + 1); tma_w2(To(), bar + 2); }
+        if (tid == 0) tma_online(To(), bar + 1);
         load_smalls(L.w, d, mi.sm[0]);
-        umma::mbar_wait(bar + 2, round & 1);
-        {   // W2^T tiles (B operand of dH1 = dZ2 W2, contraction over W2's rows) out of the W2 tiles
-            const float *w2 = reinterpret_cast<const float *>(smem + REG3);
-            float *w2t = reinterpret_cast<float *>(smem + REG3 + 32768);
-            for (int e = tid; e < HID * HID; e += NTH) {
-                const int j = e >> 6, k = e & 63, i1 = umma::tile_index(j, umma::kperm(k), HID), i2 = umma::tile_index(k, umma::kperm(j), HID);
-                w2t[i2] = w2[i1]; w2t[4096 + i2] = w2[4096 + i1];
-            }
-            umma::fence_async_smem();
-        }
         TC_STAMP(4);
         // weight-gradient accumulators; both warpgroups issue the same products on different output columns:
         // gw2 = dW2 columns [32 h, 32 h + 32), gb2 = [db2 | .] (column 0 of dZ2^T E, the same on both warpgroups),
-        // gw1 = dW1s columns [NW h, NW h + NW), gba = [db1 | dW1a] columns [16 h, 16 h + 16) (0 = bias, 1 + k = action k)
+        // gw1 = dW1s columns [NW h, NW h + NW), for NW = 64 its transpose: dW1s^T rows [64 h, 64 h + 64),
+        // gba = [db1 | dW1a] columns [16 h, 16 h + 16) (0 = bias, 1 + k = action k)
         float gw2[16], gb2[4], gw1[NW / 2], gba[8];
         float mae_acc = 0.f, db3_acc = 0.f;
         float *arena = reinterpret_cast<float *>(smem);
         const umma::Tile TA_hi = umma::make_tile(smem + AR_A_HI, 64, TL), TA_lo = umma::make_tile(smem + AR_A_LO, 64, TL);
         const umma::Tile TB_hi = umma::make_tile(smem + AR_B_HI, 64, TL), TB_lo = umma::make_tile(smem + AR_B_LO, 64, TL);
         const umma::Tile TE = umma::make_tile(smem + AR_E, 64, TL);
+        // E^T = [1 | onehot(action)]^T of the 64 rows from row b0 (this thread: columns rA, rB of the tile, rows 8 t4 .. + 8)
+        auto e_scatter = [&](int b0, int rA, int rB, int t4) {
+#pragma unroll
+            for (int p = 0; p < 2; p++) {
+                const int r = p ? rB : rA, act = mi.act[b0 + r];
+#pragma unroll
+                for (int x = 0; x < 8; x++) {
+                    const int er = t4 * 8 + x;
+                    arena[AR_E / 4 + umma::tile_index2(er, r, 64, TL)] = (er == 0 || er == act + 1) ? 1.f : 0.f;
+                }
+            }
+        };
         for (int i = 0; i < ntiles; i++) {
             const int row0 = i * 128 + h * 64;
-            if (i > 0) {   // the arena of the last tile overwrote regions 1 and 2 (tile 0's first chunk was issued in phase T)
-                if (tid == 0) tma_w1(To(), bar + 1);
+            if (i > 0) {   // the last tile's passes overwrote regions 1 and 3 (tile 0's first chunk was issued in phase T)
+                if (tid == 0) tma_online(To(), bar + 1);
                 l1_issue(a, L, mi, smem, a.lay.off_state, row0, 0);
             }
             umma::mbar_wait(bar + 1, par_w1);
             par_w1 ^= 1;
-            __syncthreads();   // also: the W2^T tiles are complete
+            __syncthreads();
             const int rows[2] = {row0 + acc_row_here(0), row0 + acc_row_here(1)};
             float h1[32], z[32], hi[32], lo[32];
             layer1_block(a, L, mi, smem, a.lay.off_state, row0, h1);
+            __syncthreads();   // both warpgroups are done with the W1 tiles: region 1 takes H1 and dZ2 below
             if (i == 0) TC_STAMP(5);
             int ai[2];
 #pragma unroll
@@ -531,10 +552,11 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                     h1[4 * j + 2 * p + 1] = fmaxf(h1[4 * j + 2 * p + 1] + wv.y, 0.f);
                 }
             }
-            // H1 and dZ2 wait in this warpgroup's (free) staging buffers while dZ2 and dH1 are formed: values that stay live
-            // across a wgmma chain besides its own operands cost the registers the chain needs, and ptxas serialises every
-            // wgmma of the kernel when a chain does not fit (C7511)
-            float *h1s = reinterpret_cast<float *>(smem + REG2 + h * 2 * SBUF) + (tid & 127);
+            // H1 and dZ2 wait in this warpgroup's half of region 1 (the W1 tiles are dead) while dZ2 and dH1 are formed:
+            // values that stay live across a wgmma chain besides its own operands cost the registers the chain needs, and
+            // ptxas serialises every wgmma of the kernel when a chain does not fit (C7511).  The staging buffers in region 2
+            // keep this tile's state rows for dW1s.
+            float *h1s = reinterpret_cast<float *>(smem + REG1 + h * HALF) + (tid & 127);
 #pragma unroll
             for (int c = 0; c < 32; c++) h1s[c * 128] = h1[c];
             acc_to_frag(h1, hi, lo);
@@ -591,10 +613,18 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 z[c] = h1s[(32 + c) * 128];
                 dz1[c] = (h1[c] > 0.f) ? dz1[c] : 0.f;
             }
+            // dZ1 waits in region 3's W2 half until its dW1s pass, so that it is not live in registers across the other
+            // passes' chains; written once both warpgroups are done with W2
+            __syncthreads();
+            float *dzs = reinterpret_cast<float *>(smem + REG3 + h * (HALF / 2)) + (tid & 127);
+#pragma unroll
+            for (int c = 0; c < 32; c++) dzs[c * 128] = dz1[c];
             if (i == 0) TC_STAMP(6);
 
             // ---- weight gradients: contractions over the batch rows, 64 rows (one warpgroup's block) per pass; the owner of the
-            //      block scatters the transposes of its rows while the other warpgroup builds E^T
+            //      block scatters the transposes of its rows while the other warpgroup builds E^T.  The dW2 | db2 passes over
+            //      both blocks come first, then the dW1s | [db1 | dW1a] passes: every output element still accumulates the
+            //      blocks in the same order, and no H1 or dZ2 stays live across the register-fed dW1s chain.
             for (int hf = 0; hf < 2; hf++) {
                 const int ft = tid_here(), h = ft >> 7, t4 = ft & 3, lane = ft & 31, warp = ft >> 5, rA = acc_row_here(0), rB = rA + 8;
                 const bool mine = h == hf;
@@ -612,24 +642,30 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                                 arena[AR_B_HI / 4 + idx] = h1[c]; arena[AR_B_LO / 4 + idx] = tf32_lo(h1[c]);     // H1^T
                             }
                 } else {
-#pragma unroll
-                    for (int p = 0; p < 2; p++) {                     // E^T: [1 | onehot(action)] of the owner's rows
-                        const int r = p ? rB : rA, act = mi.act[i * 128 + hf * 64 + r];
-#pragma unroll
-                        for (int x = 0; x < 8; x++) {
-                            const int er = t4 * 8 + x;
-                            arena[AR_E / 4 + umma::tile_index2(er, r, 64, TL)] = (er == 0 || er == act + 1) ? 1.f : 0.f;
-                        }
-                    }
+                    e_scatter(i * 128 + hf * 64, rA, rB, t4);
                 }
                 umma::fence_async_smem();
                 __syncthreads();
+                if (first) TC_STAMP(11);
                 umma::gemm3<32>(gw2, TA_hi, TA_lo, TB_hi.rows_from(32 * h), TB_lo.rows_from(32 * h), 64, !first);
                 umma::gemm3<8>(gb2, TA_hi, TA_lo, TE, TE, 64, !first, false, true);
                 umma::wg_commit();
-                // S^T: every warp reads whole state rows of this half coalesced (lane = k) and scatters them into column rq of
-                // the transposed tile.  The first four rows are prefetched into L1 under the dW2 product: held in registers
-                // across it they are spilled, and each spill store waits for its load.
+                if (NW < 64 && lane < 16 && 32 * (lane & 3) < d.obs) {   // the state rows of this block for S^T, into L1:
+                    // lane 4 ri + c = 128-byte line c of row warp + 8 ri
+                    const float *src = reinterpret_cast<const float *>(L.records + (size_t)mi.slot[i * 128 + hf * 64 + warp + 8 * (lane >> 2)] * W) +
+                                       a.lay.off_state + 32 * (lane & 3);
+                    asm volatile("prefetch.global.L1 [%0];" ::"l"(src));
+                }
+                umma::wg_wait<0>();
+                if (first) TC_STAMP(12);
+            }
+            for (int hf = 0; hf < 2; hf++) {
+                const int ft = tid_here(), h = ft >> 7, t4 = ft & 3, lane = ft & 31, warp = ft >> 5, rA = acc_row_here(0), rB = rA + 8;
+                const bool mine = h == hf;
+                const bool first = (i == 0 && hf == 0);
+                __syncthreads();   // previous products have been waited for: the arena is free
+                // NW < 64 (obs <= 64): S^T is built as a B tile.  Every warp reads whole state rows of this half coalesced
+                // (lane = k) and scatters them into column rq of the transposed tile.
                 float sv[4][4];
                 auto st_rows_load = [&](int r0) {
 #pragma unroll
@@ -652,14 +688,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                             }
                     }
                 };
-                if (lane < 16 && 32 * (lane & 3) < d.obs) {   // lane 4 ri + c: 128-byte line c of row warp + 8 ri
-                    const float *src = reinterpret_cast<const float *>(L.records + (size_t)mi.slot[i * 128 + hf * 64 + warp + 8 * (lane >> 2)] * W) +
-                                       a.lay.off_state + 32 * (lane & 3);
-                    asm volatile("prefetch.global.L1 [%0];" ::"l"(src));
-                }
-                umma::wg_wait<0>();
-                __syncthreads();
-                st_rows_load(0);
+                if constexpr (NW < 64) st_rows_load(0);
                 if (mine) {
 #pragma unroll
                     for (int j = 0; j < 8; j++)
@@ -668,24 +697,49 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
 #pragma unroll
                             for (int e = 0; e < 2; e++) {
                                 const int idx = umma::tile_index2(8 * j + 2 * t4 + e, p ? rB : rA, 64, TL), c = 4 * j + 2 * p + e;
-                                arena[AR_A_HI / 4 + idx] = dz1[c]; arena[AR_A_LO / 4 + idx] = tf32_lo(dz1[c]);   // dZ1^T
+                                const float v = reinterpret_cast<const float *>(smem + REG3 + h * (HALF / 2))[c * 128 + (ft & 127)];
+                                arena[AR_A_HI / 4 + idx] = v; arena[AR_A_LO / 4 + idx] = tf32_lo(v);               // dZ1^T
                             }
+                } else {
+                    e_scatter(i * 128 + hf * 64, rA, rB, t4);
                 }
-                st_rows_scatter(0);
-                st_rows_load(4);
-                st_rows_scatter(4);
+                if constexpr (NW < 64) {
+                    st_rows_scatter(0);
+                    st_rows_load(4);
+                    st_rows_scatter(4);
+                }
                 umma::fence_async_smem();
                 __syncthreads();
-                umma::gemm3<NW>(gw1, TA_hi, TA_lo, TB_hi.rows_from(NW * h), TB_lo.rows_from(NW * h), 64, !first);
+                if (first) TC_STAMP(13);
+                if constexpr (NW == 64) {
+                    // dW1s^T = S^T dZ1 (obs rows [64 h, 64 h + 64) on warpgroup h): A = S^T as register fragments read from the
+                    // owner's layer-1 staging buffer of K chunk h, B = the dZ1^T tile.  Each element gets the same three
+                    // products over the same K steps as dZ1^T S, the small terms in the same order (B_LO_FIRST).
+                    const float *sbuf = reinterpret_cast<const float *>(smem + REG2 + hf * 2 * SBUF + h * SBUF);
+                    float shi[32], slo[32];
+#pragma unroll
+                    for (int ks = 0; ks < 8; ks++)
+#pragma unroll
+                        for (int q = 0; q < 2; q++)
+#pragma unroll
+                            for (int p = 0; p < 2; p++) {
+                                const int o = p ? rB : rA, r = 8 * ks + t4 + 4 * q;   // A row = obs column, K = batch row
+                                umma::split_tf32(sbuf[r * 64 + (((o >> 2) ^ (r & 7)) << 2) + (o & 3)], shi[4 * ks + 2 * q + p], slo[4 * ks + 2 * q + p]);
+                            }
+                    umma::gemm3_rs<64, 8, true>(gw1, shi, slo, TA_hi, TA_lo, !first);
+                } else {
+                    umma::gemm3<NW>(gw1, TA_hi, TA_lo, TB_hi.rows_from(NW * h), TB_lo.rows_from(NW * h), 64, !first);
+                }
                 umma::gemm3<16>(gba, TA_hi, TA_lo, TE.rows_from(16 * h), TE.rows_from(16 * h), 64, !first, false, true);
                 umma::wg_commit();
                 umma::wg_wait<0>();
+                if (first) TC_STAMP(14);
             }
             umma::fence_async_smem();   // the arena was written through the generic proxy, the next W1 copy is a TMA write
             __syncthreads();            // the arena is free: the next tile's W1 copy / the gradient staging may overwrite it
         }
-        // regions 3 (W2 / W2^T, whose generic writes were fenced when W2^T was built) and 1 (the arena's first half) are
-        // free: AdamW's first chunks load during the gradient staging.
+        // regions 3 (W2 / W2^T; the arena's TB hi tile, fenced above) and 1 (the rest of the arena) are free: AdamW's
+        // first chunks load during the gradient staging.
         // Issuing them under the last tile's weight-gradient products instead made the kernel slower.
         if (a.adam_tma && tid == 0)
             for (int k = 0; k < ARING && k < nch; k++) adam_issue(k);
@@ -720,20 +774,21 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                     for (int e = 0; e < 2; e++) {
                         const int c = 8 * jb + 2 * t4 + e, x = 4 * jb + 2 * p + e;
                         gs_w2[j * 65 + 32 * h + c] = gw2[x];
-                        if (jb < NW / 8 && NW * h + c < d.obs) gs_w1[j * pitch1 + NW * h + c] = gw1[x];
+                        if (NW < 64 && jb < NW / 8 && NW * h + c < d.obs) gs_w1[j * pitch1 + NW * h + c] = gw1[x];
                         if (jb < 2) {
                             const int ce = 16 * h + c;
                             if (ce == 0) gs_b1[j] = gba[x];
                             else if (ce - 1 < d.A) gs_w1[j * pitch1 + d.obs + ce - 1] = gba[x];
                         }
                     }
+                if constexpr (NW == 64) {   // gw1 holds dW1s^T: this thread's row p is obs column 64 h + j
+                    const int k = 64 * h + j;
 #pragma unroll
-                for (int jb = 4; jb < NW / 8; jb++)
+                    for (int jb = 0; jb < 8; jb++)
 #pragma unroll
-                    for (int e = 0; e < 2; e++) {
-                        const int k = NW * h + 8 * jb + 2 * t4 + e;
-                        if (k < d.obs) gs_w1[j * pitch1 + k] = gw1[4 * jb + 2 * p + e];
-                    }
+                        for (int e = 0; e < 2; e++)
+                            if (k < d.obs) gs_w1[(8 * jb + 2 * t4 + e) * pitch1 + k] = gw1[4 * jb + 2 * p + e];
+                }
                 if (h == 0 && t4 == 0) gs_b2[j] = gb2[2 * p];
             }
             __syncthreads();
@@ -770,7 +825,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 const int n1 = HID * d.D;
                 for (int k = 0; k < nch; k++) {
                     const int s = k % ARING, uses = (nch - 1 - s) / ARING + 1;
-                    umma::mbar_wait(bar + 3 + s, (uint32_t)(round * uses + k / ARING) & 1u);
+                    umma::mbar_wait(bar + 2 + s, (uint32_t)(round * uses + k / ARING) & 1u);
                     const int i = k * ACH + 4 * tid;
                     if (i < an && (i < n1 || i >= d.oW2)) {
                         const float4 *sl = reinterpret_cast<const float4 *>(aslot(s)) + tid;
@@ -803,6 +858,15 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                             *reinterpret_cast<float2 *>(To().w2 + to) = make_float2(w.y, w.w);
                             *reinterpret_cast<float2 *>(To().w2 + 4096 + te) = make_float2(tf32_lo(w.x), tf32_lo(w.z));
                             *reinterpret_cast<float2 *>(To().w2 + 4096 + to) = make_float2(tf32_lo(w.y), tf32_lo(w.w));
+                            // W2^T: columns c .. c + 3 are its rows, row `row` its column kperm(row)
+                            float *w2t = To().w2t;
+                            const int kr = umma::kperm(row);
+                            const float wv[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+                            for (int u = 0; u < 4; u++) {
+                                const int ti = umma::tile_index(c + u, kr, HID);
+                                w2t[ti] = wv[u]; w2t[4096 + ti] = tf32_lo(wv[u]);
+                            }
                         }
                     }
                     if (k + ARING < nch) {   // every thread is done with slot s: refill it with chunk k + ARING

@@ -174,15 +174,22 @@ __device__ __forceinline__ void gemm3(float *d, Tile a_hi, Tile a_lo, Tile b_hi,
 // 3xTF32, RS form: a_hi / a_lo hold this thread's A fragments of (at most) KSTEPS K steps (4 registers each).  The registers
 // must not be written again before the products have been waited for.  A runtime ksteps < KSTEPS puts a branch into the
 // chain, and ptxas then serialises every wgmma of the kernel: pipelined kernels leave it at KSTEPS.
-template <int N, int KSTEPS>
+// B_LO_FIRST issues a_hi*b_lo before a_lo*b_hi: the small terms in the order gemm3 adds them for the transposed product
+// (B^T A^T), so that computing a transpose this way gives the same bits.
+template <int N, int KSTEPS, bool B_LO_FIRST = false>
 __device__ __forceinline__ void gemm3_rs(float *d, const float *a_hi, const float *a_lo, Tile b_hi, Tile b_lo, bool accumulate_first,
                                          int ksteps = KSTEPS) {
     wg_fence();
 #pragma unroll
     for (int ks = 0; ks < KSTEPS; ks++) {
         if (ks >= ksteps) break;
-        mma_rs<N>(d, a_lo + 4 * ks, b_hi.desc(ks), accumulate_first || ks > 0);
-        mma_rs<N>(d, a_hi + 4 * ks, b_lo.desc(ks), true);
+        if (B_LO_FIRST) {
+            mma_rs<N>(d, a_hi + 4 * ks, b_lo.desc(ks), accumulate_first || ks > 0);
+            mma_rs<N>(d, a_lo + 4 * ks, b_hi.desc(ks), true);
+        } else {
+            mma_rs<N>(d, a_lo + 4 * ks, b_hi.desc(ks), accumulate_first || ks > 0);
+            mma_rs<N>(d, a_hi + 4 * ks, b_lo.desc(ks), true);
+        }
         mma_rs<N>(d, a_hi + 4 * ks, b_hi.desc(ks), true);
     }
 }

@@ -39,14 +39,18 @@ grp.learn()
 torch.cuda.synchronize()
 s = st.cpu()[4:].double()
 # stamps written by k_dqn_tc: 0 round start, 1 row scalars + soft update done, 2 target tiles loaded, 3 phase T done,
-# 4 online tiles + W2^T ready, 5 tile 0 layer 1 done, 6 tile 0 forward / dZ2 / dH1 done, 8 weight gradients done,
-# 7 gradients staged in shared memory, 10 AdamW sweep over W1 | b1 | W2 done, 9 small-parameter tail done (round end)
+# 4 online small vectors loaded (and, before the W2^T tiles were kept in global memory, W2^T built), 5 tile 0 layer 1 done, 6 tile 0 forward / dZ2 / dH1 done, 8 weight gradients done,
+# 7 gradients staged in shared memory, 10 AdamW sweep over W1 | b1 | W2 done, 9 small-parameter tail done (round end);
+# in the weight-gradient passes of tile 0, rows 0-63: 11 dZ2^T / H1^T scattered, 12 dW2 / db2 waited for, 13 the operands
+# of dW1s ready, 14 dW1s / [db1 | dW1a] waited for (the dW2 | db2 pass over rows 64-127 lies between 12 and 13)
 phases = [("row scalars + soft upd", 0, 1), ("load target weights", 1, 2), ("phase T (layer 1 + all actions)", 2, 3),
-          ("load online weights + W2^T", 3, 4), ("tile 0: online layer 1", 4, 5), ("tile 0: fwd L2 + dZ2 + dH1", 5, 6),
-          ("rest (weight grads, other tiles)", 6, 8), ("AdamW: gradient staging", 8, 7), ("AdamW: sweep", 7, 10),
-          ("AdamW: small-parameter tail", 10, 9)]
+          ("load online weights", 3, 4), ("tile 0: online layer 1", 4, 5), ("tile 0: fwd L2 + dZ2 + dH1", 5, 6),
+          ("rest (weight grads, other tiles)", 6, 8), ("  tile 0 rows 0-63: dZ2^T / H1^T scatter", 6, 11),
+          ("  tile 0 rows 0-63: dW2 / db2 products", 11, 12), ("  tile 0: to the operands of dW1s", 12, 13),
+          ("  tile 0 rows 0-63: dW1s / [db1 | dW1a] products", 13, 14), ("AdamW: gradient staging", 8, 7),
+          ("AdamW: sweep", 7, 10), ("AdamW: small-parameter tail", 10, 9)]
 tot = (s[1:, 0] - s[:-1, 0]).mean()
 print(f"{tot:.0f} clk/round (CTA {os.environ.get('PRL_TC_PROF_CTA', '0')} with {R} learners resident)")
 for n, k, j in phases:
-    print(f"  {n:36s} {(s[:, j]-s[:, k]).mean():10.0f} clk")
-print(f"  {'AdamW (total)':36s} {(s[:, 9]-s[:, 8]).mean():10.0f} clk")
+    print(f"  {n:46s} {(s[:, j]-s[:, k]).mean():10.0f} clk")
+print(f"  {'AdamW (total)':46s} {(s[:, 9]-s[:, 8]).mean():10.0f} clk")
