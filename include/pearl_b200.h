@@ -1088,6 +1088,57 @@ int prl_cb_ts_scores(prl_cb *cb, int n, const float *state, int n_space, const f
                      const float *z_dev, const uint8_t *mask, float *out_scores, int32_t *out_index, int32_t *out_status_dev,
                      void *stream);
 
+/* ---- contextual bandit: disjoint linear bandits (one ridge regression per arm) ----------------------------------------
+ * Replaces DisjointBanditContainer of LinearBandit arms (policy_learners/contextual_bandits/disjoint_bandit.py, mode 0) and
+ * DisjointLinearBandit (disjoint_linear_bandit.py, mode 1): learn_batch, driven by PolicyLearner.learn (prl_dcb_learn) or
+ * called on a caller's batch (prl_dcb_learn_batch), and the DisjointUCBExploration / ThompsonSamplingExplorationLinearDisjoint
+ * scores of act / get_scores.  K = n_arms arms, each the ridge of prl_cb with d = obs_dim + action_dim + 1 and its own
+ * lambda, gamma and discount interval.  Per round, a row goes to arm `id` (the stored action id, or the caller's id):
+ *   mode 0: ids must lie in [0, K) (the caller checks; the reference asserts); an arm without rows adds nothing and still
+ *           takes its discounting decision and solve (the reference's null batch); its report row is (coefs_k[0], 0, 0);
+ *   mode 1: rows of ids outside [0, K) are dropped; an arm without rows is skipped (no solve); no discounting (interval 0);
+ *           x = state || act_feat[id] (action_dim columns, the constructor's action space) or state alone (action_dim 0).
+ * Rows keep their order within each arm.  1 <= K <= 1024, d <= 128, max_batch * (obs_dim + action_dim) < 2^31.  The flat buffers (device memory owned by the caller)
+ * are A f32[K][d][d], b f32[K][d], sum_weight f32[K], inv_A f32[K][d][d], coefs f32[K][d] (each arm's LinearRegression
+ * buffers as views), lam f32[K], gamma f32[K], interval f64[K], last f64[K] (last_sum_weight_when_discounted), act_feat
+ * f32[K][action_dim] (null when action_dim 0). */
+typedef struct prl_dcb_cfg {
+    int32_t obs_dim, n_arms, action_dim;
+    int32_t mode;                  /* 0: DisjointBanditContainer, 1: DisjointLinearBandit */
+    int32_t max_batch, max_rounds;
+} prl_dcb_cfg;
+typedef struct prl_dcb prl_dcb;
+int64_t prl_dcb_workspace_bytes(const prl_dcb_cfg *cfg);
+int prl_dcb_create(prl_dcb **out, const prl_dcb_cfg *cfg, float *A, float *b, float *sum_weight, float *inv_A, float *coefs,
+                   const float *lam, const float *gamma, const double *interval, double *last, const float *act_feat,
+                   void *workspace_dev);
+int prl_dcb_destroy(prl_dcb *dcb);
+int prl_dcb_set_graph(prl_dcb *dcb, int enable);
+int64_t prl_dcb_last_launches(const prl_dcb *dcb);
+/* Report (mode 0; every out pointer may be null): out_pred_dev / out_label_dev / out_weight_dev f32[rounds][batch + K],
+ * round r's rows arm by arm (arm k's rows in batch order, or its one null-batch row), the rest unwritten;
+ * out_counts_dev i32[rounds][K] = rows per arm; out_logical_dev i32[rounds][batch] = sampled indices.  A buffer of more
+ * than K actions is refused. */
+int prl_dcb_learn(prl_dcb *dcb, prl_buf *buf, int rounds, int batch, float *out_pred_dev, float *out_label_dev, float *out_weight_dev,
+                  int32_t *out_counts_dev, int32_t *out_logical_dev, void *stream);
+/* One round on a dense device batch: state f32[batch][obs_dim], or with state3d f32[batch][K][obs_dim] (arm k reads
+ * state[:, k]); arm i32[batch]; reward f32[batch]; weight f32[batch] (null: every weight 1); outputs as prl_dcb_learn's
+ * for one round. */
+int prl_dcb_learn_batch(prl_dcb *dcb, int batch, const float *state, int state3d, const int32_t *arm, const float *reward,
+                        const float *weight, float *out_pred_dev, float *out_label_dev, float *out_weight_dev, int32_t *out_counts_dev,
+                        void *stream);
+/* Scores of n states x K arms, x1 = [1, state, act_feat[k]] on arm k: out_scores f32[n][K] = x1 . coefs_k (+ alpha sigma_k
+ * when with_sigma, NaN -> 0); out_index (optional) i32[n] = first maximum where mask u8[n][K] is non-zero (as prl_cb_scores). */
+int prl_dcb_scores(prl_dcb *dcb, int n, const float *state, const float *act_feat, double alpha, int with_sigma, const uint8_t *mask,
+                   float *out_scores, int32_t *out_index, void *stream);
+/* Thompson sampling: out_theta_dev f32[K][d], arm k's draw as prl_cb_ts_sample's with lam[k] and the caller's standard
+ * normals eps_dev f32[K][d]; out_status_dev i32[K] = 0, or 1 where A_k + lambda_k I is not positive definite. */
+int prl_dcb_ts_sample(prl_dcb *dcb, const float *eps_dev, float *out_theta_dev, int32_t *out_status_dev, void *stream);
+/* Thompson scores x1 . theta_k written arm-major, out_scores f32[K][n] read as [n][K] (the reference's view of its stacked
+ * per-arm scores), and the first maximum of those rows as prl_dcb_scores. */
+int prl_dcb_ts_scores(prl_dcb *dcb, int n, const float *state, const float *act_feat, const float *theta_dev, const uint8_t *mask,
+                      float *out_scores, int32_t *out_index, void *stream);
+
 /* ---- contextual bandit: NeuralLinearBandit (neural LinUCB) -------------------------------------------------------
  * Replaces NeuralLinearBandit.learn_batch / act / get_scores (policy_learners/contextual_bandits/neural_linear_bandit.py)
  * over NeuralLinearRegression (neural_networks/contextual_bandit/neural_linear_regression.py) with two hidden layers.

@@ -299,9 +299,17 @@ try:  # pragma: no cover - depends on the environment; kept apart so the names a
     )
     from pearl.neural_networks.common.utils import LossType
     from pearl.policy_learners.exploration_modules.common.tiebreaking_strategy import TiebreakingStrategy
-    from pearl.policy_learners.exploration_modules.contextual_bandits.ucb_exploration import UCBExploration
+    from pearl.policy_learners.exploration_modules.contextual_bandits.ucb_exploration import (
+        DisjointUCBExploration, UCBExploration,
+    )
     from pearl.policy_learners.exploration_modules.contextual_bandits.thompson_sampling_exploration import (
         ThompsonSamplingExplorationLinear, ThompsonSamplingExplorationLinearDisjoint,
+    )
+    from pearl.policy_learners.contextual_bandits.disjoint_bandit import (
+        DisjointBanditContainer as _RefDisjointBanditContainer,
+    )
+    from pearl.policy_learners.contextual_bandits.disjoint_linear_bandit import (
+        DisjointLinearBandit as _RefDisjointLinearBandit,
     )
 
     HAVE_PEARL_BANDITS = True
@@ -334,8 +342,12 @@ if not HAVE_PEARL_BANDITS:
             self._enable_efficient_sampling = enable_efficient_sampling
             self.randomized_tiebreaking = randomized_tiebreaking
 
+    class DisjointUCBExploration(UCBExploration):
+        """Stand-in for DisjointUCBExploration (ucb_exploration.py:122-155): UCB with one model per arm."""
+
     class ThompsonSamplingExplorationLinearDisjoint(ThompsonSamplingExplorationLinear):
-        """Stand-in for the disjoint explorer (one model per action), which the CUDA learners refuse."""
+        """Stand-in for the disjoint explorer (thompson_sampling_exploration.py:106-142): one coefficient draw per arm's
+        model.  The disjoint CUDA learners use it; the single-ridge learners refuse it."""
 
         def __init__(self, enable_efficient_sampling: bool = False) -> None:
             super().__init__(enable_efficient_sampling=enable_efficient_sampling)
@@ -418,6 +430,78 @@ if not HAVE_PEARL_BANDITS:
                                            initial_coefs=initial_coefs)
             self.apply_discounting_interval = apply_discounting_interval
             self.last_sum_weight_when_discounted = 0.0
+
+        @property
+        def feature_dim(self) -> int:
+            return self._feature_dim
+
+        @property
+        def batch_size(self) -> int:
+            return self._batch_size
+
+        def set_history_summarization_module(self, value) -> None:
+            self._history_summarization_module = value
+
+        def reset(self, action_space) -> None:
+            pass
+
+    class _RefDisjointBanditContainer(nn.Module):
+        """Attribute-compatible stand-in for DisjointBanditContainer's constructor (policy_learners/contextual_bandits/
+        disjoint_bandit.py:44-65): same arguments and state_dict keys (`_arm_bandits.{i}.model._A`, ...)."""
+
+        def __init__(self, feature_dim: int, arm_bandits, exploration_module, training_rounds: int = 100,
+                     batch_size: int = 128) -> None:
+            super().__init__()
+            self.exploration_module = exploration_module
+            self.action_representation_module = IdentityActionRepresentationModule()
+            self._history_summarization_module = None
+            self._training_rounds, self._batch_size, self._training_steps = training_rounds, batch_size, 0
+            self.on_policy, self._is_action_continuous = False, False
+            self._feature_dim = feature_dim
+            self._arm_bandits = nn.ModuleList(arm_bandits)
+            self._n_arms = len(arm_bandits)
+            self._null_batch = None
+
+        @property
+        def n_arms(self) -> int:
+            return self._n_arms
+
+        @property
+        def models(self):
+            return [bandit.model for bandit in self._arm_bandits]
+
+        @property
+        def feature_dim(self) -> int:
+            return self._feature_dim
+
+        @property
+        def batch_size(self) -> int:
+            return self._batch_size
+
+        def set_history_summarization_module(self, value) -> None:
+            self._history_summarization_module = value
+
+        def reset(self, action_space) -> None:
+            pass
+
+    class _RefDisjointLinearBandit(nn.Module):
+        """Attribute-compatible stand-in for DisjointLinearBandit's constructor (policy_learners/contextual_bandits/
+        disjoint_linear_bandit.py:41-67): same arguments and state_dict keys (`_linear_regressions.{i}._A`, ...)."""
+
+        def __init__(self, feature_dim: int, action_space, exploration_module, l2_reg_lambda: float = 1.0,
+                     training_rounds: int = 100, batch_size: int = 128, state_features_only: bool = False) -> None:
+            super().__init__()
+            self.exploration_module = exploration_module
+            self.action_representation_module = IdentityActionRepresentationModule()
+            self._history_summarization_module = None
+            self._training_rounds, self._batch_size, self._training_steps = training_rounds, batch_size, 0
+            self.on_policy, self._is_action_continuous = False, False
+            self._feature_dim = feature_dim
+            self._linear_regressions_list = [_LinearRegression(feature_dim=feature_dim, l2_reg_lambda=l2_reg_lambda)
+                                             for _ in range(action_space.n)]
+            self._linear_regressions = nn.ModuleList(self._linear_regressions_list)
+            self._discrete_action_space = action_space
+            self._state_features_only = state_features_only
 
         @property
         def feature_dim(self) -> int:

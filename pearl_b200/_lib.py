@@ -142,6 +142,11 @@ class CbCfg(C.Structure):
                 ("discount_interval", C.c_double)]
 
 
+class DcbCfg(C.Structure):
+    _fields_ = [("obs_dim", C.c_int32), ("n_arms", C.c_int32), ("action_dim", C.c_int32), ("mode", C.c_int32),
+                ("max_batch", C.c_int32), ("max_rounds", C.c_int32)]
+
+
 class NlbCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("action_dim", C.c_int32), ("action_rep", C.c_int32),
                 ("h1", C.c_int32), ("h2", C.c_int32), ("skip", C.c_int32), ("e2e", C.c_int32), ("loss", C.c_int32),
@@ -351,6 +356,16 @@ _SIGNATURES = {
     "prl_cb_scores": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, C.c_double, C.c_int, _P, _P, _P, _P]),
     "prl_cb_ts_sample": (C.c_int, [C.c_int, C.c_double] + [_P] * 6),
     "prl_cb_ts_scores": (C.c_int, [_P, C.c_int, _P, C.c_int] + [_P] * 8),
+    "prl_dcb_workspace_bytes": (C.c_int64, [C.POINTER(DcbCfg)]),
+    "prl_dcb_create": (C.c_int, [C.POINTER(_P), C.POINTER(DcbCfg)] + [_P] * 11),
+    "prl_dcb_destroy": (C.c_int, [_P]),
+    "prl_dcb_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_dcb_last_launches": (C.c_int64, [_P]),
+    "prl_dcb_learn": (C.c_int, [_P, _P, C.c_int, C.c_int] + [_P] * 6),
+    "prl_dcb_learn_batch": (C.c_int, [_P, C.c_int, _P, C.c_int] + [_P] * 8),
+    "prl_dcb_scores": (C.c_int, [_P, C.c_int, _P, _P, C.c_double, C.c_int, _P, _P, _P, _P]),
+    "prl_dcb_ts_sample": (C.c_int, [_P] * 5),
+    "prl_dcb_ts_scores": (C.c_int, [_P, C.c_int] + [_P] * 7),
     "prl_nlb_param_count": (C.c_int64, [C.POINTER(NlbCfg)]),
     "prl_nlb_workspace_bytes": (C.c_int64, [C.POINTER(NlbCfg)]),
     "prl_nlb_create": (C.c_int, [C.POINTER(_P), C.POINTER(NlbCfg)] + [_P] * 4 + [C.c_int64] + [_P] * 7),

@@ -70,6 +70,32 @@ def _ts_failed(status: torch.Tensor, efficient: bool) -> None:
     raise ValueError("Thompson sampling: the precision matrix A + lambda I is not positive definite")
 
 
+def _check_ridge(feature_dim: int, l2_reg_lambda: float, force_pinv: bool) -> None:
+    """The ridge settings the CUDA solve refuses, for every learner built on it."""
+    if force_pinv:
+        raise NotImplementedError("force_pinv=True: the CUDA ridge solve inverts A + lambda I directly, with no "
+                                  "pseudo-inverse")
+    if not l2_reg_lambda > 0:
+        raise NotImplementedError(f"l2_reg_lambda={l2_reg_lambda}: the CUDA ridge solve needs l2_reg_lambda > 0 (the "
+                                  "reference's pinv fallback, which a singular A can reach, is not implemented)")
+    if int(feature_dim) > MAX_RIDGE_WIDTH:
+        raise NotImplementedError(f"feature_dim={feature_dim}: the CUDA ridge solve supports at most {MAX_RIDGE_WIDTH} "
+                                  "features (d = feature_dim + 1 <= 128)")
+
+
+def _refuse_negative_weights(weight: Optional[torch.Tensor]) -> None:
+    if weight is not None and bool((weight < 0).any()):      # the one host reduction, made only when a weight is given
+        raise NotImplementedError("negative weights: A + lambda I can then be singular, where the reference falls back "
+                                  "to a pseudo-inverse, which the CUDA ridge solve does not implement")
+
+
+def _check_history(learner) -> None:
+    h = getattr(learner, "_history_summarization_module", None)
+    if h is not None and any(True for _ in h.parameters()):
+        raise NotImplementedError("a history summarization module with parameters: the CUDA bandit learner reads the "
+                                  "stored states as they are")
+
+
 def _refuse_distributed() -> None:
     if torch.distributed.is_available() and torch.distributed.is_initialized():
         raise NotImplementedError("torch.distributed is initialized: the reference would all-reduce the ridge statistics, "
@@ -81,15 +107,7 @@ class B200LinearBandit(_RefLinearBandit):
                  apply_discounting_interval: float = 0.0, force_pinv: bool = False, training_rounds: int = 100,
                  batch_size: int = 128, action_representation_module=None, initial_coefs: Optional[torch.Tensor] = None, *,
                  max_rounds_per_call: int = 1024) -> None:
-        if force_pinv:
-            raise NotImplementedError("force_pinv=True: the CUDA ridge solve inverts A + lambda I directly, with no "
-                                      "pseudo-inverse")
-        if not l2_reg_lambda > 0:
-            raise NotImplementedError(f"l2_reg_lambda={l2_reg_lambda}: the CUDA ridge solve needs l2_reg_lambda > 0 (the "
-                                      "reference's pinv fallback, which a singular A can reach, is not implemented)")
-        if int(feature_dim) > MAX_RIDGE_WIDTH:
-            raise NotImplementedError(f"feature_dim={feature_dim}: the CUDA ridge solve supports at most {MAX_RIDGE_WIDTH} "
-                                      "features (d = feature_dim + 1 <= 128)")
+        _check_ridge(feature_dim, l2_reg_lambda, force_pinv)
         super().__init__(feature_dim=feature_dim, exploration_module=exploration_module, l2_reg_lambda=l2_reg_lambda,
                          gamma=gamma, apply_discounting_interval=apply_discounting_interval, force_pinv=force_pinv,
                          training_rounds=training_rounds, batch_size=batch_size,
@@ -175,10 +193,7 @@ class B200LinearBandit(_RefLinearBandit):
 
     def _check_learner(self) -> None:
         _refuse_distributed()
-        h = getattr(self, "_history_summarization_module", None)
-        if h is not None and any(True for _ in h.parameters()):
-            raise NotImplementedError("a history summarization module with parameters: the CUDA bandit learner reads the "
-                                      "stored states as they are")
+        _check_history(self)
 
     # ------------------------------------------------------------------ PolicyLearner.learn (policy_learner.py:162-195)
     def learn(self, replay_buffer: B200ReplayBuffer, trace: Optional[dict] = None) -> dict[str, Any]:
@@ -230,9 +245,7 @@ class B200LinearBandit(_RefLinearBandit):
         state, action = f32(rows(batch.state)), f32(rows(batch.action))
         reward = f32(batch.reward.reshape(B))
         weight = None if batch.weight is None else f32(batch.weight.reshape(B))
-        if weight is not None and bool((weight < 0).any()):      # the one host reduction, made only when a weight is given
-            raise NotImplementedError("negative weights: A + lambda I can then be singular, where the reference falls back "
-                                      "to a pseudo-inverse, which the CUDA ridge solve does not implement")
+        _refuse_negative_weights(weight)
         cb = self._bind(dev, int(state.shape[1]), int(action.shape[1]), 0, 0, B)
         pred = torch.empty((B, 1), dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):

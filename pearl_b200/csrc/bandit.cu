@@ -63,32 +63,6 @@ __global__ void k_cb_predict(int B, int k, const float *__restrict__ X, const fl
     if (call->out_weight) call->out_weight[o] = W[r];
 }
 
-// one warp's row x = [1, state s, action features a] of the scores (the warp's slice xw of shared memory): mu = x . coefs
-// and, with_sigma, q = x^T inv_A x, both summed over the warp
-__device__ __forceinline__ void cb_row_form(int s, int a, int obs, int act_dim, const float *__restrict__ state,
-                                            const float *__restrict__ act_feat, const float *__restrict__ inv_A,
-                                            const float *__restrict__ coefs, int with_sigma, float *x, int lane, float &mu,
-                                            float &q) {
-    const int d = obs + act_dim + 1;
-    for (int c = lane; c < d; c += 32)
-        x[c] = c == 0 ? 1.f : (c <= obs ? state[(size_t)s * obs + c - 1] : act_feat[(size_t)a * act_dim + c - 1 - obs]);
-    __syncwarp();
-    mu = 0.f; q = 0.f;
-    for (int j = lane; j < d; j += 32) {
-        mu = fmaf(x[j], coefs[j], mu);
-        if (with_sigma) {
-            float t = 0.f;
-            for (int i = 0; i < d; i++) t = fmaf(x[i], inv_A[(size_t)i * d + j], t);
-            q = fmaf(t, x[j], q);
-        }
-    }
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        mu += __shfl_xor_sync(0xffffffffu, mu, o);
-        q += __shfl_xor_sync(0xffffffffu, q, o);
-    }
-}
-
 // scores of n states x S actions, one warp per (state, action) row x = [1, state, action features a]:
 //   mu = x . coefs;  with_sigma: mu + alpha sigma, sigma = sqrt(x^T inv_A x), NaN (a negative form) -> 0
 // Thompson sampling scores x . theta through this kernel with coefs = theta and no sigma.

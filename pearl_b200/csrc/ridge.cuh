@@ -3,7 +3,9 @@
 // NeuralLinearBandit (neural_linear.cu, rows = the network's output).  The row load, the fixed-order statistics and their
 // reduction into A, b and sum_weight, the discounting decision with the fp64 Gauss-Jordan solve, and the first-maximum
 // argmax of the UCB scores.  bandit.cu's header describes the numerics.  The row load, the scoring feature rows
-// (k_cb_feat) and the argmax also serve NeuralBandit (neural_bandit.cu), which has no ridge.
+// (k_cb_feat) and the argmax also serve NeuralBandit (neural_bandit.cu), which has no ridge.  The statistics, reduction,
+// solve, sampler and score-row bodies are __device__ functions that the one-ridge kernels here and the per-arm kernels
+// of the disjoint learners (disjoint_bandit.cu) both call.
 //
 // Every kernel is `static`: each translation unit that includes this header has its own copy, so the solve's dynamic
 // shared-memory attribute is set per unit (cb_solve_prepare, called from each learner's create).
@@ -67,10 +69,11 @@ static __global__ void k_cb_feat(int m, long long r0, int S, int obs, int act_di
     for (int p = lane; p < act_dim; p += 32) x[obs + p] = act_feat[(size_t)a * act_dim + p];
 }
 
-// partial sums of the rows of chunk blockIdx.x into P[chunk][e], one entry per thread (blockIdx.y selects the entries),
-// rows in ascending order.  The rows [1, x] are staged kStage at a time with x w and y w beside them.
-static __global__ void __launch_bounds__(256) k_cb_stats(int B, int k, const float *__restrict__ X, const float *__restrict__ Y,
-                                                  const float *__restrict__ W, float *__restrict__ P) {
+// partial sums of the rows of chunk c = blockIdx.x - chunk0 (rows [c kChunk, +kChunk) of the B rows) into P[c][e], one
+// entry per thread (blockIdx.y selects the entries), rows in ascending order.  The rows [1, x] are staged kStage at a time
+// with x w and y w beside them.  The body of k_cb_stats (chunk0 = 0) and of the per-arm k_dj_stats.
+static __device__ __forceinline__ void cb_stats_chunk(int B, int k, const float *__restrict__ X, const float *__restrict__ Y,
+                                                      const float *__restrict__ W, float *__restrict__ P, unsigned chunk0) {
     __shared__ float xs[kStage][kMaxD], xws[kStage][kMaxD], yw[kStage], ws[kStage];
     const int d = k + 1, T = d * (d + 1) / 2, E = T + d + 1;
     const int e = blockIdx.y * blockDim.x + threadIdx.x;
@@ -86,7 +89,8 @@ static __global__ void __launch_bounds__(256) k_cb_stats(int B, int k, const flo
         kind = 1;
         i = e - T;
     }
-    const int r0 = blockIdx.x * kChunk, r1 = min(B, r0 + kChunk);
+    const unsigned chunk = blockIdx.x - chunk0;
+    const int r0 = chunk * kChunk, r1 = min(B, r0 + kChunk);
     float acc = 0.f;
     for (int s0 = r0; s0 < r1; s0 += kStage) {
         const int n = min(kStage, r1 - s0);
@@ -111,12 +115,18 @@ static __global__ void __launch_bounds__(256) k_cb_stats(int B, int k, const flo
                 for (int rr = 0; rr < n; rr++) acc = __fadd_rn(acc, ws[rr]);
         }
     }
-    if (e < E) P[(size_t)blockIdx.x * E + e] = acc;
+    if (e < E) P[(size_t)chunk * E + e] = acc;
 }
 
-// the chunks' partials added in ascending chunk order, then added into A (both triangles), b and sum_weight
-static __global__ void k_cb_reduce(int d, int chunks, const float *__restrict__ P, float *__restrict__ A, float *__restrict__ b,
-                            float *__restrict__ sum_weight) {
+static __global__ void __launch_bounds__(256) k_cb_stats(int B, int k, const float *__restrict__ X, const float *__restrict__ Y,
+                                                  const float *__restrict__ W, float *__restrict__ P) {
+    cb_stats_chunk(B, k, X, Y, W, P, 0);
+}
+
+// entry blockIdx.x blockDim.x + threadIdx.x of the chunks' partials added in ascending chunk order, then added into A (both triangles), b and sum_weight.
+// The body of k_cb_reduce and of the per-arm k_dj_reduce.
+static __device__ __forceinline__ void cb_reduce_entry(int d, int chunks, const float *__restrict__ P, float *__restrict__ A,
+                                                       float *__restrict__ b, float *__restrict__ sum_weight) {
     const int T = d * (d + 1) / 2, E = T + d + 1;
     const int e = blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= E) return;
@@ -136,13 +146,18 @@ static __global__ void k_cb_reduce(int d, int chunks, const float *__restrict__ 
     }
 }
 
-// _maybe_apply_discounting, then calculate_coefs.  One CTA; M = A + lambda I in fp64 shared memory [d][d], inverted in place
-// by Gauss-Jordan elimination with partial pivoting (first largest |pivot|, as LAPACK's idamax picks), the row exchanges
-// undone as column exchanges at the end.  Then round_idx advances (k_cb_predict reads the round it finished).
-static __global__ void __launch_bounds__(kSolveThreads) k_cb_solve(int d, float lam, float gamma, double interval, float *__restrict__ A,
-                                                            float *__restrict__ b, const float *__restrict__ sum_weight,
-                                                            double *__restrict__ last_discount, float *__restrict__ inv_A,
-                                                            float *__restrict__ coefs, int *__restrict__ round_idx) {
+static __global__ void k_cb_reduce(int d, int chunks, const float *__restrict__ P, float *__restrict__ A, float *__restrict__ b,
+                            float *__restrict__ sum_weight) {
+    cb_reduce_entry(d, chunks, P, A, b, sum_weight);
+}
+
+// _maybe_apply_discounting, then calculate_coefs, by one CTA: M = A + lambda I in fp64 shared memory [d][d], inverted in
+// place by Gauss-Jordan elimination with partial pivoting (first largest |pivot|, as LAPACK's idamax picks), the row
+// exchanges undone as column exchanges at the end.  The body of k_cb_solve and of the per-arm k_dj_solve.
+static __device__ __forceinline__ void cb_solve_ridge(int d, float lam, float gamma, double interval, float *__restrict__ A,
+                                                      float *__restrict__ b, const float *__restrict__ sum_weight,
+                                                      double *__restrict__ last_discount, float *__restrict__ inv_A,
+                                                      float *__restrict__ coefs) {
     extern __shared__ double sm[];
     double *M = sm, *bb = sm + (size_t)d * d;
     __shared__ double f[kMaxD];
@@ -221,7 +236,41 @@ static __global__ void __launch_bounds__(kSolveThreads) k_cb_solve(int d, float 
         for (int j = 0; j < d; j++) c = fma(M[(size_t)i * d + j], bb[j], c);
         coefs[i] = (float)c;
     }
-    if (tid == 0) *round_idx += 1;
+}
+
+// one CTA: cb_solve_ridge, then round_idx advances (k_cb_predict reads the round it finished)
+static __global__ void __launch_bounds__(kSolveThreads) k_cb_solve(int d, float lam, float gamma, double interval, float *__restrict__ A,
+                                                            float *__restrict__ b, const float *__restrict__ sum_weight,
+                                                            double *__restrict__ last_discount, float *__restrict__ inv_A,
+                                                            float *__restrict__ coefs, int *__restrict__ round_idx) {
+    cb_solve_ridge(d, lam, gamma, interval, A, b, sum_weight, last_discount, inv_A, coefs);
+    if (threadIdx.x == 0) *round_idx += 1;
+}
+
+// one warp's row x = [1, state s, action features a] of the scores (the warp's slice x of shared memory): mu = x . coefs
+// and, with_sigma, q = x^T inv_A x, both summed over the warp
+static __device__ __forceinline__ void cb_row_form(int s, int a, int obs, int act_dim, const float *__restrict__ state,
+                                            const float *__restrict__ act_feat, const float *__restrict__ inv_A,
+                                            const float *__restrict__ coefs, int with_sigma, float *x, int lane, float &mu,
+                                            float &q) {
+    const int d = obs + act_dim + 1;
+    for (int c = lane; c < d; c += 32)
+        x[c] = c == 0 ? 1.f : (c <= obs ? state[(size_t)s * obs + c - 1] : act_feat[(size_t)a * act_dim + c - 1 - obs]);
+    __syncwarp();
+    mu = 0.f; q = 0.f;
+    for (int j = lane; j < d; j += 32) {
+        mu = fmaf(x[j], coefs[j], mu);
+        if (with_sigma) {
+            float t = 0.f;
+            for (int i = 0; i < d; i++) t = fmaf(x[i], inv_A[(size_t)i * d + j], t);
+            q = fmaf(t, x[j], q);
+        }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        mu += __shfl_xor_sync(0xffffffffu, mu, o);
+        q += __shfl_xor_sync(0xffffffffu, q, o);
+    }
 }
 
 // first maximum of each state's scores over the positions whose mask is non-zero (every position when mask is null);
@@ -245,10 +294,10 @@ static __global__ void k_cb_argmax(int n, int S, const float *__restrict__ score
 // down; torch factors the index-reversed M, which is the same factorisation).  U overwrites M's upper triangle.  Then
 // U^T x = eps by forward substitution in one warp, and theta = coefs + x rounded to fp32: x has covariance
 // U^-T U^-1 = M^-1.  *status = 0, or 1 when a pivot is not positive (M is not positive definite, a NaN included), and
-// theta is then left unwritten: the reference's argument validation raises there.
-static __global__ void __launch_bounds__(kSolveThreads) k_cb_ts_sample(int d, float lam, const float *__restrict__ A,
-                                                                const float *__restrict__ coefs, const float *__restrict__ eps,
-                                                                float *__restrict__ theta, int *__restrict__ status) {
+// theta is then left unwritten: the reference's argument validation raises there.  The body of k_cb_ts_sample and of the
+// per-arm k_dj_ts_sample.
+static __device__ __forceinline__ void cb_ts_draw(int d, float lam, const float *__restrict__ A, const float *__restrict__ coefs,
+                                                  const float *__restrict__ eps, float *__restrict__ theta, int *__restrict__ status) {
     extern __shared__ double sm[];
     double *M = sm, *r = sm + (size_t)d * d;
     const int tid = threadIdx.x, nt = blockDim.x, dd = d * d;
@@ -282,6 +331,12 @@ static __global__ void __launch_bounds__(kSolveThreads) k_cb_ts_sample(int d, fl
         __syncwarp();
     }
     if (tid == 0) *status = 0;
+}
+
+static __global__ void __launch_bounds__(kSolveThreads) k_cb_ts_sample(int d, float lam, const float *__restrict__ A,
+                                                                const float *__restrict__ coefs, const float *__restrict__ eps,
+                                                                float *__restrict__ theta, int *__restrict__ status) {
+    cb_ts_draw(d, lam, A, coefs, eps, theta, status);
 }
 
 static size_t cb_solve_smem(int d) { return ((size_t)d * d + d) * sizeof(double); }
