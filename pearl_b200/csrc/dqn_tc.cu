@@ -27,8 +27,9 @@
 //            for the whole step.
 //   AdamW    gradients registers -> shared staging, then one sweep over the flat W1 | b1 | W2 range whose parameters and
 //            moments stream in by TMA bulk copies, in 16 KB chunks through an 8-slot ring in regions 3 and 1 (free once
-//            the last weight-gradient products have been waited for); 16-byte stores write the results and the
-//            operand-layout weight tiles.  b1 | b2 | W3 | b3 are updated one parameter per thread.  Shapes with
+//            the last weight-gradient products have been waited for); 16-byte stores write the results, and the new W1 | W2
+//            replace their gradients in the staging, from which a second pass writes the operand-layout weight tiles in
+//            tile order (coalesced).  b1 | b2 | W3 | b3 are updated one parameter per thread.  Shapes with
 //            D % 4 != 0 (1 or 2 actions) or parameters that are not 16-byte aligned take a scalar sweep instead.
 //
 // The weights are kept in global memory a second time IN THE OPERAND LAYOUT (hi tile = the fp32 values — the tensor
@@ -830,49 +831,59 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                     if (i < an && (i < n1 || i >= d.oW2)) {
                         const float4 *sl = reinterpret_cast<const float4 *>(aslot(s)) + tid;
                         float4 w = sl[0], mm = sl[ACH / 4], vv = sl[ACH / 2], xx = sl[3 * ACH / 4];
-                        const bool is_w1 = i < n1;
-                        int row, c;
-                        const float *gp;
-                        if (is_w1) {
-                            row = i / d.D; c = i - row * d.D;
+                        float *gp;
+                        if (i < n1) {
+                            const int row = i / d.D, c = i - row * d.D;
                             gp = gs_w1 + row * pitch1 + c;
                         } else {
                             const int e = i - d.oW2;
-                            row = e >> 6; c = e & 63;
-                            gp = gs_w2 + row * 65 + c;
+                            gp = gs_w2 + (e >> 6) * 65 + (e & 63);
                         }
                         w.x = adam_math(w.x, mm.x, vv.x, xx.x, gp[0], hs); w.y = adam_math(w.y, mm.y, vv.y, xx.y, gp[1], hs);
                         w.z = adam_math(w.z, mm.z, vv.z, xx.z, gp[2], hs); w.w = adam_math(w.w, mm.w, vv.w, xx.w, gp[3], hs);
                         *reinterpret_cast<float4 *>(L.w + i) = w; *reinterpret_cast<float4 *>(L.m + i) = mm;
                         *reinterpret_cast<float4 *>(L.v + i) = vv; *reinterpret_cast<float4 *>(L.vmax + i) = xx;
-                        // the same values in the operand-layout tiles (hi = the value, lo = residual)
-                        if (is_w1) {
-                            if (c < d.obs) {
-                                const int ti = umma::tile_index(row, c, k1);
-                                *reinterpret_cast<float4 *>(To().w1hi + ti) = w;
-                                *reinterpret_cast<float4 *>(To().w1lo + ti) = make_float4(tf32_lo(w.x), tf32_lo(w.y), tf32_lo(w.z), tf32_lo(w.w));
-                            }
-                        } else {   // kperm order: columns c, c + 2 and c + 1, c + 3 are neighbours
-                            const int te = umma::tile_index(row, umma::kperm(c), HID), to = umma::tile_index(row, umma::kperm(c + 1), HID);
-                            *reinterpret_cast<float2 *>(To().w2 + te) = make_float2(w.x, w.z);
-                            *reinterpret_cast<float2 *>(To().w2 + to) = make_float2(w.y, w.w);
-                            *reinterpret_cast<float2 *>(To().w2 + 4096 + te) = make_float2(tf32_lo(w.x), tf32_lo(w.z));
-                            *reinterpret_cast<float2 *>(To().w2 + 4096 + to) = make_float2(tf32_lo(w.y), tf32_lo(w.w));
-                            // W2^T: columns c .. c + 3 are its rows, row `row` its column kperm(row)
-                            float *w2t = To().w2t;
-                            const int kr = umma::kperm(row);
-                            const float wv[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-                            for (int u = 0; u < 4; u++) {
-                                const int ti = umma::tile_index(c + u, kr, HID);
-                                w2t[ti] = wv[u]; w2t[4096 + ti] = tf32_lo(wv[u]);
-                            }
-                        }
+                        // the new value replaces its gradient in the staging: the operand tiles are built from there below
+                        gp[0] = w.x; gp[1] = w.y; gp[2] = w.z; gp[3] = w.w;
                     }
                     if (k + ARING < nch) {   // every thread is done with slot s: refill it with chunk k + ARING
                         __syncthreads();
                         if (tid == 0) adam_issue(k + ARING);
                     }
+                }
+                __syncthreads();
+                // The operand-layout tiles from the new W1 | W2 in the staging, one 16-byte group of a tile per thread and
+                // store, in tile order: coalesced, where the sweep's own order scattered them (16-byte pieces of W1 and W2
+                // into separate sectors, W2^T one float at a time), which made the tile stores most of the sweep's store
+                // traffic.  A group is row r, columns k .. k + 3 of the tile (umma::tile_index).
+                auto group_rc = [](int p, int K, int &r, int &k) {
+                    const int rem = p % (8 * K);
+                    r = p / (8 * K) * 8 + ((rem >> 2) & 7);
+                    k = (rem >> 5) * 4;
+                };
+                auto put = [](float *hi, float *lo, int p, float4 x) {
+                    *reinterpret_cast<float4 *>(hi + p) = x;
+                    *reinterpret_cast<float4 *>(lo + p) = make_float4(tf32_lo(x.x), tf32_lo(x.y), tf32_lo(x.z), tf32_lo(x.w));
+                };
+                // kperm^-1: the W2 column at K position t of a kperm-ordered tile
+                auto kinv = [](int t) { return (t & ~7) | ((t & 3) << 1) | ((t >> 2) & 1); };
+                const NetTiles t = To();
+                for (int p = 4 * tid; p < HID * k1; p += 4 * NTH) {   // W1: columns from obs on stay zero
+                    int r, k;
+                    group_rc(p, k1, r, k);
+                    if (k < d.obs) {
+                        const float *g = gs_w1 + r * pitch1 + k;
+                        put(t.w1hi, t.w1lo, p, make_float4(g[0], g[1], g[2], g[3]));
+                    }
+                }
+                for (int p = 4 * tid; p < HID * HID; p += 4 * NTH) {
+                    int r, k;
+                    group_rc(p, HID, r, k);
+                    const float *g = gs_w2 + r * 65;   // W2 tile: row r, K positions k .. k + 3 = columns kinv(k + q)
+                    put(t.w2, t.w2 + 4096, p, make_float4(g[kinv(k)], g[kinv(k + 1)], g[kinv(k + 2)], g[kinv(k + 3)]));
+                    // W2^T tile: row r = W2 column, K positions k .. k + 3 = W2 rows kinv(k + q)
+                    put(t.w2t, t.w2t + 4096, p, make_float4(gs_w2[kinv(k) * 65 + r], gs_w2[kinv(k + 1) * 65 + r],
+                                                            gs_w2[kinv(k + 2) * 65 + r], gs_w2[kinv(k + 3) * 65 + r]));
                 }
             } else {
                 for (int row = warp; row < HID; row += 8)
