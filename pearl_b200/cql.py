@@ -11,11 +11,12 @@ CQL term as it computes it (include/pearl_b200.h).  alpha is read from `_conserv
 fallback."""
 from __future__ import annotations
 
-import torch
-
 from . import _lib
-from ._batch import available_first, checked_ids
-from .replay_buffer import _stream_ptr
+from ._batch import check_features, dense_rows, next_available_first, plugin_call, slot_ids
+
+PREFIX = "prl_cql_"
+NAME = "conservative (CQL) DQN"
+LAUNCH_INFO = dict(launches="last_launches")
 
 
 def check_config(pl, engine: str) -> None:
@@ -35,6 +36,11 @@ def alpha(pl) -> float:
     return float(a)
 
 
+def learn_args(pl) -> tuple:
+    """The arguments prl_cql_learn takes after the training-step count: alpha."""
+    return (alpha(pl),)
+
+
 def make_cfg(pl, hp: dict, max_batch: int) -> _lib.CqlCfg:
     return _lib.CqlCfg(obs_dim=pl._obs_dim, n_actions=pl._n_actions, hidden1=pl._hidden[0], hidden2=pl._hidden[1],
                        double_dqn=int(pl._double), target_update_freq=int(pl._target_update_freq), max_batch=max_batch,
@@ -48,33 +54,9 @@ def learn_batch(pl, batch) -> dict:
     `curr_unavailable_actions_mask`) defaults to every action; next-action slots that are masked are compacted away in
     order, which keeps DoubleDQN's first argmax."""
     B, A = len(batch), pl._n_actions
-    if int(batch.state.shape[-1]) != pl._obs_dim:
-        raise ValueError(f"batch.state has {int(batch.state.shape[-1])} features, the learner {pl._obs_dim}")
+    check_features(batch, pl._obs_dim)
     pl._bind(B)
     dev = pl._device
-    f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
-    state, next_state = f32(batch.state), f32(batch.next_state)
-    reward = f32(batch.reward.reshape(B))
-    term = batch.terminated.reshape(B).to(device=dev, dtype=torch.uint8).contiguous()
-    i32 = lambda t: t.to(torch.int32).contiguous()  # noqa: E731
-    action = i32(checked_ids(batch.action.to(dev), A, batch.action.dim() == 2, "batch.action").reshape(B))
-    cur = nid = cnt = None
-    ca = getattr(batch, "curr_available_actions", None)
-    if ca is not None:
-        ca = ca.to(dev)
-        cur = i32(checked_ids(ca, A, ca.dim() == 3, "batch.curr_available_actions").reshape(B, A))
-    na = getattr(batch, "next_available_actions", None)
-    if na is not None:
-        na = na.to(dev)
-        nid = checked_ids(na, A, na.dim() == 3, "batch.next_available_actions").reshape(B, A)
-        nid, cnt = available_first(nid, getattr(batch, "next_unavailable_actions_mask", None))
-    out = torch.empty(1, dtype=torch.float32, device=dev)
-    lib, h, p = pl._libh, pl._handle, _lib.ptr
-    with torch.cuda.device(dev):
-        _lib.check(lib.prl_cql_set_graph(h, int(pl.use_cuda_graph)))
-        _lib.check(lib.prl_cql_learn_batch(h, B, p(state), p(action), p(reward), p(next_state), p(term), p(cur), p(nid), p(cnt),
-                                           int(pl._training_steps), alpha(pl), p(out), _stream_ptr(dev)))
-    loss = out.item()  # also keeps the inputs alive until the round is done
-    pl._sync_step_tensors()
-    return {"loss": loss}
-
+    cur = slot_ids(batch, "curr_available_actions", B, A, dev)
+    return plugin_call(pl, B, *dense_rows(batch, B, A, dev), cur, *next_available_first(batch, B, A, dev),
+                       int(pl._training_steps), alpha(pl))

@@ -24,11 +24,10 @@
 #include <limits.h>
 #include <math.h>
 
-#include <new>
-
 #include "common.cuh"
 #include "rounds.cuh"
 #include "gemm.cuh"
+#include "qrows.cuh"
 
 using namespace prl;
 
@@ -37,64 +36,26 @@ namespace {
 constexpr int kMaxA = 255;   // next-action ids are stored as bytes
 
 // per-call block the captured round reads through
-struct CqlCall {
-    const int32_t *slots;                     // [rounds][B] (learn)
-    float *out_loss;                          // [rounds]
-    // learn_batch: the caller's dense batch
-    const float *d_state, *d_next_state, *d_reward;
-    const int32_t *d_action_id;
+struct CqlCall : QSetCall {
     const int32_t *d_curr_ids;                // [B][A] current slot ids; null: every action (slot k holds k)
-    const int32_t *d_next_ids, *d_next_cnt;   // may be null: every action available next
-    const uint8_t *d_term;
-    float decay;                              // AdamW decoupled decay 1 - lr * weight_decay
     float alpha;                              // conservative_alpha
 };
 
-// rows of one round: state, next state, reward, terminated, the next-action id of every slot with the available count, and
-// the A + 1 online slots of the row: cids[b][k] = c_b[k] for k < A, cids[b][A] = the taken action.  records == null: pack
-// the caller's dense batch.  The ring stores no current action sets: every action, as B200ReplayBuffer.sample reports.
-__global__ void k_cql_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int A, int dynamic,
+// rows of one round (load_row), and the A + 1 online slots of the row: cids[b][k] = c_b[k] for k < A, cids[b][A] = the
+// taken action.  The ring stores no current action sets: every action, as B200ReplayBuffer.sample reports.
+__global__ void __launch_bounds__(256, 8) k_cql_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int A, int dynamic,
                            const CqlCall *__restrict__ call, const int *__restrict__ round_idx, int B, float *__restrict__ S,
                            float *__restrict__ S2, float *__restrict__ R, float *__restrict__ T, int *__restrict__ cnt,
                            int *__restrict__ ids, int *__restrict__ cids) {
     const int lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (w >= B) return;
+    const QRow row = load_row<true>(records, L, obs, A, dynamic, call, round_idx, B, w, lane, S, S2, R, T, ids);
     int *crow = cids + (size_t)w * (A + 1);
-    if (!records) {
-        for (int p = lane; p < obs; p += 32) {
-            S[(size_t)w * obs + p] = call->d_state[(size_t)w * obs + p];
-            S2[(size_t)w * obs + p] = call->d_next_state[(size_t)w * obs + p];
-        }
-        const int32_t *nid = call->d_next_ids, *cid = call->d_curr_ids;
-        for (int k = lane; k < A; k += 32) {
-            ids[(size_t)w * A + k] = nid ? nid[(size_t)w * A + k] : k;
-            crow[k] = cid ? cid[(size_t)w * A + k] : k;
-        }
-        if (lane == 0) {
-            crow[A] = call->d_action_id[w];
-            R[w] = call->d_reward[w];
-            T[w] = call->d_term[w] ? 1.f : 0.f;
-            cnt[w] = call->d_next_cnt ? min(call->d_next_cnt[w], A) : A;
-        }
-        return;
-    }
-    const int32_t *slots = call->slots + (size_t)(*round_idx) * B;
-    const uint32_t *r = records + (size_t)slots[w] * L.record_words;
-    for (int p = lane; p < obs; p += 32) {
-        S[(size_t)w * obs + p] = __uint_as_float(r[L.off_state + p]);
-        S2[(size_t)w * obs + p] = __uint_as_float(r[L.off_next_state + p]);
-    }
-    const uint8_t *id8 = reinterpret_cast<const uint8_t *>(r + L.off_avail);
-    for (int k = lane; k < A; k += 32) {
-        ids[(size_t)w * A + k] = dynamic ? (int)id8[k] : k;
-        crow[k] = k;
-    }
+    const int32_t *cid = records ? nullptr : call->d_curr_ids;
+    for (int k = lane; k < A; k += 32) crow[k] = cid ? cid[(size_t)w * A + k] : k;
     if (lane == 0) {
-        const uint32_t fl = r[L.off_flags];
-        crow[A] = (int)r[L.off_action];
-        R[w] = __uint_as_float(r[L.off_reward]);
-        T[w] = (fl & 1u) ? 1.f : 0.f;
-        cnt[w] = dynamic ? min((int)((fl >> 8) & 0xffffu), A) : A;
+        crow[A] = row.action;
+        cnt[w] = row.cnt;
     }
 }
 
@@ -119,34 +80,15 @@ __global__ void __launch_bounds__(128) k_cql_target(int B, int A, int dbl, const
         const float v = k < n_ok ? sel[k] : -INFINITY;
         if (v > best || (v == best && k < bk)) { best = v; bk = k; }
     }
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int ok = __shfl_xor_sync(0xffffffffu, bk, o);
-        if (ov > best || (ov == best && ok < bk)) { best = ov; bk = ok; }
-    }
+    warp_first_max(best, bk);
     const float V = dbl ? qt[(size_t)b * A + (bk == INT_MAX ? 0 : bk)] : best;
     const float *l = q_all + (size_t)b * (A + 1);
-    // logsumexp over the A current slots: row max, then the sum of exp(l - max) (per lane in slot order, then a fixed tree)
-    float mx = -INFINITY;
-    for (int k = lane; k < A; k += 32) mx = fmaxf(mx, l[k]);
-#pragma unroll
-    for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    float s = 0.f;
-    for (int k = lane; k < A; k += 32) s += expf(l[k] - mx);
-#pragma unroll
-    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    const float alpha = call->alpha, fB = (float)B, inv_ba = 1.f / ((float)B * (float)A);
     float *d = dq + (size_t)b * (A + 1);
-    for (int k = lane; k < A; k += 32) {
-        const float p = expf(l[k] - mx) / s;
-        const float n_k = k == 0 ? (float)(A - 1) : (k == 1 ? 1.f : 0.f);
-        d[k] = __fmul_rn(alpha, __fsub_rn(__fdiv_rn(p, fB), __fmul_rn(n_k, inv_ba)));
-    }
+    cql_slot_grad(A, B, call->alpha, lane, [&](int k) { return l[k]; }, [&](int k, float g) { d[k] = g; });
     if (lane == 0) {
         const float y = __fadd_rn(__fmul_rn(__fmul_rn(V, gamma), __fsub_rn(1.f, term[b])), rew[b]);
         const float e = __fsub_rn(l[A], y);
-        d[A] = __fmul_rn(__fdiv_rn(2.f, fB), e);
+        d[A] = __fmul_rn(__fdiv_rn(2.f, (float)B), e);
         rowabs[b] = fabsf(e);
     }
 }
@@ -154,22 +96,20 @@ __global__ void __launch_bounds__(128) k_cql_target(int B, int A, int dbl, const
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_cql : Rounds<prl_cql, CqlCall> {
+struct prl_cql : FlatQ<prl_cql, CqlCall, prl_cql_cfg> {
     static constexpr const char *kFn = "prl_cql", *kName = "CQL";
-    static constexpr bool kTargetOn = true;
     static constexpr int kGraphs = 3;
-    void fill_call(CqlCall &k) const { k.decay = (float)(1.0 - cfg.lr * cfg.weight_decay); }
-    prl_cql_cfg cfg;
-    int P;
     int W1, b1, W2, b2, W3, b3;
-    float *q, *q_t, *q_m, *q_v, *q_x;
     // workspace
     float *S, *S2, *R, *T, *P1, *c1, *c2, *qa, *P1t, *c1t, *c2t, *qt, *qn, *dq, *rowabs, *dc2, *dc1, *dh1, *grad;
     int *cnt, *ids, *cids;
+    static int check(const prl_cql_cfg *c);
+    static void layout(prl_cql *s);
+    static int64_t carve(prl_cql *s, void *base);
     static int round(prl_cql *s, prl_buf *buf, int B, cudaStream_t st);
 };
 
-static void cql_layout(prl_cql *s) {
+void prl_cql::layout(prl_cql *s) {
     const prl_cql_cfg &c = s->cfg;
     const int D = c.obs_dim + c.n_actions;
     int o = 0;
@@ -179,7 +119,7 @@ static void cql_layout(prl_cql *s) {
     s->P = o;
 }
 
-static int cql_check(const prl_cql_cfg *c) {
+int prl_cql::check(const prl_cql_cfg *c) {
     PRL_REQUIRE(c, "null cfg");
     PRL_REQUIRE(c->obs_dim > 0 && c->hidden1 > 0 && c->hidden2 > 0, "dimensions must be positive");
     PRL_REQUIRE(c->n_actions >= 2 && c->n_actions <= kMaxA,
@@ -194,14 +134,8 @@ static int cql_check(const prl_cql_cfg *c) {
     return PRL_OK;
 }
 
-extern "C" int64_t prl_cql_param_count(const prl_cql_cfg *c) {
-    if (cql_check(c)) return -1;
-    prl_cql t; t.cfg = *c; cql_layout(&t);
-    return t.P;
-}
-
 // the workspace, in order; base == null: only its size
-static int64_t cql_carve(prl_cql *s, void *base) {
+int64_t prl_cql::carve(prl_cql *s, void *base) {
     const prl_cql_cfg &c = s->cfg;
     const int64_t B = c.max_batch, O = c.obs_dim, A = c.n_actions, BA = B * A, BA1 = B * (A + 1), H1 = c.hidden1, H2 = c.hidden2;
     Carve w{(char *)base};
@@ -214,25 +148,12 @@ static int64_t cql_carve(prl_cql *s, void *base) {
     s->carve_tail(w, c.max_rounds, B);
     return w.bytes;
 }
-extern "C" int64_t prl_cql_workspace_bytes(const prl_cql_cfg *c) {
-    if (cql_check(c)) return -1;
-    prl_cql t; t.cfg = *c; cql_layout(&t);
-    return cql_carve(&t, nullptr);
-}
 
+extern "C" int64_t prl_cql_param_count(const prl_cql_cfg *c) { return prl_cql::param_count(c); }
+extern "C" int64_t prl_cql_workspace_bytes(const prl_cql_cfg *c) { return prl_cql::workspace_bytes(c); }
 extern "C" int prl_cql_create(prl_cql **out, const prl_cql_cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq,
                               float *max_exp_avg_sq, int64_t adam_step, void *workspace) {
-    PRL_REQUIRE(out && w && w_target && exp_avg && exp_avg_sq && max_exp_avg_sq && workspace, "null argument");
-    int rc = cql_check(cfg);
-    if (rc) return rc;
-    prl_cql *s = new (std::nothrow) prl_cql();
-    if (!s) return fail(PRL_ENOMEM, "out of host memory");
-    s->cfg = *cfg;
-    cql_layout(s);
-    s->q = w; s->q_t = w_target; s->q_m = exp_avg; s->q_v = exp_avg_sq; s->q_x = max_exp_avg_sq;
-    s->adam_step = adam_step;
-    cql_carve(s, workspace);
-    return prl_cql::open(s, out);
+    return prl_cql::create(out, cfg, w, w_target, exp_avg, exp_avg_sq, max_exp_avg_sq, adam_step, workspace);
 }
 extern "C" int prl_cql_destroy(prl_cql *s) { return prl_cql::destroy(s); }
 extern "C" int64_t prl_cql_adam_step(const prl_cql *s) { return prl_cql::adam_step_of(s); }

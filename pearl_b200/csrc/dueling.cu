@@ -29,11 +29,10 @@
 #include <limits.h>
 #include <math.h>
 
-#include <new>
-
 #include "common.cuh"
 #include "rounds.cuh"
 #include "gemm.cuh"
+#include "qrows.cuh"
 
 using namespace prl;
 
@@ -42,17 +41,10 @@ namespace {
 constexpr int kMaxA = 255;   // next-action ids are stored as bytes
 
 // per-call block the captured round reads through
-struct DuelCall {
-    const int32_t *slots;                     // [rounds][B] (learn)
-    float *out_loss;                          // [rounds]
-    // learn_batch: the caller's dense batch
-    const float *d_state, *d_next_state, *d_reward;
-    const int32_t *d_action_id;
+struct DuelCall : QCall {
     const int32_t *d_curr_ids;                // [B][A] current slot ids
     const int32_t *d_next_ids;                // [B][A] next slot ids; null: slot k holds k
     const uint8_t *d_next_unavail;            // [B][A] 1 = unavailable; null: every slot available
-    const uint8_t *d_term;
-    float decay;                              // AdamW decoupled decay 1 - lr * weight_decay
     int query_alone;                          // the online mean runs over the query action alone (no current sets)
 };
 
@@ -67,56 +59,26 @@ __device__ __forceinline__ float slot_mean(const float *a, int K, int lane) {
 
 __device__ __forceinline__ float duel_q(float V, float adv, float mean) { return __fsub_rn(__fadd_rn(V, adv), mean); }
 
-// rows of one round: state, next state, reward, terminated, the id and unavailable flag of every next slot (slots at or
-// beyond the stored count read as id 0, as the reference pads), and the A + 1 online slots: cids[b][k] = c_b[k] for k < A,
-// cids[b][A] = the taken action.  records == null: pack the caller's dense batch.  The ring stores no current action sets:
-// every action, as B200ReplayBuffer.sample reports.
-__global__ void k_duel_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int A, int dynamic,
+// rows of one round (load_row): the id and unavailable flag of every next slot (slots at or beyond the stored count read
+// as id 0, as the reference pads), and the A + 1 online slots: cids[b][k] = c_b[k] for k < A, cids[b][A] = the taken
+// action.  The ring stores no current action sets: every action, as B200ReplayBuffer.sample reports.
+__global__ void __launch_bounds__(256, 8) k_duel_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int A, int dynamic,
                             const DuelCall *__restrict__ call, const int *__restrict__ round_idx, int B, float *__restrict__ S,
                             float *__restrict__ S2, float *__restrict__ R, float *__restrict__ T, int *__restrict__ ids,
                             int *__restrict__ un, int *__restrict__ cids) {
     const int lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (w >= B) return;
+    const QRow row = load_row<true>(records, L, obs, A, dynamic, call, round_idx, B, w, lane, S, S2, R, T, ids);
     int *crow = cids + (size_t)w * (A + 1);
     int *irow = ids + (size_t)w * A, *urow = un + (size_t)w * A;
-    if (!records) {
-        for (int p = lane; p < obs; p += 32) {
-            S[(size_t)w * obs + p] = call->d_state[(size_t)w * obs + p];
-            S2[(size_t)w * obs + p] = call->d_next_state[(size_t)w * obs + p];
-        }
-        const int32_t *nid = call->d_next_ids, *cid = call->d_curr_ids;
-        const uint8_t *nu = call->d_next_unavail;
-        for (int k = lane; k < A; k += 32) {
-            irow[k] = nid ? nid[(size_t)w * A + k] : k;
-            urow[k] = nu ? (nu[(size_t)w * A + k] ? 1 : 0) : 0;
-            crow[k] = cid ? cid[(size_t)w * A + k] : k;
-        }
-        if (lane == 0) {
-            crow[A] = call->d_action_id[w];
-            R[w] = call->d_reward[w];
-            T[w] = call->d_term[w] ? 1.f : 0.f;
-        }
-        return;
-    }
-    const int32_t *slots = call->slots + (size_t)(*round_idx) * B;
-    const uint32_t *r = records + (size_t)slots[w] * L.record_words;
-    for (int p = lane; p < obs; p += 32) {
-        S[(size_t)w * obs + p] = __uint_as_float(r[L.off_state + p]);
-        S2[(size_t)w * obs + p] = __uint_as_float(r[L.off_next_state + p]);
-    }
-    const uint32_t fl = r[L.off_flags];
-    const int cnt = dynamic ? min((int)((fl >> 8) & 0xffffu), A) : A;
-    const uint8_t *id8 = reinterpret_cast<const uint8_t *>(r + L.off_avail);
+    const int32_t *cid = records ? nullptr : call->d_curr_ids;
+    const uint8_t *nu = records ? nullptr : call->d_next_unavail;
     for (int k = lane; k < A; k += 32) {
-        irow[k] = dynamic ? (k < cnt ? (int)id8[k] : 0) : k;
-        urow[k] = k < cnt ? 0 : 1;
-        crow[k] = k;
+        if (k >= row.cnt) irow[k] = 0;
+        urow[k] = nu ? (nu[(size_t)w * A + k] ? 1 : 0) : (k < row.cnt ? 0 : 1);
+        crow[k] = cid ? cid[(size_t)w * A + k] : k;
     }
-    if (lane == 0) {
-        crow[A] = (int)r[L.off_action];
-        R[w] = __uint_as_float(r[L.off_reward]);
-        T[w] = (fl & 1u) ? 1.f : 0.f;
-    }
+    if (lane == 0) crow[A] = row.action;
 }
 
 // Bellman target and the loss gradients.  One warp per row b; lane l handles slots l, l + 32, ...
@@ -144,12 +106,7 @@ __global__ void __launch_bounds__(128) k_duel_target(int B, int A, int dbl, cons
         const float v = u[k] ? -INFINITY : duel_q(sv, sa[k], sm);
         if (v > best || (v == best && k < bk)) { best = v; bk = k; }
     }
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int ok = __shfl_xor_sync(0xffffffffu, bk, o);
-        if (ov > best || (ov == best && ok < bk)) { best = ov; bk = ok; }
-    }
+    warp_first_max(best, bk);
     float V = best;
     if (dbl) {
         const float a = at[(size_t)b * A + (bk == INT_MAX ? 0 : bk)];
@@ -190,21 +147,19 @@ struct DuelMlp { int W1, b1, W2, b2, W3, b3, in, h1, h2, out; };
 // activations of one forward pass on m rows with K advantage slots per row
 struct DuelAct { float *t1, *t2, *f, *v1, *v2, *V, *Pa, *a1, *a2, *adv; };
 
-struct prl_duel : Rounds<prl_duel, DuelCall> {
+struct prl_duel : FlatQ<prl_duel, DuelCall, prl_duel_cfg> {
     static constexpr const char *kFn = "prl_duel", *kName = "dueling DQN";
-    static constexpr bool kTargetOn = true;
     static constexpr int kGraphs = 3;
-    void fill_call(DuelCall &k) const { k.decay = (float)(1.0 - cfg.lr * cfg.weight_decay); }
-    prl_duel_cfg cfg;
-    int P;
     DuelMlp st, va, ad;
-    float *q, *q_t, *q_m, *q_v, *q_x;
     // workspace
     float *S, *S2, *R, *T;
     DuelAct on, nx;                           // online pass (kept for the backward pass); next-state pass scratch
     float *Vt, *At, *Vn, *An;                 // next-state V / advantages of the target and (DoubleDQN) online net
     float *dV, *dAdv, *rowabs, *da2, *da1, *dPa, *dv2, *dv1, *df, *dt2, *dt1, *grad;
     int *ids, *un, *cids;
+    static int check(const prl_duel_cfg *c);
+    static void layout(prl_duel *s);
+    static int64_t carve(prl_duel *s, void *base);
     static int round(prl_duel *s, prl_buf *buf, int B, cudaStream_t st);
 };
 
@@ -215,7 +170,7 @@ static void mlp_at(DuelMlp &m, int &o, int in, int h1, int h2, int out) {
     m.W3 = o; o += out * h2; m.b3 = o; o += out;
 }
 
-static void duel_layout(prl_duel *s) {
+void prl_duel::layout(prl_duel *s) {
     const prl_duel_cfg &c = s->cfg;
     int o = 0;
     mlp_at(s->st, o, c.obs_dim, c.state_h1, c.state_h2, c.feature_dim);
@@ -224,7 +179,7 @@ static void duel_layout(prl_duel *s) {
     s->P = o;
 }
 
-static int duel_check(const prl_duel_cfg *c) {
+int prl_duel::check(const prl_duel_cfg *c) {
     PRL_REQUIRE(c, "null cfg");
     PRL_REQUIRE(c->obs_dim > 0 && c->feature_dim > 0 && c->state_h1 > 0 && c->state_h2 > 0 && c->value_h1 > 0 && c->value_h2 > 0 &&
                 c->adv_h1 > 0 && c->adv_h2 > 0, "dimensions must be positive");
@@ -239,14 +194,8 @@ static int duel_check(const prl_duel_cfg *c) {
     return PRL_OK;
 }
 
-extern "C" int64_t prl_duel_param_count(const prl_duel_cfg *c) {
-    if (duel_check(c)) return -1;
-    prl_duel t; t.cfg = *c; duel_layout(&t);
-    return t.P;
-}
-
 // the workspace, in order; base == null: only its size
-static int64_t duel_carve(prl_duel *s, void *base) {
+int64_t prl_duel::carve(prl_duel *s, void *base) {
     const prl_duel_cfg &c = s->cfg;
     const int64_t B = c.max_batch, O = c.obs_dim, A = c.n_actions, F = c.feature_dim, BA = B * A, BA1 = B * (A + 1);
     Carve w{(char *)base};
@@ -266,25 +215,12 @@ static int64_t duel_carve(prl_duel *s, void *base) {
     s->carve_tail(w, c.max_rounds, B);
     return w.bytes;
 }
-extern "C" int64_t prl_duel_workspace_bytes(const prl_duel_cfg *c) {
-    if (duel_check(c)) return -1;
-    prl_duel t; t.cfg = *c; duel_layout(&t);
-    return duel_carve(&t, nullptr);
-}
 
+extern "C" int64_t prl_duel_param_count(const prl_duel_cfg *c) { return prl_duel::param_count(c); }
+extern "C" int64_t prl_duel_workspace_bytes(const prl_duel_cfg *c) { return prl_duel::workspace_bytes(c); }
 extern "C" int prl_duel_create(prl_duel **out, const prl_duel_cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq,
                                float *max_exp_avg_sq, int64_t adam_step, void *workspace) {
-    PRL_REQUIRE(out && w && w_target && exp_avg && exp_avg_sq && max_exp_avg_sq && workspace, "null argument");
-    int rc = duel_check(cfg);
-    if (rc) return rc;
-    prl_duel *s = new (std::nothrow) prl_duel();
-    if (!s) return fail(PRL_ENOMEM, "out of host memory");
-    s->cfg = *cfg;
-    duel_layout(s);
-    s->q = w; s->q_t = w_target; s->q_m = exp_avg; s->q_v = exp_avg_sq; s->q_x = max_exp_avg_sq;
-    s->adam_step = adam_step;
-    duel_carve(s, workspace);
-    return prl_duel::open(s, out);
+    return prl_duel::create(out, cfg, w, w_target, exp_avg, exp_avg_sq, max_exp_avg_sq, adam_step, workspace);
 }
 extern "C" int prl_duel_destroy(prl_duel *s) { return prl_duel::destroy(s); }
 extern "C" int64_t prl_duel_adam_step(const prl_duel *s) { return prl_duel::adam_step_of(s); }

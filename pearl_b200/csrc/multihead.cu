@@ -28,11 +28,10 @@
 #include <limits.h>
 #include <math.h>
 
-#include <new>
-
 #include "common.cuh"
 #include "rounds.cuh"
 #include "gemm.cuh"
+#include "qrows.cuh"
 
 using namespace prl;
 
@@ -42,64 +41,26 @@ constexpr int kMaxA = 255;   // next-action ids are stored as bytes
 constexpr int kColsPerLane = (kMaxA + 31) / 32;
 
 // per-call block the captured round reads through
-struct MhqCall {
-    const int32_t *slots;                     // [rounds][B] (learn)
-    float *out_loss;                          // [rounds]
-    // learn_batch: the caller's dense batch
-    const float *d_state, *d_next_state, *d_reward;
-    const int32_t *d_action_id;
+struct MhqCall : QSetCall {
     const int32_t *d_curr_ids;                // [B][A] current slot ids; null: every action (slot k holds k)
-    const int32_t *d_next_ids, *d_next_cnt;   // may be null: every action available next
-    const uint8_t *d_term;
-    float decay;                              // AdamW decoupled decay 1 - lr * weight_decay
     float alpha;                              // conservative_alpha
 };
 
-// rows of one round: state (S), next state (S2), reward, terminated, taken action, the next-action id of every slot with
-// the available count, and the current slot ids.  records == null: pack the caller's dense batch.  The ring stores no
-// current action sets: every action, as B200ReplayBuffer.sample reports.
-__global__ void k_mhq_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int A, int dynamic,
+// rows of one round (load_row): S holds the states, S2 the next states; the taken action and the current slot ids.  The
+// ring stores no current action sets: every action, as B200ReplayBuffer.sample reports.
+__global__ void __launch_bounds__(256, 8) k_mhq_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int A, int dynamic,
                            const MhqCall *__restrict__ call, const int *__restrict__ round_idx, int B, float *__restrict__ S,
                            float *__restrict__ S2, float *__restrict__ R, float *__restrict__ T, int *__restrict__ act,
                            int *__restrict__ cnt, int *__restrict__ ids, int *__restrict__ cur) {
     const int lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (w >= B) return;
-    int *irow = ids + (size_t)w * A, *crow = cur + (size_t)w * A;
-    if (!records) {
-        for (int p = lane; p < obs; p += 32) {
-            S[(size_t)w * obs + p] = call->d_state[(size_t)w * obs + p];
-            S2[(size_t)w * obs + p] = call->d_next_state[(size_t)w * obs + p];
-        }
-        const int32_t *nid = call->d_next_ids, *cid = call->d_curr_ids;
-        for (int k = lane; k < A; k += 32) {
-            irow[k] = nid ? nid[(size_t)w * A + k] : k;
-            crow[k] = cid ? cid[(size_t)w * A + k] : k;
-        }
-        if (lane == 0) {
-            act[w] = call->d_action_id[w];
-            R[w] = call->d_reward[w];
-            T[w] = call->d_term[w] ? 1.f : 0.f;
-            cnt[w] = call->d_next_cnt ? min(call->d_next_cnt[w], A) : A;
-        }
-        return;
-    }
-    const int32_t *slots = call->slots + (size_t)(*round_idx) * B;
-    const uint32_t *r = records + (size_t)slots[w] * L.record_words;
-    for (int p = lane; p < obs; p += 32) {
-        S[(size_t)w * obs + p] = __uint_as_float(r[L.off_state + p]);
-        S2[(size_t)w * obs + p] = __uint_as_float(r[L.off_next_state + p]);
-    }
-    const uint8_t *id8 = reinterpret_cast<const uint8_t *>(r + L.off_avail);
-    for (int k = lane; k < A; k += 32) {
-        irow[k] = dynamic ? (int)id8[k] : k;
-        crow[k] = k;
-    }
+    const QRow row = load_row<true>(records, L, obs, A, dynamic, call, round_idx, B, w, lane, S, S2, R, T, ids);
+    int *crow = cur + (size_t)w * A;
+    const int32_t *cid = records ? nullptr : call->d_curr_ids;
+    for (int k = lane; k < A; k += 32) crow[k] = cid ? cid[(size_t)w * A + k] : k;
     if (lane == 0) {
-        const uint32_t fl = r[L.off_flags];
-        act[w] = (int)r[L.off_action];
-        R[w] = __uint_as_float(r[L.off_reward]);
-        T[w] = (fl & 1u) ? 1.f : 0.f;
-        cnt[w] = dynamic ? min((int)((fl >> 8) & 0xffffu), A) : A;
+        act[w] = row.action;
+        cnt[w] = row.cnt;
     }
 }
 
@@ -129,12 +90,7 @@ __global__ void __launch_bounds__(128) k_mhq_head(int B, int A, int dbl, int con
         const float v = k < n_ok ? sel[nid[k]] : -INFINITY;
         if (v > best || (v == best && k < bk)) { best = v; bk = k; }
     }
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int ok = __shfl_xor_sync(0xffffffffu, bk, o);
-        if (ov > best || (ov == best && ok < bk)) { best = ov; bk = ok; }
-    }
+    warp_first_max(best, bk);
     const float V = dbl ? qt[(size_t)b * A + nid[bk == INT_MAX ? 0 : bk]] : best;
     const float *l = qo + (size_t)b * A;
     const int a = act[b];
@@ -145,25 +101,12 @@ __global__ void __launch_bounds__(128) k_mhq_head(int B, int A, int dbl, int con
 #pragma unroll
     for (int c = 0; c < kColsPerLane; c++) acc[c] = 0.f;
     if (cons) {
-        // logsumexp over the A current slots: row max, then the sum of exp(l - max) (per lane in slot order, then a fixed
-        // tree); the slot gradients are staged in shared memory and added per head column in ascending slot order
+        // the slot gradients are staged in shared memory and added per head column in ascending slot order
         const int *c_b = cur + (size_t)b * A;
-        float mx = -INFINITY;
-        for (int k = lane; k < A; k += 32) mx = fmaxf(mx, l[c_b[k]]);
-#pragma unroll
-        for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-        float s = 0.f;
-        for (int k = lane; k < A; k += 32) s += expf(l[c_b[k]] - mx);
-#pragma unroll
-        for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        const float alpha = call->alpha, fB = (float)B, inv_ba = 1.f / ((float)B * (float)A);
-        for (int k = lane; k < A; k += 32) {
-            const int id = c_b[k];
-            const float p = expf(l[id] - mx) / s;
-            const float n_k = k == 0 ? (float)(A - 1) : (k == 1 ? 1.f : 0.f);
-            sg[wb][k] = __fmul_rn(alpha, __fsub_rn(__fdiv_rn(p, fB), __fmul_rn(n_k, inv_ba)));
-            sid[wb][k] = id;
-        }
+        cql_slot_grad(A, B, call->alpha, lane, [&](int k) { return l[c_b[k]]; }, [&](int k, float g) {
+            sg[wb][k] = g;
+            sid[wb][k] = c_b[k];
+        });
         __syncwarp();
         for (int k = 0; k < A; k++) {
             const int id = sid[wb][k];
@@ -185,22 +128,21 @@ __global__ void __launch_bounds__(128) k_mhq_head(int B, int A, int dbl, int con
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_mhq : Rounds<prl_mhq, MhqCall> {
+struct prl_mhq : FlatQ<prl_mhq, MhqCall, prl_mhq_cfg> {
     static constexpr const char *kFn = "prl_mhq", *kName = "multi-head DQN";
-    static constexpr bool kTargetOn = true;
     static constexpr int kGraphs = 3;
-    void fill_call(MhqCall &k) const { k.decay = (float)(1.0 - cfg.lr * cfg.weight_decay); }
-    prl_mhq_cfg cfg;
-    int P;
     int W1, b1, W2, b2, W3, b3;
-    float *q, *q_t, *q_m, *q_v, *q_x;
     // workspace: S holds the states and, right after the round's B rows, the next states (one 2B-row online pass)
     float *S, *R, *T, *h1, *h2, *qo, *h1t, *h2t, *qt, *dq, *rowabs, *dh2, *dh1, *grad;
     int *act, *cnt, *ids, *cur;
+    static int check(const prl_mhq_cfg *c);
+    static int64_t layout(prl_mhq *s);
+    static int64_t carve(prl_mhq *s, void *base);
     static int round(prl_mhq *s, prl_buf *buf, int B, cudaStream_t st);
 };
 
-static int64_t mhq_layout(prl_mhq *s) {
+// the parameter offsets and P, set when the count stays below 2^31; returns the count
+int64_t prl_mhq::layout(prl_mhq *s) {
     const prl_mhq_cfg &c = s->cfg;
     int64_t o = 0, p[6];
     p[0] = o; o += (int64_t)c.hidden1 * c.obs_dim; p[1] = o; o += c.hidden1;
@@ -213,7 +155,7 @@ static int64_t mhq_layout(prl_mhq *s) {
     return o;
 }
 
-static int mhq_check(const prl_mhq_cfg *c) {
+int prl_mhq::check(const prl_mhq_cfg *c) {
     PRL_REQUIRE(c, "null cfg");
     PRL_REQUIRE(c->obs_dim > 0 && c->hidden1 > 0 && c->hidden2 > 0, "dimensions must be positive");
     PRL_REQUIRE(c->n_actions >= 1 && c->n_actions <= kMaxA, "n_actions must be in [1, %d]: next-action ids are stored as bytes", kMaxA);
@@ -229,19 +171,13 @@ static int mhq_check(const prl_mhq_cfg *c) {
                 "2 * max_batch * max(obs_dim, hidden1, hidden2, n_actions) = %lld must stay below 2^31 (32-bit element offsets)",
                 (long long)elems);
     prl_mhq t; t.cfg = *c;
-    const int64_t P = mhq_layout(&t);
+    const int64_t P = layout(&t);
     PRL_REQUIRE(P < ((int64_t)1 << 31), "the parameter count %lld must stay below 2^31 (32-bit element offsets)", (long long)P);
     return PRL_OK;
 }
 
-extern "C" int64_t prl_mhq_param_count(const prl_mhq_cfg *c) {
-    if (mhq_check(c)) return -1;
-    prl_mhq t; t.cfg = *c;
-    return mhq_layout(&t);
-}
-
 // the workspace, in order; base == null: only its size
-static int64_t mhq_carve(prl_mhq *s, void *base) {
+int64_t prl_mhq::carve(prl_mhq *s, void *base) {
     const prl_mhq_cfg &c = s->cfg;
     const int64_t B = c.max_batch, B2 = 2 * B, O = c.obs_dim, A = c.n_actions, H1 = c.hidden1, H2 = c.hidden2;
     Carve w{(char *)base};
@@ -253,25 +189,12 @@ static int64_t mhq_carve(prl_mhq *s, void *base) {
     s->carve_tail(w, c.max_rounds, B);
     return w.bytes;
 }
-extern "C" int64_t prl_mhq_workspace_bytes(const prl_mhq_cfg *c) {
-    if (mhq_check(c)) return -1;
-    prl_mhq t; t.cfg = *c; mhq_layout(&t);
-    return mhq_carve(&t, nullptr);
-}
 
+extern "C" int64_t prl_mhq_param_count(const prl_mhq_cfg *c) { return prl_mhq::param_count(c); }
+extern "C" int64_t prl_mhq_workspace_bytes(const prl_mhq_cfg *c) { return prl_mhq::workspace_bytes(c); }
 extern "C" int prl_mhq_create(prl_mhq **out, const prl_mhq_cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq,
                               float *max_exp_avg_sq, int64_t adam_step, void *workspace) {
-    PRL_REQUIRE(out && w && w_target && exp_avg && exp_avg_sq && max_exp_avg_sq && workspace, "null argument");
-    int rc = mhq_check(cfg);
-    if (rc) return rc;
-    prl_mhq *s = new (std::nothrow) prl_mhq();
-    if (!s) return fail(PRL_ENOMEM, "out of host memory");
-    s->cfg = *cfg;
-    mhq_layout(s);
-    s->q = w; s->q_t = w_target; s->q_m = exp_avg; s->q_v = exp_avg_sq; s->q_x = max_exp_avg_sq;
-    s->adam_step = adam_step;
-    mhq_carve(s, workspace);
-    return prl_mhq::open(s, out);
+    return prl_mhq::create(out, cfg, w, w_target, exp_avg, exp_avg_sq, max_exp_avg_sq, adam_step, workspace);
 }
 extern "C" int prl_mhq_destroy(prl_mhq *s) { return prl_mhq::destroy(s); }
 extern "C" int64_t prl_mhq_adam_step(const prl_mhq *s) { return prl_mhq::adam_step_of(s); }

@@ -23,6 +23,7 @@
 #include "common.cuh"
 #include "rounds.cuh"
 #include "gemm.cuh"
+#include "qrows.cuh"
 
 using namespace prl;
 
@@ -32,54 +33,21 @@ constexpr int kMaxQuantiles = 256;   // k_qr_loss: one thread per quantile of a 
 constexpr int kMaxA = 255;           // next-action ids are stored as bytes
 
 // per-call block the captured round reads through
-struct QrCall {
-    const int32_t *slots;                     // [rounds][B] (learn)
-    float *out_loss;                          // [rounds]
-    // learn_batch: the caller's dense batch
-    const float *d_state, *d_next_state, *d_reward;
-    const int32_t *d_action_id, *d_next_ids, *d_next_cnt;   // next ids / counts may be null: every action available
-    const uint8_t *d_term;
-    float decay;                              // AdamW decoupled decay 1 - lr * weight_decay
+struct QrCall : QSetCall {
     float beta;                               // variance weight of the risk metric (0: risk neutral)
 };
 
-// rows of one round: state, next state, action id, reward, terminated, and the next-action id of every slot (slot k holds
-// id_k; slots at and beyond the row's count are masked by k_qr_target).  records == null: pack the caller's dense batch.
-__global__ void k_qr_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int A, int dynamic,
+// rows of one round (load_row) and the taken action; slots at and beyond the row's count are masked by k_qr_target
+__global__ void __launch_bounds__(256, 8) k_qr_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, int A, int dynamic,
                           const QrCall *__restrict__ call, const int *__restrict__ round_idx, int B, float *__restrict__ S,
                           float *__restrict__ S2, int *__restrict__ act, float *__restrict__ R, float *__restrict__ T,
                           int *__restrict__ cnt, int *__restrict__ ids) {
     const int lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (w >= B) return;
-    if (!records) {
-        for (int p = lane; p < obs; p += 32) {
-            S[(size_t)w * obs + p] = call->d_state[(size_t)w * obs + p];
-            S2[(size_t)w * obs + p] = call->d_next_state[(size_t)w * obs + p];
-        }
-        const int32_t *nid = call->d_next_ids;
-        for (int k = lane; k < A; k += 32) ids[(size_t)w * A + k] = nid ? nid[(size_t)w * A + k] : k;
-        if (lane == 0) {
-            act[w] = call->d_action_id[w];
-            R[w] = call->d_reward[w];
-            T[w] = call->d_term[w] ? 1.f : 0.f;
-            cnt[w] = call->d_next_cnt ? min(call->d_next_cnt[w], A) : A;
-        }
-        return;
-    }
-    const int32_t *slots = call->slots + (size_t)(*round_idx) * B;
-    const uint32_t *r = records + (size_t)slots[w] * L.record_words;
-    for (int p = lane; p < obs; p += 32) {
-        S[(size_t)w * obs + p] = __uint_as_float(r[L.off_state + p]);
-        S2[(size_t)w * obs + p] = __uint_as_float(r[L.off_next_state + p]);
-    }
-    const uint8_t *id8 = reinterpret_cast<const uint8_t *>(r + L.off_avail);
-    for (int k = lane; k < A; k += 32) ids[(size_t)w * A + k] = dynamic ? (int)id8[k] : k;
+    const QRow row = load_row<true>(records, L, obs, A, dynamic, call, round_idx, B, w, lane, S, S2, R, T, ids);
     if (lane == 0) {
-        const uint32_t fl = r[L.off_flags];
-        act[w] = (int)r[L.off_action];
-        R[w] = __uint_as_float(r[L.off_reward]);
-        T[w] = (fl & 1u) ? 1.f : 0.f;
-        cnt[w] = dynamic ? min((int)((fl >> 8) & 0xffffu), A) : A;
+        act[w] = row.action;
+        cnt[w] = row.cnt;
     }
 }
 
@@ -113,12 +81,7 @@ __global__ void __launch_bounds__(128) k_qr_target(int B, int A, int N, const fl
         }
         if (rho > best || (rho == best && k < bk)) { best = rho; bk = k; }
     }
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-        const int ok = __shfl_xor_sync(0xffffffffu, bk, o);
-        if (ov > best || (ov == best && ok < bk)) { best = ov; bk = ok; }
-    }
+    warp_first_max(best, bk);
     const int g = bk == INT_MAX ? 0 : bk;
     const float live = __fsub_rn(1.f, term[b]), r = rew[b];
     const float *q = qt + ((size_t)b * A + g) * N;

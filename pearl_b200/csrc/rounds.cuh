@@ -1,7 +1,8 @@
 // rounds.cuh — the host half shared by every learner whose step is one fixed launch sequence per round (qrdqn.cu,
-// cql.cu, dueling.cu, sarsa.cu, sac.cu, sac_discrete.cu, td3.cu, iql.cu, ppo.cu, reinforce.cu): the per-call tail of the
-// workspace and its staging, the cache of captured rounds, the launch bookkeeping and the learn / learn_batch entries.
-// No device code.
+// cql.cu, dueling.cu, multihead.cu, sarsa.cu, sac.cu, sac_discrete.cu, td3.cu, iql.cu, ppo.cu, reinforce.cu, rc_safety.cu
+// and the bandits): the per-call tail of the workspace and its staging, the cache of captured rounds, the launch
+// bookkeeping and the learn / learn_batch entries; and, in FlatQ, the setup of the Q learners' handles over flat
+// parameter and AdamW vectors.  No device code.
 //
 // A learner's handle derives from Rounds<Self, Call> and provides
 //   cfg          its prl_*_cfg (max_batch, max_rounds, beta1, beta2, and the learning rates)
@@ -274,6 +275,47 @@ struct Rounds {
         adam_step += rounds;
         last_launches = launches;
         return PRL_OK;
+    }
+};
+
+// The handle of a Q learner bound to caller-owned flat vectors: its parameters, the target's and the three AdamW states
+// (cql.cu, dueling.cu, multihead.cu, sarsa.cu).  Self provides, besides what Rounds asks for,
+//   check        static int check(const Cfg *): the configuration refusals
+//   layout       static void layout(Self *): the parameter offsets and P from cfg
+//   carve        static int64_t carve(Self *, void *base): the workspace in order; base == null: only its size
+// Call holds `decay`, which fill_call sets.
+template <class Self, class Call, class Cfg>
+struct FlatQ : Rounds<Self, Call> {
+    static constexpr bool kTargetOn = true;
+    Cfg cfg;
+    int P;
+    float *q, *q_t, *q_m, *q_v, *q_x;         // online, target, exp_avg, exp_avg_sq, max_exp_avg_sq
+
+    void fill_call(Call &k) const { k.decay = (float)(1.0 - cfg.lr * cfg.weight_decay); }
+
+    static int64_t param_count(const Cfg *c) {
+        if (Self::check(c)) return -1;
+        Self t; t.cfg = *c; Self::layout(&t);
+        return t.P;
+    }
+    static int64_t workspace_bytes(const Cfg *c) {
+        if (Self::check(c)) return -1;
+        Self t; t.cfg = *c; Self::layout(&t);
+        return Self::carve(&t, nullptr);
+    }
+    static int create(Self **out, const Cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq, float *max_exp_avg_sq,
+                      int64_t adam_step, void *workspace) {
+        PRL_REQUIRE(out && w && w_target && exp_avg && exp_avg_sq && max_exp_avg_sq && workspace, "null argument");
+        int rc = Self::check(cfg);
+        if (rc) return rc;
+        Self *s = new (std::nothrow) Self();
+        if (!s) return fail(PRL_ENOMEM, "out of host memory");
+        s->cfg = *cfg;
+        Self::layout(s);
+        s->q = w; s->q_t = w_target; s->q_m = exp_avg; s->q_v = exp_avg_sq; s->q_x = max_exp_avg_sq;
+        s->adam_step = adam_step;
+        Self::carve(s, workspace);
+        return Self::open(s, out);
     }
 };
 

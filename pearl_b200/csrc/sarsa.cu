@@ -16,11 +16,10 @@
 // bit-reproducible run to run.
 #include <math.h>
 
-#include <new>
-
 #include "common.cuh"
 #include "rounds.cuh"
 #include "gemm.cuh"
+#include "qrows.cuh"
 
 using namespace prl;
 
@@ -29,48 +28,20 @@ namespace {
 constexpr int kMaxA = 255;   // next-action ids are stored as bytes
 
 // per-call block the captured round reads through
-struct SarsaCall {
-    const int32_t *slots;                     // [rounds][B] (learn)
-    float *out_loss;                          // [rounds]
-    // learn_batch: the caller's dense batch
-    const float *d_state, *d_next_state, *d_reward;
-    const int32_t *d_action_id, *d_next_action_id;
-    const uint8_t *d_term;
-    float decay;                              // AdamW decoupled decay 1 - lr * weight_decay
+struct SarsaCall : QCall {
+    const int32_t *d_next_action_id;
 };
 
-// rows of one round: state, next state, reward, terminated, the taken action and the committed next action (bits 24..31
-// of the record's flags word).  records == null: the caller's dense batch.
-__global__ void k_sarsa_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, const SarsaCall *__restrict__ call,
+// rows of one round (load_row), the taken action and the committed next action (bits 24..31 of the record's flags word).
+__global__ void __launch_bounds__(256, 8) k_sarsa_load(const uint32_t *__restrict__ records, prl_buf_layout L, int obs, const SarsaCall *__restrict__ call,
                              const int *__restrict__ round_idx, int B, float *__restrict__ S, float *__restrict__ S2,
                              float *__restrict__ R, float *__restrict__ T, int *__restrict__ act, int *__restrict__ nact) {
     const int lane = threadIdx.x & 31, w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     if (w >= B) return;
-    if (!records) {
-        for (int p = lane; p < obs; p += 32) {
-            S[(size_t)w * obs + p] = call->d_state[(size_t)w * obs + p];
-            S2[(size_t)w * obs + p] = call->d_next_state[(size_t)w * obs + p];
-        }
-        if (lane == 0) {
-            act[w] = call->d_action_id[w];
-            nact[w] = call->d_next_action_id[w];
-            R[w] = call->d_reward[w];
-            T[w] = call->d_term[w] ? 1.f : 0.f;
-        }
-        return;
-    }
-    const int32_t *slots = call->slots + (size_t)(*round_idx) * B;
-    const uint32_t *r = records + (size_t)slots[w] * L.record_words;
-    for (int p = lane; p < obs; p += 32) {
-        S[(size_t)w * obs + p] = __uint_as_float(r[L.off_state + p]);
-        S2[(size_t)w * obs + p] = __uint_as_float(r[L.off_next_state + p]);
-    }
+    const QRow row = load_row<false>(records, L, obs, 0, 0, call, round_idx, B, w, lane, S, S2, R, T, nullptr);
     if (lane == 0) {
-        const uint32_t fl = r[L.off_flags];
-        act[w] = (int)r[L.off_action];
-        nact[w] = (int)(fl >> 24);
-        R[w] = __uint_as_float(r[L.off_reward]);
-        T[w] = (fl & 1u) ? 1.f : 0.f;
+        act[w] = row.action;
+        nact[w] = records ? (int)(row.flags >> 24) : call->d_next_action_id[w];
     }
 }
 
@@ -89,24 +60,22 @@ __global__ void k_sarsa_target(int B, const float *__restrict__ q, const float *
 }  // namespace
 
 // ------------------------------------------------------------------ host side
-struct prl_sarsa : Rounds<prl_sarsa, SarsaCall> {
+struct prl_sarsa : FlatQ<prl_sarsa, SarsaCall, prl_sarsa_cfg> {
     static constexpr const char *kFn = "prl_sarsa", *kName = "DeepSARSA";
-    static constexpr bool kTargetOn = true;
     // an on-policy loop whose batch follows the episode length below batch_size (SARSA_method: 32) meets that many
     // sizes; a graph of a round is a few KB
     static constexpr int kGraphs = 64;
-    void fill_call(SarsaCall &k) const { k.decay = (float)(1.0 - cfg.lr * cfg.weight_decay); }
-    prl_sarsa_cfg cfg;
-    int P;
     int W1, b1, W2, b2, W3, b3;
-    float *q, *q_t, *q_m, *q_v, *q_x;
     // workspace
     float *S, *S2, *R, *T, *P1, *c1, *c2, *qa, *P1t, *c1t, *c2t, *qt, *dq, *rowabs, *dc2, *dc1, *grad;
     int *act, *nact;
+    static int check(const prl_sarsa_cfg *c);
+    static void layout(prl_sarsa *s);
+    static int64_t carve(prl_sarsa *s, void *base);
     static int round(prl_sarsa *s, prl_buf *buf, int B, cudaStream_t st);
 };
 
-static void sarsa_layout(prl_sarsa *s) {
+void prl_sarsa::layout(prl_sarsa *s) {
     const prl_sarsa_cfg &c = s->cfg;
     const int D = c.obs_dim + c.n_actions;
     int o = 0;
@@ -116,7 +85,7 @@ static void sarsa_layout(prl_sarsa *s) {
     s->P = o;
 }
 
-static int sarsa_check(const prl_sarsa_cfg *c) {
+int prl_sarsa::check(const prl_sarsa_cfg *c) {
     PRL_REQUIRE(c, "null cfg");
     PRL_REQUIRE(c->obs_dim > 0 && c->hidden1 > 0 && c->hidden2 > 0, "dimensions must be positive");
     PRL_REQUIRE(c->n_actions >= 1 && c->n_actions <= kMaxA, "n_actions must be in [1, %d]: next-action ids are stored as bytes", kMaxA);
@@ -129,17 +98,11 @@ static int sarsa_check(const prl_sarsa_cfg *c) {
     return PRL_OK;
 }
 
-extern "C" int64_t prl_sarsa_param_count(const prl_sarsa_cfg *c) {
-    if (sarsa_check(c)) return -1;
-    prl_sarsa t; t.cfg = *c; sarsa_layout(&t);
-    return t.P;
-}
-
 // rows of the layer-1 / layer-2 activations: a round needs max_batch, q_values at least the A actions of one state
 static int sarsa_qrows(const prl_sarsa_cfg &c) { return c.max_batch > c.n_actions ? c.max_batch : c.n_actions; }
 
 // the workspace, in order; base == null: only its size
-static int64_t sarsa_carve(prl_sarsa *s, void *base) {
+int64_t prl_sarsa::carve(prl_sarsa *s, void *base) {
     const prl_sarsa_cfg &c = s->cfg;
     const int64_t B = c.max_batch, O = c.obs_dim, H1 = c.hidden1, H2 = c.hidden2;
     Carve w{(char *)base};
@@ -152,25 +115,12 @@ static int64_t sarsa_carve(prl_sarsa *s, void *base) {
     s->carve_tail(w, c.max_rounds, B);
     return w.bytes;
 }
-extern "C" int64_t prl_sarsa_workspace_bytes(const prl_sarsa_cfg *c) {
-    if (sarsa_check(c)) return -1;
-    prl_sarsa t; t.cfg = *c; sarsa_layout(&t);
-    return sarsa_carve(&t, nullptr);
-}
 
+extern "C" int64_t prl_sarsa_param_count(const prl_sarsa_cfg *c) { return prl_sarsa::param_count(c); }
+extern "C" int64_t prl_sarsa_workspace_bytes(const prl_sarsa_cfg *c) { return prl_sarsa::workspace_bytes(c); }
 extern "C" int prl_sarsa_create(prl_sarsa **out, const prl_sarsa_cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq,
                                 float *max_exp_avg_sq, int64_t adam_step, void *workspace) {
-    PRL_REQUIRE(out && w && w_target && exp_avg && exp_avg_sq && max_exp_avg_sq && workspace, "null argument");
-    int rc = sarsa_check(cfg);
-    if (rc) return rc;
-    prl_sarsa *s = new (std::nothrow) prl_sarsa();
-    if (!s) return fail(PRL_ENOMEM, "out of host memory");
-    s->cfg = *cfg;
-    sarsa_layout(s);
-    s->q = w; s->q_t = w_target; s->q_m = exp_avg; s->q_v = exp_avg_sq; s->q_x = max_exp_avg_sq;
-    s->adam_step = adam_step;
-    sarsa_carve(s, workspace);
-    return prl_sarsa::open(s, out);
+    return prl_sarsa::create(out, cfg, w, w_target, exp_avg, exp_avg_sq, max_exp_avg_sq, adam_step, workspace);
 }
 extern "C" int prl_sarsa_destroy(prl_sarsa *s) { return prl_sarsa::destroy(s); }
 extern "C" int64_t prl_sarsa_adam_step(const prl_sarsa *s) { return prl_sarsa::adam_step_of(s); }

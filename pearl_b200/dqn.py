@@ -26,10 +26,7 @@ from typing import Any
 import torch
 
 from . import _lib
-from . import cql as _cql
-from . import dueling as _duel
-from . import multihead as _mh
-from . import sarsa as _sarsa_mod
+from . import cql, dueling, multihead, sarsa
 from ._batch import action_ids
 from ._compat import _RefDeepQLearning, _RefDeepSARSA, _RefDoubleDQN, TransitionBatch
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
@@ -48,7 +45,7 @@ def _linears(qnet) -> list:
 
 class _B200DQNMixin:
     _double = False
-    _sarsa = False          # DeepSARSA: prl_sarsa_* (sarsa.py)
+    _sarsa = False          # DeepSARSA (sarsa.py)
 
     def __init__(self, *args: Any, max_rounds_per_call: int = 4096, rows_per_cta: int = 0,
                  engine: str = "auto", **kwargs: Any) -> None:
@@ -58,19 +55,22 @@ class _B200DQNMixin:
         if engine not in ("auto", "simt", "tc"):
             raise ValueError("engine must be 'auto', 'simt' or 'tc'")
         self._engine = engine
-        self._conservative = bool(getattr(self, "_is_conservative", False))   # conservative (CQL) rounds: prl_cql_* (cql.py)
+        self._conservative = bool(getattr(self, "_is_conservative", False))   # conservative (CQL) rounds (cql.py)
         arm = self.action_representation_module
         if type(arm).__name__ != "OneHotActionTensorRepresentationModule":
             raise NotImplementedError("the fused Q network assumes a one-hot action representation")
         self._n_actions = int(arm.max_number_actions)
-        self._dueling = _duel.is_dueling(self._Q)       # DuelingQValueNetwork: prl_duel_* (dueling.py)
-        self._multihead = _mh.is_multihead(self._Q)     # VanillaQValueMultiHeadNetwork: prl_mhq_* (multihead.py)
+        self._dueling = dueling.is_dueling(self._Q)           # DuelingQValueNetwork (dueling.py)
+        self._multihead = multihead.is_multihead(self._Q)     # VanillaQValueMultiHeadNetwork (multihead.py)
+        # the module of the learner this instance binds (its C prefix, refusals, cfg, learn_batch); None: the fused prl_dqn
+        self._variant = sarsa if self._sarsa else dueling if self._dueling else multihead if self._multihead else \
+            cql if self._conservative else None
         if self._sarsa and (self._dueling or self._conservative or self._multihead):
-            _sarsa_mod.check_config(self, engine)
+            sarsa.check_config(self, engine)            # refused before any network shape is parsed
         if self._dueling:
-            self._obs_dim, self._duel_dims = _duel.shape_of(self._Q, self._n_actions)
+            self._obs_dim, self._duel_dims = dueling.shape_of(self._Q, self._n_actions)
         elif self._multihead:
-            self._obs_dim, self._hidden = _mh.shape_of(self._Q, self._n_actions)
+            self._obs_dim, self._hidden = multihead.shape_of(self._Q, self._n_actions)
         else:
             lin = _linears(self._Q)
             self._obs_dim = lin[0].in_features - self._n_actions
@@ -79,15 +79,8 @@ class _B200DQNMixin:
                 raise NotImplementedError("unexpected Q-network shape")
         self._max_rounds = int(max_rounds_per_call)
         self._rows_per_cta = int(rows_per_cta)
-        if self._sarsa:
-            _sarsa_mod.check_config(self, engine)
-        elif self._dueling:
-            _duel.check_config(self, engine)
-        elif self._multihead:
-            _mh.check_config(self, engine)
-        elif self._conservative:
-            _cql.check_config(self, engine)
-        if self._dueling or self._multihead or self._conservative or self._sarsa:
+        if self._variant is not None:
+            self._variant.check_config(self, engine)
             self.use_cuda_graph = True          # False: plain stream launches (profilers)
         self._handle = C.c_void_p(0)
         self._bound_ptr = None
@@ -104,12 +97,8 @@ class _B200DQNMixin:
             pass
 
     def _c(self, name: str):
-        """C entry point `name` of the learner this instance binds: prl_sarsa_* for DeepSARSA, prl_duel_* for a dueling Q
-        network, prl_mhq_* for a multi-head Q network (plain or conservative), prl_cql_* when conservative, prl_dqn_*
-        otherwise."""
-        prefix = "prl_sarsa_" if self._sarsa else "prl_duel_" if self._dueling else "prl_mhq_" if self._multihead else \
-            "prl_cql_" if self._conservative else "prl_dqn_"
-        return getattr(self._libh, prefix + name)
+        """C entry point `name` of the learner this instance binds: the variant's (prl_cql_*, ...), prl_dqn_* without one."""
+        return getattr(self._libh, (self._variant.PREFIX if self._variant is not None else "prl_dqn_") + name)
 
     def _adam_hparams(self) -> dict:
         opt = self._optimizer
@@ -150,8 +139,7 @@ class _B200DQNMixin:
         self._libh = _lib.init(device.index if device.index is not None else torch.cuda.current_device())
         hp = self._adam_hparams()
         bound_batch = max(int(need_batch), int(self._batch_size) if self._batch_size > 0 else 0, 1)
-        cfg = _sarsa_mod.make_cfg(self, hp, bound_batch) if self._sarsa else _duel.make_cfg(self, hp, bound_batch) if self._dueling else \
-            _mh.make_cfg(self, hp, bound_batch) if self._multihead else _cql.make_cfg(self, hp, bound_batch) if self._conservative else _lib.DqnCfg(
+        cfg = self._variant.make_cfg(self, hp, bound_batch) if self._variant is not None else _lib.DqnCfg(
             obs_dim=self._obs_dim, n_actions=self._n_actions, hidden1=self._hidden[0], hidden2=self._hidden[1],
             double_dqn=int(self._double), target_update_freq=int(self._target_update_freq),
             max_batch=bound_batch, max_rounds=self._max_rounds, rows_per_cta=self._rows_per_cta,
@@ -272,11 +260,8 @@ class _B200DQNMixin:
                     step=int(self._c("adam_step")(self._handle)))
 
     def launch_info(self) -> dict:
-        if self._sarsa:
-            return dict(launches=int(self._c("last_launches")(self._handle)),
-                        graph_captures=int(self._c("graph_captures")(self._handle)))
-        if self._dueling or self._multihead or self._conservative:
-            return dict(launches=int(self._c("last_launches")(self._handle)))
+        if self._variant is not None:
+            return {k: int(self._c(fn)(self._handle)) for k, fn in self._variant.LAUNCH_INFO.items()}
         a, b, c = C.c_int32(0), C.c_int32(0), C.c_int32(0)
         self._libh.prl_dqn_last_launch_info(self._handle, C.byref(a), C.byref(b), C.byref(c))
         return dict(launches=a.value, ctas=b.value, rows_per_cta=c.value)
@@ -286,17 +271,16 @@ class _B200DQNMixin:
         `learn(B200ReplayBuffer)` then applies the mean gradient of all ranks' batches, exchanged
         inside the kernel.  All ranks must call learn() with the same number of rounds and start
         from identical parameters."""
-        if self._dueling or self._multihead or self._conservative or self._sarsa:
-            raise NotImplementedError("dueling, multi-head, conservative (CQL) and DeepSARSA updates run on one GPU: "
-                                      "set_communicator is not supported")
+        if self._variant is not None:
+            raise NotImplementedError(f"{self._variant.NAME} runs on one GPU: set_communicator is not supported")
         self._bind(1)
         self._comm = comm
         _lib.check(self._libh.prl_dqn_set_comm(self._handle, comm.handle if comm is not None else None))
 
     def set_kernel_timing(self, enable: bool = True) -> None:
-        if self._dueling or self._multihead or self._conservative or self._sarsa:
-            raise NotImplementedError("kernel timing belongs to the fused DQN kernel; time dueling, multi-head, conservative and "
-                                      "DeepSARSA rounds with CUDA events")
+        if self._variant is not None:
+            raise NotImplementedError(f"kernel timing belongs to the fused DQN kernel; time {self._variant.NAME} rounds with "
+                                      "CUDA events")
         self._bind(1)
         _lib.check(self._libh.prl_dqn_set_timing(self._handle, int(enable)))
 
@@ -324,7 +308,7 @@ class _B200DQNMixin:
                     for k, v in self.learn_batch(self.preprocess_batch(batch)).items():
                         report.setdefault(k, []).append(v)
             return report
-        if self._dueling or self._multihead or self._conservative or self._sarsa:
+        if self._variant is not None:
             return self._learn_rounds(replay_buffer, bs, rounds, trace)
         self._bind(bs)
         dev = self._device
@@ -368,22 +352,18 @@ class _B200DQNMixin:
         return report
 
     def _learn_rounds(self, replay_buffer, bs: int, rounds: int, trace: bool) -> dict:
-        """learn() of the dueling, multi-head, conservative (CQL) and DeepSARSA learners over a B200ReplayBuffer: `rounds` x
-        (sample -> round) through prl_duel_learn / prl_mhq_learn and prl_cql_learn (which also take alpha) / prl_sarsa_learn
-        (which needs the committed next actions of a B200SARSAReplayBuffer).  The ring holds no current action sets, so every round uses the full set,
-        as B200ReplayBuffer.sample reports it."""
+        """learn() of a variant learner over a B200ReplayBuffer: `rounds` x (sample -> round) through its prl_*_learn, which
+        takes the variant's learn_args (alpha for CQL and multi-head) after the training-step count; DeepSARSA's needs
+        the committed next actions of a B200SARSAReplayBuffer.  The ring holds no current action sets, so every round uses
+        the full set, as B200ReplayBuffer.sample reports it."""
         from .per import B200PrioritizedReplayBuffer
         if isinstance(replay_buffer, B200PrioritizedReplayBuffer):
-            raise NotImplementedError(("DeepSARSA samples uniformly" if self._sarsa else "dueling DQN samples uniformly"
-                                       if self._dueling else "multi-head DQN samples uniformly" if self._multihead else
-                                       "conservative (CQL) updates sample uniformly")
-                                      + ": a B200PrioritizedReplayBuffer is not supported")
+            raise NotImplementedError(f"{self._variant.NAME} samples uniformly: a B200PrioritizedReplayBuffer is not supported")
         self._bind(bs)
         dev = self._device
         if replay_buffer.device != dev:
             raise RuntimeError(f"replay buffer is on {replay_buffer.device}, learner on {dev}")
-        alpha = (_mh.alpha(self),) if self._multihead else \
-            (_cql.alpha(self),) if self._conservative and not self._sarsa and not self._dueling else ()
+        extra = self._variant.learn_args(self)
         h = self._handle
         mae = torch.empty(rounds, dtype=torch.float32, device=dev)
         idx = torch.empty((rounds, bs), dtype=torch.int32, device=dev) if trace else None
@@ -395,7 +375,7 @@ class _B200DQNMixin:
             while done < rounds:
                 r = min(self._max_rounds, rounds - done)
                 off = lambda t, w=1: C.c_void_p(0) if t is None else C.c_void_p(t.data_ptr() + 4 * done * w)  # noqa: E731
-                _lib.check(self._c("learn")(h, replay_buffer.handle, r, bs, int(self._training_steps), *alpha, off(mae),
+                _lib.check(self._c("learn")(h, replay_buffer.handle, r, bs, int(self._training_steps), *extra, off(mae),
                                             off(idx, bs), stream))
                 self._training_steps += r
                 done += r
@@ -403,9 +383,7 @@ class _B200DQNMixin:
         self._sync_step_tensors()
         report = {"loss": mae.cpu().tolist()}
         if trace:
-            report.update(idx=idx, launches=int(self._c("last_launches")(h)))
-            if self._sarsa:
-                report["graph_captures"] = int(self._c("graph_captures")(h))
+            report.update(idx=idx, **self.launch_info())
         return report
 
     def _learn_prioritized(self, rb, bs: int, rounds: int, trace: bool) -> dict:
@@ -446,14 +424,8 @@ class _B200DQNMixin:
     def learn_batch(self, batch) -> dict:
         """`DeepTDLearning.learn_batch` on a caller-supplied batch (raw ids, or the one-hot
         tensors the reference's preprocess_batch produces)."""
-        if self._sarsa:
-            return _sarsa_mod.learn_batch(self, batch)
-        if self._dueling:
-            return _duel.learn_batch(self, batch)
-        if self._multihead:
-            return _mh.learn_batch(self, batch)
-        if self._conservative:
-            return _cql.learn_batch(self, batch)
+        if self._variant is not None:
+            return self._variant.learn_batch(self, batch)
         B = len(batch)
         self._bind(B)
         dev = self._device
@@ -482,10 +454,9 @@ class _B200DQNMixin:
     # ------------------------------------------------------------------ act
     def q_values(self, states: torch.Tensor, target: bool = False) -> torch.Tensor:
         """Q(s, a) for every action id: [n, obs] -> [n, n_actions]."""
-        if self._dueling:
-            return _duel.q_values(self, states, target)
-        if self._multihead:
-            return _mh.q_values(self, states, target)
+        own = getattr(self._variant, "q_values", None)
+        if own is not None:
+            return own(self, states, target)
         self._bind(1)
         dev = self._device
         s = states.to(device=dev, dtype=torch.float32).reshape(-1, self._obs_dim).contiguous()
@@ -496,11 +467,13 @@ class _B200DQNMixin:
         return out
 
     def act(self, subjective_state, available_action_space, exploit: bool = False):
-        """`DeepTDLearning.act` (deep_td_learning.py:200-254).  A dueling network's advantage mean runs over the available
-        actions only, as get_q_values does with the available set as its query."""
+        """`DeepTDLearning.act` (deep_td_learning.py:200-254).  A variant with its own q_values (dueling: the advantage mean
+        runs over the query) evaluates the available actions only, as get_q_values does with the available set as its
+        query."""
         ids = available_action_space.actions_batch.reshape(available_action_space.n, -1)[:, 0].long()
-        if self._dueling:
-            q_avail = _duel.q_values(self, torch.as_tensor(subjective_state).reshape(1, -1), False, ids.view(1, -1))[0]
+        own = getattr(self._variant, "q_values", None)
+        if own is not None:
+            q_avail = own(self, torch.as_tensor(subjective_state).reshape(1, -1), False, ids.view(1, -1))[0]
         else:
             qs = self.q_values(torch.as_tensor(subjective_state).reshape(1, -1))[0]
             q_avail = qs[ids.to(qs.device)]
@@ -521,14 +494,9 @@ class B200LearnerGroup:
     def __init__(self, learners, buffers) -> None:
         if len(learners) != len(buffers) or not learners:
             raise ValueError("need one replay buffer per learner")
-        if any(getattr(l, "_conservative", False) for l in learners):
-            raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no conservative (CQL) update")
-        if any(getattr(l, "_sarsa", False) for l in learners):
-            raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no DeepSARSA update")
-        if any(getattr(l, "_dueling", False) for l in learners):
-            raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no dueling network")
-        if any(getattr(l, "_multihead", False) for l in learners):
-            raise NotImplementedError("B200LearnerGroup runs the tensor-core DQN kernel, which has no multi-head network")
+        for l in learners:
+            if getattr(l, "_variant", None) is not None:
+                raise NotImplementedError(f"B200LearnerGroup runs the tensor-core DQN kernel, which has no {l._variant.NAME} update")
         self.learners, self.buffers = list(learners), list(buffers)
 
     def learn(self) -> list:

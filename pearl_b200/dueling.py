@@ -14,9 +14,12 @@ from __future__ import annotations
 import torch
 
 from . import _lib
-from ._batch import checked_ids
+from ._batch import check_features, dense_rows, plugin_call, slot_ids
 from .replay_buffer import _stream_ptr
 
+PREFIX = "prl_duel_"
+NAME = "dueling DQN"
+LAUNCH_INFO = dict(launches="last_launches")
 _ARCHS = ("state_arch", "value_arch", "advantage_arch")
 
 
@@ -56,6 +59,10 @@ def check_config(pl, engine: str) -> None:
     pl._adam_hparams()
 
 
+def learn_args(pl) -> tuple:
+    return ()
+
+
 def make_cfg(pl, hp: dict, max_batch: int) -> _lib.DuelCfg:
     return _lib.DuelCfg(obs_dim=pl._obs_dim, n_actions=pl._n_actions, **pl._duel_dims, double_dqn=int(pl._double),
                         target_update_freq=int(pl._target_update_freq), max_batch=max_batch, max_rounds=pl._max_rounds,
@@ -69,41 +76,19 @@ def learn_batch(pl, batch) -> dict:
     mean runs over the query action alone, as the reference's get_q_values does.  Every next slot enters the target's
     mean with the id it holds; `next_unavailable_actions_mask` only removes slots from the max / argmax."""
     B, A = len(batch), pl._n_actions
-    if int(batch.state.shape[-1]) != pl._obs_dim:
-        raise ValueError(f"batch.state has {int(batch.state.shape[-1])} features, the learner {pl._obs_dim}")
+    check_features(batch, pl._obs_dim)
     pl._bind(B)
     dev = pl._device
-    f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
-    state, next_state = f32(batch.state), f32(batch.next_state)
-    reward = f32(batch.reward.reshape(B))
-    term = batch.terminated.reshape(B).to(device=dev, dtype=torch.uint8).contiguous()
-    i32 = lambda t: t.to(torch.int32).contiguous()  # noqa: E731
-    action = i32(checked_ids(batch.action.to(dev), A, batch.action.dim() == 2, "batch.action").reshape(B))
-    cur = nid = mask = None
-    ca = getattr(batch, "curr_available_actions", None)
-    if ca is not None:
-        ca = ca.to(dev)
-        cur = i32(checked_ids(ca, A, ca.dim() == 3, "batch.curr_available_actions").reshape(B, A))
-    na = getattr(batch, "next_available_actions", None)
-    if na is not None:
-        na = na.to(dev)
-        nid = i32(checked_ids(na, A, na.dim() == 3, "batch.next_available_actions").reshape(B, A))
+    cur = slot_ids(batch, "curr_available_actions", B, A, dev)
+    nid = slot_ids(batch, "next_available_actions", B, A, dev)
     nm = getattr(batch, "next_unavailable_actions_mask", None)
-    if nm is not None:
-        mask = nm.to(dev).reshape(B, A).to(torch.uint8).contiguous()
-    out = torch.empty(1, dtype=torch.float32, device=dev)
-    lib, h, p = pl._libh, pl._handle, _lib.ptr
-    with torch.cuda.device(dev):
-        _lib.check(lib.prl_duel_set_graph(h, int(pl.use_cuda_graph)))
-        _lib.check(lib.prl_duel_learn_batch(h, B, p(state), p(action), p(reward), p(next_state), p(term), p(cur), p(nid), p(mask),
-                                            int(pl._training_steps), p(out), _stream_ptr(dev)))
-    loss = out.item()  # also keeps the inputs alive until the round is done
-    pl._sync_step_tensors()
-    return {"loss": loss}
+    mask = None if nm is None else nm.to(dev).reshape(B, A).to(torch.uint8).contiguous()
+    return plugin_call(pl, B, *dense_rows(batch, B, A, dev), cur, nid, mask, int(pl._training_steps))
 
 
 def q_values(pl, states: torch.Tensor, target: bool, ids: torch.Tensor | None = None) -> torch.Tensor:
-    """Q(s, .) at the ids [n, K] of every row (None: every action), the advantage mean over that row's K ids."""
+    """Q(s, .) at the ids [n, K] of every row (None: every action), the advantage mean over that row's K ids.  act()
+    passes the available actions as the ids."""
     pl._bind(1)
     dev = pl._device
     s = states.to(device=dev, dtype=torch.float32).reshape(-1, pl._obs_dim).contiguous()

@@ -5,7 +5,7 @@ H100 through `prl_mhq_*` (csrc/multihead.cu).
 The DQN plugin (dqn.py) keeps its binding: `_Q`, `_Q_target` and the AdamW state are views into the flat vectors it
 allocates, and a checkpoint or lr change is picked up the same way.  When the Q network is a multi-head one, the plugin
 hands the flat vectors to a `prl_mhq` handle: `learn` (over a B200ReplayBuffer) runs through its prl_mhq_* entry points,
-`learn_batch` and `q_values` through the functions here.  The network maps a state to one Q value per action; a query
+`learn_batch` through the function here.  The network maps a state to one Q value per action; a query
 slot holding id k reads head column k exactly (the reference's bmm with a one-hot slot), so a round needs one forward
 pass per state (include/pearl_b200.h).  alpha is read from `_conservative_alpha` on every call.  No CPU fallback."""
 from __future__ import annotations
@@ -13,9 +13,12 @@ from __future__ import annotations
 import torch
 
 from . import _lib
-from ._batch import available_first, checked_ids
+from ._batch import check_features, dense_rows, next_available_first, plugin_call, slot_ids
 from ._compat import VanillaQValueMultiHeadNetwork
-from .replay_buffer import _stream_ptr
+
+PREFIX = "prl_mhq_"
+NAME = "multi-head DQN"
+LAUNCH_INFO = dict(launches="last_launches")
 
 
 def is_multihead(qnet) -> bool:
@@ -63,6 +66,11 @@ def alpha(pl) -> float:
     return float(a)
 
 
+def learn_args(pl) -> tuple:
+    """The arguments prl_mhq_learn takes after the training-step count: alpha (0 when not conservative)."""
+    return (alpha(pl),)
+
+
 def make_cfg(pl, hp: dict, max_batch: int) -> _lib.MhqCfg:
     return _lib.MhqCfg(obs_dim=pl._obs_dim, n_actions=pl._n_actions, hidden1=pl._hidden[0], hidden2=pl._hidden[1],
                        double_dqn=int(pl._double), conservative=int(pl._conservative),
@@ -77,47 +85,12 @@ def learn_batch(pl, batch) -> dict:
     ignores `curr_unavailable_actions_mask`) is required, as the reference asserts.  Next-action slots that are masked are
     compacted away in order, which keeps DoubleDQN's first argmax."""
     B, A = len(batch), pl._n_actions
-    if int(batch.state.shape[-1]) != pl._obs_dim:
-        raise ValueError(f"batch.state has {int(batch.state.shape[-1])} features, the learner {pl._obs_dim}")
-    ca = getattr(batch, "curr_available_actions", None)
-    if pl._conservative and ca is None:
+    check_features(batch, pl._obs_dim)
+    if pl._conservative and getattr(batch, "curr_available_actions", None) is None:
         raise ValueError("a conservative (CQL) learn_batch needs batch.curr_available_actions, as the reference asserts")
     a = alpha(pl)
     pl._bind(B)
     dev = pl._device
-    f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
-    state, next_state = f32(batch.state), f32(batch.next_state)
-    reward = f32(batch.reward.reshape(B))
-    term = batch.terminated.reshape(B).to(device=dev, dtype=torch.uint8).contiguous()
-    i32 = lambda t: t.to(torch.int32).contiguous()  # noqa: E731
-    action = i32(checked_ids(batch.action.to(dev), A, batch.action.dim() == 2, "batch.action").reshape(B))
-    cur = nid = cnt = None
-    if pl._conservative:
-        ca = ca.to(dev)
-        cur = i32(checked_ids(ca, A, ca.dim() == 3, "batch.curr_available_actions").reshape(B, A))
-    na = getattr(batch, "next_available_actions", None)
-    if na is not None:
-        na = na.to(dev)
-        nid = checked_ids(na, A, na.dim() == 3, "batch.next_available_actions").reshape(B, A)
-        nid, cnt = available_first(nid, getattr(batch, "next_unavailable_actions_mask", None))
-    out = torch.empty(1, dtype=torch.float32, device=dev)
-    lib, h, p = pl._libh, pl._handle, _lib.ptr
-    with torch.cuda.device(dev):
-        _lib.check(lib.prl_mhq_set_graph(h, int(pl.use_cuda_graph)))
-        _lib.check(lib.prl_mhq_learn_batch(h, B, p(state), p(action), p(reward), p(next_state), p(term), p(cur), p(nid), p(cnt),
-                                           int(pl._training_steps), a, p(out), _stream_ptr(dev)))
-    loss = out.item()  # also keeps the inputs alive until the round is done
-    pl._sync_step_tensors()
-    return {"loss": loss}
-
-
-def q_values(pl, states: torch.Tensor, target: bool) -> torch.Tensor:
-    """Q(s)[a] for every action id: [n, obs] -> [n, n_actions]."""
-    pl._bind(1)
-    dev = pl._device
-    s = states.to(device=dev, dtype=torch.float32).reshape(-1, pl._obs_dim).contiguous()
-    out = torch.empty((s.shape[0], pl._n_actions), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(pl._libh.prl_mhq_q_values(pl._handle, s.shape[0], _lib.ptr(s), int(target), _lib.ptr(out), _stream_ptr(dev)))
-    torch.cuda.current_stream(dev).synchronize()
-    return out
+    cur = slot_ids(batch, "curr_available_actions", B, A, dev) if pl._conservative else None
+    return plugin_call(pl, B, *dense_rows(batch, B, A, dev), cur, *next_available_first(batch, B, A, dev),
+                       int(pl._training_steps), a)

@@ -19,7 +19,7 @@ from typing import Any, Iterable, Optional
 import torch
 
 from . import _lib
-from ._batch import available_first, checked_ids
+from ._batch import call, check_features, dense_rows, next_available_first
 from .per import B200PrioritizedReplayBuffer
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
 
@@ -184,22 +184,8 @@ class B200QuantileRegressionDeepQLearning:
         next_available_actions with next_unavailable_actions_mask; without them every action is available next).  Like
         the reference it does not advance the training-step count."""
         B, A, dev = int(batch.state.shape[0]), self._n_actions, self._device
-        if int(batch.state.shape[-1]) != self._state_dim:
-            raise ValueError(f"batch.state has {int(batch.state.shape[-1])} features, the learner {self._state_dim}")
+        check_features(batch, self._state_dim)
         self._bind(B)
-        f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
-        state, next_state, reward = f32(batch.state), f32(batch.next_state), f32(batch.reward.reshape(B))
-        term = batch.terminated.reshape(B).to(device=dev, dtype=torch.uint8).contiguous()
-        aid = checked_ids(batch.action.to(dev).reshape(B, -1), A, True, "batch.action").to(torch.int32).contiguous()
-        nid = cnt = None
-        nxt = getattr(batch, "next_available_actions", None)
-        if nxt is not None:
-            nid = checked_ids(nxt.to(dev).reshape(B, A, -1), A, True, "batch.next_available_actions")
-            nid, cnt = available_first(nid, getattr(batch, "next_unavailable_actions_mask", None))
-        out = torch.empty(1, dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(self._lib.prl_qrdqn_set_graph(self._handle, int(self.use_cuda_graph)))
-            _lib.check(self._lib.prl_qrdqn_learn_batch(self._handle, B, _lib.ptr(state), _lib.ptr(aid), _lib.ptr(reward),
-                                                       _lib.ptr(next_state), _lib.ptr(term), _lib.ptr(nid), _lib.ptr(cnt),
-                                                       self._training_steps, self._beta(), _lib.ptr(out), _stream_ptr(dev)))
-        return {"loss": float(out.item())}
+        return {"loss": call(self._lib.prl_qrdqn_set_graph, self._lib.prl_qrdqn_learn_batch, self._handle, self.use_cuda_graph, dev,
+                             B, *dense_rows(batch, B, A, dev), *next_available_first(batch, B, A, dev), self._training_steps,
+                             self._beta())}

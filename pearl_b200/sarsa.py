@@ -8,11 +8,12 @@ function here.  A round updates the target first (in the rounds the reference's 
 AdamW(amsgrad) step on mean (q - y)^2 with y = r + gamma (1 - terminated) Q'(s', a').  No CPU fallback."""
 from __future__ import annotations
 
-import torch
-
 from . import _lib
-from ._batch import checked_ids
-from .replay_buffer import _stream_ptr
+from ._batch import check_features, dense_rows, plugin_call, staged_ids
+
+PREFIX = "prl_sarsa_"
+NAME = "DeepSARSA"
+LAUNCH_INFO = dict(launches="last_launches", graph_captures="graph_captures")
 
 
 def check_config(pl, engine: str) -> None:
@@ -34,6 +35,10 @@ def make_cfg(pl, hp: dict, max_batch: int) -> _lib.SarsaCfg:
                          gamma=float(pl._discount_factor), tau=float(pl._soft_update_tau))
 
 
+def learn_args(pl) -> tuple:
+    return ()
+
+
 def learn_batch(pl, batch) -> dict:
     """`DeepTDLearning.learn_batch` with DeepSARSA's next-state values on a caller-supplied batch (raw ids, or the one-hot
     tensors the reference's preprocess_batch produces).  `next_action` is required, as the reference asserts; the
@@ -41,24 +46,9 @@ def learn_batch(pl, batch) -> dict:
     if getattr(batch, "next_action", None) is None:
         raise AssertionError("SARSA needs to have next action")
     B, A = len(batch), pl._n_actions
-    if int(batch.state.shape[-1]) != pl._obs_dim:
-        raise ValueError(f"batch.state has {int(batch.state.shape[-1])} features, the learner {pl._obs_dim}")
+    check_features(batch, pl._obs_dim)
     pl._bind(B)
     dev = pl._device
-    f32 = lambda t: t.to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
-    state, next_state = f32(batch.state), f32(batch.next_state)
-    reward = f32(batch.reward.reshape(B))
-    term = batch.terminated.reshape(B).to(device=dev, dtype=torch.uint8).contiguous()
-    i32 = lambda t: t.to(torch.int32).contiguous()  # noqa: E731
-    action = i32(checked_ids(batch.action.to(dev), A, batch.action.dim() == 2, "batch.action").reshape(B))
-    na = batch.next_action.to(dev)
-    next_action = i32(checked_ids(na, A, na.dim() == 2, "batch.next_action").reshape(B))
-    out = torch.empty(1, dtype=torch.float32, device=dev)
-    lib, h, p = pl._libh, pl._handle, _lib.ptr
-    with torch.cuda.device(dev):
-        _lib.check(lib.prl_sarsa_set_graph(h, int(pl.use_cuda_graph)))
-        _lib.check(lib.prl_sarsa_learn_batch(h, B, p(state), p(action), p(reward), p(next_state), p(next_action), p(term),
-                                             int(pl._training_steps), p(out), _stream_ptr(dev)))
-    loss = out.item()  # also keeps the inputs alive until the round is done
-    pl._sync_step_tensors()
-    return {"loss": loss}
+    state, action, reward, next_state, term = dense_rows(batch, B, A, dev)
+    next_action = staged_ids(batch.next_action, A, (B,), dev, "batch.next_action")
+    return plugin_call(pl, B, state, action, reward, next_state, next_action, term, int(pl._training_steps))
