@@ -854,6 +854,73 @@ int prl_mhq_q_values(prl_mhq *mhq, int n, const float *state, int target, float 
 int prl_mhq_set_graph(prl_mhq *mhq, int enable);
 int64_t prl_mhq_last_launches(const prl_mhq *mhq);
 
+/* ---- CNN DQN / DoubleDQN (image observations) -----------------------------------------------------
+ * Replaces CNNQValueNetwork.get_q_values and CNNQValueMultiHeadNetwork.get_q_values (neural_networks/
+ * sequential_decision_making/q_value_networks.py:713-917) with conv_block / mlp_block (neural_networks/common/utils.py:
+ * 75-198), DeepTDLearning.forward / loss / learn_batch (policy_learners/sequential_decision_making/deep_td_learning.py:
+ * 269-360) and DeepQLearning / DoubleDQN.get_next_state_values (deep_q_learning.py:130-167, double_dqn.py:29-57),
+ * driven by PolicyLearner.learn (prl_cnnq_learn: sample -> round, `rounds` times) or called on a caller's batch
+ * (prl_cnnq_learn_batch: one round).  A state is [in_c][in_h][in_w] pixel values (the ring's obs_dim = in_c in_h in_w,
+ * in (c, h, w) order); the trunk is n_conv layers Conv2d(k, stride, padding) + ReLU on state / 255, the features its
+ * output in (c, h, w) order (F values); then n_fc hidden Linear + ReLU layers and a Linear.
+ *   multi_head = 0 (CNNQValueNetwork): the FC input is features || one-hot(action), one output.
+ *   multi_head = 1 (CNNQValueMultiHeadNetwork): the FC input is the features, n_actions outputs; a slot holding id k
+ *   reads output k.
+ * Per round: when (training_steps + 1) % target_update_freq == 0, FIRST target = tau * online + (1 - tau) * target;
+ * y_b = V_b gamma (1 - terminated_b) + r_b with V_b the max over available next slots of the target values (DQN) or the
+ * target value at the first argmax of the online values (DoubleDQN); q_b = Q(s_b, a_b); one AdamW(amsgrad) step on
+ *   multi_head = 0:  L = mean_b (q_b - y_b)^2, reported mean_b |q_b - y_b|;
+ *   multi_head = 1:  L = mean_{i,j} (q_i - Y_ij)^2, reported mean_{i,j} |q_i - Y_ij|, Y_ij = y_j (DQN) or
+ *                    V_i gamma (1 - terminated_j) + r_j (DoubleDQN): the reference's get_q_values returns [B, 1] for one
+ *                    action per row (the taken actions; DoubleDQN's target lookup) and MSELoss broadcasts the pairs
+ *                    (reproduced as it computes it).
+ * 1 <= n_conv <= 4 (every conv output at least 1 x 1), 0 <= n_fc <= 2, 1 <= n_actions <= 255; the parameter count and the
+ * largest im2col / activation buffer of a 2 max_batch-image pass stay below 2^31 elements (32-bit element offsets);
+ * param_count / workspace_bytes return -1 and create returns EINVAL beyond these.  Flat layout (fp32, torch's parameter
+ * order): per conv layer W[out][in_channels k k] b[out], then per FC layer W[out][in] b[out].  Sharded buffers,
+ * continuous-action buffers, buffers of other obs_dim / n_actions, and batch / rounds above the configured maxima are
+ * rejected (EINVAL) before any launch. */
+typedef struct prl_cnnq_cfg {
+    int32_t in_c, in_h, in_w;
+    int32_t n_conv;                /* 1..4 */
+    int32_t conv_out[4], conv_kernel[4], conv_stride[4], conv_pad[4];
+    int32_t n_fc;                  /* hidden fully connected layers, 0..2 */
+    int32_t fc_hidden[2];
+    int32_t n_actions;
+    int32_t multi_head;            /* 0: CNNQValueNetwork, 1: CNNQValueMultiHeadNetwork */
+    int32_t double_dqn;            /* 0: DeepQLearning, 1: DoubleDQN */
+    int32_t target_update_freq, max_batch, max_rounds;
+    double lr, beta1, beta2, eps, weight_decay, gamma, tau;
+} prl_cnnq_cfg;
+typedef struct prl_cnnq prl_cnnq;
+int64_t prl_cnnq_param_count(const prl_cnnq_cfg *cfg);
+int64_t prl_cnnq_workspace_bytes(const prl_cnnq_cfg *cfg);
+/* w, w_target, exp_avg, exp_avg_sq, max_exp_avg_sq: device f32[param_count] owned by the caller (the argument order of
+ * prl_dqn_create); adam_step: optimizer steps already taken (torch's `step`). */
+int prl_cnnq_create(prl_cnnq **out, const prl_cnnq_cfg *cfg, float *w, float *w_target, float *exp_avg, float *exp_avg_sq,
+                    float *max_exp_avg_sq, int64_t adam_step, void *workspace_dev);
+int prl_cnnq_destroy(prl_cnnq *cnnq);
+int64_t prl_cnnq_adam_step(const prl_cnnq *cnnq);
+int prl_cnnq_set_adam_step(prl_cnnq *cnnq, int64_t step);
+/* New AdamW learning rate from the next call on; every lr-dependent scalar travels in the per-call block: no re-capture. */
+int prl_cnnq_set_lr(prl_cnnq *cnnq, double lr);
+/* training_steps = the learner's count before the call (PolicyLearner.learn increments it before each round);
+ * out_loss_dev: device f32[rounds]; out_logical_dev (optional) i32[rounds][batch] = sampled indices. */
+int prl_cnnq_learn(prl_cnnq *cnnq, prl_buf *buf, int rounds, int batch, int64_t training_steps, float *out_loss_dev,
+                   int32_t *out_logical_dev, void *stream);
+/* One round on a dense device batch: state / next_state f32[batch][in_c][in_h][in_w], action_id i32[batch], reward
+ * f32[batch], terminated u8[batch]; next_ids i32[batch][n_actions] and next_count i32[batch] (slots at and beyond it are
+ * unavailable), both null when every action is available next; training_steps = the count learn_batch sees;
+ * out_loss_dev: device f32[1]. */
+int prl_cnnq_learn_batch(prl_cnnq *cnnq, int batch, const float *state, const int32_t *action_id, const float *reward,
+                         const float *next_state, const uint8_t *terminated, const int32_t *next_ids, const int32_t *next_count,
+                         int64_t training_steps, float *out_loss_dev, void *stream);
+/* Q(s)[a] for every action (DeepTDLearning.act, deep_td_learning.py:200-254): device state f32[n][in_c][in_h][in_w] ->
+ * out_q f32[n][n_actions], online (target = 0) or target network. */
+int prl_cnnq_q_values(prl_cnnq *cnnq, int n, const float *state, int target, float *out_q_dev, void *stream);
+int prl_cnnq_set_graph(prl_cnnq *cnnq, int enable);
+int64_t prl_cnnq_last_launches(const prl_cnnq *cnnq);
+
 /* ---- DeepSARSA ------------------------------------------------------------------------------------
  * Replaces DeepSARSA.get_next_state_values (policy_learners/sequential_decision_making/deep_sarsa.py:58-75) on
  * DeepTDLearning.forward / loss / learn_batch (deep_td_learning.py:269-360) with VanillaQValueNetwork.get_q_values

@@ -6,6 +6,7 @@
 Hand-written CUDA in libpearlb200.so (C ABI: include/pearl_b200.h), called through
 ctypes; PyTorch only allocates memory and provides streams.  No CPU fallback.
 """
+from ._compat import CNNQValueMultiHeadNetwork, CNNQValueNetwork  # noqa: F401
 from ._compat import (HAVE_PEARL, DuelingQValueNetwork, OneHotActionTensorRepresentationModule, TransitionBatch,  # noqa: F401
                       VanillaQValueMultiHeadNetwork)
 from .dqn import B200DeepQLearning, B200DeepSARSA, B200DoubleDQN, B200LearnerGroup  # noqa: F401
@@ -40,4 +41,4 @@ __all__ = ["B200ReplayBuffer", "B200DeepQLearning", "B200DoubleDQN", "Transition
            "BinaryActionTensorRepresentationModule", "B200RCSafetyModuleCostCriticContinuousAction", "B200NeuralBandit",
            "SquareCBExploration", "FastCBExploration", "NoExploration", "LossType", "ThompsonSamplingExplorationLinear",
            "B200DisjointBanditContainer", "B200DisjointLinearBandit", "DisjointUCBExploration",
-           "ThompsonSamplingExplorationLinearDisjoint"]
+           "ThompsonSamplingExplorationLinearDisjoint", "CNNQValueNetwork", "CNNQValueMultiHeadNetwork"]

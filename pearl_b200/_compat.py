@@ -25,6 +25,7 @@ try:  # pragma: no cover - depends on the environment
     )
     from pearl.neural_networks.sequential_decision_making.q_value_networks import DuelingQValueNetwork
     from pearl.neural_networks.sequential_decision_making.q_value_networks import VanillaQValueMultiHeadNetwork
+    from pearl.neural_networks.sequential_decision_making.q_value_networks import CNNQValueMultiHeadNetwork, CNNQValueNetwork
     from pearl.policy_learners.sequential_decision_making.double_dqn import DoubleDQN as _RefDoubleDQN
     from pearl.policy_learners.sequential_decision_making.deep_sarsa import DeepSARSA as _RefDeepSARSA
     from pearl.policy_learners.exploration_modules.common.epsilon_greedy_exploration import EGreedyExploration
@@ -189,6 +190,57 @@ except Exception:  # ModuleNotFoundError (pearl or gymnasium missing)
         @property
         def action_dim(self) -> int:
             return self._action_dim
+
+    class _CNNQBase(nn.Module):
+        """Same constructor, module tree and state_dict keys as CNNQValueNetwork / CNNQValueMultiHeadNetwork
+        (pearl/neural_networks/sequential_decision_making/q_value_networks.py:713-917): `_model_cnn` = conv_block (Conv2d
+        then ReLU per layer, BatchNorm2d after the Conv2d with use_batch_norm_conv), `_model_fc` = mlp_block on the
+        flattened conv output (plus the one-hot action for CNNQValueNetwork)."""
+        _with_action = True
+
+        def __init__(self, input_width: int, input_height: int, input_channels_count: int, kernel_sizes, output_channels_list,
+                     strides, paddings, action_dim: int, hidden_dims_fully_connected=None, output_dim: int = 1,
+                     use_batch_norm_conv: bool = False, use_batch_norm_fully_connected: bool = False) -> None:
+            super().__init__()
+            self._input_channels, self._input_height, self._input_width = input_channels_count, input_height, input_width
+            self._output_channels, self._kernel_sizes = output_channels_list, kernel_sizes
+            self._strides, self._paddings = strides, paddings
+            self._hidden_dims_fully_connected = [] if hidden_dims_fully_connected is None else hidden_dims_fully_connected
+            self._use_batch_norm_conv = use_batch_norm_conv
+            self._use_batch_norm_fully_connected = use_batch_norm_fully_connected
+            self._output_dim = output_dim
+            layers, c, h, w = [], input_channels_count, input_height, input_width
+            for oc, k, s, p in zip(output_channels_list, kernel_sizes, strides, paddings):
+                layers.append(nn.Conv2d(c, oc, k, stride=s, padding=p))
+                if use_batch_norm_conv:
+                    layers.append(nn.BatchNorm2d(oc))
+                layers.append(nn.ReLU())
+                c = oc
+                h, w = (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
+            self._model_cnn = nn.Sequential(*layers)
+            self._mlp_input_dims = c * h * w + (action_dim if self._with_action else 0)
+            dims = [self._mlp_input_dims] + list(self._hidden_dims_fully_connected) + [output_dim]
+            blocks = [nn.Sequential(*([nn.Linear(dims[i], dims[i + 1]), nn.ReLU()]
+                                      + ([nn.BatchNorm1d(dims[i + 1])] if use_batch_norm_fully_connected else [])))
+                      for i in range(len(dims) - 2)]
+            blocks.append(nn.Sequential(nn.Linear(dims[-2], dims[-1])))
+            self._model_fc = nn.Sequential(*blocks)
+            self._state_dim = input_channels_count * input_height * input_width
+            self._action_dim = action_dim
+
+        @property
+        def state_dim(self) -> int:
+            return self._state_dim
+
+        @property
+        def action_dim(self) -> int:
+            return self._action_dim
+
+    class CNNQValueNetwork(_CNNQBase):
+        _with_action = True
+
+    class CNNQValueMultiHeadNetwork(_CNNQBase):
+        _with_action = False
 
     class _RefDeepQLearning(nn.Module):
         """Attribute-compatible stand-in for DeepQLearning's constructor

@@ -114,6 +114,16 @@ class MhqCfg(C.Structure):
                 ("tau", C.c_double)]
 
 
+class CnnqCfg(C.Structure):
+    _fields_ = [("in_c", C.c_int32), ("in_h", C.c_int32), ("in_w", C.c_int32), ("n_conv", C.c_int32),
+                ("conv_out", C.c_int32 * 4), ("conv_kernel", C.c_int32 * 4), ("conv_stride", C.c_int32 * 4),
+                ("conv_pad", C.c_int32 * 4), ("n_fc", C.c_int32), ("fc_hidden", C.c_int32 * 2), ("n_actions", C.c_int32),
+                ("multi_head", C.c_int32), ("double_dqn", C.c_int32), ("target_update_freq", C.c_int32),
+                ("max_batch", C.c_int32), ("max_rounds", C.c_int32), ("lr", C.c_double), ("beta1", C.c_double),
+                ("beta2", C.c_double), ("eps", C.c_double), ("weight_decay", C.c_double), ("gamma", C.c_double),
+                ("tau", C.c_double)]
+
+
 class SarsaCfg(C.Structure):
     _fields_ = [("obs_dim", C.c_int32), ("n_actions", C.c_int32), ("hidden1", C.c_int32), ("hidden2", C.c_int32),
                 ("target_update_freq", C.c_int32), ("max_batch", C.c_int32), ("max_rounds", C.c_int32), ("lr", C.c_double),
@@ -333,6 +343,18 @@ _SIGNATURES = {
     "prl_mhq_q_values": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
     "prl_mhq_set_graph": (C.c_int, [_P, C.c_int]),
     "prl_mhq_last_launches": (C.c_int64, [_P]),
+    "prl_cnnq_param_count": (C.c_int64, [C.POINTER(CnnqCfg)]),
+    "prl_cnnq_workspace_bytes": (C.c_int64, [C.POINTER(CnnqCfg)]),
+    "prl_cnnq_create": (C.c_int, [C.POINTER(_P), C.POINTER(CnnqCfg), _P, _P, _P, _P, _P, C.c_int64, _P]),
+    "prl_cnnq_destroy": (C.c_int, [_P]),
+    "prl_cnnq_adam_step": (C.c_int64, [_P]),
+    "prl_cnnq_set_adam_step": (C.c_int, [_P, C.c_int64]),
+    "prl_cnnq_set_lr": (C.c_int, [_P, C.c_double]),
+    "prl_cnnq_learn": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int64, _P, _P, _P]),
+    "prl_cnnq_learn_batch": (C.c_int, [_P, C.c_int] + [_P] * 7 + [C.c_int64, _P, _P]),
+    "prl_cnnq_q_values": (C.c_int, [_P, C.c_int, _P, C.c_int, _P, _P]),
+    "prl_cnnq_set_graph": (C.c_int, [_P, C.c_int]),
+    "prl_cnnq_last_launches": (C.c_int64, [_P]),
     "prl_sarsa_param_count": (C.c_int64, [C.POINTER(SarsaCfg)]),
     "prl_sarsa_workspace_bytes": (C.c_int64, [C.POINTER(SarsaCfg)]),
     "prl_sarsa_create": (C.c_int, [C.POINTER(_P), C.POINTER(SarsaCfg), _P, _P, _P, _P, _P, C.c_int64, _P]),

@@ -7,7 +7,7 @@ import subprocess
 import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SRC = [os.path.join(HERE, "csrc", f) for f in ("replay_buffer.cu", "dqn.cu", "dqn_tc.cu", "ppo.cu", "reinforce.cu", "per.cu", "sac.cu", "sac_discrete.cu", "td3.cu", "rc_safety.cu", "iql.cu", "qrdqn.cu", "cql.cu", "dueling.cu", "multihead.cu", "sarsa.cu", "bandit.cu", "neural_linear.cu", "neural_bandit.cu", "disjoint_bandit.cu", "gemm_tc.cu", "umma_test.cu")]
+SRC = [os.path.join(HERE, "csrc", f) for f in ("replay_buffer.cu", "dqn.cu", "dqn_tc.cu", "ppo.cu", "reinforce.cu", "per.cu", "sac.cu", "sac_discrete.cu", "td3.cu", "rc_safety.cu", "iql.cu", "qrdqn.cu", "cql.cu", "dueling.cu", "multihead.cu", "cnnq.cu", "sarsa.cu", "bandit.cu", "neural_linear.cu", "neural_bandit.cu", "disjoint_bandit.cu", "gemm_tc.cu", "umma_test.cu")]
 HDR = [os.path.join(HERE, "csrc", "common.cuh"), os.path.join(HERE, "csrc", "sampler.cuh"), os.path.join(HERE, "csrc", "umma.cuh"), os.path.join(HERE, "csrc", "dqn_common.cuh"), os.path.join(HERE, "csrc", "gemm.cuh"), os.path.join(HERE, "csrc", "host_runtime.cuh"), os.path.join(HERE, "csrc", "rounds.cuh"), os.path.join(HERE, "csrc", "ac_nets.cuh"), os.path.join(HERE, "csrc", "ridge.cuh"), os.path.join(os.path.dirname(HERE), "include", "pearl_b200.h")]
 OUT = os.path.join(HERE, "libpearlb200.so")
 

@@ -5,7 +5,8 @@ in one persistent CUDA kernel (libpearlb200.so), replacing
     DeepTDLearning.learn_batch     .../sequential_decision_making/deep_td_learning.py:269-360
     DeepQLearning / DoubleDQN.get_next_state_values   deep_q_learning.py:130-167, double_dqn.py:29-57
     VanillaQValueNetwork.get_q_values                 q_value_networks.py:152-174
-        (VanillaQValueMultiHeadNetwork, q_value_networks.py:185-241: multihead.py)
+        (VanillaQValueMultiHeadNetwork, q_value_networks.py:185-241: multihead.py;
+         CNNQValueNetwork / CNNQValueMultiHeadNetwork, q_value_networks.py:713-917: cnn_q.py)
     torch.optim.AdamW(amsgrad=True).step, update_target_network (common/utils.py:214-226)
 
 Constructor arguments, attributes (`_Q`, `_Q_target`, `optimizer`, `_training_steps`,
@@ -26,7 +27,7 @@ from typing import Any
 import torch
 
 from . import _lib
-from . import cql, dueling, multihead, sarsa
+from . import cnn_q, cql, dueling, multihead, sarsa
 from ._batch import action_ids
 from ._compat import _RefDeepQLearning, _RefDeepSARSA, _RefDoubleDQN, TransitionBatch
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
@@ -62,12 +63,17 @@ class _B200DQNMixin:
         self._n_actions = int(arm.max_number_actions)
         self._dueling = dueling.is_dueling(self._Q)           # DuelingQValueNetwork (dueling.py)
         self._multihead = multihead.is_multihead(self._Q)     # VanillaQValueMultiHeadNetwork (multihead.py)
+        cnn = cnn_q.is_cnn(self._Q)                           # CNNQValueNetwork / CNNQValueMultiHeadNetwork (cnn_q.py)
         # the module of the learner this instance binds (its C prefix, refusals, cfg, learn_batch); None: the fused prl_dqn
-        self._variant = sarsa if self._sarsa else dueling if self._dueling else multihead if self._multihead else \
-            cql if self._conservative else None
+        self._variant = cnn_q if cnn else sarsa if self._sarsa else dueling if self._dueling else \
+            multihead if self._multihead else cql if self._conservative else None
         if self._sarsa and (self._dueling or self._conservative or self._multihead):
             sarsa.check_config(self, engine)            # refused before any network shape is parsed
-        if self._dueling:
+        if cnn:
+            cnn_q.check_config(self, engine)            # refused before the network shape is parsed
+            self._cnn = cnn_q.shape_of(self._Q, self._n_actions)
+            self._obs_dim = self._cnn["input"][0] * self._cnn["input"][1] * self._cnn["input"][2]
+        elif self._dueling:
             self._obs_dim, self._duel_dims = dueling.shape_of(self._Q, self._n_actions)
         elif self._multihead:
             self._obs_dim, self._hidden = multihead.shape_of(self._Q, self._n_actions)
@@ -472,7 +478,10 @@ class _B200DQNMixin:
         query."""
         ids = available_action_space.actions_batch.reshape(available_action_space.n, -1)[:, 0].long()
         own = getattr(self._variant, "q_values", None)
-        if own is not None:
+        if self._variant is cnn_q:                     # a [1, C, H, W] state, as the reference's get_q_values asserts
+            qs = cnn_q.act_values(self, subjective_state)
+            q_avail = qs[ids.to(qs.device)]
+        elif own is not None:
             q_avail = own(self, torch.as_tensor(subjective_state).reshape(1, -1), False, ids.view(1, -1))[0]
         else:
             qs = self.q_values(torch.as_tensor(subjective_state).reshape(1, -1))[0]
