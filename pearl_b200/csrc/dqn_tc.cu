@@ -130,7 +130,7 @@ struct Misc {
     float rew[MAX_B], term[MAX_B];
     float redw[8][HID];
     float redmae[8], reddb3[8];
-    unsigned long long bar[2 + ARING];   // 0: target tiles; 1: online tiles; 2 + s: AdamW ring slot s
+    unsigned long long bar[3 + ARING];   // 0: target tiles; 1: online W1 tiles; 2: online W2 | W2^T tiles; 3 + s: AdamW ring slot s
     // kept here rather than in registers: the wgmma chains need the registers (section 3.1 of DESIGN.md)
     TcLearner L;                 // this CTA's learner, per-round arrays shifted to the launch's first round
     float dw3[16][NTH];          // per-thread dW3 partial sums, carried across the row tiles
@@ -353,7 +353,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     }
     uint64_t *bar = reinterpret_cast<uint64_t *>(mi.bar);
     if (tid == 0)
-        for (int i = 0; i < 2 + ARING; i++) umma::mbar_init(bar + i, 1);
+        for (int i = 0; i < 3 + ARING; i++) umma::mbar_init(bar + i, 1);
     // the operand-layout tiles follow the flat parameters (which the host may have changed between calls)
     auto To = [&] { return net_tiles(L.tiles, d.obs, true); };
     auto Tt = [&] { return net_tiles(L.tiles + net_tile_floats(d.obs) + 2 * HID * HID, d.obs, false); };
@@ -363,13 +363,25 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
     __syncthreads();
     const int k1 = k1_cols(d.obs);
     const uint32_t w1_bytes = 64u * k1 * 4, w2_bytes = 2u * HID * HID * 4;
+    // target tiles: three TMA bulk copies, W1 hi / lo into region 1 and W2 hi | lo into region 3
+    auto tma_target = [&] {
+        mbar_expect_tx(bar + 0, 2 * w1_bytes + w2_bytes);
+        bulk_g2s(smem + REG1, Tt().w1hi, w1_bytes, bar + 0);
+        bulk_g2s(smem + REG1 + HALF, Tt().w1lo, w1_bytes, bar + 0);
+        bulk_g2s(smem + REG3, Tt().w2, w2_bytes, bar + 0);
+    };
     // B-operand tiles of the online network by TMA, once per row tile (the weight-gradient passes overwrite them): W1 hi / lo
-    // into region 1, the W2 and W2^T blocks (adjacent in global memory) into region 3
-    auto tma_online = [&](const NetTiles &t, uint64_t *b) {
-        mbar_expect_tx(b, 2 * w1_bytes + 2 * w2_bytes);
-        bulk_g2s(smem + REG1, t.w1hi, w1_bytes, b);
-        bulk_g2s(smem + REG1 + HALF, t.w1lo, w1_bytes, b);
-        bulk_g2s(smem + REG3, t.w2, 2 * w2_bytes, b);
+    // into region 1 on bar[1], the W2 and W2^T blocks (adjacent in global memory) into region 3 on bar[2].  Two barriers, so
+    // that layer 1 waits for W1 only and W2 | W2^T keep loading under it.  (Issuing row tile 0's W1 inside phase T, after
+    // the last target layer 1, together with this later wait made ptxas serialise every wgmma of the NW = 64 kernel, C7520.)
+    auto tma_online_w1 = [&] {
+        mbar_expect_tx(bar + 1, 2 * w1_bytes);
+        bulk_g2s(smem + REG1, To().w1hi, w1_bytes, bar + 1);
+        bulk_g2s(smem + REG1 + HALF, To().w1lo, w1_bytes, bar + 1);
+    };
+    auto tma_online_w2 = [&] {
+        mbar_expect_tx(bar + 2, 2 * w2_bytes);
+        bulk_g2s(smem + REG3, To().w2, 2 * w2_bytes, bar + 2);
     };
     // AdamW streams W1 | b1 | W2 (one flat range; D % 4 == 0 keeps every 16-byte group inside one of the three) through the
     // ring: chunk k goes to slot k % ARING, whose barrier completes once per use
@@ -379,48 +391,82 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
         const int off = k * ACH, s = k % ARING;
         const uint32_t bytes = 4u * (an - off < ACH ? an - off : ACH);
         char *dst = aslot(s);
-        mbar_expect_tx(bar + 2 + s, 4 * bytes);
-        bulk_g2s(dst, L.w + off, bytes, bar + 2 + s);
-        bulk_g2s(dst + ACH * 4, L.m + off, bytes, bar + 2 + s);
-        bulk_g2s(dst + ACH * 8, L.v + off, bytes, bar + 2 + s);
-        bulk_g2s(dst + ACH * 12, L.vmax + off, bytes, bar + 2 + s);
+        mbar_expect_tx(bar + 3 + s, 4 * bytes);
+        bulk_g2s(dst, L.w + off, bytes, bar + 3 + s);
+        bulk_g2s(dst + ACH * 4, L.m + off, bytes, bar + 3 + s);
+        bulk_g2s(dst + ACH * 8, L.v + off, bytes, bar + 3 + s);
+        bulk_g2s(dst + ACH * 12, L.vmax + off, bytes, bar + 3 + s);
     };
-    uint32_t par_w1 = 0;   // phase parity of bar[1] (one completion per row tile)
+    // scheduled soft target update BEFORE round r's gradient step (deep_td_learning.py:283-284: (training_steps + 1) % freq == 0)
+    auto soft_due = [&](int r) { return (L.steps0 + r + 2) % a.freq == 0; };
+    // batch row tid of round r: its slot and the scalars of its record.  The slot is loaded first (row_slot), the record's
+    // scalars (row_load) once it has arrived; row_store puts them where the round reads them.  The whole record is
+    // prefetched into L2 for the round's row gathers.
+    auto row_slot = [&](int r) { return L.slots[(size_t)r * a.B + tid]; };
+    auto row_load = [&](int slot, uint32_t (&f)[3]) {
+        const uint32_t *rec = L.records + (size_t)slot * W;
+        for (int o = 0; o < W * 4; o += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char *>(rec) + o));
+        f[0] = rec[a.lay.off_action]; f[1] = rec[a.lay.off_reward]; f[2] = rec[a.lay.off_flags];
+    };
+    auto row_store = [&](int slot, const uint32_t (&f)[3]) {
+        mi.slot[tid] = slot;
+        mi.act[tid] = (int)f[0];
+        mi.rew[tid] = __uint_as_float(f[1]);
+        mi.term[tid] = (f[2] & 1u) ? 1.f : 0.f;
+        mi.cnt[tid] = (int)((f[2] >> 8) & 0xffffu);
+    };
     const umma::Tile W2_hi = umma::make_tile(smem + REG3, 64, 128), W2_lo = umma::make_tile(smem + REG3 + 16384, 64, 128);
     const umma::Tile W2T_hi = umma::make_tile(smem + REG3 + 32768, 64, 128), W2T_lo = umma::make_tile(smem + REG3 + 49152, 64, 128);
 
     for (int round = 0; round < a.rounds; round++) {
         TC_STAMP(0);
-        // ---- per-round row scalars + L2 prefetch of the NEXT round's transitions
-        if (tid < a.B) {
-            const int slot = L.slots[(size_t)round * a.B + tid];
-            const uint32_t *r = L.records + (size_t)slot * W;
-            mi.slot[tid] = slot;
-            mi.act[tid] = (int)r[a.lay.off_action];
-            mi.rew[tid] = __uint_as_float(r[a.lay.off_reward]);
-            const uint32_t fl = r[a.lay.off_flags];
-            mi.term[tid] = (fl & 1u) ? 1.f : 0.f;
-            mi.cnt[tid] = (int)((fl >> 8) & 0xffffu);
-            if (round + 1 < a.rounds) {
-                const char *nx = reinterpret_cast<const char *>(L.records + (size_t)L.slots[(size_t)(round + 1) * a.B + tid] * W);
-                for (int o = 0; o < W * 4; o += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(nx + o));
-            }
+        // ---- the row scalars of the launch's first round; those of every later round were loaded under the last AdamW sweep
+        if (round == 0 && tid < a.B) {
+            uint32_t f[3];
+            const int slot = row_slot(0);
+            row_load(slot, f);
+            row_store(slot, f);
         }
-        // ---- scheduled soft target update happens BEFORE this round's gradient step
-        //      (deep_td_learning.py:283-284: (training_steps + 1) % freq == 0)
-        const bool soft_upd = (L.steps0 + round + 2) % a.freq == 0;
+        TC_STAMP(15);
+        const bool soft_upd = soft_due(round);
         if (soft_upd) {
-            for (int i = tid; i < d.P; i += NTH) L.wt[i] = soft_update(__ldcg(L.w + i), __ldcg(L.wt + i), a.tau, a.omtau);
+            // SU parameters per thread and pass, all loaded before the first store: a store to wt may alias a later load of w
+            // for all the compiler knows, so one parameter at a time waited for an L2 round trip each.  The loads clamp their
+            // index instead of branching (a branch here made ptxas serialise the kernel's wgmma, C7520).
+            constexpr int SU = 16;
+            for (int i0 = tid; i0 < d.P; i0 += SU * NTH) {
+                float wv[SU], tv[SU];
+#pragma unroll
+                for (int u = 0; u < SU; u++) {
+                    const int i = min(i0 + u * NTH, d.P - 1);
+                    wv[u] = __ldcg(L.w + i); tv[u] = __ldcg(L.wt + i);
+                }
+#pragma unroll
+                for (int u = 0; u < SU; u++)
+                    if (i0 + u * NTH < d.P) L.wt[i0 + u * NTH] = soft_update(wv[u], tv[u], a.tau, a.omtau);
+            }
             // The operand-layout tiles get the same elementwise update IN TILE ORDER (the hi tiles hold exactly the fp32 values of
             // the flat vectors, permuted; lo = residual of the new value): coalesced 16-byte accesses instead of rebuilding the
             // target tiles from the flat vector with scattered 4-byte stores.  Same function of the same inputs: bit-identical.
+            // Four 16-byte groups per thread and pass, loaded before they are stored, as above.
             auto update_tile = [&](const float *on_hi, float *tg_hi, float *tg_lo, int n) {
-                for (int i = tid * 4; i < n; i += NTH * 4) {
-                    const float4 w = __ldcg(reinterpret_cast<const float4 *>(on_hi + i)), t = __ldcg(reinterpret_cast<const float4 *>(tg_hi + i));
-                    const float4 r = make_float4(soft_update(w.x, t.x, a.tau, a.omtau), soft_update(w.y, t.y, a.tau, a.omtau),
-                                                 soft_update(w.z, t.z, a.tau, a.omtau), soft_update(w.w, t.w, a.tau, a.omtau));
-                    *reinterpret_cast<float4 *>(tg_hi + i) = r;
-                    *reinterpret_cast<float4 *>(tg_lo + i) = make_float4(tf32_lo(r.x), tf32_lo(r.y), tf32_lo(r.z), tf32_lo(r.w));
+                for (int i0 = tid * 4; i0 < n; i0 += 4 * NTH * 4) {
+                    float4 w[4], t[4];
+#pragma unroll
+                    for (int u = 0; u < 4; u++) {
+                        const int i = min(i0 + u * NTH * 4, n - 4);
+                        w[u] = __ldcg(reinterpret_cast<const float4 *>(on_hi + i)); t[u] = __ldcg(reinterpret_cast<const float4 *>(tg_hi + i));
+                    }
+#pragma unroll
+                    for (int u = 0; u < 4; u++) {
+                        const int i = i0 + u * NTH * 4;
+                        const float4 r = make_float4(soft_update(w[u].x, t[u].x, a.tau, a.omtau), soft_update(w[u].y, t[u].y, a.tau, a.omtau),
+                                                     soft_update(w[u].z, t[u].z, a.tau, a.omtau), soft_update(w[u].w, t[u].w, a.tau, a.omtau));
+                        if (i < n) {
+                            *reinterpret_cast<float4 *>(tg_hi + i) = r;
+                            *reinterpret_cast<float4 *>(tg_lo + i) = make_float4(tf32_lo(r.x), tf32_lo(r.y), tf32_lo(r.z), tf32_lo(r.w));
+                        }
+                    }
                 }
             };
             update_tile(To().w1hi, Tt().w1hi, Tt().w1lo, HID * k1);
@@ -431,14 +477,12 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
 
         // ================= phase T: y = max_a' Q_target(s', a') * gamma * (1 - term) + r =================
         TC_STAMP(1);
-        if (tid == 0) {   // target tiles: three TMA bulk copies (regions 1 and 3 are free: every product of the last round was waited for)
-            mbar_expect_tx(bar + 0, 2 * w1_bytes + w2_bytes);
-            bulk_g2s(smem + REG1, Tt().w1hi, w1_bytes, bar + 0);
-            bulk_g2s(smem + REG1 + HALF, Tt().w1lo, w1_bytes, bar + 0);
-            bulk_g2s(smem + REG3, Tt().w2, w2_bytes, bar + 0);
-        }
+        // the target tiles (regions 1 and 3 are free: every product of the last round was waited for), unless the last round
+        // issued them already: it does when no soft update falls on this round
+        if (tid == 0 && (round == 0 || soft_upd)) tma_target();
         l1_issue(a, L, mi, smem, a.lay.off_next_state, h * 64, 0);
         if (soft_upd || round == 0) load_smalls(L.wt, d, mi.sm[1]);   // the target's small vectors only change at a soft update
+        load_smalls(L.w, d, mi.sm[0]);   // the online ones are first read in phase O: they load under the wait for the target tiles
         umma::mbar_wait(bar + 0, round & 1);
         __syncthreads();
         TC_STAMP(2);
@@ -503,8 +547,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
 
         // ================= phase O: online forward, loss, backward =================
         TC_STAMP(3);
-        if (tid == 0) tma_online(To(), bar + 1);
-        load_smalls(L.w, d, mi.sm[0]);
+        if (tid == 0) { tma_online_w1(); tma_online_w2(); }
         TC_STAMP(4);
         // weight-gradient accumulators; both warpgroups issue the same products on different output columns:
         // gw2 = dW2 columns [32 h, 32 h + 32), gb2 = [db2 | .] (column 0 of dZ2^T E, the same on both warpgroups),
@@ -531,11 +574,11 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
         for (int i = 0; i < ntiles; i++) {
             const int row0 = i * 128 + h * 64;
             if (i > 0) {   // the last tile's passes overwrote regions 1 and 3 (tile 0's first chunk was issued in phase T)
-                if (tid == 0) tma_online(To(), bar + 1);
+                if (tid == 0) { tma_online_w1(); tma_online_w2(); }
                 l1_issue(a, L, mi, smem, a.lay.off_state, row0, 0);
             }
-            umma::mbar_wait(bar + 1, par_w1);
-            par_w1 ^= 1;
+            // bar[1] and bar[2] complete once per row tile (a parity computed here, not carried across the chains)
+            umma::mbar_wait(bar + 1, (uint32_t)(round * ntiles + i) & 1u);
             __syncthreads();
             const int rows[2] = {row0 + acc_row_here(0), row0 + acc_row_here(1)};
             float h1[32], z[32], hi[32], lo[32];
@@ -560,6 +603,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             float *h1s = reinterpret_cast<float *>(smem + REG1 + h * HALF) + (tid & 127);
 #pragma unroll
             for (int c = 0; c < 32; c++) h1s[c * 128] = h1[c];
+            umma::mbar_wait(bar + 2, (uint32_t)(round * ntiles + i) & 1u);   // W2 | W2^T, loaded under layer 1
             acc_to_frag(h1, hi, lo);
             umma::gemm3_rs<HID, 8>(z, hi, lo, W2_hi, W2_lo, false);
             umma::wg_commit();
@@ -744,6 +788,13 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
         // Issuing them under the last tile's weight-gradient products instead made the kernel slower.
         if (a.adam_tma && tid == 0)
             for (int k = 0; k < ARING && k < nch; k++) adam_issue(k);
+        // this round's row scalars are dead: the next round's are loaded under AdamW and stored at its end.  Its target tiles
+        // are issued after the sweep unless a soft update, which rewrites them, comes first.
+        const bool next_rows = round + 1 < a.rounds && tid < a.B;
+        const bool stage_target = round + 1 < a.rounds && !soft_due(round + 1);
+        int nslot = 0;
+        uint32_t nf[3];
+        if (next_rows) nslot = row_slot(round + 1);
 
         TC_STAMP(8);
         // ================= AdamW ==========
@@ -794,6 +845,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
             }
             __syncthreads();
             TC_STAMP(7);
+            if (next_rows) row_load(nslot, nf);
             // 2) AdamW over the flat parameter vector, all 256 threads.  The sweep is bound by L2 round trips, not bytes: W1 | b1 |
             //    W2 arrive by TMA in chunks of ACH parameters through an ARING-slot ring in regions 3 and 1, up to 128 KB of
             //    loads in flight and no thread holding load registers.  The loads of the small vectors (b1 | b2 | W3 | b3,
@@ -826,7 +878,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 const int n1 = HID * d.D;
                 for (int k = 0; k < nch; k++) {
                     const int s = k % ARING, uses = (nch - 1 - s) / ARING + 1;
-                    umma::mbar_wait(bar + 2 + s, (uint32_t)(round * uses + k / ARING) & 1u);
+                    umma::mbar_wait(bar + 3 + s, (uint32_t)(round * uses + k / ARING) & 1u);
                     const int i = k * ACH + 4 * tid;
                     if (i < an && (i < n1 || i >= d.oW2)) {
                         const float4 *sl = reinterpret_cast<const float4 *>(aslot(s)) + tid;
@@ -852,6 +904,8 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                     }
                 }
                 __syncthreads();
+                // the ring is consumed and regions 1 and 3 are free: the next round's target tiles load under the tile pass
+                if (tid == 0 && stage_target) tma_target();
                 // The operand-layout tiles from the new W1 | W2 in the staging, one 16-byte group of a tile per thread and
                 // store, in tile order: coalesced, where the sweep's own order scattered them (16-byte pieces of W1 and W2
                 // into separate sectors, W2^T one float at a time), which made the tile stores most of the sweep's store
@@ -900,6 +954,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                     L.m[i] = mm; L.v[i] = vv; L.vmax[i] = xx;
                 }
                 __syncthreads();
+                if (tid == 0 && stage_target) tma_target();
                 rebuild_tiles(L.w, d, To(), tid);         // D % 4 != 0 or unaligned parameters: tiles from the flat vector
             }
             TC_STAMP(10);
@@ -909,6 +964,7 @@ __global__ void __launch_bounds__(NTH, 1) k_dqn_tc(const TcArgs a) {
                 L.m[si] = sm; L.v[si] = sv2; L.vmax[si] = sx;
             }
         }
+        if (next_rows) row_store(nslot, nf);
         __syncthreads();
         TC_STAMP(9);
     }

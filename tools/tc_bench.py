@@ -38,12 +38,13 @@ _lib.check(ls[0]._libh.prl_dqn_set_profile(ls[0]._handle, C.c_void_p(st.data_ptr
 grp.learn()
 torch.cuda.synchronize()
 s = st.cpu()[4:].double()
-# stamps written by k_dqn_tc: 0 round start, 1 row scalars + soft update done, 2 target tiles loaded, 3 phase T done,
+# stamps written by k_dqn_tc: 0 round start, 15 row scalars loaded (only the launch's first round loads its own), 1 soft
+# update done, 2 target tiles loaded, 3 phase T done,
 # 4 online small vectors loaded (and, before the W2^T tiles were kept in global memory, W2^T built), 5 tile 0 layer 1 done, 6 tile 0 forward / dZ2 / dH1 done, 8 weight gradients done,
 # 7 gradients staged in shared memory, 10 AdamW sweep over W1 | b1 | W2 done, 9 small-parameter tail done (round end);
 # in the weight-gradient passes of tile 0, rows 0-63: 11 dZ2^T / H1^T scattered, 12 dW2 / db2 waited for, 13 the operands
 # of dW1s ready, 14 dW1s / [db1 | dW1a] waited for (the dW2 | db2 pass over rows 64-127 lies between 12 and 13)
-phases = [("row scalars + soft upd", 0, 1), ("load target weights", 1, 2), ("phase T (layer 1 + all actions)", 2, 3),
+phases = [("row scalars", 0, 15), ("soft target update", 15, 1), ("load target weights", 1, 2), ("phase T (layer 1 + all actions)", 2, 3),
           ("load online weights", 3, 4), ("tile 0: online layer 1", 4, 5), ("tile 0: fwd L2 + dZ2 + dH1", 5, 6),
           ("rest (weight grads, other tiles)", 6, 8), ("  tile 0 rows 0-63: dZ2^T / H1^T scatter", 6, 11),
           ("  tile 0 rows 0-63: dW2 / db2 products", 11, 12), ("  tile 0: to the operands of dW1s", 12, 13),
