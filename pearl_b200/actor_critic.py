@@ -23,7 +23,6 @@ When Pearl is not installed (the GPU test box) the same public names are the sta
 same keyword arguments.  Nothing here computes anything; there is no CPU path."""
 from __future__ import annotations
 
-import ctypes as C
 from typing import Any
 
 import torch
@@ -177,11 +176,10 @@ class _B200ActorCriticMixin:
     def _optimizer_triples(self, core) -> list:  # [(optimizer, module, [exp_avg, exp_avg_sq, max_exp_avg_sq])]
         return [(self._actor_optimizer, self._actor, core._actor_state), (self._critic_optimizer, self._critic, core._critic_state)]
 
-    def _core_steps(self, core) -> tuple:        # AdamW step counts (actor, critic) the CUDA learner is at
-        raise NotImplementedError
-
-    def _restart_core(self, core, steps: tuple) -> None:   # drop the C handle; the next learn() re-creates it at `steps`
-        raise NotImplementedError
+    def _core_steps(self, core) -> tuple:
+        """The AdamW step count of each optimizer triple: the core's counts, or its one count for every optimizer."""
+        steps = core.adam_steps()
+        return steps * len(self._optimizer_triples(core)) if len(steps) == 1 else steps
 
     def _bind_extras(self, core) -> None:   # idempotent: runs on every learn()
         pass
@@ -191,7 +189,7 @@ class _B200ActorCriticMixin:
         counts (moments and parameters live in the core's vectors)."""
         steps = self._core_steps(core)
         core._actor_learning_rate, core._critic_learning_rate = lrs
-        self._restart_core(core, steps)
+        core.restart(steps)
 
     # ---- binding
     def _device_of_parameters(self) -> torch.device:
@@ -222,7 +220,7 @@ class _B200ActorCriticMixin:
             cur = self._core_steps(core)
             steps = tuple(_bind_optimizer(o, m, s3, c) for (o, m, s3), c in zip(triples, cur))
             if steps != cur:
-                self._restart_core(core, steps)
+                core.restart(steps)
         return core
 
     # the CUDA learner trains on reward - lambda * cost when the safety module has a multiplier (TD3 / DDPG / TD3BC)
@@ -292,18 +290,6 @@ if HAVE_REFERENCE:
         def _module_pairs(self, core):
             return [(self._actor, core.actor_params), (self._critic, core.critic_params), (self._critic_target, core.critic_target_params)]
 
-        def _core_steps(self, core):
-            s = int(core._lib.prl_sac_adam_step(core._handle)) if core._handle.value else int(core._adam_step)
-            return (s, s)
-
-        def _restart_core(self, core, steps):
-            if steps[0] != steps[1]:
-                raise NotImplementedError("SAC steps its actor and critics once per round: one AdamW step count")
-            if core._handle.value:
-                core._lib.prl_sac_destroy(core._handle)
-                core._handle = C.c_void_p(0)
-            core._adam_step = int(steps[0])
-
         def _bind_extras(self, core):
             """Entropy coefficient: `_log_entropy` (Parameter) and its AdamW state are the 4 floats of the CUDA learner's
             log-entropy block, `_entropy_coef` (buffer, shape kept) a view of its coefficient.  A state loaded into the
@@ -325,12 +311,12 @@ if HAVE_REFERENCE:
                 blk[1:2].copy_(st[p]["exp_avg"].reshape(1))
                 blk[2:3].copy_(st[p]["exp_avg_sq"].reshape(1))
                 blk[3:4].copy_(st[p].get("max_exp_avg_sq", st[p]["exp_avg_sq"]).reshape(1))
-            st[p] = dict(step=torch.tensor(float(self._core_steps(core)[0])), exp_avg=blk[1:2], exp_avg_sq=blk[2:3],
+            st[p] = dict(step=torch.tensor(float(core.adam_steps()[0])), exp_avg=blk[1:2], exp_avg_sq=blk[2:3],
                          max_exp_avg_sq=blk[3:4])
 
         def _after_learn(self, core):
             if self._entropy_autotune:
-                _set_steps(self._entropy_optimizer, self._core_steps(core)[0])
+                _set_steps(self._entropy_optimizer, core.adam_steps()[0])
 
     class B200SoftActorCritic(_B200ActorCriticMixin, _RefSACD):
         """Drop-in for `pearl...soft_actor_critic.SoftActorCritic` (discrete actions): VanillaActorNetwork and
@@ -368,18 +354,6 @@ if HAVE_REFERENCE:
         def _module_pairs(self, core):
             return [(self._actor, core.actor_params), (self._critic, core.critic_params), (self._critic_target, core.critic_target_params)]
 
-        def _core_steps(self, core):
-            s = int(core._lib.prl_sacd_adam_step(core._handle)) if core._handle.value else int(core._adam_step)
-            return (s, s)
-
-        def _restart_core(self, core, steps):
-            if steps[0] != steps[1]:
-                raise NotImplementedError("discrete SAC steps its actor and critics once per round: one AdamW step count")
-            if core._handle.value:
-                core._lib.prl_sacd_destroy(core._handle)
-                core._handle = C.c_void_p(0)
-            core._adam_step = int(steps[0])
-
         def _apply_learning_rates(self, core, lrs):
             core.set_learning_rates(*lrs)
 
@@ -396,7 +370,7 @@ if HAVE_REFERENCE:
             hp = _adam_lr_eps(self._entropy_optimizer)
             if hp != (core._entropy_learning_rate, core._entropy_eps):      # fixed in the handle's configuration
                 core._entropy_learning_rate, core._entropy_eps = hp
-                self._restart_core(core, self._core_steps(core))
+                core.restart()
             blk, p, st = core._log_entropy, self._log_entropy, self._entropy_optimizer.state
             if p.data_ptr() != blk.data_ptr():
                 blk[0:1].copy_(p.detach().reshape(1).to(blk))
@@ -406,11 +380,11 @@ if HAVE_REFERENCE:
             if p in st and "exp_avg" in st[p]:
                 blk[1:2].copy_(st[p]["exp_avg"].reshape(1))
                 blk[2:3].copy_(st[p]["exp_avg_sq"].reshape(1))
-            st[p] = dict(step=torch.tensor(float(self._core_steps(core)[0])), exp_avg=blk[1:2], exp_avg_sq=blk[2:3])
+            st[p] = dict(step=torch.tensor(float(core.adam_steps()[0])), exp_avg=blk[1:2], exp_avg_sq=blk[2:3])
 
         def _after_learn(self, core):
             if self._entropy_autotune:
-                _set_steps(self._entropy_optimizer, self._core_steps(core)[0])
+                _set_steps(self._entropy_optimizer, core.adam_steps()[0])
 
     class B200ProximalPolicyOptimization(_B200ActorCriticMixin, _RefPPO):
         """Drop-in for `pearl...ppo.ProximalPolicyOptimization` (discrete actions, as the reference's `_actor_loss`)."""
@@ -433,18 +407,6 @@ if HAVE_REFERENCE:
 
         def _module_pairs(self, core):
             return [(self._actor, core.actor_params), (self._critic, core.critic_params)]
-
-        def _core_steps(self, core):
-            s = int(core._lib.prl_ppo_adam_step(core._handle)) if core._handle.value else int(core._adam_step)
-            return (s, s)
-
-        def _restart_core(self, core, steps):
-            if steps[0] != steps[1]:
-                raise NotImplementedError("PPO steps actor and critic once per round: one AdamW step count")
-            if core._handle.value:
-                core._lib.prl_ppo_destroy(core._handle)
-                core._handle = C.c_void_p(0)
-            core._adam_step = int(steps[0])
 
         def preprocess_replay_buffer(self, replay_buffer, process_group=None):
             """ppo.py:201-293 on the GPU; `learn()` calls it itself (as the reference's `learn` does)."""
@@ -480,17 +442,6 @@ if HAVE_REFERENCE:
         def _module_pairs(self, core):
             return [(self._actor, core.actor_params), (self._actor_target, core.actor_target_params),
                     (self._critic, core.critic_params), (self._critic_target, core.critic_target_params)]
-
-        def _core_steps(self, core):
-            if core._handle.value:
-                return (int(core._lib.prl_td3_actor_adam_step(core._handle)), int(core._lib.prl_td3_critic_adam_step(core._handle)))
-            return tuple(int(x) for x in core._adam_steps)
-
-        def _restart_core(self, core, steps):
-            if core._handle.value:
-                core._lib.prl_td3_destroy(core._handle)
-                core._handle = C.c_void_p(0)
-            core._adam_steps = (int(steps[0]), int(steps[1]))
 
         def _bind_extras(self, core):
             """The reference's `_last_actor_loss` (TD3) is what the core's rounds without an actor update report."""
@@ -627,18 +578,6 @@ if HAVE_REFERENCE_IQL:
         def _optimizer_triples(self, core):
             return super()._optimizer_triples(core) + [(self._value_network_optimizer, self._value_network, core._value_state)]
 
-        def _core_steps(self, core):
-            s = int(core._lib.prl_iql_adam_step(core._handle)) if core._handle.value else int(core._adam_step)
-            return (s, s, s)
-
-        def _restart_core(self, core, steps):
-            if len(set(steps)) != 1:
-                raise NotImplementedError("IQL steps its actor, critics and value net once per round: one AdamW step count")
-            if core._handle.value:
-                core._lib.prl_iql_destroy(core._handle)
-                core._handle = C.c_void_p(0)
-            core._adam_step = int(steps[0])
-
         def _apply_learning_rates(self, core, lrs):
             core.set_learning_rates(*lrs, core._value_learning_rate)
 
@@ -708,18 +647,6 @@ if HAVE_REFERENCE_REINFORCE:
 
         def _module_pairs(self, core):
             return [(self._actor, core.actor_params), (self._critic, core.critic_params)]
-
-        def _core_steps(self, core):
-            s = int(core._lib.prl_reinforce_adam_step(core._handle)) if core._handle.value else int(core._adam_step)
-            return (s, s)
-
-        def _restart_core(self, core, steps):
-            if steps[0] != steps[1]:
-                raise NotImplementedError("REINFORCE steps actor and critic once per round: one AdamW step count")
-            if core._handle.value:
-                core._lib.prl_reinforce_destroy(core._handle)
-                core._handle = C.c_void_p(0)
-            core._adam_step = int(steps[0])
 
         def _apply_learning_rates(self, core, lrs):
             core.set_learning_rates(*lrs)
@@ -814,10 +741,10 @@ if HAVE_REFERENCE_QRDQN:
             if lr != core._learning_rate:
                 core.set_learning_rate(lr)
             if not _is_bound(self._optimizer, self._Q, core._state):
-                cur = core._current_adam_step()
+                cur = core.adam_steps()[0]
                 step = _bind_optimizer(self._optimizer, self._Q, core._state, cur)
                 if step != cur:
-                    core._restart(step)
+                    core.restart((step,))
             core._variance_weighting_coefficient = _qrdqn_beta(getattr(self, "safety_module", None))
             core._training_rounds, core._batch_size = int(self._training_rounds), int(self._batch_size)
             core._training_steps = int(self._training_steps)
@@ -830,7 +757,7 @@ if HAVE_REFERENCE_QRDQN:
             core = self._ensure_core()
             report = core.learn(replay_buffer)
             self._training_steps = int(core._training_steps)
-            _set_steps(self._optimizer, core._current_adam_step())
+            _set_steps(self._optimizer, core.adam_steps()[0])
             return report
 
         def learn_batch(self, batch) -> dict:
@@ -838,7 +765,7 @@ if HAVE_REFERENCE_QRDQN:
             reference it does not advance the training-step count."""
             core = self._ensure_core()
             report = core.learn_batch(batch)
-            _set_steps(self._optimizer, core._current_adam_step())
+            _set_steps(self._optimizer, core.adam_steps()[0])
             return report
 
 else:

@@ -23,11 +23,14 @@ from typing import Any, Iterable, Optional
 import torch
 
 from . import _lib
+from ._core import FlatCore, _bounds
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
-from .sac import _bounds
 
 
-class B200ImplicitQLearning:
+class B200ImplicitQLearning(FlatCore):
+    _ABI = "prl_iql"
+    _ONE_STEP = "IQL steps its actor, critics and value net once per round: one AdamW step count"
+
     def __init__(self, state_dim: int, action_space: Any = None, actor_hidden_dims: Optional[Iterable[int]] = None,
                  critic_hidden_dims: Optional[Iterable[int]] = None, value_critic_hidden_dims: Optional[Iterable[int]] = None,
                  value_critic_learning_rate: float = 1e-3, actor_learning_rate: float = 1e-3, critic_learning_rate: float = 1e-3,
@@ -35,10 +38,7 @@ class B200ImplicitQLearning:
                  batch_size: int = 128, expectile: float = 0.5, temperature_advantage_weighted_regression: float = 0.5,
                  advantage_clamp: float = 100.0, *, n_actions: Optional[int] = None, low=None, high=None,
                  device: Optional[torch.device | str | int] = None, max_rounds_per_call: int = 1024, seed: Optional[int] = None) -> None:
-        self._device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        if self._device.index is None:
-            self._device = torch.device("cuda", torch.cuda.current_device())
-        self._lib = _lib.init(self._device.index)
+        self._open(device, training_rounds, batch_size, max_rounds_per_call, seed)
         dims = [list(d or []) for d in (actor_hidden_dims, critic_hidden_dims, value_critic_hidden_dims)]
         if any(len(d) != 2 for d in dims):
             raise NotImplementedError("the CUDA IQL learner is built for two hidden layers in the actor, each critic and the value net")
@@ -57,18 +57,9 @@ class B200ImplicitQLearning:
         self._actor_learning_rate, self._critic_learning_rate = float(actor_learning_rate), float(critic_learning_rate)
         self._value_learning_rate = float(value_critic_learning_rate)
         self._critic_soft_update_tau, self._discount_factor = float(critic_soft_update_tau), float(discount_factor)
-        self._training_rounds, self._batch_size = int(training_rounds), int(batch_size)
         self._expectile = float(expectile)
         self._temperature = float(temperature_advantage_weighted_regression)
         self._advantage_clamp = float(advantage_clamp)
-        self._max_rounds = max(int(max_rounds_per_call), 1)
-        self._training_steps = 0
-        self.use_cuda_graph = True       # False: plain stream launches (profilers)
-        self._handle = C.c_void_p(0)
-        self._bound_batch = 0
-        self._gen = torch.Generator(device=self._device)
-        if seed is not None:
-            self._gen.manual_seed(int(seed))
         cfg = self._cfg(1)
         pa, pc, pv = (int(self._lib.prl_iql_actor_param_count(C.byref(cfg))), int(self._lib.prl_iql_critic_param_count(C.byref(cfg))),
                       int(self._lib.prl_iql_value_param_count(C.byref(cfg))))
@@ -83,7 +74,6 @@ class B200ImplicitQLearning:
         self._actor_state = [torch.zeros(pa, dtype=f32, device=dev) for _ in range(3)]      # exp_avg, exp_avg_sq, max_exp_avg_sq
         self._critic_state = [torch.zeros(2 * pc, dtype=f32, device=dev) for _ in range(3)]
         self._value_state = [torch.zeros(pv, dtype=f32, device=dev) for _ in range(3)]
-        self._adam_step = 0
 
     # ------------------------------------------------------------------ parameters
     def _cfg(self, max_batch: int) -> _lib.IqlCfg:
@@ -103,38 +93,17 @@ class B200ImplicitQLearning:
         """Actor and critics: Xavier-uniform weights, biases 0.01 (neural_networks/common/utils.py xavier_init_weights, as
         actor_critic_base.py and twin_critic.py apply it).  Value net: torch's default nn.Linear initialisation
         (VanillaValueNetwork is not re-initialised): weights and biases U(-1/sqrt(fan_in), 1/sqrt(fan_in))."""
-        def fill(vec, shapes, xavier):
-            off, fan_in = 0, 1
-            for shp in shapes:
-                n = shp[0] * (shp[1] if len(shp) == 2 else 1)
-                if len(shp) == 2:
-                    fan_in = shp[1]
-                    bound = (6.0 / (shp[0] + shp[1])) ** 0.5 if xavier else fan_in ** -0.5
-                    vec[off:off + n].uniform_(-bound, bound, generator=self._gen)
-                elif xavier:
-                    vec[off:off + n].fill_(0.01)
-                else:
-                    vec[off:off + n].uniform_(-fan_in ** -0.5, fan_in ** -0.5, generator=self._gen)
-                off += n
-            assert off == vec.numel()
         sa, sc, sv = self._shapes()
-        fill(self.actor_params, sa, True)
-        pc = self.critic_params.numel() // 2
-        fill(self.critic_params[:pc], sc, True)
-        fill(self.critic_params[pc:], sc, True)
-        fill(self.value_params, sv, False)
+        self._fill(self.actor_params, sa)
+        self._fill(self.critic_params, 2 * sc)
+        self._fill(self.value_params, sv, xavier=False)
 
     def load_parameters(self, actor, q1, q2, value, q1_target=None, q2_target=None) -> None:
         """Flat fp32 vectors in `torch.nn.Module.parameters()` order of the reference networks (VanillaActorNetwork or
         VanillaContinuousActorNetwork, VanillaQValueNetwork over state || action, VanillaValueNetwork)."""
-        t = lambda x: torch.as_tensor(x, dtype=torch.float32).reshape(-1).to(self._device)  # noqa: E731
-        pc = self.critic_params.numel() // 2
-        self.actor_params.copy_(t(actor))
-        self.critic_params[:pc].copy_(t(q1))
-        self.critic_params[pc:].copy_(t(q2))
-        self.value_params.copy_(t(value))
-        self.critic_target_params[:pc].copy_(t(q1 if q1_target is None else q1_target))
-        self.critic_target_params[pc:].copy_(t(q2 if q2_target is None else q2_target))
+        pc, c, t = self.critic_params.numel() // 2, self.critic_params, self.critic_target_params
+        self._load((self.actor_params, actor), (c[:pc], q1), (c[pc:], q2), (self.value_params, value),
+                   (t[:pc], q1 if q1_target is None else q1_target), (t[pc:], q2 if q2_target is None else q2_target))
 
     def set_learning_rates(self, actor_learning_rate: float, critic_learning_rate: float, value_critic_learning_rate: float) -> None:
         """New AdamW learning rates from the next call on; the C handle and its captured graphs are kept."""
@@ -144,86 +113,35 @@ class B200ImplicitQLearning:
             _lib.check(self._lib.prl_iql_set_lr(self._handle, self._actor_learning_rate, self._critic_learning_rate,
                                                 self._value_learning_rate))
 
-    @property
-    def batch_size(self) -> int:
-        return self._batch_size
-
-    @property
-    def training_rounds(self) -> int:
-        return self._training_rounds
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None) and self._handle.value:
-                self._lib.prl_iql_destroy(self._handle)
-                self._handle = C.c_void_p(0)
-        except Exception:
-            pass
-
-    def _bind(self, need_batch: int) -> None:
-        if self._handle.value and need_batch <= self._bound_batch:
-            return
-        if self._handle.value:
-            self._adam_step = int(self._lib.prl_iql_adam_step(self._handle))
-            self._lib.prl_iql_destroy(self._handle)
-            self._handle = C.c_void_p(0)
-        cfg = self._cfg(max(need_batch, self._batch_size if self._batch_size > 0 else need_batch))
-        self._workspace = torch.empty(int(self._lib.prl_iql_workspace_bytes(C.byref(cfg))), dtype=torch.uint8, device=self._device)
-        h = C.c_void_p(0)
+    def _create(self, h, cfg) -> int:
         p = _lib.ptr
-        with torch.cuda.device(self._device):
-            _lib.check(self._lib.prl_iql_create(
-                C.byref(h), C.byref(cfg), p(self.actor_params), p(self._actor_state[0]), p(self._actor_state[1]), p(self._actor_state[2]),
-                p(self.critic_params), p(self._critic_state[0]), p(self._critic_state[1]), p(self._critic_state[2]),
-                p(self.critic_target_params), p(self.value_params), p(self._value_state[0]), p(self._value_state[1]),
-                p(self._value_state[2]), p(self._low), p(self._high), self._adam_step, p(self._workspace)))
-        self._handle, self._bound_batch = h, cfg.max_batch
+        return self._lib.prl_iql_create(
+            C.byref(h), C.byref(cfg), p(self.actor_params), p(self._actor_state[0]), p(self._actor_state[1]), p(self._actor_state[2]),
+            p(self.critic_params), p(self._critic_state[0]), p(self._critic_state[1]), p(self._critic_state[2]),
+            p(self.critic_target_params), p(self.value_params), p(self._value_state[0]), p(self._value_state[1]),
+            p(self._value_state[2]), p(self._low), p(self._high), self._adam_steps[0], p(self._workspace))
 
     def _bits(self, rounds: int) -> torch.Tensor:
         """The round's two `torch.randint(0, 2, (1,))` draws of the reference (value loss, then actor loss), in one draw."""
         return torch.randint(0, 2, (rounds, 2)).to(device=self._device, dtype=torch.int32)
 
-    @staticmethod
-    def _report(host: torch.Tensor) -> dict:
-        return {"value_loss": host[0].tolist(), "actor_loss": host[2].tolist(), "critic_loss": host[1].tolist()}
+    # the rows of prl_iql_learn's outputs each report key reads
+    _ROWS = {"value_loss": 0, "actor_loss": 2, "critic_loss": 1}
 
     # ------------------------------------------------------------------ PolicyLearner.learn (policy_learner.py:162-204)
     def learn(self, replay_buffer: B200ReplayBuffer, trace: Optional[dict] = None) -> dict:
-        if not isinstance(replay_buffer, B200ReplayBuffer):
-            raise TypeError("B200ImplicitQLearning learns from a B200ReplayBuffer (GPU-resident ring)")
-        if len(replay_buffer) == 0:
+        if not self._accepts(replay_buffer, not self._discrete,
+                             f"IQL configured for {'discrete' if self._discrete else 'continuous'} actions needs a replay buffer "
+                             f"with is_action_continuous={not self._discrete}"):
             return {}
-        if bool(replay_buffer.is_action_continuous) == self._discrete:
-            raise ValueError(f"IQL configured for {'discrete' if self._discrete else 'continuous'} actions needs a replay buffer with "
-                             f"is_action_continuous={not self._discrete}")
-        B = len(replay_buffer) if (self._batch_size == -1 or len(replay_buffer) < self._batch_size) else self._batch_size
+        B = self._batch(len(replay_buffer))
         self._bind(B)
-        R, dev = self._training_rounds, self._device
-        report = {"value_loss": [], "actor_loss": [], "critic_loss": []}
-        idx_all = []
-        done = 0
-        while done < R:
-            r = min(self._max_rounds, R - done)
+
+        def chunk(r, done, out, idx):
             bits = self._bits(r)
-            out = torch.empty((3, r), dtype=torch.float32, device=dev)
-            idx = torch.empty((r, B), dtype=torch.int32, device=dev) if trace is not None else None
-            replay_buffer._rng_push()
-            with torch.cuda.device(dev):
-                _lib.check(self._lib.prl_iql_set_graph(self._handle, int(self.use_cuda_graph)))
-                _lib.check(self._lib.prl_iql_learn(self._handle, replay_buffer.handle, r, B, _lib.ptr(bits), _lib.ptr(out[0]),
-                                                   _lib.ptr(out[1]), _lib.ptr(out[2]), _lib.ptr(idx) if idx is not None else None,
-                                                   _stream_ptr(dev)))
-            replay_buffer._rng_pull()
-            for k, v in self._report(out.cpu()).items():
-                report[k] += v
-            if idx is not None:
-                idx_all.append(idx.cpu())
-            done += r
-        self._training_steps += R
-        if trace is not None:
-            trace["idx"] = torch.cat(idx_all)
-            trace["launches"] = int(self._lib.prl_iql_last_launches(self._handle))
-        return report
+            return self._lib.prl_iql_learn(self._handle, replay_buffer.handle, r, B, _lib.ptr(bits), _lib.ptr(out[0]), _lib.ptr(out[1]),
+                                           _lib.ptr(out[2]), _lib.ptr(idx), _stream_ptr(self._device))
+        return self._rounds(replay_buffer, B, trace, 3, self._ROWS, chunk)
 
     def _action_ids(self, a: torch.Tensor) -> torch.Tensor:
         """Action ids from the one-hot rows the reference's preprocess_batch produces, or from raw ids ([B] or [B, 1])."""
@@ -260,4 +178,5 @@ class B200ImplicitQLearning:
             _lib.check(self._lib.prl_iql_learn_batch(self._handle, B, _lib.ptr(state), _lib.ptr(act), _lib.ptr(aid), _lib.ptr(reward),
                                                      _lib.ptr(next_state), _lib.ptr(term), _lib.ptr(bits), _lib.ptr(out[0]),
                                                      _lib.ptr(out[1]), _lib.ptr(out[2]), _stream_ptr(dev)))
-        return {k: v[0] for k, v in self._report(out.cpu()).items()}
+        host = out.cpu()
+        return {k: host[row].tolist()[0] for k, row in self._ROWS.items()}

@@ -21,8 +21,8 @@ from typing import Any, Iterable, Optional
 import torch
 
 from . import _lib
+from ._core import Handle, _bounds, fill_like_reference
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
-from .sac import _bounds
 from .td3 import B200TD3
 
 try:  # pragma: no cover - depends on the environment
@@ -45,8 +45,9 @@ def _td3_core(policy_learner) -> B200TD3:
                               f"(pearl_b200), not {type(policy_learner).__name__}")
 
 
-class _CostStep:
+class _CostStep(Handle):
     """The CUDA cost-critic step: flat twin cost critic, its target, AdamW vectors and the C handle."""
+    _ABI = "prl_rcsafety"
 
     def __init__(self, state_dim: int, action_dim: int, critic_hidden_dims, *, critic_learning_rate: float, cost_discount_factor: float,
                  critic_soft_update_tau: float, device: torch.device, seed: Optional[int] = None) -> None:
@@ -61,7 +62,7 @@ class _CostStep:
         self.use_cuda_graph = True
         self._handle = C.c_void_p(0)
         self._bound = (0, 0, 0)               # (max_batch, actor_h1, actor_h2) of the handle
-        self._adam_step = 0
+        self._adam_steps = (0,)
         pc = int(self._lib.prl_rcsafety_param_count(C.byref(self._cfg(1, 1, 1))))
         f32 = torch.float32
         self.params = torch.empty(2 * pc, dtype=f32, device=device)
@@ -69,15 +70,8 @@ class _CostStep:
         if seed is not None:
             gen.manual_seed(int(seed))
         O, A, (c1, c2) = self._state_dim, self._action_dim, dims
-        off = 0
-        for net in range(2):     # Xavier-uniform weights, biases 0.01, as the reference's VanillaQValueNetwork
-            for shp in [(c1, O + A), (c1,), (c2, c1), (c2,), (1, c2), (1,)]:
-                n = shp[0] * (shp[1] if len(shp) == 2 else 1)
-                if len(shp) == 2:
-                    self.params[off:off + n].uniform_(-(6.0 / sum(shp)) ** 0.5, (6.0 / sum(shp)) ** 0.5, generator=gen)
-                else:
-                    self.params[off:off + n].fill_(0.01)
-                off += n
+        # Xavier-uniform weights, biases 0.01, as the reference's VanillaQValueNetwork
+        fill_like_reference(self.params, 2 * [(c1, O + A), (c1,), (c2, c1), (c2,), (1, c2), (1,)], gen)
         self.target_params = self.params.clone()
         self.state = [torch.zeros(2 * pc, dtype=f32, device=device) for _ in range(3)]   # exp_avg, exp_avg_sq, max_exp_avg_sq
         self._out = torch.zeros(3, dtype=torch.float64, device=device)
@@ -88,35 +82,18 @@ class _CostStep:
 
     @property
     def adam_step(self) -> int:
-        return int(self._lib.prl_rcsafety_adam_step(self._handle)) if self._handle.value else self._adam_step
-
-    def restart(self, step: Optional[int] = None) -> None:
-        """Drop the C handle; the next call re-creates it (with the current learning rate) at `step` or the current count."""
-        step = self.adam_step if step is None else int(step)
-        if self._handle.value:
-            self._lib.prl_rcsafety_destroy(self._handle)
-            self._handle = C.c_void_p(0)
-        self._adam_step = step
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None) and self._handle.value:
-                self._lib.prl_rcsafety_destroy(self._handle)
-                self._handle = C.c_void_p(0)
-        except Exception:
-            pass
+        return self.adam_steps()[0]
 
     def _bind(self, batch: int, h1: int, h2: int) -> None:
         if self._handle.value and batch <= self._bound[0] and (h1, h2) == self._bound[1:]:
             return
-        step = self.adam_step
-        self.restart(step)
+        self.restart()
         cfg = self._cfg(batch, h1, h2)
         self._workspace = torch.empty(int(self._lib.prl_rcsafety_workspace_bytes(C.byref(cfg))), dtype=torch.uint8, device=self._device)
         h, p = C.c_void_p(0), _lib.ptr
         with torch.cuda.device(self._device):
             _lib.check(self._lib.prl_rcsafety_create(C.byref(h), C.byref(cfg), p(self.params), p(self.state[0]), p(self.state[1]),
-                                                     p(self.state[2]), p(self.target_params), step, p(self._workspace)))
+                                                     p(self.state[2]), p(self.target_params), self._adam_steps[0], p(self._workspace)))
         self._handle, self._bound = h, (batch, h1, h2)
 
     def run(self, replay_buffer: B200ReplayBuffer, core: B200TD3, batch: int, lam: float, constraint_value: float, lr_lambda: float,
@@ -333,7 +310,7 @@ if HAVE_REFERENCE_RC:  # pragma: no cover - depends on the environment
                 cur = step.adam_step
                 got = _bind_optimizer(self.cost_critic_optimizer, self.cost_critic, step.state, cur)
                 if got != cur:
-                    step.restart(got)
+                    step.restart((got,))
             return step
 
         def _after_step(self, step):

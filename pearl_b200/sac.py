@@ -14,32 +14,21 @@ from typing import Any, Iterable, Optional
 import torch
 
 from . import _lib
+from ._core import FlatCore, _bounds
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
 
 
-def _bounds(action_space, low, high, device):
-    if action_space is not None:
-        low, high = getattr(action_space, "low"), getattr(action_space, "high")
-    if low is None or high is None:
-        raise ValueError("continuous SAC needs a box action space (`action_space.low/.high`) or explicit low/high")
-    lo = torch.as_tensor(low, dtype=torch.float32).reshape(-1).to(device).contiguous()
-    hi = torch.as_tensor(high, dtype=torch.float32).reshape(-1).to(device).contiguous()
-    if lo.shape != hi.shape:
-        raise ValueError("low / high shapes differ")
-    return lo, hi
+class B200ContinuousSoftActorCritic(FlatCore):
+    _ABI = "prl_sac"
+    _ONE_STEP = "SAC steps its actor and critics once per round: one AdamW step count"
 
-
-class B200ContinuousSoftActorCritic:
     def __init__(self, state_dim: int, action_space: Any = None, actor_hidden_dims: Optional[Iterable[int]] = None,
                  critic_hidden_dims: Optional[Iterable[int]] = None, actor_learning_rate: float = 1e-3,
                  critic_learning_rate: float = 1e-3, critic_soft_update_tau: float = 0.005, discount_factor: float = 0.99,
                  training_rounds: int = 100, batch_size: int = 256, entropy_coef: float = 0.2, entropy_autotune: bool = True,
                  *, low=None, high=None, device: Optional[torch.device | str | int] = None, max_rounds_per_call: int = 1024,
                  seed: Optional[int] = None) -> None:
-        self._device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        if self._device.index is None:
-            self._device = torch.device("cuda", torch.cuda.current_device())
-        self._lib = _lib.init(self._device.index)
+        self._open(device, training_rounds, batch_size, max_rounds_per_call, seed)
         actor_hidden_dims, critic_hidden_dims = list(actor_hidden_dims or []), list(critic_hidden_dims or [])
         if len(actor_hidden_dims) != 2 or len(critic_hidden_dims) != 2:
             raise NotImplementedError("the CUDA SAC learner is built for two hidden layers in the actor and in each critic")
@@ -49,16 +38,7 @@ class B200ContinuousSoftActorCritic:
         self._actor_hidden_dims, self._critic_hidden_dims = actor_hidden_dims, critic_hidden_dims
         self._actor_learning_rate, self._critic_learning_rate = float(actor_learning_rate), float(critic_learning_rate)
         self._critic_soft_update_tau, self._discount_factor = float(critic_soft_update_tau), float(discount_factor)
-        self._training_rounds, self._batch_size = int(training_rounds), int(batch_size)
         self._entropy_autotune = bool(entropy_autotune)
-        self._max_rounds = max(int(max_rounds_per_call), 1)
-        self._training_steps = 0
-        self.use_cuda_graph = True       # False: plain stream launches (profilers)
-        self._handle = C.c_void_p(0)
-        self._bound_batch = 0
-        self._gen = torch.Generator(device=self._device)
-        if seed is not None:
-            self._gen.manual_seed(int(seed))
         cfg = self._cfg(1)
         pa, pc = int(self._lib.prl_sac_actor_param_count(C.byref(cfg))), int(self._lib.prl_sac_critic_param_count(C.byref(cfg)))
         dev, f32 = self._device, torch.float32
@@ -70,7 +50,6 @@ class B200ContinuousSoftActorCritic:
         self._critic_state = [torch.zeros(2 * pc, dtype=f32, device=dev) for _ in range(3)]
         self._log_entropy = torch.zeros(4, dtype=f32, device=dev)                              # value + its AdamW state
         self._entropy_coef = torch.full((1,), 1.0 if entropy_autotune else float(entropy_coef), dtype=f32, device=dev)
-        self._adam_step = 0
 
     # ------------------------------------------------------------------ parameters
     def _cfg(self, max_batch: int) -> _lib.SacCfg:
@@ -90,116 +69,44 @@ class B200ContinuousSoftActorCritic:
     def _init_like_reference(self) -> None:
         """Xavier-uniform weights, biases 0.01 (neural_networks/common/utils.py:201-205, applied to the actor at
         actor_critic_base.py:154 and to both critics at twin_critic.py:36-60)."""
-        def fill(vec, shapes):
-            off = 0
-            for shp in shapes:
-                if len(shp) == 2:
-                    n = shp[0] * shp[1]
-                    bound = (6.0 / (shp[0] + shp[1])) ** 0.5
-                    vec[off:off + n].uniform_(-bound, bound, generator=self._gen)
-                else:
-                    n = shp[0]
-                    vec[off:off + n].fill_(0.01)
-                off += n
-            assert off == vec.numel()
-        fill(self.actor_params, self._actor_shapes())
-        pc = self.critic_params.numel() // 2
-        fill(self.critic_params[:pc], self._critic_shapes())
-        fill(self.critic_params[pc:], self._critic_shapes())
+        self._fill(self.actor_params, self._actor_shapes())
+        self._fill(self.critic_params, 2 * self._critic_shapes())
 
     def load_parameters(self, actor, q1, q2, q1_target=None, q2_target=None) -> None:
         """Flat fp32 vectors in `torch.nn.Module.parameters()` order of the reference networks (actor: body, fc_mu,
         fc_std; critics: VanillaQValueNetwork)."""
-        t = lambda x: torch.as_tensor(x, dtype=torch.float32).reshape(-1).to(self._device)  # noqa: E731
-        pc = self.critic_params.numel() // 2
-        self.actor_params.copy_(t(actor))
-        self.critic_params[:pc].copy_(t(q1))
-        self.critic_params[pc:].copy_(t(q2))
-        self.critic_target_params[:pc].copy_(t(q1 if q1_target is None else q1_target))
-        self.critic_target_params[pc:].copy_(t(q2 if q2_target is None else q2_target))
+        pc, c, t = self.critic_params.numel() // 2, self.critic_params, self.critic_target_params
+        self._load((self.actor_params, actor), (c[:pc], q1), (c[pc:], q2), (t[:pc], q1 if q1_target is None else q1_target),
+                   (t[pc:], q2 if q2_target is None else q2_target))
 
     @property
     def entropy_coef(self) -> float:
         return float(self._entropy_coef.item())
 
-    @property
-    def batch_size(self) -> int:
-        return self._batch_size
-
-    @property
-    def training_rounds(self) -> int:
-        return self._training_rounds
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None) and self._handle.value:
-                self._lib.prl_sac_destroy(self._handle)
-                self._handle = C.c_void_p(0)
-        except Exception:
-            pass
-
-    def _bind(self, need_batch: int) -> None:
-        if self._handle.value and need_batch <= self._bound_batch:
-            return
-        if self._handle.value:
-            self._adam_step = int(self._lib.prl_sac_adam_step(self._handle))
-            self._lib.prl_sac_destroy(self._handle)
-            self._handle = C.c_void_p(0)
-        cfg = self._cfg(max(need_batch, self._batch_size if self._batch_size > 0 else need_batch))
-        nbytes = int(self._lib.prl_sac_workspace_bytes(C.byref(cfg)))
-        self._workspace = torch.empty(nbytes, dtype=torch.uint8, device=self._device)
-        h = C.c_void_p(0)
+    def _create(self, h, cfg) -> int:
         p = _lib.ptr
-        with torch.cuda.device(self._device):
-            _lib.check(self._lib.prl_sac_create(
-                C.byref(h), C.byref(cfg), p(self.actor_params), p(self._actor_state[0]), p(self._actor_state[1]),
-                p(self._actor_state[2]), p(self.critic_params), p(self._critic_state[0]), p(self._critic_state[1]),
-                p(self._critic_state[2]), p(self.critic_target_params), p(self._log_entropy), p(self._entropy_coef),
-                p(self._low), p(self._high), self._adam_step, p(self._workspace)))
-        self._handle, self._bound_batch = h, cfg.max_batch
+        return self._lib.prl_sac_create(
+            C.byref(h), C.byref(cfg), p(self.actor_params), p(self._actor_state[0]), p(self._actor_state[1]), p(self._actor_state[2]),
+            p(self.critic_params), p(self._critic_state[0]), p(self._critic_state[1]), p(self._critic_state[2]),
+            p(self.critic_target_params), p(self._log_entropy), p(self._entropy_coef), p(self._low), p(self._high),
+            self._adam_steps[0], p(self._workspace))
 
     # ------------------------------------------------------------------ PolicyLearner.learn (policy_learner.py:162-204)
     def learn(self, replay_buffer: B200ReplayBuffer, noise: Optional[torch.Tensor] = None, trace: Optional[dict] = None) -> dict:
-        if not isinstance(replay_buffer, B200ReplayBuffer):
-            raise TypeError("B200ContinuousSoftActorCritic learns from a B200ReplayBuffer (GPU-resident ring)")
-        if len(replay_buffer) == 0:
+        if not self._accepts(replay_buffer, True, "continuous SAC needs a replay buffer with is_action_continuous=True"):
             return {}
-        if not replay_buffer.is_action_continuous:
-            raise ValueError("continuous SAC needs a replay buffer with is_action_continuous=True")
-        B = len(replay_buffer) if (self._batch_size == -1 or len(replay_buffer) < self._batch_size) else self._batch_size
+        B = self._batch(len(replay_buffer))
         self._bind(B)
-        R, A, dev = self._training_rounds, self._action_dim, self._device
-        report = {"actor_loss": [], "critic_loss": []}
-        if self._entropy_autotune:
-            report["entropy_coef"] = []
-        idx_all = []
-        done = 0
-        while done < R:
-            r = min(self._max_rounds, R - done)
+        A, dev = self._action_dim, self._device
+
+        def chunk(r, done, out, idx):
             if noise is not None:
                 nz = noise[done:done + r].to(device=dev, dtype=torch.float32).contiguous()
                 if tuple(nz.shape) != (r, 2, B, A):
                     raise ValueError(f"noise must be [rounds, 2, {B}, {A}]")
             else:
                 nz = torch.randn((r, 2, B, A), dtype=torch.float32, device=dev, generator=self._gen)
-            out = torch.empty((3, r), dtype=torch.float32, device=dev)
-            idx = torch.empty((r, B), dtype=torch.int32, device=dev) if trace is not None else None
-            replay_buffer._rng_push()
-            with torch.cuda.device(dev):
-                _lib.check(self._lib.prl_sac_set_graph(self._handle, int(self.use_cuda_graph)))
-                _lib.check(self._lib.prl_sac_learn(self._handle, replay_buffer.handle, r, B, _lib.ptr(nz), _lib.ptr(out[0]),
-                                                   _lib.ptr(out[1]), _lib.ptr(out[2]), _lib.ptr(idx) if idx is not None else None,
-                                                   _stream_ptr(dev)))
-            replay_buffer._rng_pull()
-            host = out.cpu()
-            report["actor_loss"] += host[0].tolist()
-            report["critic_loss"] += host[1].tolist()
-            if self._entropy_autotune:
-                report["entropy_coef"] += host[2].tolist()
-            if idx is not None:
-                idx_all.append(idx.cpu())
-            done += r
-        self._training_steps += R
-        if trace is not None:
-            trace["idx"] = torch.cat(idx_all)
-        return report
+            return self._lib.prl_sac_learn(self._handle, replay_buffer.handle, r, B, _lib.ptr(nz), _lib.ptr(out[0]), _lib.ptr(out[1]),
+                                           _lib.ptr(out[2]), _lib.ptr(idx), _stream_ptr(dev))
+        rows = {"actor_loss": 0, "critic_loss": 1, "entropy_coef": 2} if self._entropy_autotune else {"actor_loss": 0, "critic_loss": 1}
+        return self._rounds(replay_buffer, B, trace, 3, rows, chunk)

@@ -16,11 +16,13 @@ from typing import Any, Iterable, Optional
 import torch
 
 from . import _lib
+from ._core import FlatCore, _bounds
 from .replay_buffer import B200ReplayBuffer, _stream_ptr
-from .sac import _bounds
 
 
-class B200TD3:
+class B200TD3(FlatCore):
+    _ABI = "prl_td3"
+    _STEPS = ("_actor_adam_step", "_critic_adam_step")
     _default_freq, _default_noise, _default_clip = 2, 0.2, 0.5
 
     def __init__(self, state_dim: int, action_space: Any = None, actor_hidden_dims: Optional[Iterable[int]] = None,
@@ -31,10 +33,7 @@ class B200TD3:
                  actor_update_noise_clip: Optional[float] = None, *, low=None, high=None,
                  device: Optional[torch.device | str | int] = None, max_rounds_per_call: int = 1024, seed: Optional[int] = None,
                  lambda_constraint: Optional[float] = None, safety_module: Any = None) -> None:
-        self._device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
-        if self._device.index is None:
-            self._device = torch.device("cuda", torch.cuda.current_device())
-        self._lib = _lib.init(self._device.index)
+        self._open(device, training_rounds, batch_size, max_rounds_per_call, seed)
         actor_hidden_dims, critic_hidden_dims = list(actor_hidden_dims or []), list(critic_hidden_dims or [])
         if len(actor_hidden_dims) != 2 or len(critic_hidden_dims) != 2:
             raise NotImplementedError("the CUDA TD3 / DDPG learner is built for two hidden layers in the actor and in each critic")
@@ -45,22 +44,13 @@ class B200TD3:
         self._actor_learning_rate, self._critic_learning_rate = float(actor_learning_rate), float(critic_learning_rate)
         self._actor_soft_update_tau, self._critic_soft_update_tau = float(actor_soft_update_tau), float(critic_soft_update_tau)
         self._discount_factor = float(discount_factor)
-        self._training_rounds, self._batch_size = int(training_rounds), int(batch_size)
         self._actor_update_freq = int(self._default_freq if actor_update_freq is None else actor_update_freq)
         self._actor_update_noise = float(self._default_noise if actor_update_noise is None else actor_update_noise)
         self._actor_update_noise_clip = float(self._default_clip if actor_update_noise_clip is None else actor_update_noise_clip)
-        self._max_rounds = max(int(max_rounds_per_call), 1)
-        self._training_steps = 0
         self._last_actor_loss = 0.0    # what rounds without an actor update report (td3.py:104,122)
         # the reward-constrained multiplier: `lambda_constraint` when set, else the safety module's, else no shaping
         self.lambda_constraint = None if lambda_constraint is None else float(lambda_constraint)
         self.safety_module = safety_module
-        self.use_cuda_graph = True
-        self._handle = C.c_void_p(0)
-        self._bound_batch = 0
-        self._gen = torch.Generator(device=self._device)
-        if seed is not None:
-            self._gen.manual_seed(int(seed))
         cfg = self._cfg(1)
         pa, pc = int(self._lib.prl_td3_actor_param_count(C.byref(cfg))), int(self._lib.prl_td3_critic_param_count(C.byref(cfg)))
         dev, f32 = self._device, torch.float32
@@ -71,7 +61,6 @@ class B200TD3:
         self.critic_target_params = self.critic_params.clone()
         self._actor_state = [torch.zeros(pa, dtype=f32, device=dev) for _ in range(3)]      # exp_avg, exp_avg_sq, max_exp_avg_sq
         self._critic_state = [torch.zeros(2 * pc, dtype=f32, device=dev) for _ in range(3)]
-        self._adam_steps = (0, 0)
 
     def _cfg(self, max_batch: int) -> _lib.Td3Cfg:
         return _lib.Td3Cfg(self._state_dim, self._action_dim, self._actor_hidden_dims[0], self._actor_hidden_dims[1],
@@ -85,82 +74,33 @@ class B200TD3:
 
     def _init_like_reference(self) -> None:
         """Xavier-uniform weights, biases 0.01 (neural_networks/common/utils.py:201-205, actor_critic_base.py:154, twin_critic.py:36-60)."""
-        def fill(vec, shapes):
-            off = 0
-            for shp in shapes:
-                n = shp[0] * (shp[1] if len(shp) == 2 else 1)
-                if len(shp) == 2:
-                    bound = (6.0 / (shp[0] + shp[1])) ** 0.5
-                    vec[off:off + n].uniform_(-bound, bound, generator=self._gen)
-                else:
-                    vec[off:off + n].fill_(0.01)
-                off += n
-            assert off == vec.numel()
         sa, sc = self._shapes()
-        fill(self.actor_params, sa)
-        pc = self.critic_params.numel() // 2
-        fill(self.critic_params[:pc], sc)
-        fill(self.critic_params[pc:], sc)
+        self._fill(self.actor_params, sa)
+        self._fill(self.critic_params, 2 * sc)
 
     def load_parameters(self, actor, q1, q2, actor_target=None, q1_target=None, q2_target=None) -> None:
         """Flat fp32 vectors in `torch.nn.Module.parameters()` order of the reference networks."""
-        t = lambda x: torch.as_tensor(x, dtype=torch.float32).reshape(-1).to(self._device)  # noqa: E731
-        pc = self.critic_params.numel() // 2
-        self.actor_params.copy_(t(actor))
-        self.actor_target_params.copy_(t(actor if actor_target is None else actor_target))
-        self.critic_params[:pc].copy_(t(q1)); self.critic_params[pc:].copy_(t(q2))
-        self.critic_target_params[:pc].copy_(t(q1 if q1_target is None else q1_target))
-        self.critic_target_params[pc:].copy_(t(q2 if q2_target is None else q2_target))
+        pc, c, t = self.critic_params.numel() // 2, self.critic_params, self.critic_target_params
+        self._load((self.actor_params, actor), (self.actor_target_params, actor if actor_target is None else actor_target),
+                   (c[:pc], q1), (c[pc:], q2), (t[:pc], q1 if q1_target is None else q1_target),
+                   (t[pc:], q2 if q2_target is None else q2_target))
 
-    @property
-    def batch_size(self) -> int:
-        return self._batch_size
-
-    @property
-    def training_rounds(self) -> int:
-        return self._training_rounds
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None) and self._handle.value:
-                self._lib.prl_td3_destroy(self._handle)
-                self._handle = C.c_void_p(0)
-        except Exception:
-            pass
-
-    def _bind(self, need_batch: int) -> None:
-        if self._handle.value and need_batch <= self._bound_batch:
-            return
-        if self._handle.value:
-            self._adam_steps = (int(self._lib.prl_td3_actor_adam_step(self._handle)), int(self._lib.prl_td3_critic_adam_step(self._handle)))
-            self._lib.prl_td3_destroy(self._handle)
-            self._handle = C.c_void_p(0)
-        cfg = self._cfg(max(need_batch, self._batch_size if self._batch_size > 0 else need_batch))
-        self._workspace = torch.empty(self._workspace_bytes(cfg), dtype=torch.uint8, device=self._device)
-        h = C.c_void_p(0)
+    def _create(self, h, cfg) -> int:
         p = _lib.ptr
-        args = (p(self.actor_params), p(self._actor_state[0]), p(self._actor_state[1]), p(self._actor_state[2]), p(self.actor_target_params),
-                p(self.critic_params), p(self._critic_state[0]), p(self._critic_state[1]), p(self._critic_state[2]),
-                p(self.critic_target_params), p(self._low), p(self._high), self._adam_steps[0], self._adam_steps[1], p(self._workspace))
-        with torch.cuda.device(self._device):
-            _lib.check(self._create(h, cfg, args))
-            # a handle re-created mid-training reports the learner's last actor loss, not 0, until its next actor update
-            _lib.check(self._lib.prl_td3_set_last_actor_loss(h, float(self._last_actor_loss)))
-        self._handle, self._bound_batch = h, cfg.max_batch
+        _lib.check(self._create_with(h, cfg, (
+            p(self.actor_params), p(self._actor_state[0]), p(self._actor_state[1]), p(self._actor_state[2]), p(self.actor_target_params),
+            p(self.critic_params), p(self._critic_state[0]), p(self._critic_state[1]), p(self._critic_state[2]),
+            p(self.critic_target_params), p(self._low), p(self._high), self._adam_steps[0], self._adam_steps[1], p(self._workspace))))
+        # a handle re-created mid-training reports the learner's last actor loss, not 0, until its next actor update
+        return self._lib.prl_td3_set_last_actor_loss(h, float(self._last_actor_loss))
 
-    def _workspace_bytes(self, cfg) -> int:
-        return int(self._lib.prl_td3_workspace_bytes(C.byref(cfg)))
-
-    def _create(self, h, cfg, args) -> int:
+    def _create_with(self, h, cfg, args) -> int:
         return self._lib.prl_td3_create(C.byref(h), C.byref(cfg), *args)
 
     def set_learning_rates(self, actor_lr: float, critic_lr: float) -> None:
         """New AdamW learning rates: the handle is re-created with them at the current step counts (parameters, moments and
         the last actor loss live outside it)."""
-        if self._handle.value:
-            self._adam_steps = (int(self._lib.prl_td3_actor_adam_step(self._handle)), int(self._lib.prl_td3_critic_adam_step(self._handle)))
-            self._lib.prl_td3_destroy(self._handle)
-            self._handle = C.c_void_p(0)
+        self.restart()
         self._actor_learning_rate, self._critic_learning_rate = float(actor_lr), float(critic_lr)
 
     def set_last_actor_loss(self, value: float) -> None:
@@ -194,46 +134,23 @@ class B200TD3:
 
     # ------------------------------------------------------------------ PolicyLearner.learn (policy_learner.py:162-204)
     def learn(self, replay_buffer: B200ReplayBuffer, noise: Optional[torch.Tensor] = None, trace: Optional[dict] = None) -> dict:
-        if not isinstance(replay_buffer, B200ReplayBuffer):
-            raise TypeError(f"{type(self).__name__} learns from a B200ReplayBuffer (GPU-resident ring)")
-        if len(replay_buffer) == 0:
+        if not self._accepts(replay_buffer, True, "TD3 / DDPG need a replay buffer with is_action_continuous=True"):
             return {}
-        if not replay_buffer.is_action_continuous:
-            raise ValueError("TD3 / DDPG need a replay buffer with is_action_continuous=True")
         lam = self._cost_lambda()
         if lam is not None and not replay_buffer.has_cost:
             raise ValueError("a reward-constrained multiplier is set but the replay buffer stores no costs (the reference "
                              "fails on batch.cost = None)")
-        B = len(replay_buffer) if (self._batch_size == -1 or len(replay_buffer) < self._batch_size) else self._batch_size
+        B = self._batch(len(replay_buffer))
         self._bind(B)
         self._before_call()
         with torch.cuda.device(self._device):
             _lib.check(self._lib.prl_td3_set_cost_lambda(self._handle, int(lam is not None), 0.0 if lam is None else lam))
-        R, dev = self._training_rounds, self._device
-        report = {"actor_loss": [], "critic_loss": []}
-        idx_all = []
-        done = 0
-        while done < R:
-            r = min(self._max_rounds, R - done)
+
+        def chunk(r, done, out, idx):
             nz = self._noise(noise, r, B, done)
-            out = torch.empty((2, r), dtype=torch.float32, device=dev)
-            idx = torch.empty((r, B), dtype=torch.int32, device=dev) if trace is not None else None
-            replay_buffer._rng_push()
-            with torch.cuda.device(dev):
-                _lib.check(self._lib.prl_td3_set_graph(self._handle, int(self.use_cuda_graph)))
-                _lib.check(self._lib.prl_td3_learn(self._handle, replay_buffer.handle, r, B, int(self._training_steps), _lib.ptr(nz),
-                                                   _lib.ptr(out[0]), _lib.ptr(out[1]), _lib.ptr(idx) if idx is not None else None,
-                                                   _stream_ptr(dev)))
-            replay_buffer._rng_pull()
-            host = out.cpu()
-            report["actor_loss"] += host[0].tolist()
-            report["critic_loss"] += host[1].tolist()
-            if idx is not None:
-                idx_all.append(idx.cpu())
-            self._training_steps += r
-            done += r
-        if trace is not None:
-            trace["idx"] = torch.cat(idx_all)
+            return self._lib.prl_td3_learn(self._handle, replay_buffer.handle, r, B, int(self._training_steps), _lib.ptr(nz),
+                                           _lib.ptr(out[0]), _lib.ptr(out[1]), _lib.ptr(idx), _stream_ptr(self._device))
+        report = self._rounds(replay_buffer, B, trace, 2, {"actor_loss": 0, "critic_loss": 1}, chunk)
         self._last_actor_loss = float(report["actor_loss"][-1])
         return report
 
@@ -305,7 +222,7 @@ class B200TD3BC(B200TD3):
     def _workspace_bytes(self, cfg) -> int:
         return int(self._lib.prl_td3bc_workspace_bytes(C.byref(cfg), C.byref(self._bc_cfg())))
 
-    def _create(self, h, cfg, args) -> int:
+    def _create_with(self, h, cfg, args) -> int:
         return self._lib.prl_td3bc_create(C.byref(h), C.byref(cfg), C.byref(self._bc_cfg()), _lib.ptr(self.behavior_params), *args)
 
     def _before_call(self) -> None:

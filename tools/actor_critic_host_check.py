@@ -16,6 +16,7 @@ import torch  # noqa: E402
 
 import pearl_b200  # noqa: E402
 from pearl_b200 import actor_critic as ac  # noqa: E402
+from pearl_b200._core import Handle  # noqa: E402
 from pearl.action_representation_modules.one_hot_action_representation_module import OneHotActionTensorRepresentationModule  # noqa: E402
 from pearl.utils.instantiations.spaces.box_action import BoxActionSpace  # noqa: E402
 from pearl.utils.instantiations.spaces.discrete_action import DiscreteActionSpace  # noqa: E402
@@ -29,9 +30,11 @@ def mlp_count(i, h1, h2, o):
     return h1 * i + h1 + h2 * h1 + h2 + o * h2 + o
 
 
-class Stub:
-    """What the binding touches of pearl_b200.sac / td3 / ppo learners."""
+class Stub(Handle):
+    """What the binding touches of pearl_b200.sac / td3 / ppo learners.  It never has a C handle, so adam_steps() and
+    restart() are the real lifecycle code working on the saved counts."""
     made = []
+    _ONE_STEP = "one AdamW step count"
 
     def __init__(self, **kw):
         self.kw, self._device, self._handle, self._lib = kw, CPU, C.c_void_p(0), None
@@ -48,7 +51,8 @@ class Stub:
         self.actor_target_params, self.critic_target_params = z(pa), z(pc)
         self._actor_state, self._critic_state = [z(pa) for _ in range(3)], [z(pc) for _ in range(3)]
         self._log_entropy, self._entropy_coef = z(4), torch.ones(1)
-        self._adam_step, self._adam_steps, self._training_steps = 0, (0, 0), 0
+        self._adam_steps, self._training_steps = (0, 0) if self.kind in ("td3", "ddpg") else (0,), 0
+        self._last_actor_loss = 0.0
         self._training_rounds, self._batch_size = kw["training_rounds"], kw["batch_size"]
         self._actor_learning_rate, self._critic_learning_rate = float(kw["actor_learning_rate"]), float(kw["critic_learning_rate"])
         Stub.made.append(self)
@@ -61,10 +65,15 @@ class Stub:
             t += 0.5
         self._log_entropy += 0.25
         self._entropy_coef.copy_(torch.exp(self._log_entropy[:1]))
-        self._adam_step += R
-        self._adam_steps = (self._adam_steps[0] + (R + 1) // 2, self._adam_steps[1] + R)
+        if len(self._adam_steps) == 2:    # TD3 / DDPG: the actor steps every other round
+            self._adam_steps = (self._adam_steps[0] + (R + 1) // 2, self._adam_steps[1] + R)
+        else:
+            self._adam_steps = (self._adam_steps[0] + R,)
         self._training_steps += R
         return {"actor_loss": [0.0] * R, "critic_loss": [0.0] * R}
+
+    def set_last_actor_loss(self, value):
+        self._last_actor_loss = float(value)
 
 
 def stub(kind):
@@ -127,7 +136,7 @@ l2._training_steps = l._training_steps
 assert l.compare(l2) == "", l.compare(l2)
 l2.learn(Buf())
 core2 = l2._b200
-assert core2 is not core and core2._adam_step == 8 + 4
+assert core2 is not core and core2._adam_steps == (8 + 4,)
 assert torch.equal(core2._actor_state[0], core._actor_state[0] + 0.5) and torch.equal(core2.actor_params, core.actor_params + 1)
 assert float(l2._log_entropy) == 0.5 + 0.25 and float(l2._actor_optimizer.state[next(l2._actor.parameters())]["step"]) == 12
 
@@ -137,20 +146,26 @@ sd2 = l2.state_dict()
 l.load_state_dict(sd2)
 assert not ac._is_bound(l._actor_optimizer, l._actor, core._actor_state)          # torch swapped the state tensors
 l.learn(Buf())
-assert ac._is_bound(l._actor_optimizer, l._actor, core._actor_state) and core._adam_step == 12 + 4
+assert ac._is_bound(l._actor_optimizer, l._actor, core._actor_state) and core._adam_steps == (12 + 4,)
 assert torch.equal(core._actor_state[1], core2._actor_state[1] + 0.5)
 
 # a learning-rate change (scheduler / user) reaches the CUDA learner: same vectors, same step count, new rate
 restarts = []
-orig_restart = type(l)._restart_core
-type(l)._restart_core = lambda self, c, steps: (restarts.append(steps), orig_restart(self, c, steps))[1]
+orig_restart = type(core).restart
+type(core).restart = lambda self, steps=None: (restarts.append(steps), orig_restart(self, steps))[1]
 l.learn(Buf())
 assert restarts == []                                        # nothing changed: the handle is kept
 l._actor_optimizer.param_groups[0]["lr"] = 1e-5
-at = core._adam_step
+at, = core.adam_steps()
 l.learn(Buf())
-assert restarts == [(at, at)] and core._actor_learning_rate == 1e-5 and core._critic_learning_rate == 7e-4 and core._adam_step == at + 4
-type(l)._restart_core = orig_restart
+assert restarts == [(at, at)] and core._actor_learning_rate == 1e-5 and core._critic_learning_rate == 7e-4 and core.adam_steps() == (at + 4,)
+type(core).restart = orig_restart
+# a learner with one step count refuses counts that differ
+try:
+    core.restart((at, at + 1))
+    raise SystemExit("differing step counts must be refused")
+except NotImplementedError:
+    pass
 
 # fixed entropy coefficient
 lf = pearl_b200.B200ContinuousSoftActorCritic(**dict(kw, entropy_autotune=False, entropy_coef=0.3))
